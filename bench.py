@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — RGB-D frames/s of the per-frame surfel reconstruction hot path on B200.
+"""bench.py — RGB-D frames/s of the per-frame surfel reconstruction hot path on H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl product|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl product|reference] [--dump-outputs DIR]
   torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One STEP = one pass over a whole synthetic TUM-fr1/desk-shaped 640x480 RGB-D stream
@@ -12,7 +12,7 @@ same work. At N > 1 every rank processes its own stream (BASELINE.json configs[3
 streams, one per GPU, weak scaling, no collective on the data path).
 
   value : whole-job frames/s with the stream resident in HBM (770 MB of frames per step,
-          larger than the 126 MB L2, so no L2 flush is needed between steps)
+          larger than the 50 MB L2, so no L2 flush is needed between steps)
   e2e   : the same through HOST (pinned) frame buffers: every raw depth map and colour image
           is uploaded inside the timed region (copy stream overlapped with compute, as the
           reference's main loop does) and the CUDASurfelBuffersCPU arrays are transferred back
@@ -23,10 +23,16 @@ streams, one per GPU, weak scaling, no collective on the data path).
           min-depth/association loop; the reference ships no CPU implementation) on a bounded
           sample of the same stream, on the box's host cores
 
---impl reference runs the reference's OWN kernels (unmodified .cu files rebuilt for sm_100a,
+--impl reference runs the reference's OWN kernels (unmodified .cu files rebuilt for sm_90a,
 oracle/_ref/libsurfel_ref.so) through the same stream runner and prints the same line with
 "impl": "reference". The reference implements this path only in CUDA, so its arm runs on the
 same GPU; see DESIGN.md §7.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed: the
+CUDASurfelBuffersCPU arrays of the final cloud (TransferAllToCPU), sampled at the surfels nearest
+to 262 144 fixed points on the scene's surfaces (slot order is not reproducible, see dump_outputs),
+and the step's counts, as DIR/<name>.npy (float32 / float64, fixed shapes). The input stream is
+seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -63,7 +69,7 @@ def measured_peaks():
     if p.exists():
         j = json.loads(p.read_text())
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 700 W card)"
 
 
 class ClockSampler:
@@ -131,26 +137,6 @@ def timed_steps(info, device, step_fn, warmup, steps):
     return e0.elapsed_time(e1), last
 
 
-def ncu_traffic(kernel, width):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of `kernel` from the committed
-    `ncu --set full` capture of THIS configuration (profiles/*_C2_*_traffic.json for the 640-wide streams,
-    *_C3_* for the 1280-wide one; written by tools/ncu_summary.py, latest round wins), or None."""
-    tag = {640: "_C2_", 1280: "_C3_"}.get(width)
-    best = None
-    if tag is None:
-        return None
-    for path in sorted((ROOT / "profiles").glob("*_traffic.json")):
-        if tag not in path.name:
-            continue
-        try:
-            entry = json.loads(path.read_text())["kernels"].get(kernel)
-        except (OSError, ValueError, KeyError):
-            continue
-        if entry:
-            best = float(entry["dram_bytes_per_launch"])
-    return best
-
-
 def algorithmic_bytes(kernel, c):
     """DESIGN.md §5: algorithmic bytes of one launch. c: P, K, valid, N, V, S, M, A."""
     P, K, N, V, S_, M, A, D = c["P"], c["K"], c["N"], c["V"], c["S"], c["M"], c["A"], c["D"]
@@ -213,6 +199,57 @@ def cpu_baseline(stream, pp, ip, cam, rows, frame, budget_s=24.0, runs=3, max_fr
                       f"no CPU Integrate)"}
 
 
+DUMP_PROBES = 1 << 18   # 9.4 MB of dumped arrays, well inside the 64 MB budget
+
+
+def probe_points(stream, first, last, count):
+    """`count` fixed points on the scene's surfaces, a function of the seeded input stream only: pixels with a
+    measurement, drawn with a fixed seed from the integrated frames and unprojected with their frames' poses."""
+    rng = np.random.default_rng(0)
+    cam, frames, height, width = stream.camera, stream.depth.shape[0], stream.depth.shape[1], stream.depth.shape[2]
+    f = rng.integers(first, min(last, frames), 4 * count)
+    v = rng.integers(0, height, 4 * count)
+    u = rng.integers(0, width, 4 * count)
+    index = [torch.from_numpy(i).to(stream.depth.device) for i in (f, v, u)]
+    # (gathered as int16: CUDA has no uint16 gather)
+    z = stream.depth.view(torch.int16)[tuple(index)].cpu().numpy().view(np.uint16).astype(np.float64)
+    keep = np.flatnonzero(z > 0)[:count]
+    f, v, u, z = f[keep], v[keep], u[keep], z[keep] / stream.depth_scaling
+    local = np.stack([(u + 0.5 - cam.cx) / cam.fx * z, (v + 0.5 - cam.cy) / cam.fy * z, z], axis=1)
+    pose = stream.global_T_frame[f].astype(np.float64)
+    return np.einsum("nij,nj->ni", pose[:, :, :3], local) + pose[:, :, 3]
+
+
+def dump_outputs(out_dir, rec, stats, stream, first, last):
+    """What a caller of the timed path receives after a step: the CUDASurfelBuffersCPU arrays of the cloud
+    (TransferAllToCPU at the step's last frame) and the step's counts.
+
+    The slot order of the cloud is not reproducible (which of several supporting surfels wins a pixel feeds back
+    into how many surfels each frame creates, and float atomics round differently from run to run), so the rows
+    are sampled by place, not by slot: for each of DUMP_PROBES fixed points on the scene's surfaces
+    (probe_points), the row of the nearest surfel that is not merged away. Every file has the same shape from run
+    to run and from build to build. Stamps are written as float64 (exact)."""
+    from scipy.spatial import cKDTree
+    out_dir.mkdir(parents=True, exist_ok=True)
+    buffers = rec.TransferAllToCPU(None, last - 1)
+    n = int(buffers["surfel_count"])
+    arrays = {k: (v[:n].astype(np.float64) if v.dtype == np.uint32 else v[:n])
+              for k, v in buffers.items() if k.endswith("_buffer")}
+    live = np.flatnonzero(arrays["surfel_radius_squared_buffer"] >= 0)
+    probes = probe_points(stream, first, last, DUMP_PROBES)
+    if len(live):
+        xyz = np.stack([arrays[f"surfel_{c}_buffer"][live] for c in "xyz"], axis=1).astype(np.float64)
+        _, nearest = cKDTree(xyz).query(probes)
+        rows = live[nearest]
+        sampled = {k: a[rows] for k, a in arrays.items()}
+    else:
+        sampled = {k: np.full(len(probes), np.nan, dtype=a.dtype) for k, a in arrays.items()}
+    sampled["stream_counts"] = np.array([stats.frames_integrated, stats.surfels_size, stats.surfel_count],
+                                        dtype=np.float64)
+    for name, a in sampled.items():
+        np.save(out_dir / f"{name}.npy", a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -229,7 +266,11 @@ def main():
     ap.add_argument("--erosion-radius", type=int, default=2, help="depth_erosion_radius (reference default 2)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1 (the timed steps are what the line reports and --dump-outputs writes)")
     warmup = max(args.warmup, 3)
 
     # stdout carries exactly one JSON line: NCCL's version banner (NCCL_DEBUG=VERSION) goes to stdout too
@@ -268,6 +309,8 @@ def main():
     ms_max, frames_total = D.aggregate(info, ms, frames_per_step * args.steps, device)
     ms_per_rank = D.gather_values(info, ms / args.steps, device)
     value = frames_total / (ms_max * 1e-3)
+    if args.dump_outputs and info.rank == 0:
+        dump_outputs(Path(args.dump_outputs), rec, stats, stream, first, last)
 
     # ---- e2e: host (pinned) frames in, CUDASurfelBuffersCPU arrays out ----
     host_depth = stream.depth.cpu().pin_memory()
@@ -373,7 +416,7 @@ def main():
         b = algorithmic_bytes(dom, counters)
         dur = kernel_table[dom]["mean_us"] * 1e-6
         achieved = b / dur / 1e9
-        roofline.update({"kernel": dom, "achieved": achieved, "frac": achieved / peak, "traffic": ncu_traffic(dom, cam.width),
+        roofline.update({"kernel": dom, "achieved": achieved, "frac": achieved / peak,
                          "algorithmic_bytes_per_launch": b, "mean_launch_us": kernel_table[dom]["mean_us"],
                          "pipelined_launch_us": kernel_table[dom].get("pipelined_us"),
                          "achieved_pipelined": b / (kernel_table[dom].get("pipelined_us", float("nan")) * 1e-6) / 1e9,
@@ -393,7 +436,7 @@ def main():
         else:
             cpu = {"value": value, "unit": "frames/s", "cores": 1, "kind": "reference",
                    "sample": "full workload; the reference implements this path only as CUDA kernels, so its arm "
-                             "runs them (rebuilt unmodified for sm_100a) on the same GPU, driven by one host thread"}
+                             "runs them (rebuilt unmodified for sm_90a) on the same GPU, driven by one host thread"}
 
     if info.rank == 0:
         line = {

@@ -1,5 +1,5 @@
 /*
- * surfel_b200.h — C ABI of libsurfel_b200.so, the Blackwell-native (sm_100a)
+ * surfel_b200.h — C ABI of libsurfel_b200.so, the Hopper-native (sm_90a)
  * replacement for the per-frame surfel reconstruction hot path of
  * puzzlepaint/surfelmeshing.
  *
@@ -19,7 +19,7 @@
  *    available from sm_last_error(). (Reference: no return values, CUDA errors
  *    abort through LOG(FATAL), libvis/src/libvis/cuda/cuda_util.h:35-49. The
  *    C++ adapter in surfel_b200_adapter.h maps non-zero to LOG(FATAL).)
- *  - There is NO CPU fallback: if the CUDA runtime or an sm_100 device is not
+ *  - There is NO CPU fallback: if the CUDA runtime or an sm_90 device is not
  *    available the calls fail with SM_ERR_CUDA.
  */
 #ifndef SURFEL_B200_H_
@@ -99,7 +99,7 @@ void sm_default_integrate_params(sm_integrate_params* p);
 void sm_default_preprocess_params(sm_preprocess_params* p);
 
 const char* sm_last_error(void);
-/* Library/arch identification string, e.g. "surfel_b200 sm_100a". */
+/* Library/arch identification string, e.g. "surfel_b200 0.1 (sm_90a)". */
 const char* sm_version(void);
 
 /* ---- lifecycle ----------------------------------------------------------

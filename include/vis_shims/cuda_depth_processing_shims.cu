@@ -6,7 +6,7 @@
 // :459-510, :573-587, :629-633) on top of the C ABI of libsurfel_b200.so. A maintainer of the
 // reference replaces cuda_depth_processing.cu by this file in the SurfelMeshing target
 // (applications/surfel_meshing/CMakeLists.txt:5-12) and links libsurfel_b200.so; main.cc:1015-1191 then
-// runs the sm_100a kernels without a source change. Compiled against the reference's own headers, so
+// runs the sm_90a kernels without a source change. Compiled against the reference's own headers, so
 // a signature mismatch is a compile error; oracle/Makefile builds it into
 // oracle/_ref/libsurfel_shimref.so (the reference's restated host glue + these shims) for
 // tests/test_parity_gpu.py::test_vis_depth_processing_shims.

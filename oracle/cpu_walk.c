@@ -15,7 +15,7 @@
  *   cw_associate   APP/cuda_surfel_reconstruction_kernels.cu:1466-1557 (min depth),
  *                  :1586-1808 (association)
  * Parity status: "parity unpinned" by reference tests (the reference has none for this
- * path); pinned against the reference's own kernels run on a B200 (tests/golden/, produced
+ * path); pinned against the reference's own kernels run on the GPU (tests/golden/, produced
  * by tests/golden/make_golden.py through oracle/_ref/libsurfel_ref.so). IEEE division,
  * expf and sqrtf replace the GPU's approximate MUFU ops, so u16 results may differ from the
  * GPU by 1 LSB on a small fraction of pixels (tolerance stated in tests/test_cpu_walk.py).

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE (oracle).  C entry points around the reference's own CPU meshing
 // (applications/surfel_meshing/src/surfel_meshing/{surfel_meshing.cc,octree.cc}, compiled unmodified from
-// /root/reference by oracle/Makefile against oracle/eigen_shim and oracle/libvis_stubs): BASELINE config 1, the
+// the reference sources (REF) by oracle/Makefile against oracle/eigen_shim and oracle/libvis_stubs): BASELINE config 1, the
 // pattern of the reference's triangulation test (test/test_triangulation.cc:57-98): fill CUDASurfelsCPU ->
 // IntegrateCUDABuffers -> CheckRemeshing -> Triangulate.
 //

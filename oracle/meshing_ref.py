@@ -2,8 +2,8 @@
 
 The library is the reference's own CPU meshing (surfel_meshing.cc + octree.cc compiled unmodified by oracle/Makefile
 against oracle/eigen_shim and oracle/libvis_stubs) behind oracle/meshing_driver.cc: BASELINE config 1 (random surfels
--> octree k-NN + Triangulate(), the pattern of the reference's test/test_triangulation.cc). Needs /root/reference at
-BUILD time only.
+-> octree k-NN + Triangulate(), the pattern of the reference's test/test_triangulation.cc). Needs the reference sources
+(oracle/Makefile: REF) at BUILD time only.
 """
 from __future__ import annotations
 

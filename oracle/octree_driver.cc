@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE (oracle).  C entry points around the reference's own CPU octree
-// (applications/surfel_meshing/src/surfel_meshing/octree.{h,cc}, compiled unmodified from /root/reference by
+// (applications/surfel_meshing/src/surfel_meshing/octree.{h,cc}, compiled unmodified from the reference sources (REF) by
 // oracle/Makefile against oracle/eigen_shim) so that the GPU radius k-NN (SURVEY §8 f4) can be checked against
 // CompressedOctree::FindNearestSurfelsWithinRadius (octree.cc:433-470) itself, plus a restatement of the brute-force
 // checker the reference's own octree test uses (test/test_octree.cc:116-149).  Only tests/, smoke() and the

@@ -3,7 +3,7 @@
 The library is the reference's own CPU octree (applications/surfel_meshing/src/surfel_meshing/octree.cc, compiled
 unmodified by oracle/Makefile against oracle/eigen_shim) behind the C entry points of oracle/octree_driver.cc, plus
 a restatement of the brute-force checker of the reference's octree test (test/test_octree.cc:116-149). It needs
-/root/reference at BUILD time only; the built .so travels to the GPU box.
+the reference sources (oracle/Makefile: REF) at BUILD time only.
 """
 from __future__ import annotations
 

@@ -3,7 +3,7 @@
 // Eigen-/Qt-free driver around the UNMODIFIED reference kernels. The three
 // reference translation units (APP/cuda_surfel_reconstruction_kernels.cu,
 // APP/cuda_depth_processing.cu, libvis/src/libvis/cuda/cuda_buffer.cu, plus
-// loguru.cpp) are compiled where they lie under /root/reference by
+// loguru.cpp) are compiled where they lie under the reference sources (REF) by
 // oracle/Makefile and linked with this file into oracle/_ref/libsurfel_ref.so.
 // Nothing from the reference is copied into the repository.
 //
@@ -385,7 +385,7 @@ int Preprocess(smref_reconstruction* r, cudaStream_t stream, const sm_preprocess
 extern "C" {
 
 const char* smref_last_error(void) { return g_error.c_str(); }
-const char* smref_version(void) { return "surfel_ref oracle (reference kernels rebuilt for sm_100a)"; }
+const char* smref_version(void) { return "surfel_ref oracle (reference kernels rebuilt for sm_90a)"; }
 
 int smref_create(smref_reconstruction** out, uint64_t max_surfel_count, int32_t width, int32_t height, float fx,
                  float fy, float cx, float cy) {

@@ -1,4 +1,4 @@
-"""surfelmeshing_b200 — Blackwell-native (sm_100a) per-frame surfel reconstruction.
+"""surfelmeshing_b200 — Hopper-native (sm_90a, H100) per-frame surfel reconstruction.
 
 Drop-in for the hot path of puzzlepaint/surfelmeshing: depth pre-processing and
 CUDASurfelReconstruction::Integrate()/Regularize() as hand-written CUDA kernels behind a

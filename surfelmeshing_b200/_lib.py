@@ -1,9 +1,9 @@
 """ctypes bindings of the C ABI declared in include/surfel_b200.h.
 
 The same signatures are exported twice:
-  * libsurfel_b200.so   (prefix `sm_`)    -- the product: hand-written sm_100a kernels
+  * libsurfel_b200.so   (prefix `sm_`)    -- the product: hand-written sm_90a kernels
   * oracle/_ref/libsurfel_ref.so (prefix `smref_`) -- TEST INFRASTRUCTURE: the reference's
-    own kernels rebuilt for sm_100a behind the same ABI. Only tests/, __graft_entry__.smoke()
+    own kernels rebuilt for sm_90a behind the same ABI. Only tests/, __graft_entry__.smoke()
     and bench.py's reference arm load it (see `load_reference_oracle`).
 
 There is no CPU fallback: if the product library is missing or cannot be loaded the

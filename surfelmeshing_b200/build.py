@@ -1,9 +1,9 @@
-"""Build recipe for libsurfel_b200.so (hand-written sm_100a kernels + the C ABI).
+"""Build recipe for libsurfel_b200.so (hand-written sm_90a kernels + the C ABI).
 
 `python -m surfelmeshing_b200.build` compiles every .cu under csrc/ with nvcc for
-sm_100a only (no fallback architectures) and links them in-tree into
-surfelmeshing_b200/libsurfel_b200.so, so that the library travels to the GPU box
-with the repository snapshot.
+sm_90a (H100) only (no fallback architectures) and links them in-tree into
+surfelmeshing_b200/libsurfel_b200.so, so that the package is importable from the
+repository tree.
 
 Flags: -ftz=true -fmad=false. The kernels spell out every fp32 operation (csrc/sm_math.cuh)
 in the order of the reference's -use_fast_math SASS; -fmad=false guarantees the compiler
@@ -25,7 +25,7 @@ HEADERS = ["sm_math.cuh", "sm_kernels.cuh", "sm_handle.cuh", "../../include/surf
 
 NVCC_FLAGS = [
     "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo",
     "-ftz=true", "-fmad=false", "-prec-div=true", "-prec-sqrt=true",
     "-Xcompiler", "-fPIC",
@@ -66,7 +66,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
                 raise RuntimeError(f"nvcc failed on {src}")
             (obj_dir / (src + ".ptxas.log")).write_text(res.stderr)
     if force or _stale(LIB_PATH, objects):
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", str(LIB_PATH), *map(str, objects)]
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", str(LIB_PATH), *map(str, objects)]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:
             sys.stderr.write(" ".join(cmd) + "\n" + res.stdout + res.stderr)

@@ -299,9 +299,9 @@ int CreateImpl(sm_reconstruction* r, uint64_t max_surfel_count, int32_t width, i
     // One shared-memory carve-out for every kernel of the library (SM_B200_CARVEOUT, percent of
     // the 228 KB; -1 = leave it to the driver). k_blend needs ~100 KB per block and everything else
     // a few KB; left to the driver, the SMs keep switching between configurations and the gather
-    // kernels (integrate, update_neighbors, regularisation) ran 1.5-2x slower after a blend
-    // (measured: 9.9k -> 11.7k frames/s with one configuration). 47 % selects the 132 KB
-    // configuration, the smallest that holds a blend block, and leaves 96 KB of L1 to the gathers.
+    // kernels (integrate, update_neighbors, regularisation) slow down after a blend. 47 % selects
+    // the 132 KB configuration (an H100 SM offers 0, 8, 16, 32, 64, 100, 132, 164, 196
+    // and 228 KB), the smallest that holds a blend block, and leaves 124 KB of L1 to the gathers.
     // Function attributes and occupancy are per device: configured for every handle.
     const char* e = std::getenv("SM_B200_CARVEOUT");
     const int percent = e ? std::atoi(e) : 47;
@@ -431,7 +431,7 @@ void sm_default_preprocess_params(sm_preprocess_params* p) {
 }
 
 const char* sm_last_error(void) { return g_last_error.c_str(); }
-const char* sm_version(void) { return "surfel_b200 0.1 (sm_100a)"; }
+const char* sm_version(void) { return "surfel_b200 0.1 (sm_90a)"; }
 uint64_t sm_kernel_launch_count(void) { return g_launches.load(); }
 
 int sm_profile_kernels(int32_t enable) {

@@ -1,4 +1,4 @@
-// integrate.cu — per-frame surfel reconstruction kernels for sm_100a (SURVEY §8 a6-a13).
+// integrate.cu — per-frame surfel reconstruction kernels for sm_90a (SURVEY §8 a6-a13).
 //
 // Replaces the ~36 launches and 2 host synchronisations of
 // CUDASurfelReconstruction::Integrate() (APP/cuda_surfel_reconstruction.cc:112-291) by 9
@@ -516,10 +516,11 @@ __global__ void __launch_bounds__(kBlock) k_merge(DeviceState d, FrameParams f) 
 //   3. walks the lists level by level (one thread per pixel, one barrier per level) doing the
 //      reference's float arithmetic; the search for level k + 1 runs beside the update of level k.
 // Tile 32 x 40 (VGA: 20 x 12 = 240 tiles): with the halo of a radius-12 blend the region is 64 x 62 pixels,
-// 61 KB of shared memory, so TWO blocks share an SM and all tiles of a VGA frame are resident at once;
+// 61 KB of shared memory, so TWO blocks share an SM and all tiles of a VGA frame are resident at once
+// (264 block slots on the 132 SMs of an H100);
 // both bit rasters of a level search (2 x 124 words) take one pass of the 256 threads. The kernel is a
 // chain of ~11 barrier-separated levels with little work each: what counts is how many tiles are in
-// flight per SM, not the work per tile (round 1: 80 x 32 tiles, 1 block per SM, 120 blocks: 20 us).
+// flight per SM, not the work per tile (round 1: 80 x 32 tiles, 1 block per SM, 120 blocks).
 constexpr int kBlendTileW = 32, kBlendTileH = 40;
 constexpr int kBlendBlock = 256;
 constexpr int kMaxBlendRadius = 64;
@@ -914,8 +915,10 @@ __device__ __forceinline__ void integrate_or_conflict(const FrameParams& f, cons
     const float cw = fadd(weight, confidence);
     s.confidence = (cw < f.max_surfel_confidence) ? cw : f.max_surfel_confidence;
     const float normalization_factor = frcp(cw);
-    s.x = fmul(normalization_factor, ffma(s.x, confidence, fmul(g.x, weight)));
-    s.y = fmul(normalization_factor, ffma(confidence, s.y, fmul(g.y, weight)));
+    // The reference's sm_90a SASS contracts all three coordinates as fma(g, w, c * s) (its sm_100a build
+    // contracts x as fma(s, c, g * w) and y as fma(c, s, g * w)).
+    s.x = fmul(normalization_factor, ffma(g.x, weight, fmul(confidence, s.x)));
+    s.y = fmul(normalization_factor, ffma(g.y, weight, fmul(confidence, s.y)));
     s.z = fmul(normalization_factor, ffma(g.z, weight, fmul(confidence, s.z)));
     const float nx = ffma(gn.x, weight, fmul(confidence, s.nx));
     const float ny = ffma(gn.y, weight, fmul(confidence, s.ny));

@@ -4,7 +4,7 @@
 // (APP/octree.cc:313-470) for the <= 64 nearest surfels within a squared radius, once per surfel it
 // triangulates (APP/surfel_meshing.cc:421, <false, true>: completed surfels excluded) and once per surfel it resets
 // for remeshing (APP/surfel_meshing.cc:821, <true, false>: free surfels excluded). One query walks a lazily sorted
-// compressed octree on one thread (~3.5 us for 10^4 points on this container's CPU).
+// compressed octree on one thread.
 //
 // Here the cloud is binned once per snapshot into a hashed uniform grid (counting sort by bucket: count, exclusive
 // scan, scatter of {x, y, z, index} records, so that a cell is one contiguous run of 16-byte records) and queries run

@@ -1,4 +1,4 @@
-// regularize.cu — surfel regularisation for sm_100a (SURVEY §8 a14 + the second half of a12).
+// regularize.cu — surfel regularisation for sm_90a (SURVEY §8 a14 + the second half of a12).
 //
 // Replaces RegularizeSurfelsCUDA (APP/cuda_surfel_reconstruction_kernels.cu:2099-2410: Clear,
 // Accumulate, Step, Update = 4 sweeps over all slots) and

@@ -23,26 +23,24 @@ struct TieBreakConfig {
   u32 lane_shift;        // what is in effect: lane_request, or 0 when the wave is not a multiple of it
   u32 mul, mul_inv;      // derived from wave and lane_shift
 };
-// Defaults (DESIGN.md section 4 / profiles/r02_race_stats.md have the measurements that picked them):
-// wave = the reference's AssociateSurfels launch wave on a B200 (1024-thread blocks, 31 registers ->
-// 2 blocks x 148 SMs = 296 blocks of slots); inside a wave and a kind the lower slot won 100 % of the pairs
-// that sit in one warp, ~49 % across the warps of one block and 52 - 70 % across blocks (the warps of a wave in a
-// shuffled order that keeps the lanes of a warp in order, and a quarter of the pixels in plain slot order). The
-// blocks of the FIRST wave start together; those of the later waves start one by one as earlier blocks retire, so
-// there arrival follows the slot order more closely (lower slot wins 80 % instead of 70 %) and a secondary
-// association beats a primary one of the same wave 5.4 % of the time instead of 0.6 %: separate fractions for the
-// first wave, the second (at VGA sizes only partly filled) and the later ones (1 % / 1.5 % / 3 % early secondaries,
-// 25 % / 45 % / 45 % of the pixels in slot order) put the per-frame merge flags at 1.2x the reference's own run-to-run
-// difference and the free-running totals of the 500- and 1000-frame VGA streams inside the reference's spread
-// (1280x960: -0.1 % slots, -0.06 % merges).
-constexpr u32 kDefaultTieBreakWave = 296 * 1024;
+// Defaults (DESIGN.md section 4; tools/race_stats.py + tools/race_sets_fit.py on an H100: 641 k contested pixels of
+// 31 teacher-forced frames of the 500-frame VGA stream): wave = the reference's AssociateSurfels launch wave on an
+// H100 (1024-thread blocks, 31 registers -> 2 blocks x 132 SMs = 264 blocks of slots; the earlier wave won all
+// 16 569 contests between two waves). Inside a wave and a kind the lower slot won 100 % of the pairs that sit in one
+// warp, ~49 % across the warps of one block and 50 - 74 % across blocks (the warps of a wave in a shuffled order
+// that keeps the lanes of a warp in order, and a share of the pixels in plain slot order); a secondary association
+// beat a primary one of its wave 2.9 % of the time. Separate fractions for the first wave, the second (at VGA sizes
+// only partly filled) and the later ones (1.5 % / 2 % / 4 % early secondaries, 25 % / 45 % / 45 % of the pixels in
+// slot order) put the free-running totals of the 500-frame VGA stream within 0.12 % (merges) and 0.03 % (slots) of
+// the reference's mean, less than half of its run-to-run spread.
+constexpr u32 kDefaultTieBreakWave = 264 * 1024;
 constexpr u32 kDefaultTieBreakLaneShift = 5;
 constexpr u32 kDefaultTieBreakWaveOffset = 0;
-constexpr double kDefaultTieBreakEarlyFraction = 0.01;
+constexpr double kDefaultTieBreakEarlyFraction = 0.015;
 constexpr double kDefaultTieBreakIndexOrderFraction = 0.25;
-constexpr double kDefaultTieBreakEarlyFractionLater = 0.03;
+constexpr double kDefaultTieBreakEarlyFractionLater = 0.04;
 constexpr double kDefaultTieBreakIndexOrderFractionLater = 0.45;
-constexpr double kDefaultTieBreakEarlyFractionSecond = 0.015;
+constexpr double kDefaultTieBreakEarlyFractionSecond = 0.02;
 TieBreak MakeTieBreak(const TieBreakConfig& cfg, u32 frame_index);
 int SetTieBreakWave(TieBreakConfig* cfg, u32 wave, u32 capacity);   // uses cfg->lane_request
 

@@ -65,16 +65,16 @@ constexpr u32 kActiveBit = 0x80000000u;      // VisEntry.idx: surfel was active 
 // PixelAssoc.x while a frame is processed: the arrival key of the winning association. The
 // reference lets the first atomicCAS win (kernels.cu:1688): which of several supporters of a pixel
 // becomes its supporting surfel is a race. The product takes the minimum of a key that orders the
-// associations the way the reference's race resolves ON AVERAGE (measured, tools/race_stats.py,
-// profiles/r02_race_stats.md) and is reproducible. Most significant first:
+// associations the way the reference's race resolves ON AVERAGE (measured on an H100, tools/race_stats.py,
+// DESIGN.md section 4) and is reproducible. Most significant first:
 //   wave   slots are grouped into launch waves of W slots (the reference's 1024-thread blocks are
 //          scheduled in slot order; of two supporters in different waves the earlier wave won
-//          18 406 times out of 18 407);
+//          16 569 times out of 16 569);
 //   late   set for a secondary-pixel association (a reference thread handles its primary pixel first:
-//          inside a wave a secondary beat a primary in 2.3 % of the contests) - except for a
+//          inside a wave a secondary beat a primary in 2.9 % of the contests) - except for a
 //          pseudo-random fraction `early` of them, which compete like primaries;
 //   order  inside a wave: slot order for a pseudo-random fraction of the PIXELS (per frame), a per-frame
-//          pseudo-random permutation of the slots for the others (the lower slot won 72 % of the
+//          pseudo-random permutation of the slots for the others (the lower slot won 74 % of the
 //          same-kind pairs, whatever their distance).
 // W = 0 selects the plain rule of round 1: late (= secondary) first, then lowest slot index.
 constexpr u32 kSecondaryBit = 0x80000000u;
@@ -284,9 +284,9 @@ inline unsigned long long* TimelineSlot(const DeviceState& d, u32 frame, int ker
 }
 
 // SM_B200_PDL: 0 = never, 1 (default) = only launches marked as dependents (LaunchDependent: the
-// kernel follows its producer on the same stream), 2 = every launch. Marking everything costs
-// ~3 % in the multi-stream frame pipeline (early-launched kernels take SM slots from the kernels
-// of the other streams).
+// kernel follows its producer on the same stream), 2 = every launch. Marking everything slows the
+// multi-stream frame pipeline down (early-launched kernels take SM slots from the kernels of the
+// other streams; measured on a 148-SM GPU, not re-measured on an H100).
 int PdlMode();
 int ScaleGrid(int blocks);  // SM_B200_GRID_PERCENT measurement hook (integrate.cu)
 

@@ -7,7 +7,7 @@
 // single differing ulp into different surfel counts, so the kernels in this
 // directory are compiled with -ftz=true -fmad=false and spell every float
 // operation out through the helpers below, in the operation order read from
-// the reference's sm_100a SASS (SURVEY.md Appendix B; tools/sass_arith.sh).
+// the reference's compiled SASS (SURVEY.md Appendix B; tools/sass_arith.sh).
 // Nothing here is ever contracted or re-associated by the compiler.
 #pragma once
 

@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(kBlock) k_delta_select(DeviceState d, DeltaArg
 // over all slots (UpdateSurfelVertexBufferCUDAKernel<4 bools>, UpdateNeighborIndexBufferCUDAKernel,
 // UpdateNormalVertexBufferCUDAKernel, kernels.cu:274-514); here ONE sweep reads every row once and
 // writes whichever of the three (plain device) buffers the caller passes. Arithmetic as in the
-// reference's sm_100a SASS: colour ramps are sat(fma) * 255.99 -> F2I.U32.TRUNC, the normal end point
+// reference's compiled SASS: colour ramps are sat(fma) * 255.99 -> F2I.U32.TRUNC, the normal end point
 // is fma(MUFU.SQRT(r^2), n, p).
 // ---------------------------------------------------------------------------------------------
 struct VizArgs {

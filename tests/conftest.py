@@ -2,7 +2,6 @@
 import sys
 from pathlib import Path
 
-import numpy as np
 import pytest
 
 ROOT = Path(__file__).resolve().parents[1]
@@ -11,13 +10,14 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with `-m gpu`)")
 
 
 @pytest.fixture(scope="session")
 def golden():
     """Known-answer set produced by the reference's own kernels (tests/golden/make_golden.py)."""
-    return np.load(ROOT / "tests" / "golden" / "golden_320x240.npz")
+    from tests.util import load_golden
+    return load_golden()
 
 
 @pytest.fixture(scope="session")
@@ -28,10 +28,10 @@ def product():
 
 @pytest.fixture(scope="session")
 def reference():
-    """The reference's kernels rebuilt for sm_100a (oracle/_ref); skips when not built."""
+    """The reference's kernels rebuilt for sm_90a (oracle/_ref); skips when not built."""
     from surfelmeshing_b200 import _lib
     if not _lib.REF_LIB_PATH.exists():
-        pytest.skip("oracle/_ref/libsurfel_ref.so not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/libsurfel_ref.so not built (needs the reference sources at build time)")
     return _lib.load_reference_oracle()
 
 
@@ -40,5 +40,5 @@ def shimref():
     """Reference host glue linked against the vis:: link shims (oracle/_ref/libsurfel_shimref.so)."""
     from surfelmeshing_b200 import _lib
     if not _lib.SHIM_LIB_PATH.exists():
-        pytest.skip("oracle/_ref/libsurfel_shimref.so not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/libsurfel_shimref.so not built (needs the reference sources at build time)")
     return _lib.load_shim_oracle()

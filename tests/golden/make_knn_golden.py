@@ -1,6 +1,6 @@
 """Writes tests/golden/knn_golden.npz: answers of the REFERENCE's CPU octree (oracle/_ref/liboctree_ref.so, i.e.
 applications/surfel_meshing/src/surfel_meshing/octree.cc compiled by oracle/Makefile) for the seeded cases of
-tests/knn_cases.py. Run in the dev container (needs /root/reference to build the oracle):
+tests/knn_cases.py. Run where the reference sources are present (oracle/Makefile: REF builds the oracle):
 
     make -C oracle ref && python tests/golden/make_knn_golden.py
 """

@@ -1,7 +1,7 @@
 // Host-side statistics of the supporting-surfel arrival key (csrc/sm_kernels.cuh) with the library's default
 // parameters: how often the lower slot / the primary association wins, by where the two slots sit in the modelled
 // launch. Printed as "name value" lines; tests/test_tiebreak_host.py compares them with what was measured on the
-// reference (profiles/r02_race_stats.md).
+// reference (DESIGN.md section 4).
 #include <cstdio>
 #include <cstdlib>
 #include <random>

@@ -31,10 +31,10 @@ def test_library_exports_every_declared_symbol(product):
     assert "smref_" not in out.stdout and "cw_" not in out.stdout
 
 
-def test_library_is_sm100a_only(product):
+def test_library_is_sm90a_only(product):
     out = subprocess.run(["cuobjdump", "--list-elf", str(product.path)], capture_output=True, text=True)
     archs = set(re.findall(r"sm_(\d+a?)", out.stdout))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_default_params_match_reference_defaults(product):

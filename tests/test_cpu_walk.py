@@ -1,5 +1,5 @@
 """The CPU restatement (oracle/cpu_walk.c) against the golden vectors produced by the
-reference's own kernels on a B200.
+reference's own kernels.
 
 The GPU evaluates exp/div/sqrt with approximate MUFU ops under -use_fast_math, the CPU walk
 with IEEE libm, so the comparison is statistical: u16 depth maps may differ by 1 LSB on a

@@ -13,9 +13,10 @@ from oracle import cpu_walk
 from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams
-from tests.test_parity_gpu import ENVELOPE_FACTOR, envelope_floors, envelope_limit
-from tests.util import (INTEGRATE_ROWS, INVALID, NEIGHBOR_ROWS, check_state_invariants, count_mismatch, golden_camera,
-                        golden_params, other_frames)
+from tests.test_parity_gpu import (ENVELOPE_FACTOR, envelope_floors, envelope_limit, golden_final_state,
+                                   golden_reconstruction)
+from tests.util import (INTEGRATE_ROWS, INVALID, NEIGHBOR_ROWS, check_state_invariants, count_mismatch, digest,
+                        golden_camera, golden_params, oracle_answers, other_frames)
 
 pytestmark = pytest.mark.gpu
 
@@ -165,39 +166,44 @@ def test_delta_transfer_equals_full_transfer(product):
 # f3: visualisation buffers
 # ---------------------------------------------------------------------------------------
 
-@pytest.mark.parametrize("mode", ["color", "last_update", "creation", "radii", "normals"])
-def test_visualization_buffers_against_oracle(product, reference, mode):
-    """One fused sweep against the reference's three kernels (kernels.cu:274-514, run unmodified into
-    plain device buffers): vertex buffer (incl. the NaN that hides replaced surfels), neighbour line
-    indices, normal line vertices: bit-exact."""
-    cam, st, pp, ip = stream_and_params(320, 240, 30, 8)
-    first, last = st.integrated_range()
-    rec_r = make(cam, 400_000, reference)
-    rec_r.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
-                     first, last)
-    rows, n, merges = rec_r.dump_state()
-    rec_p = make(cam, 400_000)
-    rec_p.load_state(rows, merges)
+VISUALIZATION_MODES = ["color", "last_update", "creation", "radii", "normals"]
+
+
+def visualization_params(mode, last, n):
     # hidden vertices: surfels created after the last triangulation whose slot the mesh already knows
-    params = dict(frame_index=last, latest_triangulated_frame_index=last - 8, latest_mesh_surfel_count=n - 100,
-                  surfel_integration_active_window_size=12 if mode == "last_update" else 2**31 - 1,
-                  visualize_last_update_timestamp=mode == "last_update", visualize_creation_timestamp=mode == "creation",
-                  visualize_radii=mode == "radii", visualize_normals=mode == "normals")
-    outs = []
-    for rec in (rec_p, rec_r):
-        vertex = torch.zeros((n, 4), dtype=torch.float32, device="cuda")
-        nbr = torch.zeros((n, 8), dtype=torch.int32, device="cuda")
-        nrm = torch.zeros((n, 6), dtype=torch.float32, device="cuda")
-        rec.UpdateVisualizationBuffers(None, vertex_buffer=vertex, neighbor_index_buffer=nbr, normal_vertex_buffer=nrm,
-                                       **params)
-        torch.cuda.synchronize()
-        outs.append((vertex.cpu().numpy(), nbr.cpu().numpy(), nrm.cpu().numpy()))
-    for k, name in enumerate(("vertex", "neighbour index", "normal vertex")):
-        assert count_mismatch(outs[0][k], outs[1][k]) == 0, name
-    hidden = np.isnan(outs[0][0][:, 0])
+    return dict(frame_index=last, latest_triangulated_frame_index=last - 2, latest_mesh_surfel_count=n - 100,
+                surfel_integration_active_window_size=2 if mode == "last_update" else 2**31 - 1,
+                visualize_last_update_timestamp=mode == "last_update", visualize_creation_timestamp=mode == "creation",
+                visualize_radii=mode == "radii", visualize_normals=mode == "normals")
+
+
+def visualization_outputs(rec, n, params):
+    """Vertex buffer, neighbour line indices and normal line vertices of one UpdateVisualizationBuffers()."""
+    vertex = torch.zeros((n, 4), dtype=torch.float32, device="cuda")
+    nbr = torch.zeros((n, 8), dtype=torch.int32, device="cuda")
+    nrm = torch.zeros((n, 6), dtype=torch.float32, device="cuda")
+    rec.UpdateVisualizationBuffers(None, vertex_buffer=vertex, neighbor_index_buffer=nbr, normal_vertex_buffer=nrm, **params)
+    torch.cuda.synchronize()
+    return {"vertex": vertex.cpu().numpy(), "neighbour index": nbr.cpu().numpy(), "normal vertex": nrm.cpu().numpy()}
+
+
+@pytest.mark.parametrize("mode", VISUALIZATION_MODES)
+def test_visualization_buffers_against_oracle(golden, product, mode):
+    """One fused sweep against the reference's three kernels (kernels.cu:274-514, run unmodified into
+    plain device buffers) on the reference's state after the golden frames: vertex buffer (incl. the NaN
+    that hides replaced surfels), neighbour line indices, normal line vertices: bit-exact against the
+    reference's recorded answers (tests/golden/make_oracle_answers.py)."""
+    rows, n, merges, last = golden_final_state(golden)
+    answers = oracle_answers()[f"visualization/{mode}"]
+    assert digest(rows) == answers["inputs"]
+    rec_p = golden_reconstruction(golden)
+    rec_p.load_state(rows, merges)
+    params = visualization_params(mode, last, n)
+    outs = visualization_outputs(rec_p, n, params)
+    assert [k for k, v in outs.items() if digest(v) != answers[k]] == [], "buffers differing from the reference"
+    hidden = np.isnan(outs["vertex"][:, 0])
     assert hidden.any() and not hidden.all()
     # a null pointer skips that buffer
-    vertex = torch.full((n, 4), 7.0, dtype=torch.float32, device="cuda")
     rec_p.UpdateVisualizationBuffers(None, vertex_buffer=None, neighbor_index_buffer=None, normal_vertex_buffer=None,
                                      **params)
 
@@ -396,25 +402,29 @@ def test_race_bound_rows_inside_the_reference_envelope(product, reference):
     assert exact_checked > 500, "the exact neighbour-link comparison covered a meaningful number of surfels"
 
 
-def test_free_running_stream_inside_the_reference_envelope(product, reference):
+def free_running_case():
+    return stream_and_params(640, 480, 500, 0)
+
+
+def stream_totals(s):
+    return [int(s.surfels_size), int(s.surfel_count), int(s.surfels_size) - int(s.surfel_count)]
+
+
+def test_free_running_stream_inside_the_reference_envelope(product):
     """BASELINE config 2, full length (500 frames / 492 integrated): the free-running product against the
     free-running oracle. The oracle differs from ITSELF between runs (its races feed back through the
-    cloud); the product's deviation from the oracle's mean must stay within 3x the oracle's own spread over six
-    runs (three runs can land within 60 merges of each other where the run-to-run standard deviation is 150;
-    + a floor of 0.1 %) for slots, live surfels and merges. Measured with the default rule: slots +0.06 %,
-    merges +0.35 % (profiles/r02_race_stats.md)."""
-    cam, st, pp, ip = stream_and_params(640, 480, 500, 0)
+    cloud, and its totals vary more between processes than within one); the product's deviation from the
+    oracle's mean must stay within 3x the oracle's own spread over six recorded runs, each in a process of its
+    own (+ a floor of 0.1 %), for slots, live surfels and merges (DESIGN.md section 4)."""
+    cam, st, pp, ip = free_running_case()
     first, last = st.integrated_range()
-    rec_r, rec_p = make(cam, 5_000_000, reference), make(cam, 5_000_000)
-    runs = []
-    for _ in range(6):
-        rec_r.reset()
-        s = rec_r.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp,
-                             ip, first, last)
-        runs.append((int(s.surfels_size), int(s.surfel_count), int(s.surfels_size) - int(s.surfel_count)))
+    answers = oracle_answers()["free_running"]
+    assert digest(st.depth.cpu().numpy()) == answers["inputs"], "the seeded input stream changed"
+    runs = answers["runs"]   # six runs of the oracle, each in a process of its own (tests/golden/make_oracle_answers.py)
+    rec_p = make(cam, 5_000_000)
     s = rec_p.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
                          first, last)
-    mine = (int(s.surfels_size), int(s.surfel_count), int(s.surfels_size) - int(s.surfel_count))
+    mine = stream_totals(s)
     for k, name in enumerate(("surfels_size", "surfel_count", "merges")):
         values = [r[k] for r in runs]
         mean, spread = float(np.mean(values)), max(values) - min(values)

@@ -1,7 +1,15 @@
 """Helpers shared by the parity tests."""
+import hashlib
+import io
+import json
+import lzma
+from pathlib import Path
+
 import numpy as np
 
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams
+
+GOLDEN_DIR = Path(__file__).resolve().parent / "golden"
 
 # Rows of the surfel SoA that Integrate() determines from deterministic rasters only
 # (everything except smooth positions, neighbour links and scratch rows).
@@ -21,6 +29,48 @@ def count_mismatch(a, b, mask=None):
     if mask is not None:
         ne &= mask
     return int(ne.sum())
+
+
+def digest(a):
+    """sha256 of an array's bytes (with its dtype and shape): the stored form of a bit-exact known answer."""
+    a = np.ascontiguousarray(a)
+    h = hashlib.sha256(f"{a.dtype.str}{a.shape}".encode())
+    h.update(a.tobytes())
+    return h.hexdigest()
+
+
+def load_npz_xz(path):
+    with lzma.open(path) as f:
+        data = np.load(io.BytesIO(f.read()))
+        return {k: data[k] for k in data.files}
+
+
+def load_golden(name="golden_320x240"):
+    """The known-answer set written by tests/golden/make_golden.py: `<name>_meta.npz` (camera, poses, frame range,
+    digests of the input stream), the input stream (`<name>_inputs_a/b.npz.xz`: colour and the first half of the
+    depth maps / the second half) and one lzma-compressed npz per integrated frame with the reference's outputs."""
+    meta = np.load(GOLDEN_DIR / f"{name}_meta.npz")
+    out = {k: meta[k] for k in meta.files if k not in ("depth_sha256", "color_sha256", "depth_shape", "stream_id")}
+    a, b = (load_npz_xz(GOLDEN_DIR / f"{name}_inputs_{part}.npz.xz") for part in "ab")
+    out["depth"], out["color"] = np.concatenate([a["depth"], b["depth"]]), a["color"]
+    assert digest(out["depth"]) == str(meta["depth_sha256"][0]), "stored input depth does not match its digest"
+    assert digest(out["color"]) == str(meta["color_sha256"][0]), "stored input colour does not match its digest"
+    first, last = [int(v) for v in out["frames"]]
+    for frame in range(first, last):
+        out.update(load_npz_xz(GOLDEN_DIR / f"{name}_f{frame}.npz.xz"))
+    return out
+
+
+_ORACLE_ANSWERS = None
+
+
+def oracle_answers():
+    """The reference kernels' recorded answers on the seeded inputs of the parity tests
+    (tests/golden/oracle_answers.json, written by tests/golden/make_oracle_answers.py)."""
+    global _ORACLE_ANSWERS
+    if _ORACLE_ANSWERS is None:
+        _ORACLE_ANSWERS = json.loads((GOLDEN_DIR / "oracle_answers.json").read_text())
+    return _ORACLE_ANSWERS
 
 
 def golden_params(golden):

@@ -8,11 +8,11 @@ out=$root/variants/build_$name
 mkdir -p $out
 objs=""
 for f in api pipeline transfer preprocess integrate regularize knn; do
-  nvcc -std=c++17 -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -ftz=true -fmad=false -prec-div=true -prec-sqrt=true \
+  nvcc -std=c++17 -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -ftz=true -fmad=false -prec-div=true -prec-sqrt=true \
        -Xcompiler -fPIC "$@" -c $root/surfelmeshing_b200/csrc/$f.cu -o $out/$f.o &
   objs="$objs $out/$f.o"
 done
 wait
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o $root/variants/lib_$name.so $objs
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o $root/variants/lib_$name.so $objs
 rm -rf $out
 echo $root/variants/lib_$name.so

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""profiles/rNN_sass.md: per-kernel SASS evidence from the built library (cuobjdump -sass): counts of the
+"""probe_out/<tag>_sass.md: per-kernel SASS evidence from the built library (cuobjdump -sass): counts of the
 memory / async-copy / SFU mnemonics that the design claims, and the instruction window around the TMA load."""
 import re
 import subprocess
@@ -30,7 +30,7 @@ def main():
             continue
         if name and re.search(r"/\*[0-9a-f]{4}\*/", line):
             kernels[name].append(re.sub(r"/\* 0x[0-9a-f]+ \*/", "", line).strip())
-    out = [f"# {tag}: SASS evidence (`cuobjdump -sass surfelmeshing_b200/libsurfel_b200.so`, sm_100a only)\n",
+    out = [f"# {tag}: SASS evidence (`cuobjdump -sass surfelmeshing_b200/libsurfel_b200.so`, sm_90a only)\n",
            "Instruction counts per kernel (static code, not executed counts). `UTMALDG` = `cp.async.bulk.tensor` (TMA) load, "
            "`SYNCS` = mbarrier operations, `LDG.E.128` / `STG.E.128` = 128-bit global accesses, `REDG.E.ADD.F32x4` = vector float "
            "atomics, `MUFU.*` = SFU approximations mirrored from the reference's fast-math SASS.\n",
@@ -49,8 +49,9 @@ def main():
             i = next(i for i, ln in enumerate(lines) if "UTMALDG" in ln)
             out += ["", f"## TMA tile fill of `{k}` (window around the load)\n", "```"] + lines[max(0, i - 14): i + 12] + ["```"]
             break
-    (ROOT / "profiles" / f"{tag}_sass.md").write_text("\n".join(out) + "\n")
-    print(ROOT / "profiles" / f"{tag}_sass.md")
+    (ROOT / "probe_out").mkdir(exist_ok=True)
+    (ROOT / "probe_out" / f"{tag}_sass.md").write_text("\n".join(out) + "\n")
+    print(ROOT / "probe_out" / f"{tag}_sass.md")
 
 
 if __name__ == "__main__":

@@ -1,12 +1,13 @@
 """Offline look at how the reference's association race resolves (input: the supporter-set dump of
 tools/race_stats.py, <out>_sets.npz): for pairs of supporters of one pixel, who wins as a function of where the two
-threads sit in the reference's launch (wave = 296 blocks x 1024 threads, block, warp, lane)."""
+threads sit in the reference's launch (wave = 2 blocks per SM x SMs x 1024 threads, block, warp, lane;
+the SM count is the second argument, 132 = H100 SXM by default)."""
 import sys
 from collections import defaultdict
 
 import numpy as np
 
-W = 296 * 1024
+W = 2 * (int(sys.argv[2]) if len(sys.argv) > 2 else 132) * 1024
 
 
 def main():
@@ -43,9 +44,10 @@ def main():
         diff_block = same_wave & (blk_a != blk_b)
         report("different block", diff_block)
         db = blk_b - blk_a
-        for lo, hi in ((1, 1), (2, 7), (8, 31), (32, 147), (148, 148), (149, 295)):
+        sms = W // 2048
+        for lo, hi in ((1, 1), (2, 7), (8, 31), (32, sms - 1), (sms, sms), (sms + 1, 2 * sms - 1)):
             report(f"block distance {lo}-{hi}", diff_block & (db >= lo) & (db <= hi))
-        report("different block, same SM parity (d % 148 == 0)", diff_block & (db % 148 == 0))
+        report(f"different block, same SM parity (d % {sms} == 0)", diff_block & (db % sms == 0))
         # does the position inside the block matter across blocks?
         for name, m in (("a earlier in its block than b", (ra % 1024) < (rb % 1024)), ("a later in its block than b", (ra % 1024) > (rb % 1024))):
             report("different block, " + name, diff_block & m)
