@@ -162,6 +162,25 @@ int sm_median_filter_and_densify_depth_map(
     void* stream, int32_t iterations, int32_t width, int32_t height,
     const uint16_t* in_depth, size_t in_pitch, uint16_t* out_depth, size_t out_pitch,
     uint16_t* scratch, size_t scratch_pitch);
+/* The input downscaling of --pyramid_level (APP/main.cc:299-303), which the reference runs on the CPU
+ * inside its upload loop (main.cc:946-981). Device buffers, pitches in bytes.
+ * sm_downscale_using_median_while_excluding replaces Image<u16>::DownscaleUsingMedianWhileExcluding
+ * (libvis image.h:1003-1050; main.cc:951-952): output pixel (x, y) is the median of the input block
+ * [W x / out_width, W (x + 1) / out_width) x [H y / out_height, H (y + 1) / out_height) (integer
+ * division) without the values equal to value_to_ignore, value_to_ignore if none is left; for an even
+ * count the middle value closer to the float average, the upper one on a tie. Blocks up to 16 x 16.
+ * sm_color_image_pyramid replaces ImagePyramid(color, levels) (libvis image_cache.h:205-282; main.cc:
+ * 973-981): `levels` rounds of Image<Vec3u8>::DownscaleToHalfSize (image.h:929-948), a/4 + b/4 + c/4 +
+ * d/4 per channel with each quarter truncated; out is (width >> levels) x (height >> levels) packed
+ * uchar3; levels == 0 copies. Both return SM_ERR_INVALID_ARGUMENT for an empty output or one larger than
+ * the input, blocks larger than 16 x 16, levels outside [0, 4] or a size that is odd at some level. */
+int sm_downscale_using_median_while_excluding(void* stream, uint16_t value_to_ignore,
+                                              int32_t in_width, int32_t in_height,
+                                              const uint16_t* in, size_t in_pitch,
+                                              int32_t out_width, int32_t out_height,
+                                              uint16_t* out, size_t out_pitch);
+int sm_color_image_pyramid(void* stream, int32_t levels, int32_t width, int32_t height,
+                           const uint8_t* in, size_t in_pitch, uint8_t* out, size_t out_pitch);
 int sm_erode_depth_map(void* stream, int32_t radius /* 0 = copy w/o border */,
                        int32_t width, int32_t height,
                        const uint16_t* in_depth, size_t in_pitch,
@@ -400,7 +419,16 @@ int sm_stream_run(sm_reconstruction* r, void* stream, const sm_stream_desc* s,
  *   (APP/cuda_surfel_reconstruction_kernels.cu:1688); DESIGN.md section 4 has the measurements behind the defaults.
  *   "median_filter_and_densify_iterations": sm_stream_run applies that many
  *   MedianFilterAndDensifyDepthMap passes (APP/main.cc:207-252, 927-939) to every raw depth map
- *   as it enters the device-side frame ring (default 0, as in the reference). */
+ *   as it enters the device-side frame ring (default 0, as in the reference).
+ *   "pyramid_level" (integer in [0, 4], default 0, APP/main.cc:299-303 --pyramid_level L): sm_stream_run
+ *   reconstructs at 1 / 2^L of the sensor resolution. sm_stream_desc.width/height and the depth/colour frames
+ *   are then the sensor's, width and height must be divisible by 2^L and (width >> L, height >> L) must be the
+ *   handle's size (create the handle with the camera scaled by 1 / 2^L, libvis Camera::Scaled); every raw
+ *   depth map and colour image is downscaled on the upload stream as sm_downscale_using_median_while_excluding
+ *   and sm_color_image_pyramid do (host frames through full-size staging, device frames in place;
+ *   stats.h2d_bytes counts the full-size uploads). Like the reference (main.cc:946-949) a level above 0
+ *   cannot be combined with median_filter_and_densify_iterations > 0: sm_stream_run then returns
+ *   SM_ERR_INVALID_ARGUMENT, whatever the order of the sm_configure calls. */
 int sm_configure(sm_reconstruction* r, const char* key, double value);
 
 /* Number of kernel launches issued by this library since load (all handles). */

@@ -161,6 +161,8 @@ _PRODUCT_ONLY = {
     "frame_counters": (C.c_int, [_P, _P, C.POINTER(C.c_uint64 * 4)]),
     "configure": (C.c_int, [_P, C.c_char_p, C.c_double]),
     "median_filter_and_densify_depth_map": (C.c_int, [_P, _I, _I, _I, _P, _SZ, _P, _SZ, _P, _SZ]),
+    "downscale_using_median_while_excluding": (C.c_int, [_P, _U16, _I, _I, _P, _SZ, _I, _I, _P, _SZ]),
+    "color_image_pyramid": (C.c_int, [_P, _I, _I, _I, _P, _SZ, _P, _SZ]),
     "transfer_delta_to_cpu": (C.c_int, [_P, _P, _U32, C.POINTER(TransferToken), _P, _P, _P, _P, _P, _P, _P, _P,
                                         C.POINTER(TransferStats)]),
     "knn_create": (C.c_int, [C.POINTER(_P), _U32]),

@@ -153,7 +153,8 @@ const char* KernelName(int id) {
       "k_clear", "k_bilateral_outlier", "k_bilateral_generic", "k_outlier", "k_erode_normals_radii", "k_erode",
       "k_normals", "k_radii", "k_project", "k_associate", "k_merge", "k_blend", "k_integrate", "k_update_neighbors",
       "k_new_surfel_scan", "k_create_surfels", "k_reg_accumulate", "k_reg_step", "k_reg_copy_only",
-      "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_project_tail"};
+      "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_project_tail",
+      "k_downscale_depth_median", "k_downscale_color"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -496,6 +497,7 @@ int sm_destroy(sm_reconstruction* r) {
   cudaFree(r->scratch_B);
   cudaFree(r->blend_src);
   cudaFree(r->median_stage[0]); cudaFree(r->median_stage[1]);
+  cudaFree(r->pyramid_depth_stage); cudaFree(r->pyramid_color_stage);
   FreeTransferBuffers(r);
   for (int i = 0; i < 2; ++i) {
     if (r->pipe.ev_create[i]) cudaEventDestroy(r->pipe.ev_create[i]);
@@ -565,6 +567,19 @@ int sm_median_filter_and_densify_depth_map(void* stream, int32_t iterations, int
                                            size_t out_pitch, uint16_t* scratch, size_t scratch_pitch) {
   return StageMedianDensify(static_cast<cudaStream_t>(stream), iterations, width, height, in_depth, in_pitch, out_depth,
                             out_pitch, scratch, scratch_pitch);
+}
+
+int sm_downscale_using_median_while_excluding(void* stream, uint16_t value_to_ignore, int32_t in_width,
+                                              int32_t in_height, const uint16_t* in, size_t in_pitch,
+                                              int32_t out_width, int32_t out_height, uint16_t* out,
+                                              size_t out_pitch) {
+  return StageDownscaleMedian(static_cast<cudaStream_t>(stream), value_to_ignore, in_width, in_height, in, in_pitch,
+                              out_width, out_height, out, out_pitch);
+}
+
+int sm_color_image_pyramid(void* stream, int32_t levels, int32_t width, int32_t height, const uint8_t* in,
+                           size_t in_pitch, uint8_t* out, size_t out_pitch) {
+  return StageColorPyramid(static_cast<cudaStream_t>(stream), levels, width, height, in, in_pitch, out, out_pitch);
 }
 
 int sm_erode_depth_map(void* stream, int32_t radius, int32_t width, int32_t height, const uint16_t* in_depth,
@@ -817,6 +832,8 @@ int sm_stream_run(sm_reconstruction* r, void* stream_v, const sm_stream_desc* s,
 //   "tiebreak_index_order_fraction"  fraction of the pixels whose supporters are ordered by slot index inside a wave
 //   "median_filter_and_densify_iterations"  sm_stream_run: MedianFilterAndDensifyDepthMap passes over every raw
 //                              depth map on its way into the frame ring (APP/main.cc:435, 927-939; default 0)
+//   "pyramid_level"            sm_stream_run: frames are 2^L times the handle's size and are downscaled on their
+//                              way into the frame rings (APP/main.cc:299-303, 946-981; default 0)
 int sm_configure(sm_reconstruction* r, const char* key, double value) {
   if (!r || !key) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_configure: null argument");
   const std::string k(key);
@@ -856,6 +873,11 @@ int sm_configure(sm_reconstruction* r, const char* key, double value) {
   if (k == "median_filter_and_densify_iterations") {
     if (value < 0 || value > 16 || value != static_cast<int>(value)) return SetError(SM_ERR_INVALID_ARGUMENT, "median_filter_and_densify_iterations must be an integer in [0, 16]");
     r->median_iterations = static_cast<int>(value);
+    return SM_OK;
+  }
+  if (k == "pyramid_level") {
+    if (value < 0 || value > 4 || value != static_cast<int>(value)) return SetError(SM_ERR_INVALID_ARGUMENT, "pyramid_level must be an integer in [0, 4]");
+    r->pyramid_level = static_cast<int>(value);
     return SM_OK;
   }
   return SetError(SM_ERR_INVALID_ARGUMENT, "sm_configure: unknown key");

@@ -49,7 +49,8 @@ int EnvInt(const char* name, int fallback) {
   return (e && e[0]) ? std::atoi(e) : fallback;
 }
 
-int EnsureRunBuffers(sm_reconstruction* r, bool on_host, bool depth_ring) {
+int EnsureRunBuffers(sm_reconstruction* r, bool on_host, bool depth_ring, bool color_ring, int source_width,
+                     int source_height) {
   const int W = r->d.width, H = r->d.height;
   if (!r->run_depth[0]) {
     for (int i = 0; i < kSets; ++i) {
@@ -94,11 +95,26 @@ int EnsureRunBuffers(sm_reconstruction* r, bool on_host, bool depth_ring) {
       SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b), &r->ring_depth_pitch, W * sizeof(u16), H));
     }
   }
-  if (on_host && r->ring_color.empty()) {
+  if (color_ring && r->ring_color.empty()) {
     r->ring_color.assign(kColorRing, nullptr);
     for (auto& b : r->ring_color) {
       SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b), &r->ring_color_pitch, W * 3, H));
     }
+  }
+  // host frames at a pyramid level: full-size staging on the upload stream (one frame at a time)
+  if (on_host && r->pyramid_level > 0 &&
+      (r->pyramid_stage_width != source_width || r->pyramid_stage_height != source_height)) {
+    SM_CUDA(cudaFree(r->pyramid_depth_stage));
+    SM_CUDA(cudaFree(r->pyramid_color_stage));
+    r->pyramid_depth_stage = nullptr;
+    r->pyramid_color_stage = nullptr;
+    r->pyramid_stage_width = r->pyramid_stage_height = 0;
+    SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->pyramid_depth_stage), &r->pyramid_depth_stage_pitch,
+                            source_width * sizeof(u16), source_height));
+    SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->pyramid_color_stage), &r->pyramid_color_stage_pitch,
+                            static_cast<size_t>(source_width) * 3, source_height));
+    r->pyramid_stage_width = source_width;
+    r->pyramid_stage_height = source_height;
   }
   if (r->median_iterations > 0 && !r->median_stage[0]) {
     for (int i = 0; i < 2; ++i) {
@@ -116,8 +132,12 @@ struct RunContext {
   const sm_integrate_params* ip;
   int W, H, K, half, first, last;
   size_t frame_elems;
+  int pyramid;            // input pyramid level: the stream's frames are (W << pyramid) x (H << pyramid)
+  int source_W, source_H;
+  size_t source_elems;    // pixels of one frame of the stream
   bool on_host;           // depth / colour frames are in (pinned) host memory
-  bool depth_ring;        // raw depth maps pass through the device-side ring (host frames, or median densify on)
+  bool depth_ring;        // raw depth maps pass through the device-side ring (host frames, median densify or pyramid)
+  bool color_ring;        // colour images pass through the device-side ring (host frames or pyramid)
   int base_slot;          // Counters::surfel_count slot before the first frame
   uint64_t h2d = 0;
 
@@ -128,7 +148,7 @@ struct RunContext {
     return s->depth + frame_elems * frame;
   }
   const uint8_t* Color(int frame, size_t* pitch) const {
-    if (on_host) { *pitch = r->ring_color_pitch; return reinterpret_cast<const uint8_t*>(r->ring_color[frame % kColorRing]); }
+    if (color_ring) { *pitch = r->ring_color_pitch; return reinterpret_cast<const uint8_t*>(r->ring_color[frame % kColorRing]); }
     *pitch = static_cast<size_t>(W) * 3;
     return s->color + 3 * frame_elems * frame;
   }
@@ -151,7 +171,22 @@ struct RunContext {
   // MedianFilterAndDensifyDepthMap passes when configured (main.cc:927-939, there on the CPU).
   int EnqueueRawFrame(int frame) {
     u16* const slot = r->ring_depth[frame % kDepthRing];
-    const u16* const src = s->depth + frame_elems * frame;
+    const u16* const src = s->depth + source_elems * frame;
+    if (pyramid > 0) {
+      // DownscaleUsingMedianWhileExcluding(0, W, H) of the full-size map (main.cc:951-952, there on the
+      // CPU); host frames are uploaded full-size first, device frames are read in place
+      const u16* full = src;
+      size_t full_pitch = source_W * sizeof(u16);
+      if (on_host) {
+        SM_CUDA(cudaMemcpy2DAsync(r->pyramid_depth_stage, r->pyramid_depth_stage_pitch, src, full_pitch, full_pitch,
+                                  source_H, cudaMemcpyHostToDevice, r->upload_stream));
+        h2d += source_elems * sizeof(u16);
+        full = r->pyramid_depth_stage;
+        full_pitch = r->pyramid_depth_stage_pitch;
+      }
+      return StageDownscaleMedian(r->upload_stream, 0, source_W, source_H, full, full_pitch, W, H, slot,
+                                  r->ring_depth_pitch);
+    }
     const int n = r->median_iterations;
     u16* const target = n > 0 ? r->median_stage[0] : slot;
     const size_t target_pitch = n > 0 ? r->median_stage_pitch : r->ring_depth_pitch;
@@ -164,6 +199,20 @@ struct RunContext {
     return SM_OK;
   }
   int EnqueueColorFrame(int frame) {
+    if (pyramid > 0) {
+      // ImagePyramid(color, pyramid) (main.cc:973-981, there on the CPU)
+      const uint8_t* full = s->color + 3 * source_elems * frame;
+      size_t full_pitch = static_cast<size_t>(source_W) * 3;
+      if (on_host) {
+        SM_CUDA(cudaMemcpy2DAsync(r->pyramid_color_stage, r->pyramid_color_stage_pitch, full, full_pitch, full_pitch,
+                                  source_H, cudaMemcpyHostToDevice, r->upload_stream));
+        h2d += source_elems * 3;
+        full = r->pyramid_color_stage;
+        full_pitch = r->pyramid_color_stage_pitch;
+      }
+      return StageColorPyramid(r->upload_stream, pyramid, source_W, source_H, full, full_pitch,
+                               reinterpret_cast<u8*>(r->ring_color[frame % kColorRing]), r->ring_color_pitch);
+    }
     SM_CUDA(cudaMemcpy2DAsync(r->ring_color[frame % kColorRing], r->ring_color_pitch, s->color + 3 * frame_elems * frame,
                               static_cast<size_t>(W) * 3, static_cast<size_t>(W) * 3, H, cudaMemcpyHostToDevice,
                               r->upload_stream));
@@ -210,7 +259,7 @@ int RunStreams(RunContext& c, cudaStream_t stream, bool pipelined, uint32_t* int
         if (st != SM_OK) return st;
       }
       uploaded_until = frame + half;
-      if (c.on_host) {
+      if (c.color_ring) {
         const int st = c.EnqueueColorFrame(frame);
         if (st != SM_OK) return st;
       }
@@ -466,7 +515,7 @@ int RunGraph(RunContext& c, cudaStream_t stream, uint32_t* integrated) {
         if (st != SM_OK) return st;
       }
       uploaded_until = pre + half;
-      if (c.on_host) {
+      if (c.color_ring) {
         // the colour slot held frame pre - kColorRing, last read by the step that integrated it
         const int last_color_step = pre - kColorRing;
         if (last_color_step >= it0) SM_CUDA(cudaStreamWaitEvent(r->upload_stream, r->iteration_done[(last_color_step - it0) % kIterationEvents], 0));
@@ -588,7 +637,22 @@ int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s
   RunContext c;
   c.r = r; c.s = s; c.pp = pp; c.ip = ip;
   c.W = r->d.width; c.H = r->d.height;
-  if (s->width != c.W || s->height != c.H) return SetError(SM_ERR_INVALID_ARGUMENT, "stream size mismatch");
+  c.pyramid = r->pyramid_level;
+  if (c.pyramid > 0) {
+    // main.cc:946-949
+    if (r->median_iterations > 0) {
+      return SetError(SM_ERR_INVALID_ARGUMENT, "pyramid_level > 0 cannot be combined with median_filter_and_densify_iterations > 0");
+    }
+    const int step = 1 << c.pyramid;
+    if (s->width <= 0 || s->height <= 0 || s->width % step != 0 || s->height % step != 0 ||
+        (s->width >> c.pyramid) != c.W || (s->height >> c.pyramid) != c.H) {
+      return SetError(SM_ERR_INVALID_ARGUMENT, "stream size must be the handle's size times 2^pyramid_level");
+    }
+  } else if (s->width != c.W || s->height != c.H) {
+    return SetError(SM_ERR_INVALID_ARGUMENT, "stream size mismatch");
+  }
+  c.source_W = s->width; c.source_H = s->height;
+  c.source_elems = static_cast<size_t>(c.source_W) * c.source_H;
   c.K = pp->outlier_filtering_frame_count;
   c.half = c.K / 2;
   if (c.K < 2 || c.K > 8 || first_frame < c.half || last_frame > s->frame_count - c.half || first_frame > last_frame) {
@@ -598,9 +662,10 @@ int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s
   c.first = first_frame; c.last = last_frame;
   c.frame_elems = static_cast<size_t>(c.W) * c.H;
   c.on_host = s->frames_on_host != 0;
-  c.depth_ring = c.on_host || r->median_iterations > 0;
+  c.depth_ring = c.on_host || r->median_iterations > 0 || c.pyramid > 0;
+  c.color_ring = c.on_host || c.pyramid > 0;
   c.base_slot = r->count_slot;
-  int status = EnsureRunBuffers(r, c.on_host, c.depth_ring);
+  int status = EnsureRunBuffers(r, c.on_host, c.depth_ring, c.color_ring, c.source_W, c.source_H);
   if (status != SM_OK) return status;
   const unsigned long long launches_before = LaunchCount();
   const auto host_t0 = std::chrono::steady_clock::now();

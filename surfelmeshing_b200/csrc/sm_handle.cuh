@@ -100,6 +100,13 @@ struct sm_reconstruction {
   // (APP/main.cc:435 --median_filter_and_densify_iterations, default 0) and their staging buffers
   int median_iterations = 0;
   smb::u16* median_stage[2] = {nullptr, nullptr}; size_t median_stage_pitch = 0;
+  // Input pyramid level (APP/main.cc:299-303 --pyramid_level, default 0): sm_stream_run takes frames of
+  // 2^L times the handle's size and downscales them on the upload stream; host frames pass through
+  // full-size staging buffers of pyramid_stage_width x pyramid_stage_height pixels.
+  int pyramid_level = 0;
+  smb::u16* pyramid_depth_stage = nullptr; size_t pyramid_depth_stage_pitch = 0;
+  smb::u8* pyramid_color_stage = nullptr; size_t pyramid_color_stage_pitch = 0;
+  int pyramid_stage_width = 0, pyramid_stage_height = 0;
   std::vector<cudaEvent_t> iteration_done;   // frame graph: one event per iteration slot (ring reuse)
   // delta transfer (transfer.cu): operation counter, per-operation regularisation thresholds, staging
   smb::u32 op_epoch = 0;

@@ -24,7 +24,8 @@ enum KernelId {
   KID_CLEAR = 0, KID_BILATERAL_OUTLIER, KID_BILATERAL_GENERIC, KID_OUTLIER, KID_ERODE_NORMALS_RADII, KID_ERODE,
   KID_NORMALS, KID_RADII, KID_PROJECT, KID_ASSOCIATE, KID_MERGE, KID_BLEND, KID_INTEGRATE, KID_UPDATE_NEIGHBORS,
   KID_NEW_SURFEL_SCAN, KID_CREATE_SURFELS, KID_REG_ACCUMULATE, KID_REG_STEP, KID_REG_COPY_ONLY,
-  KID_EXPORT_VERTICES, KID_MEDIAN_DENSIFY, KID_DELTA_SELECT, KID_VIZ_BUFFERS, KID_PROJECT_TAIL, KID_COUNT
+  KID_EXPORT_VERTICES, KID_MEDIAN_DENSIFY, KID_DELTA_SELECT, KID_VIZ_BUFFERS, KID_PROJECT_TAIL, KID_DOWNSCALE_DEPTH,
+  KID_DOWNSCALE_COLOR, KID_COUNT
 };
 const char* KernelName(int id);
 bool ProfilingEnabled();
@@ -392,6 +393,12 @@ int StageErode(cudaStream_t stream, int radius, int width, int height, const u16
                size_t out_pitch);
 int StageMedianDensify(cudaStream_t stream, int iterations, int width, int height, const u16* in, size_t in_pitch,
                        u16* out, size_t out_pitch, u16* scratch, size_t scratch_pitch);
+// The input downscaling of --pyramid_level: median depth blocks of up to 16 x 16 pixels, and `levels`
+// (0-4) colour halvings of packed uchar3 in one launch (levels == 0 copies).
+int StageDownscaleMedian(cudaStream_t stream, u16 value_to_ignore, int in_width, int in_height, const u16* in,
+                         size_t in_pitch, int out_width, int out_height, u16* out, size_t out_pitch);
+int StageColorPyramid(cudaStream_t stream, int levels, int width, int height, const u8* in, size_t in_pitch, u8* out,
+                      size_t out_pitch);
 int StageNormals(cudaStream_t stream, float observation_angle_threshold_deg, float depth_scaling, float fx, float fy,
                  float cx, float cy, int width, int height, const u16* in, size_t in_pitch, u16* out, size_t out_pitch,
                  float2* normals, size_t normals_pitch);

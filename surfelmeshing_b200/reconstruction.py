@@ -136,6 +136,38 @@ def MedianFilterAndDensifyDepthMap(stream, iterations, input_depth, output_depth
     return output_depth
 
 
+def DownscaleUsingMedianWhileExcluding(stream, value_to_ignore, output_width, output_height, input_depth,
+                                       output_depth=None, lib: Optional[Library] = None):
+    """Image<u16>::DownscaleUsingMedianWhileExcluding (libvis image.h:1003-1050; APP/main.cc:951-952, there on
+    the CPU): each output pixel is the median of its input block without `value_to_ignore`. Returns the
+    [output_height, output_width] output tensor."""
+    lib = lib or _lib.load_product()
+    H, W = input_depth.shape
+    if output_depth is None:
+        output_depth = torch.zeros((int(output_height), int(output_width)), dtype=torch.uint16,
+                                   device=input_depth.device)
+    ip, ipitch = _raster(input_depth)
+    op, opitch = _raster(output_depth)
+    lib.call("downscale_using_median_while_excluding", _stream_handle(stream), int(value_to_ignore), W, H, ip, ipitch,
+             int(output_width), int(output_height), op, opitch)
+    return output_depth
+
+
+def ImagePyramid(stream, color, pyramid_level, output=None, lib: Optional[Library] = None):
+    """ImagePyramid(color, pyramid_level) (libvis image_cache.h:205-282; APP/main.cc:973-981, there on the CPU):
+    `pyramid_level` rounds of DownscaleToHalfSize on a [H, W, 3] uint8 image. Returns the
+    [H >> level, W >> level, 3] output tensor."""
+    lib = lib or _lib.load_product()
+    H, W = color.shape[:2]
+    level = int(pyramid_level)
+    if output is None:
+        output = torch.zeros((max(H >> level, 1), max(W >> level, 1), 3), dtype=torch.uint8, device=color.device)
+    ip, ipitch = _raster(color, 3)
+    op, opitch = _raster(output, 3)
+    lib.call("color_image_pyramid", _stream_handle(stream), level, W, H, ip, ipitch, op, opitch)
+    return output
+
+
 def ErodeDepthMapCUDA(stream, radius, input_depth, output_depth, lib: Optional[Library] = None):
     lib = lib or _lib.load_product()
     ip, ipitch = _raster(input_depth)
@@ -371,7 +403,8 @@ class CUDASurfelReconstruction:
         """Frame loop of APP/main.cc:885-1223 over frames [first_frame, last_frame).
 
         depth [F,H,W] uint16 and color [F,H,W,3] uint8 are either CUDA tensors (device-resident
-        stream) or pinned CPU tensors (uploaded frame by frame inside the call)."""
+        stream) or pinned CPU tensors (uploaded frame by frame inside the call). H and W are the
+        handle's size, or 2^L times it with configure("pyramid_level", L)."""
         on_host = not depth.is_cuda
         assert depth.is_contiguous() and color.is_contiguous() and color.is_cuda == depth.is_cuda
         if on_host:
@@ -381,7 +414,9 @@ class CUDASurfelReconstruction:
         l = np.ascontiguousarray(np.asarray(frame_T_global, np.float32).reshape(F, 12))
         o = np.ascontiguousarray(np.asarray(others_TR_reference, np.float32).reshape(F, -1, 12))
         assert o.shape[1] == pp.outlier_filtering_frame_count
-        desc = StreamDesc(self.width, self.height, F, 1 if on_host else 0, depth.data_ptr(), color.data_ptr(),
+        H, W = depth.shape[1:3]
+        assert tuple(color.shape[1:3]) == (H, W)
+        desc = StreamDesc(W, H, F, 1 if on_host else 0, depth.data_ptr(), color.data_ptr(),
                           g.ctypes.data, l.ctypes.data, o.ctypes.data)
         stats = StreamStats()
         self.lib.call("stream_run", self._h, _stream_handle(stream), C.byref(desc), C.byref(pp), C.byref(ip),

@@ -41,6 +41,15 @@ class Camera:
         s = width / 640.0
         return Camera(width, height, 525.0 * s, 525.0 * s, 320.0 * s, 240.0 * s)
 
+    def scaled(self, level: int) -> "Camera":
+        """The camera of pyramid level `level`, as libvis Camera::Scaled(1 / 2^level) builds it (camera.h:1564-1573,
+        pinhole ScaleParameters near :954; APP/main.cc:751): sizes int(factor * size + 0.5) in double,
+        fx, fy, cx, cy multiplied by the float factor in float (cx, cy are pixel-corner coordinates)."""
+        factor = np.float32(1.0) / np.float32(2.0 ** level)
+        scale = lambda v: float(np.float32(v) * factor)
+        return Camera(int(float(factor) * self.width + 0.5), int(float(factor) * self.height + 0.5), scale(self.fx),
+                      scale(self.fy), scale(self.cx), scale(self.cy))
+
     def valid_region_radius(self) -> float:
         """333 px at VGA (main.cc default), scaled with the image (SURVEY §8d)."""
         return 333.0 * self.width / 640.0
