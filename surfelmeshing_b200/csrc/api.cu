@@ -263,6 +263,7 @@ int IntegrateImpl(sm_reconstruction* r, cudaStream_t stream, u32 frame_index, co
   int status = IntegrateFrame(stream, r->d, f, p.do_blending != 0, r->rasters_cleared, r->plan, &r->events);
   r->rasters_cleared = false;
   if (status != SM_OK) return status;
+  NoteIntegratedFrame(r->d, frame_index);
   const int old_slot = r->count_slot;
   r->count_slot = (r->count_slot + 1) % kCountSlots;  // k_new_surfel_scan wrote the next slot
   if (r->events.enabled) cudaEventRecord(r->events.ev[12], stream);
@@ -332,9 +333,14 @@ int CreateImpl(sm_reconstruction* r, uint64_t max_surfel_count, int32_t width, i
     SM_CUDA(cudaMalloc(&r->vis_set[i], sizeof(VisEntry) * padded));
     SM_CUDA(cudaMalloc(&r->seg_count_set[i], sizeof(u32) * (padded / kSegment)));
     SM_CUDA(cudaMalloc(&r->merge_flag_set[i], padded));
+    SM_CUDA(cudaMalloc(&r->upd_list_set[i], sizeof(uint2) * padded));
+    SM_CUDA(cudaMalloc(&r->upd_count_set[i], sizeof(u32)));
   }
   d.assoc = r->assoc_set[0]; d.first_depth = r->first_depth_set[0]; d.supported = r->supported_set[0];
   d.vis = r->vis_set[0]; d.seg_count = r->seg_count_set[0]; d.merge_flag = r->merge_flag_set[0];
+  d.upd_list = r->upd_list_set[0]; d.upd_count = r->upd_count_set[0];
+  d.reg_t_prev = 0;
+  d.reg_full_sweep = 1;  // smooth_next is undefined
   SM_CUDA(cudaMalloc(&d.new_list, sizeof(u32) * P));
   SM_CUDA(cudaMalloc(&d.new_flag, P));
   SM_CUDA(cudaMalloc(&d.new_index, sizeof(u32) * P));
@@ -488,6 +494,7 @@ int sm_destroy(sm_reconstruction* r) {
   cudaFree(d.surfels); cudaFree(d.gradient); cudaFree(r->smooth_alt); cudaFree(d.new_list);
   for (int i = 0; i < kSets; ++i) {
     cudaFree(r->vis_set[i]); cudaFree(r->seg_count_set[i]); cudaFree(r->merge_flag_set[i]);
+    cudaFree(r->upd_list_set[i]); cudaFree(r->upd_count_set[i]);
     cudaFree(r->assoc_set[i]); cudaFree(r->first_depth_set[i]); cudaFree(r->supported_set[i]);
     cudaFree(r->run_depth[i]); cudaFree(r->run_depth_pre[i]); cudaFree(r->run_normals[i]); cudaFree(r->run_radius[i]);
   }
@@ -720,6 +727,7 @@ int sm_load_state(sm_reconstruction* r, void* stream_v, const float* host_rows, 
   // the loaded rows 3-5 are the current smooth-position buffer again
   r->d.smooth = r->d.surfels + static_cast<size_t>(SM_ROW_SMOOTH_X) * r->d.stride;
   r->d.smooth_next = r->smooth_alt;
+  r->d.reg_full_sweep = 1;  // smooth_next is undefined
   if (surfels_size > 0) {
     SM_CUDA(cudaMemcpy2DAsync(r->d.surfels, r->d.stride * sizeof(float), host_rows,
                               host_row_stride_elems * sizeof(float), surfels_size * sizeof(float), SM_ROW_COUNT,

@@ -156,6 +156,7 @@ struct RunContext {
     DeviceState d = r->d;
     d.assoc = r->assoc_set[set]; d.first_depth = r->first_depth_set[set]; d.supported = r->supported_set[set];
     d.vis = r->vis_set[set]; d.seg_count = r->seg_count_set[set]; d.merge_flag = r->merge_flag_set[set];
+    d.upd_list = r->upd_list_set[set]; d.upd_count = r->upd_count_set[set];
     return d;
   }
   FrameParams Params(int frame, int set) const {
@@ -306,6 +307,7 @@ int RunStreams(RunContext& c, cudaStream_t stream, bool pipelined, uint32_t* int
     SM_CUDA(cudaStreamWaitEvent(pipelined ? r->pipe.front : stream, r->pre_done[set], 0));
     r->d.assoc = r->assoc_set[set]; r->d.first_depth = r->first_depth_set[set]; r->d.supported = r->supported_set[set];
     r->d.vis = r->vis_set[set]; r->d.seg_count = r->seg_count_set[set]; r->d.merge_flag = r->merge_flag_set[set];
+    r->d.upd_list = r->upd_list_set[set]; r->d.upd_count = r->upd_count_set[set];
     if (pipelined) {
       RecordOperation(r, static_cast<int>(static_cast<u32>(frame) - static_cast<u32>(c.ip->regularization_frame_window_size)));
       const FrameParams f = c.Params(frame, set);
@@ -543,6 +545,7 @@ int RunGraph(RunContext& c, cudaStream_t stream, uint32_t* integrated) {
         if (status != SM_OK) return status;
       }
       const int old_slot = f.count_slot, new_slot = (f.count_slot + 1) % kCountSlots;
+      if (active(crit)) NoteIntegratedFrame(d, static_cast<u32>(frame));
       for (int i = 0; i < (disable_denoising ? 1 : iterations); ++i) {
         KernelLaunch* first = &launches[l.reg0 + (disable_denoising ? 0 : 2 * i)];
         KernelLaunch* second = disable_denoising ? nullptr : first + 1;
@@ -554,8 +557,11 @@ int RunGraph(RunContext& c, cudaStream_t stream, uint32_t* integrated) {
           smooth_next = smooth;
           smooth = filled;
           d.smooth = smooth; d.smooth_next = smooth_next;
+          NoteRegStep(d, static_cast<u32>(frame), c.ip->regularization_frame_window_size);
         }
       }
+      r->d.reg_t_prev = d.reg_t_prev;   // the next step's SetState starts from here
+      r->d.reg_full_sweep = d.reg_full_sweep;
       if (active(crit)) ++*integrated;
     }
     {  // front: frame `front`
@@ -623,6 +629,7 @@ int RunGraph(RunContext& c, cudaStream_t stream, uint32_t* integrated) {
     const DeviceState last_set = c.SetState((c.last - 1) % kSets);
     r->d.assoc = last_set.assoc; r->d.first_depth = last_set.first_depth; r->d.supported = last_set.supported;
     r->d.vis = last_set.vis; r->d.seg_count = last_set.seg_count; r->d.merge_flag = last_set.merge_flag;
+    r->d.upd_list = last_set.upd_list; r->d.upd_count = last_set.upd_count;
   }
   r->count_slot = c.CountSlot(c.last);
   SM_CUDA(cudaEventRecord(r->graph_exit, gs));

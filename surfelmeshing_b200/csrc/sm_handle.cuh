@@ -81,6 +81,8 @@ struct sm_reconstruction {
   smb::VisEntry* vis_set[smb::kSets] = {};
   smb::u32* seg_count_set[smb::kSets] = {};
   smb::u8* merge_flag_set[smb::kSets] = {};
+  uint2* upd_list_set[smb::kSets] = {};
+  smb::u32* upd_count_set[smb::kSets] = {};
   // stream-runner buffers (pre-processing outputs per buffer set)
   smb::u16* run_depth[smb::kSets] = {}; size_t run_depth_pitch = 0;
   float2* run_normals[smb::kSets] = {}; size_t run_normals_pitch = 0;

@@ -198,6 +198,11 @@ struct DeviceState {
   VisEntry* vis;         // capacity (rounded up to kSegment)
   u32* seg_count;        // capacity / kSegment
   u8* merge_flag;        // per list position
+  // Neighbour-update work list, filled by k_integrate: {slot, x | y << 16} of every surfel that passes the
+  // gates of k_update_neighbors up to the occlusion test (x, y: its pixel after the integration), in
+  // arbitrary order. Capacity as vis; the count is reset by k_project.
+  uint2* upd_list;
+  u32* upd_count;
   u8* new_flag;          // W*H
   u32* new_index;        // W*H
   u32* new_list;         // W*H: pixel (seq index) of the k-th new surfel
@@ -209,9 +214,16 @@ struct DeviceState {
   float4* gradient;
   // Smooth positions (the reference's rows 3-5), double-buffered: [3][stride] each. `smooth` is the
   // current buffer (initially the SoA rows themselves); the regularisation step reads it and writes
-  // every slot of `smooth_next`, then the two are swapped on the host (no separate update sweep).
+  // slots of `smooth_next` it has to (see reg_t_prev), then the two are swapped on the host (no separate
+  // update sweep).
   float* smooth;
   float* smooth_next;
+  // Host-side bookkeeping of the two smooth buffers (regularize.cu). Invariant: a slot whose stamp is below
+  // reg_t_prev holds the same smooth position in both buffers, unless reg_full_sweep is set (the second
+  // buffer is undefined: after sm_create, sm_load_state, sm_reset). reg_t_prev is int(frame - window) of the
+  // previous k_reg_step sweep, lowered to a frame index that k_integrate stamps below it.
+  int reg_t_prev;
+  int reg_full_sweep;
   // Device timeline (diagnostics, sm_timeline_enable): [frame % timeline_frames][kernel id]{first block start,
   // last block end} in %globaltimer nanoseconds; null when disabled.
   unsigned long long* timeline;
@@ -455,6 +467,15 @@ int ExportVertices(cudaStream_t stream, const DeviceState& d, int count_slot, in
 // `remove_replaced_below`: if >= 0, slot of the surfel count below which neighbour links to
 // surfels with the detach flag are dropped first (UpdateNeighborsCUDARemoveReplacedNeighbors
 // fused into the first sweep); -1 = no removal.
+// Bookkeeping of DeviceState::reg_t_prev on the host: after every k_reg_step sweep, and for every
+// Integrate() (k_integrate stamps surfels with its frame index, which may lie below the last threshold).
+inline void NoteRegStep(DeviceState& d, u32 frame_index, int window) {
+  d.reg_t_prev = static_cast<int>(frame_index - static_cast<u32>(window));
+  d.reg_full_sweep = 0;
+}
+inline void NoteIntegratedFrame(DeviceState& d, u32 frame_index) {
+  if (static_cast<int>(frame_index) < d.reg_t_prev) d.reg_t_prev = static_cast<int>(frame_index);
+}
 // Rebuilds row kRowMeta from the stamp and colour rows of slots [0, count) (after sm_load_state).
 int RebuildMetaRow(cudaStream_t stream, const DeviceState& d, u32 count, int sm_count);
 int RegularizeSurfels(cudaStream_t stream, DeviceState& d, bool disable_denoising, u32 frame_index,
