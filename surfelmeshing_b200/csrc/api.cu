@@ -154,7 +154,7 @@ const char* KernelName(int id) {
       "k_normals", "k_radii", "k_project", "k_associate", "k_merge", "k_blend", "k_integrate", "k_update_neighbors",
       "k_new_surfel_scan", "k_create_surfels", "k_reg_accumulate", "k_reg_step", "k_reg_copy_only",
       "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_project_tail",
-      "k_downscale_depth_median", "k_downscale_color"};
+      "k_downscale_depth_median", "k_downscale_color", "k_reg_mirror", "k_reg_pack"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -322,9 +322,9 @@ int CreateImpl(sm_reconstruction* r, uint64_t max_surfel_count, int32_t width, i
   const size_t scan_tiles = (P + kSegment - 1) / kSegment;
   SM_CUDA(cudaMalloc(&d.surfels, sizeof(float) * SM_ROW_COUNT * d.stride));
   SM_CUDA(cudaMalloc(&d.gradient, sizeof(float4) * d.stride));
-  SM_CUDA(cudaMalloc(&r->smooth_alt, sizeof(float) * 3 * d.stride));
-  d.smooth = d.surfels + static_cast<size_t>(SM_ROW_SMOOTH_X) * d.stride;  // rows 3-5 are contiguous
-  d.smooth_next = r->smooth_alt;
+  SM_CUDA(cudaMalloc(&r->reg_records, sizeof(float4) * 2 * d.stride));
+  d.smooth = r->reg_records;
+  d.smooth_next = r->reg_records + d.stride;
   SM_CUDA(cudaMemset(d.gradient, 0, sizeof(float4) * d.stride));
   for (int i = 0; i < kSets; ++i) {
     SM_CUDA(cudaMalloc(&r->assoc_set[i], sizeof(PixelAssoc) * P));
@@ -491,7 +491,7 @@ int sm_destroy(sm_reconstruction* r) {
   cudaGetLastError();
   DestroyFrameGraph(r->graph);
   DeviceState& d = r->d;
-  cudaFree(d.surfels); cudaFree(d.gradient); cudaFree(r->smooth_alt); cudaFree(d.new_list);
+  cudaFree(d.surfels); cudaFree(d.gradient); cudaFree(r->reg_records); cudaFree(d.new_list);
   for (int i = 0; i < kSets; ++i) {
     cudaFree(r->vis_set[i]); cudaFree(r->seg_count_set[i]); cudaFree(r->merge_flag_set[i]);
     cudaFree(r->upd_list_set[i]); cudaFree(r->upd_count_set[i]);
@@ -656,9 +656,11 @@ int sm_transfer_all_to_cpu(sm_reconstruction* r, void* stream_v, uint32_t /*fram
   const size_t bytes = sizeof(float) * n;
   const float* s = r->d.surfels;
   const size_t st = r->d.stride;
-  SM_CUDA(cudaMemcpyAsync(x, r->d.smooth + 0 * st, bytes, cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaMemcpyAsync(y, r->d.smooth + 1 * st, bytes, cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaMemcpyAsync(z, r->d.smooth + 2 * st, bytes, cudaMemcpyDeviceToHost, stream));
+  const int mirrored = MirrorRegRecords(stream, r->d, n, r->sm_count);   // rows 3-5 <- the current records
+  if (mirrored != SM_OK) return mirrored;
+  SM_CUDA(cudaMemcpyAsync(x, s + SM_ROW_SMOOTH_X * st, bytes, cudaMemcpyDeviceToHost, stream));
+  SM_CUDA(cudaMemcpyAsync(y, s + SM_ROW_SMOOTH_Y * st, bytes, cudaMemcpyDeviceToHost, stream));
+  SM_CUDA(cudaMemcpyAsync(z, s + SM_ROW_SMOOTH_Z * st, bytes, cudaMemcpyDeviceToHost, stream));
   SM_CUDA(cudaMemcpyAsync(radius_squared, s + SM_ROW_RADIUS_SQUARED * st, bytes, cudaMemcpyDeviceToHost, stream));
   SM_CUDA(cudaMemcpyAsync(nx, s + SM_ROW_NORMAL_X * st, bytes, cudaMemcpyDeviceToHost, stream));
   SM_CUDA(cudaMemcpyAsync(ny, s + SM_ROW_NORMAL_Y * st, bytes, cudaMemcpyDeviceToHost, stream));
@@ -708,12 +710,11 @@ int sm_dump_state(sm_reconstruction* r, void* stream_v, float* host_rows, uint64
   if (merge_count) *merge_count = r->host_counters->merge_count;
   if (host_rows && n > host_row_stride_elems) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_dump_state: host rows shorter than surfels_size()");
   if (host_rows && n > 0) {
+    // rows 3-5 and 15: the mirror of the current regularisation records (DeviceState::smooth)
+    const int mirrored = MirrorRegRecords(stream, r->d, n, r->sm_count);
+    if (mirrored != SM_OK) return mirrored;
     SM_CUDA(cudaMemcpy2DAsync(host_rows, host_row_stride_elems * sizeof(float), r->d.surfels,
                               r->d.stride * sizeof(float), n * sizeof(float), SM_ROW_COUNT, cudaMemcpyDeviceToHost,
-                              stream));
-    // rows 3-5: the current smooth-position buffer (may be the second one, DeviceState::smooth)
-    SM_CUDA(cudaMemcpy2DAsync(host_rows + SM_ROW_SMOOTH_X * host_row_stride_elems, host_row_stride_elems * sizeof(float),
-                              r->d.smooth, r->d.stride * sizeof(float), n * sizeof(float), 3, cudaMemcpyDeviceToHost,
                               stream));
     SM_CUDA(cudaStreamSynchronize(stream));
   }
@@ -724,10 +725,7 @@ int sm_load_state(sm_reconstruction* r, void* stream_v, const float* host_rows, 
                   uint32_t surfels_size, uint32_t merge_count) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   if (surfels_size > r->d.capacity) return SetError(SM_ERR_CAPACITY, "sm_load_state: state larger than the surfel cap");
-  // the loaded rows 3-5 are the current smooth-position buffer again
-  r->d.smooth = r->d.surfels + static_cast<size_t>(SM_ROW_SMOOTH_X) * r->d.stride;
-  r->d.smooth_next = r->smooth_alt;
-  r->d.reg_full_sweep = 1;  // smooth_next is undefined
+  r->d.reg_full_sweep = 1;  // as after sm_create (both record buffers are packed below)
   if (surfels_size > 0) {
     SM_CUDA(cudaMemcpy2DAsync(r->d.surfels, r->d.stride * sizeof(float), host_rows,
                               host_row_stride_elems * sizeof(float), surfels_size * sizeof(float), SM_ROW_COUNT,
@@ -738,9 +736,10 @@ int sm_load_state(sm_reconstruction* r, void* stream_v, const float* host_rows, 
     for (int row : zero_rows) {
       SM_CUDA(cudaMemsetAsync(r->d.surfels + row * r->d.stride, 0, surfels_size * sizeof(float), stream));
     }
-    // bookkeeping rows the library keeps in the reference's unused rows 14 / 15 (sm_kernels.cuh)
+    // bookkeeping row the library keeps in the reference's unused row 14 (sm_kernels.cuh)
     SM_CUDA(cudaMemsetAsync(r->d.surfels + kRowMergeEpoch * r->d.stride, 0, surfels_size * sizeof(float), stream));
-    const int status = RebuildMetaRow(stream, r->d, surfels_size, r->sm_count);
+    // both regularisation record buffers from the loaded rows 3-5, stamps and colours
+    const int status = PackRegRecords(stream, r->d, surfels_size, r->sm_count);
     if (status != SM_OK) return status;
   }
   Counters c{};

@@ -51,8 +51,6 @@ namespace {
 
 #define SM_S(row, i) d.surfels[static_cast<size_t>(row) * d.stride + (i)]
 #define SM_SU(row, i) reinterpret_cast<u32*>(d.surfels)[static_cast<size_t>(row) * d.stride + (i)]
-#define SM_SMOOTH(axis, i) d.smooth[static_cast<size_t>(axis) * d.stride + (i)]  // current smooth-position buffer
-#define SM_SMOOTH_NEXT(axis, i) d.smooth_next[static_cast<size_t>(axis) * d.stride + (i)]  // the other one
 
 constexpr int kBlock = 256;
 
@@ -1007,11 +1005,13 @@ __device__ __forceinline__ bool integrate_entry(const DeviceState& d, const Fram
       SM_SU(SM_ROW_LAST_UPDATE_STAMP, idx) = 0;
       SM_S(SM_ROW_RADIUS_SQUARED, idx) = -1.0f;
       reinterpret_cast<u8*>(&SM_SU(SM_ROW_COLOR, idx))[3] = 1;
-      SM_SU(kRowMeta, idx) = kMetaDetachBit;      // stamp 0, detach flag set
       SM_SU(kRowMergeEpoch, idx) = f.op_epoch;    // when it was merged (delta transfer)
-      // its stamp drops below every window: both smooth buffers have to hold its position (regularize.cu)
-      SM_SMOOTH_NEXT(0, idx) = SM_SMOOTH(0, idx); SM_SMOOTH_NEXT(1, idx) = SM_SMOOTH(1, idx);
-      SM_SMOOTH_NEXT(2, idx) = SM_SMOOTH(2, idx);
+      // Its stamp drops below every window: both record buffers have to hold its smooth position, and both
+      // the new meta word (stamp 0, detach flag set; DeviceState::smooth).
+      float4 record = d.smooth[idx];
+      record.w = __uint_as_float(kMetaDetachBit);
+      d.smooth[idx] = record;
+      d.smooth_next[idx] = record;
       return false;
     }
     if (!(e.x & kActiveBit)) return false;
@@ -1050,14 +1050,20 @@ __device__ __forceinline__ bool integrate_entry(const DeviceState& d, const Fram
       SM_S(SM_ROW_NORMAL_X, idx) = s.nx; SM_S(SM_ROW_NORMAL_Y, idx) = s.ny; SM_S(SM_ROW_NORMAL_Z, idx) = s.nz;
       SM_SU(SM_ROW_COLOR, idx) = s.color;
       if (s.stamped) {
-        // every path that changes the colour's flag byte also stamps the surfel
+        // every path that changes the colour's flag byte also stamps the surfel; the meta word goes to both
+        // record buffers (DeviceState::smooth), with the new smooth position after a replacement
         SM_SU(SM_ROW_LAST_UPDATE_STAMP, idx) = f.frame_index;
-        SM_SU(kRowMeta, idx) = f.frame_index | (((s.color >> 24) & 1u) ? kMetaDetachBit : 0u);
+        const u32 meta = f.frame_index | (((s.color >> 24) & 1u) ? kMetaDetachBit : 0u);
+        if (s.replaced) {
+          const float4 record = make_float4(s.smooth_x, s.smooth_y, s.smooth_z, __uint_as_float(meta));
+          d.smooth[idx] = record;
+          d.smooth_next[idx] = record;
+        } else {
+          store_reg_meta(d.smooth, idx, meta);
+          store_reg_meta(d.smooth_next, idx, meta);
+        }
       }
       if (s.replaced) {
-        // both smooth buffers (regularize.cu)
-        SM_SMOOTH(0, idx) = s.smooth_x; SM_SMOOTH(1, idx) = s.smooth_y; SM_SMOOTH(2, idx) = s.smooth_z;
-        SM_SMOOTH_NEXT(0, idx) = s.smooth_x; SM_SMOOTH_NEXT(1, idx) = s.smooth_y; SM_SMOOTH_NEXT(2, idx) = s.smooth_z;
         SM_SU(SM_ROW_CREATION_STAMP, idx) = f.frame_index;
 #pragma unroll
         for (int i = 0; i < 4; ++i) SM_SU(SM_ROW_NEIGHBOR0 + i, idx) = kInvalidIndex;
@@ -1362,9 +1368,10 @@ __global__ void __launch_bounds__(kBlock) k_create_surfels(DeviceState d, FrameP
       const u32 q = neighbor_index[direction];
       if (q == kInvalidIndex) continue;
       ndist[direction] = squared_norm(fsub(SM_S(SM_ROW_X, q), g.x), fsub(SM_S(SM_ROW_Y, q), g.y), fsub(SM_S(SM_ROW_Z, q), g.z));
-      nsx[direction] = SM_SMOOTH(0, q);
-      nsy[direction] = SM_SMOOTH(1, q);
-      nsz[direction] = SM_SMOOTH(2, q);
+      const float4 record = d.smooth[q];   // smooth position: one 16-byte gather
+      nsx[direction] = record.x;
+      nsy[direction] = record.y;
+      nsz[direction] = record.z;
     }
     float sum_x = 0.f, sum_y = 0.f, sum_z = 0.f;
     int existing_neighbor_count_plus_1 = 1;
@@ -1392,7 +1399,6 @@ __global__ void __launch_bounds__(kBlock) k_create_surfels(DeviceState d, FrameP
     SM_S(SM_ROW_CONFIDENCE, idx) = 1.0f;
     SM_SU(SM_ROW_CREATION_STAMP, idx) = f.frame_index;
     SM_SU(SM_ROW_LAST_UPDATE_STAMP, idx) = f.frame_index;
-    SM_SU(kRowMeta, idx) = f.frame_index;
     SM_S(SM_ROW_RADIUS_SQUARED, idx) = radius_squared;
     // The reference leaves rows 11-16 and 23 uninitialised; here rows 11-13 and 23 are always
     // zero and the regularisation accumulates in d.gradient, zero between calls (regularize.cu).
@@ -1403,9 +1409,10 @@ __global__ void __launch_bounds__(kBlock) k_create_surfels(DeviceState d, FrameP
     const float sx = fmul(fadd(g.x, sum_x), rcp_count);
     const float sy = fmul(fadd(g.y, sum_y), rcp_count);
     const float sz = fmul(fadd(g.z, sum_z), rcp_count);
-    // both smooth buffers (regularize.cu)
-    SM_SMOOTH(0, idx) = sx; SM_SMOOTH(1, idx) = sy; SM_SMOOTH(2, idx) = sz;
-    SM_SMOOTH_NEXT(0, idx) = sx; SM_SMOOTH_NEXT(1, idx) = sy; SM_SMOOTH_NEXT(2, idx) = sz;
+    // both record buffers (DeviceState::smooth): meta word = the stamp, detach flag clear
+    const float4 record = make_float4(sx, sy, sz, __uint_as_float(f.frame_index));
+    d.smooth[idx] = record;
+    d.smooth_next[idx] = record;
   }
 }
 
@@ -1417,9 +1424,10 @@ __global__ void __launch_bounds__(kBlock) k_export_vertices(DeviceState d, int c
   for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const bool merged = SM_S(SM_ROW_RADIUS_SQUARED, i) < 0.f;
     const float nan = __int_as_float(0x7fffffff);
-    position_buffer[3 * i + 0] = merged ? nan : SM_SMOOTH(0, i);
-    position_buffer[3 * i + 1] = merged ? nan : SM_SMOOTH(1, i);
-    position_buffer[3 * i + 2] = merged ? nan : SM_SMOOTH(2, i);
+    const float4 smooth = d.smooth[i];
+    position_buffer[3 * i + 0] = merged ? nan : smooth.x;
+    position_buffer[3 * i + 1] = merged ? nan : smooth.y;
+    position_buffer[3 * i + 2] = merged ? nan : smooth.z;
     const u32 c = SM_SU(SM_ROW_COLOR, i);
     color_buffer[3 * i + 0] = c & 0xFF;
     color_buffer[3 * i + 1] = (c >> 8) & 0xFF;

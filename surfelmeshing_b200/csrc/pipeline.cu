@@ -499,8 +499,8 @@ int RunGraph(RunContext& c, cudaStream_t stream, uint32_t* integrated) {
   const int it0 = c.first - 2;
 
   // smooth-position double buffer as the host tracks it (swapped by every denoising iteration)
-  float* smooth = r->d.smooth;
-  float* smooth_next = r->d.smooth_next;
+  float4* smooth = r->d.smooth;
+  float4* smooth_next = r->d.smooth_next;
 
   auto active = [&](int frame) { return frame >= c.first && frame < c.last; };
   auto clamp_frame = [&](int frame) { return frame < c.first ? c.first : (frame >= c.last ? c.last - 1 : frame); };
@@ -553,7 +553,7 @@ int RunGraph(RunContext& c, cudaStream_t stream, uint32_t* integrated) {
                            c.ip->radius_factor_for_regularization_neighbors, c.ip->regularizer_weight,
                            c.ip->regularization_frame_window_size, new_slot, i == 0 ? old_slot : -1);
         if (!disable_denoising && active(crit)) {  // k_reg_step fills the other smooth buffer
-          float* const filled = smooth_next;
+          float4* const filled = smooth_next;
           smooth_next = smooth;
           smooth = filled;
           d.smooth = smooth; d.smooth_next = smooth_next;

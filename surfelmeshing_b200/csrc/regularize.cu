@@ -14,6 +14,10 @@
 // surfels are created with zeros, Accumulate only adds into surfels inside the regularisation
 // window, and exactly those are reset by k_reg_step). The SoA rows 11-13 / 23 stay zero.
 // Float atomics make the accumulated gradients order-dependent, as in the reference.
+//
+// Smooth positions live in 16-byte regularisation records {x, y, z, stamp | detach << 31}, double-buffered
+// (DeviceState::smooth): a neighbour costs one gather (one 32-byte sector) in either sweep, where separate
+// rows cost one sector per value.
 
 #include <algorithm>
 #include <cstdlib>
@@ -26,12 +30,12 @@ namespace {
 
 #define SM_S(row, i) d.surfels[static_cast<size_t>(row) * d.stride + (i)]
 #define SM_SU(row, i) reinterpret_cast<u32*>(d.surfels)[static_cast<size_t>(row) * d.stride + (i)]
-#define SM_SMOOTH(axis, i) d.smooth[static_cast<size_t>(axis) * d.stride + (i)]
-#define SM_SMOOTH_NEXT(axis, i) d.smooth_next[static_cast<size_t>(axis) * d.stride + (i)]
 
 constexpr int kBlock = 256;
-// Minimum resident blocks per SM of the two sweeps (0 = whatever the register count gives: 4 and 5).
-// A/B hook (tools/build_variant.sh): more resident warps against spills.
+// Minimum resident blocks per SM of the two sweeps (1 = whatever the register count gives: 64 and 56 registers,
+// 4 blocks of 256 threads each). A/B hook (tools/build_variant.sh): more resident warps against spills. On an
+// H100 at 400 W (tools/ab_probe.py, VGA stream, median of 5 passes) 6 blocks (40 registers, spills in both
+// sweeps) ran 8 926 frames/s and 8 blocks (32 registers) 7 600, against 8 990-9 643 for the default.
 #ifndef SM_REG_ACCUMULATE_MIN_BLOCKS
 #define SM_REG_ACCUMULATE_MIN_BLOCKS 1
 #endif
@@ -84,15 +88,16 @@ __global__ void __launch_bounds__(kBlock, SM_REG_ACCUMULATE_MIN_BLOCKS) k_reg_ac
     }
     if ((nbr[0] & nbr[1] & nbr[2] & nbr[3]) == kInvalidIndex) continue;  // no neighbours at all
 
-    // batch 1: detach flag + stamp of the neighbours (one gather each: row kRowMeta), and this surfel's
-    // own attributes
-    u32 meta[4];
+    // batch 1: the record of each neighbour (detach flag + stamp and smooth position in one 16-byte gather),
+    // and this surfel's own attributes
+    float4 rec[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const u32 q = nbr[k] != kInvalidIndex ? nbr[k] : i;
-      meta[k] = SM_SU(kRowMeta, q);
+      rec[k] = d.smooth[q];
     }
-    const float sx = SM_SMOOTH(0, i), sy = SM_SMOOTH(1, i), sz = SM_SMOOTH(2, i);
+    const float4 self = d.smooth[i];
+    const float sx = self.x, sy = self.y, sz = self.z;
     const float nx = SM_S(SM_ROW_NORMAL_X, i), ny = SM_S(SM_ROW_NORMAL_Y, i), nz = SM_S(SM_ROW_NORMAL_Z, i);
     const float radius_squared = SM_S(SM_ROW_RADIUS_SQUARED, i);
 
@@ -102,24 +107,16 @@ __global__ void __launch_bounds__(kBlock, SM_REG_ACCUMULATE_MIN_BLOCKS) k_reg_ac
     int neighbor_count = 0;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      if (i < n_remove && nbr[k] != kInvalidIndex && (meta[k] & kMetaDetachBit)) {
+      const u32 meta = __float_as_uint(rec[k].w);
+      if (i < n_remove && nbr[k] != kInvalidIndex && (meta & kMetaDetachBit)) {
         nbr[k] = kInvalidIndex;
         SM_SU(SM_ROW_NEIGHBOR0 + k, i) = kInvalidIndex;
       }
-      use[k] = nbr[k] != kInvalidIndex && !outside_window(meta[k] & ~kMetaDetachBit, p);
+      use[k] = nbr[k] != kInvalidIndex && !outside_window(meta & ~kMetaDetachBit, p);
       neighbor_count += use[k] ? 1 : 0;
     }
     if (neighbor_count == 0) continue;
 
-    // batch 2: smooth positions of the neighbours
-    float qx[4], qy[4], qz[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const u32 q = use[k] ? nbr[k] : i;
-      qx[k] = SM_SMOOTH(0, q);
-      qy[k] = SM_SMOOTH(1, q);
-      qz[k] = SM_SMOOTH(2, q);
-    }
     const float max_distance_squared = fmul(radius_squared, p.radius_factor_squared);
     const float rcp_count = frcp(i2f(neighbor_count));
     const float factor = fmul(fadd(p.regularizer_weight, p.regularizer_weight), rcp_count);  // 2 * w / count
@@ -128,9 +125,9 @@ __global__ void __launch_bounds__(kBlock, SM_REG_ACCUMULATE_MIN_BLOCKS) k_reg_ac
     for (int k = 0; k < 4; ++k) {
       if (!use[k]) continue;
       const u32 q = nbr[k];
-      const float dx = fsub(qx[k], sx);
-      const float dy = fsub(qy[k], sy);
-      const float dz = fsub(qz[k], sz);
+      const float dx = fsub(rec[k].x, sx);
+      const float dy = fsub(rec[k].y, sy);
+      const float dz = fsub(rec[k].z, sz);
       const float f = fmul(factor, ffma(nz, dz, ffma(nx, dx, fmul(ny, dy))));
       // kernels.cu:2173-2176: four float atomicAdds; here one 16-byte vector atomic (sm_90+), the
       // same four fp32 additions in the same (arbitrary) arrival order
@@ -158,15 +155,14 @@ __global__ void __launch_bounds__(kBlock, SM_REG_STEP_MIN_BLOCKS) k_reg_step(Dev
       // Not regularised (kernels.cu:2206): the smooth position carries over to the next buffer. It already
       // is there unless the previous sweep moved it (DeviceState::reg_t_prev; stamps below t_prev were below
       // that sweep's threshold too, and every other writer of smooth positions writes both buffers).
-      if (p.full_sweep || static_cast<int>(stamp) >= p.t_prev) {
-        SM_SMOOTH_NEXT(0, i) = SM_SMOOTH(0, i); SM_SMOOTH_NEXT(1, i) = SM_SMOOTH(1, i); SM_SMOOTH_NEXT(2, i) = SM_SMOOTH(2, i);
-      }
+      if (p.full_sweep || static_cast<int>(stamp) >= p.t_prev) d.smooth_next[i] = d.smooth[i];
       continue;
     }
     u32 nbr[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) nbr[k] = SM_SU(SM_ROW_NEIGHBOR0 + k, i);
-    const float sx = SM_SMOOTH(0, i), sy = SM_SMOOTH(1, i), sz = SM_SMOOTH(2, i);
+    const float4 self = d.smooth[i];
+    const float sx = self.x, sy = self.y, sz = self.z;
     const float nx = SM_S(SM_ROW_NORMAL_X, i), ny = SM_S(SM_ROW_NORMAL_Y, i), nz = SM_S(SM_ROW_NORMAL_Z, i);
     // Data term (factor 2) + neighbour-induced terms.
     const float4 accumulated = d.gradient[i];
@@ -175,21 +171,19 @@ __global__ void __launch_bounds__(kBlock, SM_REG_STEP_MIN_BLOCKS) k_reg_step(Dev
     float gz = ffma(fsub(sz, SM_S(SM_ROW_Z, i)), 2.0f, accumulated.z);
     int neighbor_count = 0;
     float rx = 0.f, ry = 0.f, rz = 0.f;
-    float qx[4], qy[4], qz[4];
+    float4 rec[4];   // smooth positions of the neighbours: one 16-byte gather each
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const u32 q = nbr[k] != kInvalidIndex ? nbr[k] : i;
-      qx[k] = SM_SMOOTH(0, q);
-      qy[k] = SM_SMOOTH(1, q);
-      qz[k] = SM_SMOOTH(2, q);
+      rec[k] = d.smooth[q];
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (nbr[k] == kInvalidIndex) continue;
       ++neighbor_count;
-      const float dx = fsub(qx[k], sx);
-      const float dy = fsub(qy[k], sy);
-      const float dz = fsub(qz[k], sz);
+      const float dx = fsub(rec[k].x, sx);
+      const float dy = fsub(rec[k].y, sy);
+      const float dz = fsub(rec[k].z, sz);
       const float normal_dot_difference = ffma(nz, dz, ffma(nx, dx, fmul(ny, dy)));
       rx = ffma(-nx, normal_dot_difference, rx);
       ry = ffma(-ny, normal_dot_difference, ry);
@@ -207,11 +201,10 @@ __global__ void __launch_bounds__(kBlock, SM_REG_STEP_MIN_BLOCKS) k_reg_step(Dev
     const float max_step_length = fsqrt_approx(SM_S(SM_ROW_RADIUS_SQUARED, i));
     const float step_length = fmul(step_factor, gradient_length);
     if (step_length > max_step_length) step_factor = fmul(step_factor, fmul(max_step_length, frcp(step_length)));
-    // The new smooth position goes to the other buffer (the neighbours still read the old one);
-    // this surfel's accumulator, read by nobody else in this sweep, is reset for the next call.
-    SM_SMOOTH_NEXT(0, i) = ffma(step_factor, -gx, sx);
-    SM_SMOOTH_NEXT(1, i) = ffma(step_factor, -gy, sy);
-    SM_SMOOTH_NEXT(2, i) = ffma(step_factor, -gz, sz);
+    // The new smooth position goes to the other buffer (the neighbours still read the old one), with the
+    // meta word carried over; this surfel's accumulator, read by nobody else in this sweep, is reset for
+    // the next call.
+    d.smooth_next[i] = make_float4(ffma(step_factor, -gx, sx), ffma(step_factor, -gy, sy), ffma(step_factor, -gz, sz), self.w);
     d.gradient[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
@@ -232,28 +225,50 @@ __global__ void __launch_bounds__(kBlock) k_reg_copy_only(DeviceState d, RegPara
       }
     }
     if (outside_window(SM_SU(SM_ROW_LAST_UPDATE_STAMP, i), p)) continue;
-    // both buffers (see RegParams::t_prev)
-    const float x = SM_S(SM_ROW_X, i), y = SM_S(SM_ROW_Y, i), z = SM_S(SM_ROW_Z, i);
-    SM_SMOOTH(0, i) = x; SM_SMOOTH(1, i) = y; SM_SMOOTH(2, i) = z;
-    SM_SMOOTH_NEXT(0, i) = x; SM_SMOOTH_NEXT(1, i) = y; SM_SMOOTH_NEXT(2, i) = z;
+    // both buffers (see RegParams::t_prev), meta word unchanged
+    const float4 record = make_float4(SM_S(SM_ROW_X, i), SM_S(SM_ROW_Y, i), SM_S(SM_ROW_Z, i), d.smooth[i].w);
+    d.smooth[i] = record;
+    d.smooth_next[i] = record;
   }
 }
 
 }  // namespace
 
 namespace {
-__global__ void __launch_bounds__(kBlock) k_rebuild_meta(DeviceState d, u32 count) {
+__global__ void __launch_bounds__(kBlock) k_reg_pack(DeviceState d, u32 count) {
+  pdl_prologue();
   for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
     const u32 flag = (SM_SU(SM_ROW_COLOR, i) >> 24) == 1u ? kMetaDetachBit : 0u;
-    SM_SU(kRowMeta, i) = (SM_SU(SM_ROW_LAST_UPDATE_STAMP, i) & ~kMetaDetachBit) | flag;
+    const u32 meta = (SM_SU(SM_ROW_LAST_UPDATE_STAMP, i) & ~kMetaDetachBit) | flag;
+    const float4 record = make_float4(SM_S(SM_ROW_SMOOTH_X, i), SM_S(SM_ROW_SMOOTH_Y, i), SM_S(SM_ROW_SMOOTH_Z, i),
+                                      __uint_as_float(meta));
+    d.smooth[i] = record;
+    d.smooth_next[i] = record;
+  }
+}
+
+__global__ void __launch_bounds__(kBlock) k_reg_mirror(DeviceState d, u32 count) {
+  pdl_prologue();
+  for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
+    const float4 record = d.smooth[i];
+    SM_S(SM_ROW_SMOOTH_X, i) = record.x;
+    SM_S(SM_ROW_SMOOTH_Y, i) = record.y;
+    SM_S(SM_ROW_SMOOTH_Z, i) = record.z;
+    SM_SU(kRowMeta, i) = __float_as_uint(record.w);
   }
 }
 }  // namespace
 
-int RebuildMetaRow(cudaStream_t stream, const DeviceState& d, u32 count, int sm_count) {
+int PackRegRecords(cudaStream_t stream, const DeviceState& d, u32 count, int sm_count) {
   if (count == 0) return SM_OK;
-  k_rebuild_meta<<<sm_count * 4, kBlock, 0, stream>>>(d, count);
-  return CheckLaunch("rebuild meta row");
+  { LaunchScope scope(stream, KID_REG_PACK); LaunchKernel(k_reg_pack, dim3(sm_count * 4), dim3(kBlock), 0, stream, d, count); }
+  return CheckLaunch("pack regularisation records");
+}
+
+int MirrorRegRecords(cudaStream_t stream, const DeviceState& d, u32 count, int sm_count) {
+  if (count == 0) return SM_OK;
+  { LaunchScope scope(stream, KID_REG_MIRROR); LaunchKernel(k_reg_mirror, dim3(sm_count * 4), dim3(kBlock), 0, stream, d, count); }
+  return CheckLaunch("mirror regularisation records");
 }
 
 int DescribeRegularize(KernelLaunch* first, KernelLaunch* second, bool skip, const LaunchPlan& plan,
@@ -299,7 +314,7 @@ int RegularizeSurfels(cudaStream_t stream, DeviceState& d, bool disable_denoisin
   if (n == 1) return CheckLaunch("regularize (copy only)");
   LaunchOnStream(stream, second, true);
   // k_reg_step completed the other smooth buffer: it is the current one from here on
-  float* const filled = d.smooth_next;
+  float4* const filled = d.smooth_next;
   d.smooth_next = d.smooth;
   d.smooth = filled;
   NoteRegStep(d, frame_index, regularization_frame_window_size);

@@ -88,7 +88,7 @@ struct sm_reconstruction {
   float2* run_normals[smb::kSets] = {}; size_t run_normals_pitch = 0;
   float* run_radius[smb::kSets] = {}; size_t run_radius_pitch = 0;
   smb::u16* run_depth_pre[smb::kSets] = {};   // pre-blend copy of run_depth (merge runs next to blend)
-  float* smooth_alt = nullptr;    // second smooth-position buffer (DeviceState::smooth / smooth_next)
+  float4* reg_records = nullptr;  // [2][stride]: both regularisation record buffers (DeviceState::smooth / smooth_next)
   // multi-stream pipeline of round 1 (SM_B200_GRAPH=0)
   smb::PipelineCtx pipe{};
   cudaStream_t pre_stream = nullptr;

@@ -43,7 +43,6 @@ namespace {
 
 #define SM_S(row, i) d.surfels[static_cast<size_t>(row) * d.stride + (i)]
 #define SM_SU(row, i) reinterpret_cast<u32*>(d.surfels)[static_cast<size_t>(row) * d.stride + (i)]
-#define SM_SMOOTH(axis, i) d.smooth[static_cast<size_t>(axis) * d.stride + (i)]
 
 constexpr int kBlock = 256;
 
@@ -84,9 +83,10 @@ __global__ void __launch_bounds__(kBlock) k_delta_select(DeviceState d, DeltaArg
     a.index[k] = i;
     float* v = a.values + k;
     const size_t c = a.capacity;
-    v[0 * c] = SM_SMOOTH(0, i);
-    v[1 * c] = SM_SMOOTH(1, i);
-    v[2 * c] = SM_SMOOTH(2, i);
+    const float4 smooth = d.smooth[i];
+    v[0 * c] = smooth.x;
+    v[1 * c] = smooth.y;
+    v[2 * c] = smooth.z;
     v[3 * c] = radius_squared;
     v[4 * c] = SM_S(SM_ROW_NORMAL_X, i);
     v[5 * c] = SM_S(SM_ROW_NORMAL_Y, i);
@@ -120,7 +120,8 @@ __device__ __forceinline__ u32 pack_rgb(u32 r, u32 g, u32 b) { return (r & 0xFFu
 __global__ void __launch_bounds__(kBlock) k_viz_buffers(DeviceState d, VizArgs a) {
   const u32 n = d.counters->surfel_count[a.count_slot];
   for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float sx = SM_SMOOTH(0, i), sy = SM_SMOOTH(1, i), sz = SM_SMOOTH(2, i);
+    const float4 smooth = d.smooth[i];
+    const float sx = smooth.x, sy = smooth.y, sz = smooth.z;
     if (a.vertex) {
       // kernels.cu:287-351
       const u32 creation_stamp = SM_SU(SM_ROW_CREATION_STAMP, i);
@@ -185,7 +186,9 @@ int FullTransfer(sm_reconstruction* r, cudaStream_t stream, u32 n, float* const 
   const size_t bytes = sizeof(float) * n;
   const float* s = r->d.surfels;
   const size_t st = r->d.stride;
-  const float* src[7] = {r->d.smooth + 0 * st, r->d.smooth + 1 * st, r->d.smooth + 2 * st,
+  const int mirrored = MirrorRegRecords(stream, r->d, n, r->sm_count);   // rows 3-5 <- the current records
+  if (mirrored != SM_OK) return mirrored;
+  const float* src[7] = {s + SM_ROW_SMOOTH_X * st, s + SM_ROW_SMOOTH_Y * st, s + SM_ROW_SMOOTH_Z * st,
                          s + SM_ROW_RADIUS_SQUARED * st, s + SM_ROW_NORMAL_X * st, s + SM_ROW_NORMAL_Y * st,
                          s + SM_ROW_NORMAL_Z * st};
   for (int k = 0; k < 7; ++k) SM_CUDA(cudaMemcpyAsync(out[k], src[k], bytes, cudaMemcpyDeviceToHost, stream));
