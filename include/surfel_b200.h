@@ -409,6 +409,82 @@ int sm_stream_run(sm_reconstruction* r, void* stream, const sm_stream_desc* s,
                   const sm_preprocess_params* pp, const sm_integrate_params* ip,
                   int32_t first_frame, int32_t last_frame, sm_stream_stats* stats);
 
+/* The K = other_count outlier-filter transforms of reference frame `frame` (APP/main.cc:1039-1058) from
+ * per-frame poses (frame_count x 12 each, host): out[k] for the other frame o = frame - (k + 1) (k < K/2)
+ * or frame + (k - K/2 + 1) (k >= K/2), the layout sm_preprocess and sm_stream_desc.others_TR_reference
+ * take. Host only, no device needed. With A = frame_T_global[o] and B = global_T_frame[frame], both with
+ * their translation column multiplied by depth_scaling, out[k] = A . B, which equals the reference's
+ * (ref_T_global_scaled . global_T_other_scaled)^-1 without an explicit inverse. Every value is converted
+ * to double and every entry is evaluated as
+ *     m[r][c] = ((A[r][0] * B[0][c] + A[r][1] * B[1][c]) + A[r][2] * B[2][c])            (c < 3)
+ *     m[r][3] = (((A[r][0] * B[0][3] + A[r][1] * B[1][3]) + A[r][2] * B[2][3]) + A[r][3])
+ * (A[r][3] = double(frame_T_global[o][4 r + 3]) * double(depth_scaling), likewise B[k][3]), then rounded to
+ * float once. SM_ERR_INVALID_ARGUMENT for other_count not in {2, 4, 6, 8}, NULL pointers, or a frame without
+ * K/2 neighbours on both sides in [0, frame_count). */
+int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32_t frame_count,
+                                 const float* global_T_frame, const float* frame_T_global,
+                                 int32_t frame, float* out /* other_count x 12 */);
+
+/* ---- incremental stream sessions (the frame loop of APP/main.cc:885-1293, one frame per call) ----------
+ * A session runs the same pipeline as sm_stream_run on frames that arrive one at a time. The k-th pushed
+ * frame has frame index first_frame_index + k (first_frame_index + frames pushed < 2^30); frame_width x
+ * frame_height is the sensor size, as sm_stream_desc.width/height (the handle's size, or 2^L times it with
+ * "pyramid_level" L). A frame is integrated once its K/2 successors were pushed (K = pp's
+ * outlier_filtering_frame_count, 2, 4, 6 or 8); the first K/2 and the last K/2 frames of a session are never
+ * integrated (main.cc:987-992). The session computes frame f's outlier-filter transforms, as
+ * sm_outlier_filter_transforms does, from the pushed poses when frame f + K/2 arrives (pp.depth_scaling).
+ *
+ * In frame-graph mode pushing frame p launches the step {integrate p - K/2 - 2, associate p - K/2 - 1,
+ * pre-process p - K/2}, so status.last_integrated_frame becomes p - K/2 - 2; sm_session_end launches the
+ * remaining steps. The session runs serially on `stream` wherever sm_stream_run does (sm_enable_timings,
+ * sm_profile_kernels, a bilateral radius other than 6, SM_B200_GRAPH=0); a push of frame p then integrates
+ * p - K/2.
+ *
+ * Frames: with frame_on_host != 0, depth / colour are host memory, pageable or pinned. The push copies them
+ * into pinned staging owned by the library before it returns (main.cc:942-944, 974-976), so the caller may
+ * reuse the buffers at once; it blocks only while that staging slot's previous frame is still being
+ * uploaded. Otherwise they are device memory: they are copied (or downscaled / median-filtered, as in
+ * sm_stream_run) into the library's rings on an internal upload stream after the work enqueued on `stream`
+ * before the push, and `stream` waits for that copy, so work the caller enqueues on `stream` after the push
+ * may overwrite them. depth is u16 rows, colour packed u8x3 rows, pitches in bytes.
+ *
+ * Between pushes, calls on `stream` see the state after status.last_integrated_frame, and the next push's
+ * work waits for them: the hand-off calls (sm_transfer_all_to_cpu, sm_transfer_delta_to_cpu,
+ * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
+ * sm_frame_counters, sm_knn_build_from_reconstruction, sm_surfel_count / sm_surfels_size) and
+ * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
+ * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which
+ * that frame's Integrate() applies in the next step. The device merge counter then already includes them, so
+ * the push snapshots it first, and while the session is open the count queries report the snapshot:
+ * sm_surfel_count and sm_dump_state's merge_count are those after Integrate(last_integrated_frame), as
+ * in the reference (sm_export_vertices' non-NaN count == sm_surfel_count, main.cc:150).
+ *
+ * While a session is open, sm_integrate, sm_preprocess, sm_stream_run, sm_reset, sm_load_state,
+ * sm_configure, sm_enable_timings, sm_timeline_enable and a second sm_session_begin return
+ * SM_ERR_INVALID_ARGUMENT and leave the handle unchanged; so do sm_session_push / sm_session_end without
+ * one. A push with bad arguments (NULL pointers, a pitch below the row size) returns
+ * SM_ERR_INVALID_ARGUMENT without consuming the frame; the session stays open. A CUDA error drains the
+ * device and closes the session. sm_destroy ends an open session first.
+ *
+ * sm_session_end fills `stats` as sm_stream_run does, for the whole session: frames_integrated,
+ * surfels_size / surfel_count after it, the kernel launches since sm_session_begin, h2d_bytes = the
+ * sensor-size depth and colour bytes of every host frame pushed (0 for device frames), d2h_bytes = the
+ * counters fetched at the end, host_enqueue_ms = host time inside begin, the pushes and end. */
+typedef struct sm_session_status {
+  uint32_t frames_pushed;          /* since sm_session_begin */
+  uint32_t frames_integrated;      /* since sm_session_begin */
+  int64_t last_integrated_frame;   /* frame index of the newest integrated frame, -1 = none yet */
+} sm_session_status;
+
+int sm_session_begin(sm_reconstruction* r, void* stream, const sm_preprocess_params* pp,
+                     const sm_integrate_params* ip, int32_t frame_width, int32_t frame_height,
+                     uint32_t first_frame_index);
+int sm_session_push(sm_reconstruction* r, const uint16_t* depth, size_t depth_pitch,
+                    const uint8_t* color, size_t color_pitch, int32_t frame_on_host,
+                    const float global_T_frame[12], const float frame_T_global[12],
+                    sm_session_status* status /* may be NULL */);
+int sm_session_end(sm_reconstruction* r, sm_stream_stats* stats /* may be NULL */);
+
 /* Named tuning knobs of a handle (no counterpart in the reference). Keys:
  *   "tiebreak_wave" (slots per launch wave of the reference's association kernel; 0 = the plain rule "primary-pixel
  *   association before secondary, then lowest index"), "tiebreak_lanes" (consecutive slots that keep their order: a

@@ -111,6 +111,12 @@ class StreamStats(C.Structure):
     ]
 
 
+class SessionStatus(C.Structure):
+    """sm_session_status: progress of an incremental session after a push."""
+    _fields_ = [("frames_pushed", C.c_uint32), ("frames_integrated", C.c_uint32),
+                ("last_integrated_frame", C.c_int64)]
+
+
 _P = C.c_void_p
 _SZ = C.c_size_t
 _F = C.c_float
@@ -173,6 +179,10 @@ _PRODUCT_ONLY = {
     "knn_batch_host": (C.c_int, [_P, _P, _U32, _P, _P, _P, _P, _F, _F, _I, _P, _P, _P]),
     "timeline_enable": (C.c_int, [_P, _I]),
     "timeline_read": (C.c_int, [_P, C.POINTER(C.c_uint64), _I]),
+    "outlier_filter_transforms": (C.c_int, [_I, _F, _I, _P, _P, _I, _P]),
+    "session_begin": (C.c_int, [_P, _P, C.POINTER(PreprocessParams), C.POINTER(IntegrateParams), _I, _I, _U32]),
+    "session_push": (C.c_int, [_P, _P, _SZ, _P, _SZ, _I, _P, _P, C.POINTER(SessionStatus)]),
+    "session_end": (C.c_int, [_P, C.POINTER(StreamStats)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

@@ -7,7 +7,8 @@ repository tree.
 
 Flags: -ftz=true -fmad=false. The kernels spell out every fp32 operation (csrc/sm_math.cuh)
 in the order of the reference's -use_fast_math SASS; -fmad=false guarantees the compiler
-contracts nothing on its own.
+contracts nothing on its own. -ffp-contract=off does the same for the host compiler, whose default
+would fuse the documented products and sums of sm_outlier_filter_transforms on hosts with FMA units.
 """
 from __future__ import annotations
 
@@ -29,6 +30,7 @@ NVCC_FLAGS = [
     "-O3", "-lineinfo",
     "-ftz=true", "-fmad=false", "-prec-div=true", "-prec-sqrt=true",
     "-Xcompiler", "-fPIC",
+    "-Xcompiler", "-ffp-contract=off",   # host code too (sm_outlier_filter_transforms documents its order)
     "-Xptxas", "-v",
 ]
 

@@ -189,10 +189,21 @@ using namespace smb;
     }                                                                                        \
   } while (0)
 
+namespace {
+// Calls that would change what an open session builds on (sm_session_begin, include/surfel_b200.h).
+int RejectInSession(const char* call) {
+  return SetError(SM_ERR_INVALID_ARGUMENT, (std::string(call) + ": a stream session is open on this handle (sm_session_end first)").c_str());
+}
+}  // namespace
+
 namespace smb {
 
 int FetchCounters(sm_reconstruction* r, cudaStream_t stream) {
   SM_CUDA(cudaMemcpyAsync(r->host_counters, r->d.counters, sizeof(Counters), cudaMemcpyDeviceToHost, stream));
+  if (r->reported_merge_count) {   // an open frame-graph session (pipeline.cu: SessionPush)
+    SM_CUDA(cudaMemcpyAsync(&r->host_counters->merge_count, r->reported_merge_count, sizeof(u32), cudaMemcpyDeviceToHost,
+                            stream));
+  }
   SM_CUDA(cudaStreamSynchronize(stream));
   if (r->host_counters->capacity_overflow) {
     return SetError(SM_ERR_CAPACITY, "surfel cap exceeded: new surfels of at least one frame were dropped "
@@ -487,6 +498,7 @@ int sm_create(sm_reconstruction** out, uint64_t max_surfel_count, int32_t width,
 
 int sm_destroy(sm_reconstruction* r) {
   if (!r) return SM_OK;
+  if (r->session) SessionEnd(r, nullptr);   // drains the open session
   cudaDeviceSynchronize();
   cudaGetLastError();
   DestroyFrameGraph(r->graph);
@@ -527,6 +539,7 @@ int sm_destroy(sm_reconstruction* r) {
 }
 
 int sm_reset(sm_reconstruction* r, void* stream) {
+  if (r->session) return RejectInSession("sm_reset");
   SM_CUDA(cudaMemsetAsync(r->d.counters, 0, sizeof(Counters), static_cast<cudaStream_t>(stream)));
   r->count_slot = 0;
   r->rasters_cleared = false;
@@ -540,6 +553,8 @@ int sm_preprocess(sm_reconstruction* r, void* stream, const sm_preprocess_params
                   size_t raw_pitch, const uint16_t* const* other_depths, const size_t* other_pitches,
                   const float* others_TR_reference, uint16_t* out_depth, size_t out_depth_pitch, float* out_normals,
                   size_t out_normals_pitch, float* out_radius, size_t out_radius_pitch) {
+  // the frame pipeline of a session pre-processes through the same scratch_B
+  if (r->session) return RejectInSession("sm_preprocess");
   const int status = PreprocessFused(static_cast<cudaStream_t>(stream), *p, r->d.width, r->d.height, r->fx, r->fy,
                                      r->cx, r->cy, raw_depth, raw_pitch, other_depths, other_pitches,
                                      others_TR_reference, r->scratch_B, r->scratch_B_pitch, out_depth,
@@ -618,6 +633,7 @@ int sm_integrate(sm_reconstruction* r, void* stream, uint32_t frame_index, const
                  uint16_t* depth, size_t depth_pitch, const float* normals, size_t normals_pitch, const float* radius,
                  size_t radius_pitch, const uint8_t* color, size_t color_pitch, const float global_T_local[12],
                  const float local_T_global[12]) {
+  if (r->session) return RejectInSession("sm_integrate");
   return IntegrateImpl(r, static_cast<cudaStream_t>(stream), frame_index, *p, depth, depth_pitch, normals,
                        normals_pitch, radius, radius_pitch, color, color_pitch, global_T_local, local_T_global);
 }
@@ -697,6 +713,7 @@ int sm_get_timings(sm_reconstruction* r, float out_ms[7]) {
 }
 
 int sm_enable_timings(sm_reconstruction* r, int32_t enable) {
+  if (r->session) return RejectInSession("sm_enable_timings");
   r->events.enabled = enable != 0;
   return SM_OK;
 }
@@ -724,6 +741,7 @@ int sm_dump_state(sm_reconstruction* r, void* stream_v, float* host_rows, uint64
 int sm_load_state(sm_reconstruction* r, void* stream_v, const float* host_rows, uint64_t host_row_stride_elems,
                   uint32_t surfels_size, uint32_t merge_count) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (r->session) return RejectInSession("sm_load_state");
   if (surfels_size > r->d.capacity) return SetError(SM_ERR_CAPACITY, "sm_load_state: state larger than the surfel cap");
   r->d.reg_full_sweep = 1;  // as after sm_create (both record buffers are packed below)
   if (surfels_size > 0) {
@@ -801,6 +819,7 @@ int sm_frame_counters(sm_reconstruction* r, void* stream_v, uint64_t out[4]) {
 
 int sm_timeline_enable(sm_reconstruction* r, int32_t frames) {
   if (r == nullptr || frames < 0) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_timeline_enable: bad arguments");
+  if (r->session) return RejectInSession("sm_timeline_enable");
   SM_CUDA(cudaDeviceSynchronize());
   if (r->d.timeline) {
     cudaFree(r->d.timeline);
@@ -830,7 +849,44 @@ int sm_timeline_read(sm_reconstruction* r, uint64_t* out, int32_t frames) {
 int sm_stream_run(sm_reconstruction* r, void* stream_v, const sm_stream_desc* s, const sm_preprocess_params* pp,
                   const sm_integrate_params* ip, int32_t first_frame, int32_t last_frame, sm_stream_stats* stats) {
   if (!r || !s || !pp || !ip) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_stream_run: null argument");
+  if (r->session) return RejectInSession("sm_stream_run");
   return StreamRun(r, static_cast<cudaStream_t>(stream_v), s, pp, ip, first_frame, last_frame, stats);
+}
+
+int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32_t frame_count,
+                                 const float* global_T_frame, const float* frame_T_global, int32_t frame, float* out) {
+  if (!global_T_frame || !frame_T_global || !out) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: null argument");
+  if (other_count < 2 || other_count > 8 || other_count % 2 != 0)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: other_count must be 2, 4, 6 or 8");
+  const int half = other_count / 2;
+  if (frame < half || frame >= frame_count - half)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: the frame needs other_count/2 frames on both sides (main.cc:987-992)");
+  const float* ref = global_T_frame + 12 * static_cast<size_t>(frame);
+  for (int i = 0; i < half; ++i) {
+    OutlierFilterTransform(depth_scaling, ref, frame_T_global + 12 * static_cast<size_t>(frame - (i + 1)), out + 12 * i);
+    OutlierFilterTransform(depth_scaling, ref, frame_T_global + 12 * static_cast<size_t>(frame + (i + 1)), out + 12 * (half + i));
+  }
+  return SM_OK;
+}
+
+// An incremental session on the handle (pipeline.cu).
+int sm_session_begin(sm_reconstruction* r, void* stream, const sm_preprocess_params* pp, const sm_integrate_params* ip,
+                     int32_t frame_width, int32_t frame_height, uint32_t first_frame_index) {
+  if (!r || !pp || !ip) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_begin: null argument");
+  return SessionBegin(r, static_cast<cudaStream_t>(stream), pp, ip, frame_width, frame_height, first_frame_index);
+}
+
+int sm_session_push(sm_reconstruction* r, const uint16_t* depth, size_t depth_pitch, const uint8_t* color,
+                    size_t color_pitch, int32_t frame_on_host, const float global_T_frame[12],
+                    const float frame_T_global[12], sm_session_status* status) {
+  if (!r) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_push: null argument");
+  return SessionPush(r, depth, depth_pitch, color, color_pitch, frame_on_host != 0, global_T_frame, frame_T_global,
+                     status);
+}
+
+int sm_session_end(sm_reconstruction* r, sm_stream_stats* stats) {
+  if (!r) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_end: null argument");
+  return SessionEnd(r, stats);
 }
 
 // Named tuning / experiment knobs of a handle (no counterpart in the reference):
@@ -843,6 +899,7 @@ int sm_stream_run(sm_reconstruction* r, void* stream_v, const sm_stream_desc* s,
 //                              way into the frame rings (APP/main.cc:299-303, 946-981; default 0)
 int sm_configure(sm_reconstruction* r, const char* key, double value) {
   if (!r || !key) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_configure: null argument");
+  if (r->session) return RejectInSession("sm_configure");
   const std::string k(key);
   if (k == "tiebreak_wave") {
     if (value < 0 || value > 2147483647.0) return SetError(SM_ERR_INVALID_ARGUMENT, "tiebreak_wave out of range");

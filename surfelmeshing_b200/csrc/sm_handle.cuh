@@ -46,6 +46,8 @@ int SetTieBreakWave(TieBreakConfig* cfg, u32 wave, u32 capacity);   // uses cfg-
 
 struct FrameGraph;  // pipeline.cu
 void DestroyFrameGraph(FrameGraph* g);
+struct StreamSession;  // pipeline.cu: an open sm_session_begin
+void DestroySession(StreamSession* s);
 
 }  // namespace smb
 
@@ -122,6 +124,11 @@ struct sm_reconstruction {
   cudaStream_t graph_stream = nullptr;
   cudaEvent_t graph_exit = nullptr;
   smb::FrameGraph* graph = nullptr;
+  // incremental session (sm_session_begin .. sm_session_end); nullptr = none open
+  smb::StreamSession* session = nullptr;
+  // Set while a frame-graph session is open: a device copy of Counters::merge_count as of the newest integrated
+  // frame, which FetchCounters reports instead (the front half of a step already counted the next frame's merges).
+  const smb::u32* reported_merge_count = nullptr;
 };
 
 namespace smb {
@@ -149,4 +156,11 @@ int UpdateVisualizationBuffers(sm_reconstruction* r, cudaStream_t stream, const 
 // pipeline.cu
 int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
               const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats);
+int SessionBegin(sm_reconstruction* r, cudaStream_t stream, const sm_preprocess_params* pp,
+                 const sm_integrate_params* ip, int width, int height, uint32_t first_frame_index);
+int SessionPush(sm_reconstruction* r, const u16* depth, size_t depth_pitch, const uint8_t* color, size_t color_pitch,
+                bool on_host, const float* global_T_frame, const float* frame_T_global, sm_session_status* status);
+int SessionEnd(sm_reconstruction* r, sm_stream_stats* stats);
+// out (3x4) = scale(other_T_global) . scale(global_T_ref) (sm_outlier_filter_transforms)
+void OutlierFilterTransform(float depth_scaling, const float* global_T_ref, const float* other_T_global, float* out);
 }  // namespace smb

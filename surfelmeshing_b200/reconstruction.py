@@ -19,8 +19,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import (IntegrateParams, Library, PreprocessParams, StreamDesc, StreamStats, TransferStats, TransferToken,
-                   VisualizationParams)
+from ._lib import (IntegrateParams, Library, PreprocessParams, SessionStatus, StreamDesc, StreamStats, TransferStats,
+                   TransferToken, VisualizationParams)
 
 BUFFER_NAMES = ["surfel_x_buffer", "surfel_y_buffer", "surfel_z_buffer", "surfel_radius_squared_buffer",
                 "surfel_normal_x_buffer", "surfel_normal_y_buffer", "surfel_normal_z_buffer",
@@ -422,3 +422,116 @@ class CUDASurfelReconstruction:
         self.lib.call("stream_run", self._h, _stream_handle(stream), C.byref(desc), C.byref(pp), C.byref(ip),
                       int(first_frame), int(last_frame), C.byref(stats))
         return stats
+
+    def session(self, pp: PreprocessParams, ip: IntegrateParams, frame_size, first_frame_index: int = 0,
+                stream=None) -> "StreamSession":
+        """An incremental session (sm_session_begin): the frame loop of APP/main.cc:885-1293 with frames pushed
+        one at a time. `frame_size` = (width, height) of the sensor frames. Use as a context manager::
+
+            with rec.session(pp, ip, (640, 480)) as s:
+                for depth, color, g, l in frames:
+                    s.push(depth, color, g, l)
+            s.stats   # StreamStats of sm_session_end
+        """
+        return StreamSession(self, pp, ip, frame_size, first_frame_index, stream)
+
+
+def _dtype_name(a) -> str:
+    """'uint16', 'uint8', ... of a torch tensor or a numpy-convertible array."""
+    if isinstance(a, torch.Tensor):
+        return str(a.dtype).replace("torch.", "")
+    return np.asarray(a).dtype.name
+
+
+def _frame_arg(a, channels: int):
+    """(pointer, pitch in bytes, on_host, keep-alive) of a depth [H, W] or colour [H, W, 3] frame: a CUDA tensor
+    (row-pitched), or any CPU tensor / array (copied to a contiguous array if it is not row-pitched)."""
+    if isinstance(a, torch.Tensor) and a.is_cuda:
+        ptr, pitch = _raster(a, channels)
+        return ptr, pitch, 0, a
+    if isinstance(a, torch.Tensor):
+        a = a.numpy()
+    a = np.asarray(a)
+    inner_ok = a.ndim == (2 if channels == 1 else 3) and a.strides[-1] == a.itemsize and (
+        channels == 1 or a.strides[1] == channels * a.itemsize)
+    if not inner_ok or a.strides[0] <= 0:
+        a = np.ascontiguousarray(a)
+    return C.c_void_p(a.ctypes.data), a.strides[0], 1, a
+
+
+class StreamSession:
+    """An open sm_session_begin on a CUDASurfelReconstruction (see CUDASurfelReconstruction.session)."""
+
+    def __init__(self, rec: CUDASurfelReconstruction, pp: PreprocessParams, ip: IntegrateParams, frame_size,
+                 first_frame_index: int = 0, stream=None):
+        self.rec, self.pp, self.ip = rec, pp, ip
+        self.width, self.height = (int(v) for v in frame_size)
+        self.stream = _stream_handle(stream)
+        self.stats: Optional[StreamStats] = None
+        rec.lib.call("session_begin", rec._h, self.stream, C.byref(pp), C.byref(ip), self.width, self.height,
+                     int(first_frame_index))
+        self.open = True
+
+    def push(self, depth, color, global_T_frame, frame_T_global) -> SessionStatus:
+        """sm_session_push: depth [H, W] uint16 and colour [H, W, 3] uint8 as CUDA tensors or any CPU tensor /
+        array (copied into pinned staging before the call returns), and the frame's two 3x4 poses."""
+        if tuple(depth.shape[:2]) != (self.height, self.width) or tuple(color.shape[:2]) != (self.height, self.width):
+            raise ValueError(f"frames must be {self.height} x {self.width}")
+        if _dtype_name(depth) != "uint16" or _dtype_name(color) != "uint8" or len(color.shape) != 3 or color.shape[2] != 3:
+            raise ValueError("depth must be uint16 [H, W] and colour uint8 [H, W, 3]")
+        dp, dpitch, d_host, _keep_d = _frame_arg(depth, 1)
+        cp, cpitch, c_host, _keep_c = _frame_arg(color, 3)
+        if d_host != c_host:
+            raise ValueError("depth and colour must both be CUDA tensors or both host memory")
+        g = _mat12(global_T_frame)
+        l = _mat12(frame_T_global)
+        status = SessionStatus()
+        self.rec.lib.call("session_push", self.rec._h, dp, dpitch, cp, cpitch, d_host, g.ctypes.data_as(C.c_void_p),
+                          l.ctypes.data_as(C.c_void_p), C.byref(status))
+        return status
+
+    def end(self) -> StreamStats:
+        """sm_session_end: integrates what is left and returns the session's StreamStats."""
+        if self.open:
+            self.open = False
+            stats = StreamStats()
+            self.rec.lib.call("session_end", self.rec._h, C.byref(stats))
+            self.stats = stats
+        return self.stats
+
+    def __enter__(self) -> "StreamSession":
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        if exc_type is None:
+            self.end()
+        elif self.open:   # an error inside the block: drain and close without masking it
+            self.open = False
+            self.rec.lib.fn["session_end"](self.rec._h, None)
+        return False
+
+
+def outlier_filter_transforms(global_T_frame, frame_T_global, frame: int, other_count: int, depth_scaling: float,
+                              lib: Optional[Library] = None) -> np.ndarray:
+    """sm_outlier_filter_transforms: the [K, 3, 4] float32 transforms of reference frame `frame`
+    (APP/main.cc:1039-1058) from [F, 3, 4] poses."""
+    lib = lib or _lib.load_product()
+    g = np.ascontiguousarray(np.asarray(global_T_frame, np.float32).reshape(-1, 12))
+    l = np.ascontiguousarray(np.asarray(frame_T_global, np.float32).reshape(-1, 12))
+    assert g.shape == l.shape
+    out = np.zeros((int(other_count), 12), np.float32)
+    lib.call("outlier_filter_transforms", int(other_count), float(depth_scaling), g.shape[0], g.ctypes.data_as(C.c_void_p),
+             l.ctypes.data_as(C.c_void_p), int(frame), out.ctypes.data_as(C.c_void_p))
+    return out.reshape(-1, 3, 4)
+
+
+def stream_outlier_filter_transforms(global_T_frame, frame_T_global, other_count: int, depth_scaling: float,
+                                     lib: Optional[Library] = None) -> np.ndarray:
+    """[F, K, 3, 4] float32 for sm_stream_run / stream_run, by sm_outlier_filter_transforms; frames without K/2
+    neighbours get identity (as synthetic.others_TR_reference)."""
+    F = np.asarray(global_T_frame).reshape(-1, 12).shape[0]
+    half = int(other_count) // 2
+    out = np.tile(np.eye(4, dtype=np.float32)[:3][None, None], (F, int(other_count), 1, 1))
+    for frame in range(half, F - half):
+        out[frame] = outlier_filter_transforms(global_T_frame, frame_T_global, frame, other_count, depth_scaling, lib)
+    return out

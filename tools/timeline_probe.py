@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Device timeline of the frame pipeline (sm_timeline_enable): per-kernel start/end stamps
-written by the kernels themselves while sm_stream_run pipelines the stream. Prints the mean
-duration per kernel, the frame period and a few consecutive frames as a Gantt table; writes the
+written by the kernels themselves while sm_stream_run pipelines the stream (or, with --session, while a session
+is pushed the same frames from device memory). Prints the mean duration per kernel, the frame period, the time
+per frame in which no kernel of the pipeline runs, and a few consecutive frames as a Gantt table; writes the
 raw stamps to probe_out/timeline.csv."""
 import argparse
 import ctypes as C
@@ -23,6 +24,7 @@ def main():
     ap.add_argument("--show", type=int, default=450, help="first frame of the Gantt table")
     ap.add_argument("--count", type=int, default=3)
     ap.add_argument("--out", default="probe_out/timeline.csv")
+    ap.add_argument("--session", action="store_true", help="push the frames through a session instead")
     args = ap.parse_args()
     lib = _lib.load_product()
     cam = S.Camera.tum(640, 480)
@@ -41,8 +43,14 @@ def main():
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        stats = rec.stream_run(None, depth, color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
-                               f0, f1)
+        if args.session:
+            with rec.session(pp, ip, (cam.width, cam.height)) as s:
+                for f in range(args.frames):
+                    s.push(depth[f], color[f], st.global_T_frame[f], st.frame_T_global[f])
+            stats = s.stats
+        else:
+            stats = rec.stream_run(None, depth, color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp,
+                                   ip, f0, f1)
         e1.record()
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1)
@@ -71,6 +79,17 @@ def main():
     kp = names.index("k_project")
     period = np.diff(start[lo:hi, kp]) / 1e3
     print(f"frame period (project start to project start): mean {period.mean():.2f} us  median {np.median(period):.2f}")
+    # device time without any pipeline kernel running, between the first kernel of frame lo and frame hi's k_project
+    w0, w1 = start[lo][valid[lo]].min(), start[hi, kp]
+    spans = sorted((s_, e_) for f in range(lo - 3, hi + 3) for s_, e_, ok in zip(start[f], end[f], valid[f])
+                   if ok and e_ > w0 and s_ < w1)
+    idle, cursor = 0.0, w0
+    for s_, e_ in spans:
+        if s_ > cursor:
+            idle += s_ - cursor
+        cursor = max(cursor, e_)
+    idle += max(0.0, w1 - cursor)
+    print(f"no pipeline kernel running: {idle / 1e3 / (hi - lo):.2f} us per frame")
     t0 = start[args.show, kp]
     for f in range(args.show, args.show + args.count):
         rows = [(start[f, k], end[f, k], names[k]) for k in range(kcount) if valid[f, k]]
