@@ -302,6 +302,53 @@ int sm_update_visualization_buffers(sm_reconstruction* r, void* stream, const sm
                                     float* vertex_buffer, uint32_t* neighbor_index_buffer,
                                     float* normal_vertex_buffer);
 
+/* ---- rendering the surfel cloud into any pinhole camera (DESIGN.md section 1 row f7, section 5.5) ----
+ * The reference shows the cloud in its Qt/OpenGL render window, where a geometry shader draws each surfel of
+ * the UpdateVisualizationBuffers vertex buffer as a splat (APP/surfel_meshing_render_window.cc:239-300,
+ * 948-1003). sm_render_surfels draws it without a display: every surfel as an oriented disk, into a
+ * deterministic z-buffer, from any camera and at any image size (independent of the handle's camera).
+ *
+ * Slots i in [0, surfels_size()) with radius_squared (row 7) > 0 are drawn (merged surfels, radius^2 < 0, are
+ * not). The disk has centre s = the current SMOOTH position (what TransferAllToCPU, the viewer and the meshing
+ * thread see), normal n = rows 8-10, squared radius row 7 and colour the low three bytes of row 24. Per
+ * surfel, in fp32 with denormals flushed to zero, no contraction:
+ *   1. c = view_T_global * s (per row: t = s.y*r.y; t = fma(s.x, r.x, t); t = fma(s.z, r.z, t); t + r.w) and
+ *      m = R(view_T_global) * n (the same without + r.w).
+ *   2. The surfel is skipped unless near_depth <= c.z <= far_depth.
+ *   3. For pixel (px, py): dx = ((float(px) + 0.5f) - cx) / fx and dy = ((float(py) + 0.5f) - cy) / fy
+ *      (IEEE division), the ray (dx, dy, 1); den = fma(m.z, 1, fma(m.x, dx, m.y*dy)) and
+ *      num = fma(m.z, c.z, fma(m.x, c.x, m.y*c.y)); the pixel is skipped if den == 0; t = num / den (IEEE)
+ *      must be finite and > 0; e = (t*dx - c.x, t*dy - c.y, t - c.z); the pixel is covered iff
+ *      fma(e.z, e.z, fma(e.x, e.x, e.y*e.y)) <= radius^2. There is no back-face culling.
+ *   4. A covered pixel proposes the key (bits(t) << 32) | i and keeps the smallest key: the nearest surfel
+ *      wins, equal depths go to the lower slot, so the images do not depend on the order of the GPU's work.
+ *   5. Outputs from the winning key: depth = t, index = i, colour = the low three bytes of row 24 (r, g, b),
+ *      normal = m (camera frame, not re-normalised). Pixels without a covering surfel get 0 and
+ *      SM_INVALID_SURFEL_INDEX.
+ * Each surfel only tests the pixels of a screen rectangle that contains every pixel step 3 can accept (the
+ * projection of its bounding sphere, rounded outwards); a sphere that reaches the camera plane tests the whole
+ * image. Which pixels are covered is decided by step 3 alone.
+ *
+ * Outputs are device buffers of height rows, pitches in bytes, any of them NULL but not all: depth f32,
+ * colour packed u8x3, normal f32x3, index u32. Bytes past a row's width x element size stay untouched.
+ * Asynchronous on `stream`, no host synchronisation; surfels_size() is read on the device. The handle keeps
+ * an 8-byte-per-pixel key raster and a list of large splats: the first call, and a call with a larger
+ * image, allocate them (sm_create allocates nothing for rendering). Only reads the surfel state.
+ * SM_ERR_INVALID_ARGUMENT (and no launch) for width or height <= 0, fx or fy zero or not finite, cx, cy or a
+ * pose entry not finite, near_depth <= 0 or far_depth <= near_depth (either NaN included), a non-NULL output
+ * whose pitch is below its row size, or all outputs NULL. */
+typedef struct sm_render_params {
+  int32_t width, height;        /* output image size */
+  float fx, fy, cx, cy;         /* pinhole intrinsics, pixel-corner convention as sm_create */
+  float near_depth, far_depth;  /* metres: a surfel is drawn iff near_depth <= its camera-space z <= far_depth */
+} sm_render_params;
+int sm_render_surfels(sm_reconstruction* r, void* stream, const sm_render_params* p,
+                      const float view_T_global[12],     /* 3x4 row-major, global -> camera */
+                      float* depth, size_t depth_pitch,
+                      uint8_t* color, size_t color_pitch,
+                      float* normal, size_t normal_pitch,
+                      uint32_t* index, size_t index_pitch);
+
 /* ---- radius-limited k-nearest-neighbour queries for the meshing thread (SURVEY section 8 f4) ----
  * Replaces CompressedOctree::FindNearestSurfelsWithinRadius<include_completed_surfels, include_free_surfels>
  * (octree.h:471, octree.cc:313-470; callers surfel_meshing.cc:421 <false, true> and :821 <true, false>) for a BATCH of
@@ -451,7 +498,7 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * Between pushes, calls on `stream` see the state after status.last_integrated_frame, and the next push's
  * work waits for them: the hand-off calls (sm_transfer_all_to_cpu, sm_transfer_delta_to_cpu,
  * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
- * sm_frame_counters, sm_knn_build_from_reconstruction, sm_surfel_count / sm_surfels_size) and
+ * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_surfel_count / sm_surfels_size) and
  * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
  * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which
  * that frame's Integrate() applies in the next step. The device merge counter then already includes them, so

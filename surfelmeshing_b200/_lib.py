@@ -117,6 +117,12 @@ class SessionStatus(C.Structure):
                 ("last_integrated_frame", C.c_int64)]
 
 
+class RenderParams(C.Structure):
+    """sm_render_params: output size, pinhole intrinsics (pixel-corner convention) and the depth range drawn."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_float), ("fy", C.c_float),
+                ("cx", C.c_float), ("cy", C.c_float), ("near_depth", C.c_float), ("far_depth", C.c_float)]
+
+
 _P = C.c_void_p
 _SZ = C.c_size_t
 _F = C.c_float
@@ -183,6 +189,7 @@ _PRODUCT_ONLY = {
     "session_begin": (C.c_int, [_P, _P, C.POINTER(PreprocessParams), C.POINTER(IntegrateParams), _I, _I, _U32]),
     "session_push": (C.c_int, [_P, _P, _SZ, _P, _SZ, _I, _P, _P, C.POINTER(SessionStatus)]),
     "session_end": (C.c_int, [_P, C.POINTER(StreamStats)]),
+    "render_surfels": (C.c_int, [_P, _P, C.POINTER(RenderParams), _P, _P, _SZ, _P, _SZ, _P, _SZ, _P, _SZ]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

@@ -154,7 +154,8 @@ const char* KernelName(int id) {
       "k_normals", "k_radii", "k_project", "k_associate", "k_merge", "k_blend", "k_integrate", "k_update_neighbors",
       "k_new_surfel_scan", "k_create_surfels", "k_reg_accumulate", "k_reg_step", "k_reg_copy_only",
       "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_project_tail",
-      "k_downscale_depth_median", "k_downscale_color", "k_reg_mirror", "k_reg_pack"};
+      "k_downscale_depth_median", "k_downscale_color", "k_reg_mirror", "k_reg_pack", "k_render_splat",
+      "k_render_large", "k_render_resolve"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -518,6 +519,7 @@ int sm_destroy(sm_reconstruction* r) {
   cudaFree(r->median_stage[0]); cudaFree(r->median_stage[1]);
   cudaFree(r->pyramid_depth_stage); cudaFree(r->pyramid_color_stage);
   FreeTransferBuffers(r);
+  FreeRenderBuffers(r);
   for (int i = 0; i < 2; ++i) {
     if (r->pipe.ev_create[i]) cudaEventDestroy(r->pipe.ev_create[i]);
     if (r->pipe.ev_update[i]) cudaEventDestroy(r->pipe.ev_update[i]);
@@ -700,6 +702,14 @@ int sm_update_visualization_buffers(sm_reconstruction* r, void* stream, const sm
                                     normal_vertex_buffer);
 }
 
+int sm_render_surfels(sm_reconstruction* r, void* stream, const sm_render_params* p, const float view_T_global[12],
+                      float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch, float* normal,
+                      size_t normal_pitch, uint32_t* index, size_t index_pitch) {
+  if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_surfels: null argument");
+  return RenderSurfels(r, static_cast<cudaStream_t>(stream), *p, view_T_global, depth, depth_pitch, color, color_pitch,
+                       normal, normal_pitch, index, index_pitch);
+}
+
 int sm_export_vertices(sm_reconstruction* r, void* stream, float* position_buffer, uint8_t* color_buffer) {
   return ExportVertices(static_cast<cudaStream_t>(stream), r->d, r->count_slot, r->sm_count, position_buffer,
                         color_buffer);
@@ -827,7 +837,7 @@ int sm_timeline_enable(sm_reconstruction* r, int32_t frames) {
     r->d.timeline_frames = 0;
   }
   if (frames == 0) return SM_OK;
-  const size_t slots = static_cast<size_t>(frames) * KID_COUNT;
+  const size_t slots = static_cast<size_t>(frames) * KID_TIMELINE_COUNT;
   SM_CUDA(cudaMalloc(&r->d.timeline, slots * 2 * sizeof(unsigned long long)));
   std::vector<unsigned long long> init(slots * 2);
   for (size_t i = 0; i < slots; ++i) { init[2 * i] = ~0ull; init[2 * i + 1] = 0ull; }
@@ -841,7 +851,15 @@ int sm_timeline_read(sm_reconstruction* r, uint64_t* out, int32_t frames) {
   if (r->d.timeline == nullptr || frames != static_cast<int32_t>(r->d.timeline_frames))
     return SetError(SM_ERR_INVALID_ARGUMENT, "sm_timeline_read: timeline not enabled with this frame count");
   SM_CUDA(cudaDeviceSynchronize());
-  SM_CUDA(cudaMemcpy(out, r->d.timeline, static_cast<size_t>(frames) * KID_COUNT * 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  // Rows of sm_profile_kernel_count() columns; the kernels without a timeline column read "not launched".
+  const size_t row = 2 * sizeof(uint64_t) * KID_COUNT, device_row = 2 * sizeof(uint64_t) * KID_TIMELINE_COUNT;
+  for (int32_t f = 0; f < frames; ++f) {
+    for (int k = KID_TIMELINE_COUNT; k < KID_COUNT; ++k) {
+      out[(static_cast<size_t>(f) * KID_COUNT + k) * 2] = ~0ull;
+      out[(static_cast<size_t>(f) * KID_COUNT + k) * 2 + 1] = 0ull;
+    }
+  }
+  SM_CUDA(cudaMemcpy2D(out, row, r->d.timeline, device_row, device_row, frames, cudaMemcpyDeviceToHost));
   return SM_OK;
 }
 

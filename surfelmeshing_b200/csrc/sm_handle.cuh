@@ -129,6 +129,12 @@ struct sm_reconstruction {
   // Set while a frame-graph session is open: a device copy of Counters::merge_count as of the newest integrated
   // frame, which FetchCounters reports instead (the front half of a step already counted the next frame's merges).
   const smb::u32* reported_merge_count = nullptr;
+  // sm_render_surfels scratch (render.cu), allocated by the first render: the key raster (all keys "empty"
+  // between calls), the large-splat list (capacity slots) and its count (zero between calls), resident grids.
+  unsigned long long* render_keys = nullptr; size_t render_key_capacity = 0;   // in pixels
+  smb::u32* render_large_list = nullptr;
+  smb::u32* render_large_count = nullptr;
+  int render_splat_blocks = 0, render_large_blocks = 0;
 };
 
 namespace smb {
@@ -153,6 +159,11 @@ int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_inde
                   uint32_t* last_update_stamp, sm_transfer_stats* stats);
 int UpdateVisualizationBuffers(sm_reconstruction* r, cudaStream_t stream, const sm_visualization_params& p, float* vertex,
                                uint32_t* neighbor_index, float* normal_vertex);
+// render.cu
+int RenderSurfels(sm_reconstruction* r, cudaStream_t stream, const sm_render_params& p, const float* view_T_global,
+                  float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch, float* normal,
+                  size_t normal_pitch, uint32_t* index, size_t index_pitch);
+void FreeRenderBuffers(sm_reconstruction* r);
 // pipeline.cu
 int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
               const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats);

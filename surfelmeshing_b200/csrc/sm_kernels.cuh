@@ -25,7 +25,11 @@ enum KernelId {
   KID_NORMALS, KID_RADII, KID_PROJECT, KID_ASSOCIATE, KID_MERGE, KID_BLEND, KID_INTEGRATE, KID_UPDATE_NEIGHBORS,
   KID_NEW_SURFEL_SCAN, KID_CREATE_SURFELS, KID_REG_ACCUMULATE, KID_REG_STEP, KID_REG_COPY_ONLY,
   KID_EXPORT_VERTICES, KID_MEDIAN_DENSIFY, KID_DELTA_SELECT, KID_VIZ_BUFFERS, KID_PROJECT_TAIL, KID_DOWNSCALE_DEPTH,
-  KID_DOWNSCALE_COLOR, KID_REG_MIRROR, KID_REG_PACK, KID_COUNT
+  KID_DOWNSCALE_COLOR, KID_REG_MIRROR, KID_REG_PACK,
+  // The kernels below this id have a column in the device timeline (DeviceState::timeline, [frame][column]); the
+  // render kernels (render.cu) run outside the frame pipeline and have none.
+  KID_TIMELINE_COUNT,
+  KID_RENDER_SPLAT = KID_TIMELINE_COUNT, KID_RENDER_LARGE, KID_RENDER_RESOLVE, KID_COUNT
 };
 const char* KernelName(int id);
 bool ProfilingEnabled();
@@ -292,7 +296,7 @@ struct TimelineScope {
   unsigned long long* slot;
   __device__ __forceinline__ explicit TimelineScope(unsigned long long* s) : slot(s) { begin(); }
   __device__ __forceinline__ TimelineScope(const DeviceState& d, u32 frame, int kernel_id)
-      : slot(d.timeline ? d.timeline + (static_cast<size_t>(frame % d.timeline_frames) * KID_COUNT + kernel_id) * 2 : nullptr) {
+      : slot(d.timeline ? d.timeline + (static_cast<size_t>(frame % d.timeline_frames) * KID_TIMELINE_COUNT + kernel_id) * 2 : nullptr) {
     begin();
   }
   __device__ __forceinline__ void begin() {
@@ -304,7 +308,7 @@ struct TimelineScope {
 };
 // Host side: slot of (frame, kernel id) for kernels that do not take a DeviceState.
 inline unsigned long long* TimelineSlot(const DeviceState& d, u32 frame, int kernel_id) {
-  return d.timeline ? d.timeline + (static_cast<size_t>(frame % d.timeline_frames) * KID_COUNT + kernel_id) * 2 : nullptr;
+  return d.timeline ? d.timeline + (static_cast<size_t>(frame % d.timeline_frames) * KID_TIMELINE_COUNT + kernel_id) * 2 : nullptr;
 }
 
 // SM_B200_PDL: 0 = never, 1 (default) = only launches marked as dependents (LaunchDependent: the

@@ -19,8 +19,10 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import (IntegrateParams, Library, PreprocessParams, SessionStatus, StreamDesc, StreamStats, TransferStats,
-                   TransferToken, VisualizationParams)
+from ._lib import (IntegrateParams, Library, PreprocessParams, RenderParams, SessionStatus, StreamDesc, StreamStats,
+                   TransferStats, TransferToken, VisualizationParams)
+
+RENDER_OUTPUTS = ("depth", "color", "normal", "index")
 
 BUFFER_NAMES = ["surfel_x_buffer", "surfel_y_buffer", "surfel_z_buffer", "surfel_radius_squared_buffer",
                 "surfel_normal_x_buffer", "surfel_normal_y_buffer", "surfel_normal_z_buffer",
@@ -320,6 +322,37 @@ class CUDASurfelReconstruction:
         ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
         self.lib.call("update_visualization_buffers", self._h, _stream_handle(stream), C.byref(p), ptr(vertex_buffer),
                       ptr(neighbor_index_buffer), ptr(normal_vertex_buffer))
+
+    def render(self, view_T_global, width: int, height: int, fx: float, fy: float, cx: float, cy: float,
+               near: float = 0.1, far: float = 100.0, stream=None, outputs=RENDER_OUTPUTS) -> dict:
+        """sm_render_surfels: the current cloud drawn as oriented disks (smooth position, normal, radius, colour)
+        into a pinhole camera of any size; the nearest disk wins a pixel, equal depths the lower slot.
+
+        view_T_global: 3x4 global-to-camera transform; fx, fy, cx, cy in the pixel-corner convention of the
+        handle's camera; surfels with camera-space z outside [near, far] are not drawn. Returns the requested
+        CUDA tensors, enqueued on `stream` (not synchronised): "depth" float32 [H, W] metres (0 = empty),
+        "color" uint8 [H, W, 3], "normal" float32 [H, W, 3] camera-frame normal (0 = empty), "index" int32
+        [H, W] surfel slot (-1 = empty)."""
+        outputs = tuple(outputs)
+        unknown = [o for o in outputs if o not in RENDER_OUTPUTS]
+        if unknown or not outputs:
+            raise ValueError(f"outputs must be a non-empty subset of {RENDER_OUTPUTS}, got {outputs}")
+        H, W = int(height), int(width)
+        shapes = {"depth": ((H, W), torch.float32), "color": ((H, W, 3), torch.uint8),
+                  "normal": ((H, W, 3), torch.float32), "index": ((H, W), torch.int32)}
+        out = {k: torch.empty(shapes[k][0], dtype=shapes[k][1], device="cuda") for k in outputs}
+        if isinstance(stream, torch.cuda.Stream):
+            for t in out.values():
+                t.record_stream(stream)   # allocated on the current stream, written on `stream`
+        args = []
+        for k in RENDER_OUTPUTS:
+            t = out.get(k)
+            args += [C.c_void_p(t.data_ptr()), t.stride(0) * t.element_size()] if t is not None else [None, 0]
+        p = RenderParams(W, H, float(fx), float(fy), float(cx), float(cy), float(near), float(far))
+        T = _mat12(view_T_global)
+        self.lib.call("render_surfels", self._h, _stream_handle(stream), C.byref(p), T.ctypes.data_as(C.c_void_p),
+                      *args)
+        return out
 
     def ExportVertices(self, stream, position_buffer: torch.Tensor, color_buffer: torch.Tensor):
         """cuda_surfel_reconstruction.cc:405-410."""
