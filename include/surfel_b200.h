@@ -425,8 +425,7 @@ int sm_download_rasters(sm_reconstruction* r, void* stream,
  * (APP/main.cc:902-995); otherwise they are device-resident.
  * The call never synchronises with the host inside the loop and overlaps the
  * kernels of three consecutive frames (one instantiated CUDA graph per frame
- * step on an internal stream, DESIGN.md section 5; SM_B200_GRAPH=0 selects the
- * multi-stream event pipeline instead); `stream` only brackets the call: work enqueued on it
+ * step on an internal stream, DESIGN.md section 5); `stream` only brackets the call: work enqueued on it
  * before the call is complete before the first frame starts, work enqueued
  * after the call sees all frames integrated. The call itself returns after
  * one synchronisation at the end (to fetch the counters for `stats`). With
@@ -484,14 +483,13 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * In frame-graph mode pushing frame p launches the step {integrate p - K/2 - 2, associate p - K/2 - 1,
  * pre-process p - K/2}, so status.last_integrated_frame becomes p - K/2 - 2; sm_session_end launches the
  * remaining steps. The session runs serially on `stream` wherever sm_stream_run does (sm_enable_timings,
- * sm_profile_kernels, a bilateral radius other than 6, SM_B200_GRAPH=0); a push of frame p then integrates
- * p - K/2.
+ * sm_profile_kernels); a push of frame p then integrates p - K/2.
  *
  * Frames: with frame_on_host != 0, depth / colour are host memory, pageable or pinned. The push copies them
  * into pinned staging owned by the library before it returns (main.cc:942-944, 974-976), so the caller may
  * reuse the buffers at once; it blocks only while that staging slot's previous frame is still being
  * uploaded. Otherwise they are device memory: they are copied (or downscaled / median-filtered, as in
- * sm_stream_run) into the library's rings on an internal upload stream after the work enqueued on `stream`
+ * sm_stream_run) into the library's rings after the work enqueued on `stream`
  * before the push, and `stream` waits for that copy, so work the caller enqueues on `stream` after the push
  * may overwrite them. depth is u16 rows, colour packed u8x3 rows, pitches in bytes.
  *

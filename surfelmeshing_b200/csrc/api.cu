@@ -153,9 +153,8 @@ const char* KernelName(int id) {
       "k_clear", "k_bilateral_outlier", "k_bilateral_generic", "k_outlier", "k_erode_normals_radii", "k_erode",
       "k_normals", "k_radii", "k_project", "k_associate", "k_merge", "k_blend", "k_integrate", "k_update_neighbors",
       "k_new_surfel_scan", "k_create_surfels", "k_reg_accumulate", "k_reg_step", "k_reg_copy_only",
-      "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_project_tail",
-      "k_downscale_depth_median", "k_downscale_color", "k_reg_mirror", "k_reg_pack", "k_render_splat",
-      "k_render_large", "k_render_resolve"};
+      "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_downscale_depth_median",
+      "k_downscale_color", "k_reg_mirror", "k_reg_pack", "k_render_splat", "k_render_large", "k_render_resolve"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -520,16 +519,9 @@ int sm_destroy(sm_reconstruction* r) {
   cudaFree(r->pyramid_depth_stage); cudaFree(r->pyramid_color_stage);
   FreeTransferBuffers(r);
   FreeRenderBuffers(r);
-  for (int i = 0; i < 2; ++i) {
-    if (r->pipe.ev_create[i]) cudaEventDestroy(r->pipe.ev_create[i]);
-    if (r->pipe.ev_update[i]) cudaEventDestroy(r->pipe.ev_update[i]);
-    if (r->pre_done[i]) cudaEventDestroy(r->pre_done[i]);
-    if (r->int_done[i]) cudaEventDestroy(r->int_done[i]);
-  }
-  for (cudaStream_t st : {r->pre_stream, r->pipe.crit, r->pipe.front, r->pipe.side, r->upload_stream, r->graph_stream})
+  for (cudaStream_t st : {r->upload_stream, r->graph_stream})
     if (st) cudaStreamDestroy(st);
-  for (cudaEvent_t e : {r->pipe.ev_assoc, r->pipe.ev_merge, r->pipe.ev_blend, r->pipe.ev_integrate, r->pipe.ev_reg,
-                        r->entry_event, r->upload_done, r->graph_exit})
+  for (cudaEvent_t e : {r->entry_event, r->upload_done, r->graph_exit})
     if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : r->iteration_done) if (e) cudaEventDestroy(e);
   for (u16* b : r->ring_depth) cudaFree(b);

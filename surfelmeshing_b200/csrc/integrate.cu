@@ -32,8 +32,8 @@
 // reference: first atomicCAS wins), merge decisions read the pre-merge state. Both are legal
 // outcomes of the reference.
 //
-// Host side at the end of the file: IntegrateFrame (one stream, stage events) and
-// IntegrateFramePipelined (the frame DAG over the streams of PipelineCtx, sm_kernels.cuh).
+// Host side at the end of the file: IntegrateFrame (one stream, stage events) and DescribeFrameKernel (the
+// launches as descriptors, which the frame graph of pipeline.cu is built from).
 
 #include <algorithm>
 #include <cstdio>
@@ -163,21 +163,14 @@ __global__ void __launch_bounds__(kBlock) k_clear(DeviceState d) {
 // ---------------------------------------------------------------------------------------
 constexpr int kProjectBlock = 512;  // 2 slots per thread, kSegment slots per block-iteration
 
-// `part`: which list segments the launch covers. The surfels created by the previous frame occupy the
-// slots [count before the previous frame, count before this frame): every segment entirely below them
-// only needs the previous frame's INTEGRATION, so the frame graph projects those (kProjectMain) beside
-// the previous frame's creation kernel and the remaining tail (kProjectTail) after it.
-enum { kProjectAll = 0, kProjectMain = 1, kProjectTail = 2 };
-
-__global__ void __launch_bounds__(kProjectBlock) k_project(DeviceState d, FrameParams f, int part) {
+__global__ void __launch_bounds__(kProjectBlock) k_project(DeviceState d, FrameParams f) {
   pdl_prologue();
   if (f.skip) return;
-  const TimelineScope timeline_scope(d, f.frame_index, part == kProjectTail ? KID_PROJECT_TAIL : KID_PROJECT);
+  const TimelineScope timeline_scope(d, f.frame_index, KID_PROJECT);
   __shared__ u32 warp_totals[kProjectBlock / 32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const u32 first_seg_if_all = blockIdx.x;
 
-  if (blockIdx.x == 0 && part != kProjectMain) {
+  if (blockIdx.x == 0) {
     // Reset the state of this frame's new-surfel scan and neighbour-update list (run after several kernel
     // boundaries).
     const int tiles = (d.width * d.height + kSegment - 1) / kSegment;
@@ -199,15 +192,9 @@ __global__ void __launch_bounds__(kProjectBlock) k_project(DeviceState d, FrameP
     return r;
   };
   SlotRows rows = {};
-  if (part != kProjectTail && (static_cast<size_t>(first_seg_if_all) + 1) * kSegment <= d.stride) rows = fetch(first_seg_if_all);
-  // Count before the previous frame (3-slot history, sm_kernels.cuh). kProjectMain must not read the
-  // current count: the previous frame's scan, which writes it, may still be running.
-  const u32 n_before = part == kProjectAll ? 0u : d.counters->surfel_count[(f.count_slot + kCountSlots - 1) % kCountSlots];
-  const u32 seg_begin = part == kProjectTail ? n_before / kSegment : 0u;
-  const u32 n = part == kProjectMain ? (n_before / kSegment) * kSegment
-                                     : d.counters->surfel_count[f.count_slot];   // slots [seg_begin * kSegment, n)
-  if (part == kProjectTail && static_cast<u64>(seg_begin + blockIdx.x) * kSegment < n) rows = fetch(seg_begin + blockIdx.x);
-  for (u32 seg = seg_begin + blockIdx.x; static_cast<u64>(seg) * kSegment < n; seg += gridDim.x) {
+  if ((static_cast<size_t>(blockIdx.x) + 1) * kSegment <= d.stride) rows = fetch(blockIdx.x);
+  const u32 n = d.counters->surfel_count[f.count_slot];
+  for (u32 seg = blockIdx.x; static_cast<u64>(seg) * kSegment < n; seg += gridDim.x) {
     const u32 base = seg * kSegment + threadIdx.x * 2;
     const SlotRows cur = rows;
     if (static_cast<u64>(seg + gridDim.x) * kSegment < n) rows = fetch(seg + gridDim.x);
@@ -1446,12 +1433,6 @@ size_t BlendSmemBytes(int radius) {
   return rn16 * 14 + mask_words * 11 * 4 + 16;
 }
 constexpr size_t kBlendSmemLimit = 224 * 1024;  // one region per block has to fit an SM
-
-#define SM_EV(call)                                                              \
-  do {                                                                           \
-    const cudaError_t e_ = (call);                                               \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, cudaGetErrorString(e_)); \
-  } while (0)
 }  // namespace
 
 int DescribeFrameKernel(FrameKernel which, const LaunchPlan& plan, const DeviceState& d, const FrameParams& f,
@@ -1460,11 +1441,7 @@ int DescribeFrameKernel(FrameKernel which, const LaunchPlan& plan, const DeviceS
   const int scan_tiles = (d.width * d.height + kSegment - 1) / kSegment;
   switch (which) {
     case FK_PROJECT:
-    case FK_PROJECT_MAIN:
       out->Reset(reinterpret_cast<const void*>(k_project), dim3(plan.project), dim3(kProjectBlock), 0, KID_PROJECT);
-      break;
-    case FK_PROJECT_TAIL:  // the segments that hold the previous frame's new surfels: a handful
-      out->Reset(reinterpret_cast<const void*>(k_project), dim3(plan.sm_count), dim3(kProjectBlock), 0, KID_PROJECT_TAIL);
       break;
     case FK_ASSOCIATE:
       out->Reset(reinterpret_cast<const void*>(k_associate), dim3(plan.associate), dim3(kBlock), 0, KID_ASSOCIATE);
@@ -1498,9 +1475,6 @@ int DescribeFrameKernel(FrameKernel which, const LaunchPlan& plan, const DeviceS
   }
   out->Arg(d);
   out->Arg(f);
-  if (which == FK_PROJECT) out->Arg(static_cast<int>(kProjectAll));
-  if (which == FK_PROJECT_MAIN) out->Arg(static_cast<int>(kProjectMain));
-  if (which == FK_PROJECT_TAIL) out->Arg(static_cast<int>(kProjectTail));
   return SM_OK;
 }
 
@@ -1550,65 +1524,6 @@ int IntegrateFrame(cudaStream_t stream, const DeviceState& d, const FrameParams&
   record(11);
   if (status != SM_OK) return status;
   return CheckLaunch("integrate");
-}
-
-// The multi-stream frame pipeline of round 1 (SM_B200_GRAPH=0; the frame graph of pipeline.cu
-// replaces it by default): every hand-over between streams is an event record + wait.
-int IntegrateFramePipelined(cudaStream_t stream, PipelineCtx* pc, int set, DeviceState& d, const FrameParams& f,
-                            bool do_blending, const RegularizeArgs& reg, const LaunchPlan& plan) {
-  cudaStream_t crit = pc->crit, side = pc->side;
-  int status = SM_OK;
-  auto launch = [&](cudaStream_t s, FrameKernel which, bool dependent) {
-    if (status == SM_OK) status = LaunchFrameKernel(s, which, plan, d, f, dependent);
-  };
-  // front: project -> associate -> blend. Needs the surfels as the previous
-  // frame's integration and creation left them.
-  if (pc->have_frame) SM_EV(cudaStreamWaitEvent(stream, pc->ev_create[set ^ 1], 0));
-  launch(stream, FK_PROJECT, false);
-  launch(stream, FK_ASSOCIATE, true);
-  SM_EV(cudaEventRecord(pc->ev_assoc, stream));
-  // side: merge decisions (read the pre-blend depth copy) beside the blending
-  SM_EV(cudaStreamWaitEvent(side, pc->ev_assoc, 0));
-  launch(side, FK_MERGE, false);
-  SM_EV(cudaEventRecord(pc->ev_merge, side));
-  if (do_blending) launch(stream, FK_BLEND, true);
-  SM_EV(cudaEventRecord(pc->ev_blend, stream));
-  // side: new-surfel flags + scan need the blended depth and the final association rasters
-  SM_EV(cudaStreamWaitEvent(side, pc->ev_blend, 0));
-  launch(side, FK_SCAN, false);
-  // crit: the cycle that bounds the frame rate, one stream, back to back:
-  //   [regularisation of the previous frame] -> integrate -> update_neighbors -> regularisation
-  // (the integration rewrites what the previous regularisation reads, and this frame's
-  // regularisation needs the neighbour links and the new surfels).
-  SM_EV(cudaStreamWaitEvent(crit, pc->ev_blend, 0));
-  SM_EV(cudaStreamWaitEvent(crit, pc->ev_merge, 0));
-  launch(crit, FK_INTEGRATE, false);
-  SM_EV(cudaEventRecord(pc->ev_integrate, crit));
-  launch(crit, FK_UPDATE_NEIGHBORS, true);
-  SM_EV(cudaEventRecord(pc->ev_update[set], crit));
-  // side: create the new surfels once the integration is through (kernels.cu order: after the
-  // neighbour update, which does not touch the new slots)
-  SM_EV(cudaStreamWaitEvent(side, pc->ev_integrate, 0));
-  launch(side, FK_CREATE, false);
-  SM_EV(cudaEventRecord(pc->ev_create[set], side));
-  SM_EV(cudaStreamWaitEvent(crit, pc->ev_create[set], 0));
-  if (status != SM_OK) return status;
-  status = CheckLaunch("integrate (pipelined)");
-  if (status != SM_OK) return status;
-  const int old_slot = f.count_slot, new_slot = (f.count_slot + 1) % kCountSlots;
-  NoteIntegratedFrame(d, f.frame_index);
-  if (reg.disable_denoising) {
-    status = RegularizeSurfels(crit, d, true, f.frame_index, reg.radius_factor, reg.regularizer_weight, reg.window,
-                               new_slot, old_slot, plan);
-  } else {
-    for (int i = 0; i < reg.iterations && status == SM_OK; ++i) {
-      status = RegularizeSurfels(crit, d, false, f.frame_index, reg.radius_factor, reg.regularizer_weight, reg.window,
-                                 new_slot, i == 0 ? old_slot : -1, plan);
-    }
-  }
-  SM_EV(cudaEventRecord(pc->ev_reg, crit));
-  pc->have_frame = true;
-  return status;
 }
 
 int ExportVertices(cudaStream_t stream, const DeviceState& d, int count_slot, int sm_count, float* position_buffer,
@@ -1661,13 +1576,6 @@ int ConfigureIntegrateKernels(int carveout_percent, LaunchPlan* plan) {
   plan->merge = resident(k_merge, kBlock, 4);
   plan->integrate = resident(k_integrate, kBlock, 3);
   plan->update_neighbors = resident(k_update_neighbors, kBlock, 3);
-  if (const char* pe = std::getenv("SM_B200_OFFCHAIN_GRID_PERCENT")) {  // see ConfigureRegularizeKernels
-    const int percent = std::atoi(pe);
-    if (percent > 0 && percent < 100) {
-      plan->update_neighbors = std::max(sm_count, plan->update_neighbors * percent / 100);
-      plan->merge = std::max(sm_count, plan->merge * percent / 100);
-    }
-  }
   return SM_OK;
 }
 

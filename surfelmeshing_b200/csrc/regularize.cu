@@ -342,15 +342,6 @@ int ConfigureRegularizeKernels(int carveout_percent, LaunchPlan* plan) {
   plan->reg_accumulate = resident(k_reg_accumulate);
   plan->reg_step = resident(k_reg_step);
   plan->reg_copy = resident(k_reg_copy_only);
-  // SM_B200_OFFCHAIN_GRID_PERCENT (A/B hook): fraction of the resident grid for the sweeps that are not on
-  // the dependency chain that ends a frame step, so that the chain's kernels find free SM resources.
-  if (const char* pe = std::getenv("SM_B200_OFFCHAIN_GRID_PERCENT")) {
-    const int percent = std::atoi(pe);
-    if (percent > 0 && percent < 100) {
-      plan->reg_accumulate = std::max(plan->sm_count, plan->reg_accumulate * percent / 100);
-      plan->reg_step = std::max(plan->sm_count, plan->reg_step * percent / 100);
-    }
-  }
   return SM_OK;
 }
 

@@ -91,10 +91,7 @@ struct sm_reconstruction {
   float* run_radius[smb::kSets] = {}; size_t run_radius_pitch = 0;
   smb::u16* run_depth_pre[smb::kSets] = {};   // pre-blend copy of run_depth (merge runs next to blend)
   float4* reg_records = nullptr;  // [2][stride]: both regularisation record buffers (DeviceState::smooth / smooth_next)
-  // multi-stream pipeline of round 1 (SM_B200_GRAPH=0)
-  smb::PipelineCtx pipe{};
-  cudaStream_t pre_stream = nullptr;
-  cudaEvent_t pre_done[2] = {nullptr, nullptr}, int_done[2] = {nullptr, nullptr}, entry_event = nullptr;
+  cudaEvent_t entry_event = nullptr;   // sm_stream_run / sm_session_begin: the start of the frame loop on the caller's stream
   // host-resident streams: raw-depth / colour rings filled by the upload stream
   std::vector<smb::u16*> ring_depth; size_t ring_depth_pitch = 0;
   std::vector<uchar3*> ring_color; size_t ring_color_pitch = 0;
@@ -111,7 +108,7 @@ struct sm_reconstruction {
   smb::u16* pyramid_depth_stage = nullptr; size_t pyramid_depth_stage_pitch = 0;
   smb::u8* pyramid_color_stage = nullptr; size_t pyramid_color_stage_pitch = 0;
   int pyramid_stage_width = 0, pyramid_stage_height = 0;
-  std::vector<cudaEvent_t> iteration_done;   // frame graph: one event per iteration slot (ring reuse)
+  std::vector<cudaEvent_t> iteration_done;   // frame loop: one event per step slot (ring reuse)
   // delta transfer (transfer.cu): operation counter, per-operation regularisation thresholds, staging
   smb::u32 op_epoch = 0;
   uint64_t state_generation = 1;   // bumped by sm_reset / sm_load_state

@@ -24,8 +24,8 @@ enum KernelId {
   KID_CLEAR = 0, KID_BILATERAL_OUTLIER, KID_BILATERAL_GENERIC, KID_OUTLIER, KID_ERODE_NORMALS_RADII, KID_ERODE,
   KID_NORMALS, KID_RADII, KID_PROJECT, KID_ASSOCIATE, KID_MERGE, KID_BLEND, KID_INTEGRATE, KID_UPDATE_NEIGHBORS,
   KID_NEW_SURFEL_SCAN, KID_CREATE_SURFELS, KID_REG_ACCUMULATE, KID_REG_STEP, KID_REG_COPY_ONLY,
-  KID_EXPORT_VERTICES, KID_MEDIAN_DENSIFY, KID_DELTA_SELECT, KID_VIZ_BUFFERS, KID_PROJECT_TAIL, KID_DOWNSCALE_DEPTH,
-  KID_DOWNSCALE_COLOR, KID_REG_MIRROR, KID_REG_PACK,
+  KID_EXPORT_VERTICES, KID_MEDIAN_DENSIFY, KID_DELTA_SELECT, KID_VIZ_BUFFERS, KID_DOWNSCALE_DEPTH, KID_DOWNSCALE_COLOR,
+  KID_REG_MIRROR, KID_REG_PACK,
   // The kernels below this id have a column in the device timeline (DeviceState::timeline, [frame][column]); the
   // render kernels (render.cu) run outside the frame pipeline and have none.
   KID_TIMELINE_COUNT,
@@ -312,9 +312,8 @@ inline unsigned long long* TimelineSlot(const DeviceState& d, u32 frame, int ker
 }
 
 // SM_B200_PDL: 0 = never, 1 (default) = only launches marked as dependents (LaunchDependent: the
-// kernel follows its producer on the same stream), 2 = every launch. Marking everything slows the
-// multi-stream frame pipeline down (early-launched kernels take SM slots from the kernels of the
-// other streams; measured on a 148-SM GPU, not re-measured on an H100).
+// kernel follows its producer on the same stream), 2 = every launch. Applies to stream launches
+// (sm_preprocess, sm_integrate, the serial mode of sm_stream_run), not to the nodes of the frame graph.
 int PdlMode();
 int ScaleGrid(int blocks);  // SM_B200_GRID_PERCENT measurement hook (integrate.cu)
 
@@ -356,7 +355,7 @@ struct KernelLaunch {
   size_t smem;
   int kernel_id;                 // KernelId
   int arg_count;
-  void* args[4];                 // point into storage
+  void* args[6];                 // point into storage
   alignas(64) unsigned char storage[2304];
   size_t used;
   void Reset(const void* f, dim3 g, dim3 b, size_t shared, int id) {
@@ -400,14 +399,19 @@ int PreprocessFused(cudaStream_t stream, const sm_preprocess_params& p, int widt
                     float* clear_first_depth, u8* clear_supported, u16* out_depth_copy = nullptr,
                     size_t out_depth_copy_pitch = 0, unsigned long long* timeline_bilateral = nullptr,
                     unsigned long long* timeline_tail = nullptr, const TensorMapStorage* scratch_B_map = nullptr);
-// The same two launches as descriptors (frame graph). `skip`: placeholder launches.
-int DescribePreprocess(KernelLaunch* bilateral, KernelLaunch* tail, bool skip, const sm_preprocess_params& p, int width,
-                       int height, float fx, float fy, float cx, float cy, const u16* raw, size_t raw_pitch,
-                       const u16* const* other_depths, const size_t* other_pitches, const float* others_TR_reference,
-                       u16* scratch_B, size_t scratch_B_pitch, u16* out_depth, size_t out_depth_pitch,
-                       float2* out_normals, size_t out_normals_pitch, float* out_radius, size_t out_radius_pitch,
-                       uint4* clear_assoc, float* clear_first_depth, u8* clear_supported, u16* out_depth_copy,
-                       size_t out_depth_copy_pitch, unsigned long long* timeline_bilateral,
+// Bilateral filter radius (cuda_depth_processing.cu:135). Radius 6 has the fused bilateral + outlier kernel.
+inline int BilateralRadius(const sm_preprocess_params& p) {
+  return static_cast<int>(p.bilateral_filter_radius_factor * p.bilateral_filter_sigma_xy + 0.5f);
+}
+// The same launches as descriptors (frame graph): bilateral + outlier fused at radius 6 (`outlier` unused), else
+// k_bilateral_generic and k_outlier in place on scratch_B; then the tail. `skip`: placeholder launches.
+int DescribePreprocess(KernelLaunch* bilateral, KernelLaunch* outlier, KernelLaunch* tail, bool skip,
+                       const sm_preprocess_params& p, int width, int height, float fx, float fy, float cx, float cy,
+                       const u16* raw, size_t raw_pitch, const u16* const* other_depths, const size_t* other_pitches,
+                       const float* others_TR_reference, u16* scratch_B, size_t scratch_B_pitch, u16* out_depth,
+                       size_t out_depth_pitch, float2* out_normals, size_t out_normals_pitch, float* out_radius,
+                       size_t out_radius_pitch, uint4* clear_assoc, float* clear_first_depth, u8* clear_supported,
+                       u16* out_depth_copy, size_t out_depth_copy_pitch, unsigned long long* timeline_bilateral,
                        unsigned long long* timeline_tail, const TensorMapStorage* scratch_B_map);
 int StageBilateral(cudaStream_t stream, float sigma_xy, float sigma_value_factor, u16 value_to_ignore,
                    float radius_factor, u16 max_depth, float depth_valid_region_radius, int width, int height,
@@ -442,38 +446,11 @@ int IntegrateFrame(cudaStream_t stream, const DeviceState& d, const FrameParams&
                    bool rasters_already_cleared, const LaunchPlan& plan, const IntegrateEvents* events);
 // Kernels of one Integrate() as descriptors (stream launches and frame-graph nodes).
 enum FrameKernel { FK_PROJECT = 0, FK_ASSOCIATE, FK_MERGE, FK_BLEND, FK_INTEGRATE, FK_UPDATE_NEIGHBORS, FK_SCAN, FK_CREATE,
-                   FK_PROJECT_MAIN, FK_PROJECT_TAIL, FK_COUNT };
+                   FK_COUNT };
 int DescribeFrameKernel(FrameKernel which, const LaunchPlan& plan, const DeviceState& d, const FrameParams& f,
                         KernelLaunch* out);
 int ClearAssociationRasters(cudaStream_t stream, const DeviceState& d);
 
-// Streams / events of the frame pipeline used by sm_stream_run. The kernels of one frame form a
-// DAG (project -> associate -> {merge | blend} -> integrate -> {update_neighbors | create}, scan
-// after blend, regularisation after update_neighbors + create) and consecutive frames are chained
-// by integrate(f + 1) after regularisation(f) and project(f + 1) after create(f). Three internal
-// streams (the caller's stream only brackets the run):
-//   front                : project, associate, blend of frame f + 1 while frame f regularises
-//   crit  (high priority): integrate, update_neighbors, regularisation - the cycle that bounds the
-//                          frame rate, kept back to back on one stream
-//   side  (high priority): merge, new-surfel scan, create - short kernels that gate the others
-struct PipelineCtx {
-  cudaStream_t front;
-  cudaStream_t crit;
-  cudaStream_t side;
-  cudaEvent_t ev_assoc, ev_merge, ev_blend, ev_integrate;  // transient, re-recorded every frame
-  cudaEvent_t ev_create[2], ev_update[2];                   // per buffer set (frame parity)
-  cudaEvent_t ev_reg;                                       // regularisation of the latest frame
-  bool have_frame;
-};
-struct RegularizeArgs {
-  bool disable_denoising;
-  int iterations;
-  float radius_factor, regularizer_weight;
-  int window;
-};
-// One frame through the DAG, including its regularisation. `set`: frame parity (buffer set).
-int IntegrateFramePipelined(cudaStream_t stream, PipelineCtx* pc, int set, DeviceState& d, const FrameParams& f,
-                            bool do_blending, const RegularizeArgs& reg, const LaunchPlan& plan);
 int ExportVertices(cudaStream_t stream, const DeviceState& d, int count_slot, int sm_count, float* position_buffer,
                    u8* color_buffer);
 

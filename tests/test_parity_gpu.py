@@ -543,7 +543,7 @@ def test_full_size_stream_properties(product, sigma):
                           st.frame_T_global, st.others_TR_reference, pp, ip, first, last)
     assert sh.h2d_bytes > 0
     assert abs(int(sh.surfels_size) - int(sp.surfels_size)) <= 0.002 * sp.surfels_size + 5
-    # sm_stream_run spreads a frame's kernels over several streams (PipelineCtx); with stage timings
+    # sm_stream_run overlaps the kernels of three frames in its frame graph; with stage timings
     # enabled it runs them one after the other on the caller's stream. Same result either way
     # (up to the float-atomic rounding that also separates two runs of the reference).
     rec_s = R.CUDASurfelReconstruction(2_000_000, 640, 480, cam_.fx, cam_.fy, cam_.cx, cam_.cy)
@@ -555,9 +555,9 @@ def test_full_size_stream_properties(product, sigma):
     assert len(rec_s.GetTimings()) == 7
 
 
-def test_device_timeline_of_the_frame_pipeline(product):
-    """sm_timeline_enable: the kernels stamp their own start / end while sm_stream_run pipelines the
-    frames over its streams. The stamps must respect the data dependencies of the frame DAG
+def test_device_timeline_of_the_frame_graph(product):
+    """sm_timeline_enable: the kernels stamp their own start / end while sm_stream_run overlaps three
+    frames in its frame graph. The stamps must respect the data dependencies of the frame DAG
     (DESIGN.md): associate after project, integrate after blend and merge, regularisation after
     the neighbour update and the creation, the next frame's integration after this frame's
     regularisation, the next frame's projection after this frame's creation."""
@@ -603,12 +603,7 @@ def test_device_timeline_of_the_frame_pipeline(product):
         if f + 1 < last:
             assert start(f + 1, "k_integrate") >= end(f, "k_reg_step")
             assert start(f + 1, "k_project") >= end(f, "k_integrate")
-            # the segments that hold frame f's new surfels are projected after its creation kernel: by the
-            # one projection launch, or by the tail launch when the frame graph splits the projection
-            split = buf[f + 1, k["k_project_tail"], 0] != never
-            assert start(f + 1, "k_project_tail" if split else "k_project") >= end(f, "k_create_surfels")
-            if split:
-                assert start(f + 1, "k_associate") >= end(f + 1, "k_project_tail")
+            assert start(f + 1, "k_project") >= end(f, "k_create_surfels")
 
 
 LARGE_FRAME_FIRST_ROWS = (0, 1, 2, 7, 8, 9, 10, 17, 18, 24)

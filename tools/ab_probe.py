@@ -17,8 +17,7 @@ from surfelmeshing_b200 import _lib, synthetic as S  # noqa: E402
 from surfelmeshing_b200 import reconstruction as R  # noqa: E402
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams  # noqa: E402
 
-KNOBS = ("SM_B200_GRAPH", "SM_B200_GRAPH_PDL", "SM_B200_SPLIT_PROJECT", "SM_B200_TAIL_FILL", "SM_B200_PDL",
-         "SM_B200_CARVEOUT", "SM_B200_GRAPH_PRIO", "SM_B200_OFFCHAIN_GRID_PERCENT", "SM_B200_GRID_PERCENT", "SM_B200_TIEBREAK")
+KNOBS = ("SM_B200_TAIL_FILL", "SM_B200_PDL", "SM_B200_CARVEOUT", "SM_B200_GRID_PERCENT", "SM_B200_TIEBREAK")
 
 
 def main():
@@ -29,6 +28,8 @@ def main():
     ap.add_argument("--cap", type=int, default=5_000_000)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--host", action="store_true", help="pinned host frames (e2e path)")
+    ap.add_argument("--sigma-xy", type=float, default=None,
+                    help="bilateral_filter_sigma_xy (default 3: radius 6, the fused kernel; 2 gives radius 4)")
     ap.add_argument("--lib", action="append", default=[], help="name=path of another product build")
     ap.add_argument("--config", action="append", default=[],
                     help="name:KEY=VAL+KEY=VAL[+lib=name]; 'default' is always run first and last")
@@ -59,6 +60,8 @@ def main():
         depth, color = depth.cpu().pin_memory(), color.cpu().pin_memory()
     pp = PreprocessParams.defaults()
     pp.depth_valid_region_radius = cam.valid_region_radius()
+    if args.sigma_xy is not None:
+        pp.bilateral_filter_sigma_xy = args.sigma_xy
     ip = IntegrateParams.defaults()
     f0, f1 = st.integrated_range()
     torch.cuda.synchronize()
