@@ -17,7 +17,8 @@ from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, SurfelError
 from tests.util import (GOLDEN_DIR, INTEGRATE_ROWS, INVALID, NEIGHBOR_ROWS, SMOOTH_ROWS, check_state_invariants,
-                        count_mismatch, digest, golden_camera, golden_params, load_npz_xz, oracle_answers, other_frames)
+                        count_mismatch, digest, golden_camera, golden_params, link_stable_slots, load_npz_xz,
+                        oracle_answers, other_frames, regularization_threshold, smooth_violations)
 
 pytestmark = pytest.mark.gpu
 
@@ -220,19 +221,123 @@ def envelope_limit(env, floor):
     return ENVELOPE_FACTOR * env + 4.0 * float(np.sqrt(max(env, 1))) + floor
 
 
-def race_envelope(state_b, state_a, n_before):
-    """What a SECOND run of the oracle (B) differs from the first (A) in, on the race-bound rows of the
-    slots that existed before the frame: (differing merge flags, |merge count difference|, differing
-    neighbour-link rows). The product is held to a multiple of this (compare_integrate)."""
-    rows_b, _, merges_b = state_b
+# Number of extra oracle runs (B) a live-oracle test measures the reference's envelope with. A single B draw can
+# land low (two runs of the reference happen to agree unusually well on a frame), and a test family with hundreds of
+# envelope checks then fails now and then on an unchanged build; the envelope is the largest of several draws.
+ORACLE_B_RUNS = 3
+
+
+def race_envelope(states_b, state_a, n_before):
+    """What further runs of the oracle (B) differ from the first (A) in, on the race-bound rows of the slots that
+    existed before the frame: (differing merge flags, |merge count difference|, differing neighbour-link rows), each
+    the largest over the B runs. The product is held to a multiple of this (compare_integrate)."""
     rows_a, _, merges_a = state_a
-    flags = int(((rows_b[7, :n_before] < 0) != (rows_a[7, :n_before] < 0)).sum())
     nb = list(NEIGHBOR_ROWS)
-    links = int((rows_b[nb, :n_before].view(np.uint32) != rows_a[nb, :n_before].view(np.uint32)).any(axis=0).sum())
-    return flags, abs(int(merges_b) - int(merges_a)), links
+    out = (0, 0, 0)
+    for rows_b, _, merges_b in states_b:
+        flags = int(((rows_b[7, :n_before] < 0) != (rows_a[7, :n_before] < 0)).sum())
+        links = int((rows_b[nb, :n_before].view(np.uint32) != rows_a[nb, :n_before].view(np.uint32)).any(axis=0).sum())
+        out = tuple(max(a, b) for a, b in zip(out, (flags, abs(int(merges_b) - int(merges_a)), links)))
+    return out
 
 
-def compare_integrate(mine_rasters, mine_depth, mine_state, ref_rasters, ref_depth, ref_state, n_before, envelope=None):
+def smooth_floor(n_before):
+    """Floor of the smooth-position envelope: a neighbour link that differs (link floor of envelope_floors) moves the
+    smooth positions of the up to four slots it touches through their accumulated gradients."""
+    return max(24, n_before // 200)
+
+
+# Measured (H100 80GB HBM3, 700 W, October 2026; three full suite runs, 573 frames with an envelope): the product broke
+# the smooth bound on at most 281 of 48 624 link-stable slots where the B runs broke it on up to 461 of the same set;
+# the largest product count relative to its oracle figure was 253 against 198 (17 100 slots). Golden frames: 0, 8, 22
+# and 27 of 8 206 - 11 130 slots (<= 0.3 %).
+# Without a second oracle run (golden vectors) at most this fraction of the link-stable slots may break the smooth
+# tolerance: the bound of test_smooth_positions_close_to_oracle.
+SMOOTH_GOLDEN_FRACTION = 0.02
+
+
+def compare_smooth(rows_m, rows_r, frame_index, window, iterations, rows_b=(), n_before=0, label=""):
+    """Smooth positions (rows 3-5) after a regularisation that started from the same state in both runs.
+    - outside the window (int(stamp) < int(frame_index - window), stamps and merge flags equal): bit-exact; no
+      sweep moves them, so both still hold the position they started from (the library's partial sweep has to
+      carry these over between its two record buffers);
+    - `iterations` == 0 (copy only, no float atomics): bit-exact for every in-window slot whose position rows,
+      stamp and merge flag agree;
+    - otherwise, on the link-stable slots (util.link_stable_slots): |delta| <= 1e-4 |p| + 1e-5 m per component
+      except for at most envelope_limit(env, smooth_floor) slots, env = the most slots of that set on which a further
+      oracle run (`rows_b`, a list) breaks the same bound against the first, or SMOOTH_GOLDEN_FRACTION of the set
+      without one. The set is taken from the product against oracle A, so env also counts the slots whose links
+      differ between the two oracle runs."""
+    stamps_m, stamps_r = rows_m[18].view(np.int32), rows_r[18].view(np.int32)
+    same = ((rows_m[7] < 0) == (rows_r[7] < 0)) & (stamps_m == stamps_r)
+    outside = stamps_m < regularization_threshold(frame_index, window)
+    smooth_bits = lambda rows: rows[list(SMOOTH_ROWS)].view(np.uint32)
+    differs = np.any(smooth_bits(rows_m) != smooth_bits(rows_r), axis=0)
+    assert int((differs & same & outside).sum()) == 0, f"{label}smooth positions outside the regularisation window"
+    if iterations == 0:
+        same_position = np.all(rows_m[0:3].view(np.uint32) == rows_r[0:3].view(np.uint32), axis=0)
+        assert int((differs & same & ~outside & same_position).sum()) == 0, f"{label}copy-only smooth positions"
+        return
+    stable = link_stable_slots(rows_m, rows_r)
+    got = smooth_violations(rows_m, rows_r, stable)
+    if not len(rows_b):
+        limit = SMOOTH_GOLDEN_FRACTION * int(stable.sum())
+        env = None
+    else:
+        env = max(smooth_violations(rows, rows_r, stable) for rows in rows_b)
+        limit = envelope_limit(env, smooth_floor(n_before))
+    print(f"{label}smooth: {got} of {int(stable.sum())} link-stable slots outside 1e-4 |p| + 1e-5 m "
+          f"(oracle B: {env}, window {int((~outside).sum())}, n = {rows_m.shape[1]})")
+    assert got <= limit, (label, got, env, int(stable.sum()))
+
+
+def link_attribution(walk, mine_rasters, ref_rasters, rows_m, rows_r, n_before):
+    """Where the neighbour links of the product and oracle A may legitimately differ. `walk` = the frame's inputs
+    (rows before the frame, frame index, (fx, fy, cx, cy), frame_T_global, pre-blend depth, normals, IntegrateParams).
+    The CPU walk (oracle/cpu_walk.c) recomputes every pixel's supporter set from the state before the frame; the
+    product's supporting surfel of every contested pixel must be a member of it (a legal race outcome). A slot's links
+    may then differ only if it has an association within 3 pixels of a pixel the two runs resolved differently (the
+    integration can move a surfel by a pixel before its neighbourhood is read, as in test_round2_gpu), or if it or one
+    of its link targets merged differently. Returns (differing link rows outside that set, slots in it)."""
+    if n_before == 0:
+        return 0, 0   # an empty cloud: no slot had links, and no pixel had a supporter
+    from tests.test_round2_gpu import supporter_sets
+    from oracle import cpu_walk
+    from scipy import ndimage
+    fx, fy, cx, cy = walk["camera"]
+    ip = walk["ip"]
+    _, ev_p, ev_k = cpu_walk.associate_events(walk["rows"], walk["frame_index"], fx, fy, cx, cy, walk["frame_T_global"],
+                                              walk["depth"], walk["normals"], ip.sensor_noise_factor,
+                                              ip.normal_compatibility_threshold_deg, ip.depth_scaling)
+    sets = supporter_sets(ev_p, ev_k)
+    cnt = ref_rasters["supporting_surfel_counts"].reshape(-1)
+    sup_m, sup_r = mine_rasters["supporting_surfels"].reshape(-1), ref_rasters["supporting_surfels"].reshape(-1)
+    contested = np.flatnonzero(cnt > 1)
+    checked = outside = 0
+    for p in contested:
+        s = sets.get(int(p))
+        if s is None or len(s) != cnt[p]:
+            continue  # CPU and GPU floats disagree on a borderline gate: not a statement about the winner
+        checked += 1
+        outside += int(sup_m[p] not in s)
+    assert outside == 0 and checked >= 0.9 * len(contested), ("supporting surfel outside the supporter set",
+                                                              checked, len(contested), outside)
+    H, W = ref_rasters["supporting_surfel_counts"].shape
+    resolved = ((cnt > 1) & (sup_m != sup_r)).reshape(H, W)
+    near = ndimage.binary_dilation(resolved, structure=np.ones((3, 3), bool), iterations=3).reshape(-1)
+    attributable = np.zeros(n_before, bool)
+    slots = (ev_k[near[ev_p]] & 0x7FFFFFFF).astype(np.int64)
+    attributable[slots[slots < n_before]] = True
+    nb = list(NEIGHBOR_ROWS)
+    links_m, links_r = rows_m[nb, :n_before].view(np.uint32), rows_r[nb, :n_before].view(np.uint32)
+    bad = np.flatnonzero((rows_m[7, :n_before] < 0) != (rows_r[7, :n_before] < 0))
+    attributable |= np.isin(np.arange(n_before), bad) | np.isin(links_m, bad).any(axis=0) | np.isin(links_r, bad).any(axis=0)
+    differ = (links_m != links_r).any(axis=0)
+    return int((differ & ~attributable).sum()), int(attributable.sum())
+
+
+def compare_integrate(mine_rasters, mine_depth, mine_state, ref_rasters, ref_depth, ref_state, n_before, states_b=(),
+                      ip=None, frame_index=None, walk=None):
     """Contract for one teacher-forced Integrate():
     - min-depth raster, supporting counts, conflicting surfels, new-surfel flags + scan indices,
       surfel count: bit-exact;
@@ -243,11 +348,18 @@ def compare_integrate(mine_rasters, mine_depth, mine_state, ref_rasters, ref_dep
     - depth sums: 1e-6 relative (float atomics);
     - per-surfel attributes written by the integration (position, confidence, radius, normal,
       stamps, colour) bit-exact for every surfel whose merge decision agrees (merging reads the
-      supporting surfel, so it inherits its nondeterminism): with `envelope` (race_envelope of a second
-      oracle run) the differing merge flags, the merge-count difference and the differing neighbour-link
-      rows stay within ENVELOPE_FACTOR x the reference's own run-to-run difference (+ a floor); without
-      one (golden vectors: a single recorded run) within small absolute bounds;
-    - smooth positions within 1e-4 relative where neighbour links agree."""
+      supporting surfel, so it inherits its nondeterminism): with `states_b` (the states of further
+      oracle runs; race_envelope) the differing merge flags and the merge-count difference stay within
+      ENVELOPE_FACTOR x the reference's own run-to-run difference (+ a floor); without them (golden vectors: a
+      single recorded run) within small absolute bounds;
+    - neighbour links: with `walk` (the frame's inputs, link_attribution) every supporting surfel of a contested
+      pixel is one of the pixel's supporters, and a link differs only on slots next to a pixel the two runs resolved
+      differently or touched by a differing merge (up to the tolerance of test_round2_gpu's exact-link check);
+      without it, the differing link rows stay within the envelope (+ a floor fitted at VGA);
+    - smooth positions: compare_smooth with the frame's regularisation window and sweep count (`ip`,
+      `frame_index`): bit-exact outside the window and for copy-only frames, otherwise 1e-4 relative
+      (+ 1e-5 m) on the slots whose own and neighbours' links and merge flags agree, up to the envelope."""
+    envelope = race_envelope(states_b, ref_state, n_before) if len(states_b) else None
     for k in DETERMINISTIC_RASTERS:
         assert count_mismatch(mine_rasters[k], ref_rasters[k]) == 0, k
     depth_diff = np.abs(mine_depth.astype(np.int32) - ref_depth.astype(np.int32))
@@ -273,7 +385,13 @@ def compare_integrate(mine_rasters, mine_depth, mine_state, ref_rasters, ref_dep
         # (two oracle runs can differ on dozens of flags and still count the same number of merges: the count
         #  envelope is the larger of the two figures)
         assert abs(int(merges_m) - int(merges_r)) <= envelope_limit(max(env_count, env_flags), flag_floor), (merges_m, merges_r, env_count, env_flags)
-        assert link_rows_differ <= envelope_limit(env_links, link_floor), (link_rows_differ, env_links)
+        if walk is None:
+            assert link_rows_differ <= envelope_limit(env_links, link_floor), (link_rows_differ, env_links)
+        else:
+            unexplained, attributable = link_attribution(walk, mine_rasters, ref_rasters, rows_m, rows_r, n_before)
+            print(f"links: {unexplained} differing rows away from differently resolved pixels and merges "
+                  f"({attributable} slots near them)")
+            assert unexplained <= 2 * env_links // 10 + 4, (unexplained, env_links)
     else:
         assert (~same_merge).sum() <= max(20, 0.004 * n_r), "merge decisions differ only inside the reference's envelope"
         assert abs(int(merges_m) - int(merges_r)) <= max(20, 0.004 * n_r)
@@ -283,6 +401,10 @@ def compare_integrate(mine_rasters, mine_depth, mine_state, ref_rasters, ref_dep
     for row in INTEGRATE_ROWS:
         assert count_mismatch(rows_m[row], rows_r[row], same_merge) <= allowed, f"row {row}"
     check_state_invariants(rows_m, n_m)
+    assert ip is not None and frame_index is not None, "the smooth-position contract needs the frame's parameters"
+    compare_smooth(rows_m, rows_r, frame_index, ip.regularization_frame_window_size,
+                   ip.regularization_iterations_per_integration_iteration,
+                   rows_b=[state[0] for state in states_b], n_before=n_before, label=f"frame {frame_index}: ")
 
 
 def test_integrate_teacher_forced_against_golden(golden, product):
@@ -305,48 +427,162 @@ def test_integrate_teacher_forced_against_golden(golden, product):
             "supporting_surfels", "supporting_surfel_depth_sums")}
         n_r, merges_r = [int(v) for v in golden[f"f{frame}_counts"]]
         compare_integrate(rec.download_rasters(), d.cpu().numpy(), rec.dump_state(), ref_rasters,
-                          golden[f"f{frame}_blended_depth"], (golden[f"f{frame}_state"], n_r, merges_r), n_prev)
+                          golden[f"f{frame}_blended_depth"], (golden[f"f{frame}_state"], n_r, merges_r), n_prev, ip=ip,
+                          frame_index=frame)
         assert rec.surfels_size() == n_r
 
 
-@pytest.mark.parametrize("variant", ["default", "no_blending", "reg0", "reg2", "window20", "blend_radius5"])
-def test_integrate_teacher_forced_live_oracle(product, reference, variant):
-    """640x480, several frames, product re-synchronised to the oracle's state before every frame."""
-    cam_ = S.Camera.tum(640, 480)
-    st = S.make_stream(cam_, 13, stream_id=11, device="cuda")
-    W, H = 640, 480
+# Cameras of the live-oracle cases: intrinsics in the pixel-corner convention, and the depth scaling of the stream,
+# the pre-processing and the integration.
+LIVE_CAMERAS = {
+    "tum": (S.Camera.tum(640, 480), 5000.0),
+    "tum_fr1": (S.Camera(640, 480, 517.3, 516.5, 319.1, 255.8), 5000.0),    # TUM RGB-D fr1 calibration
+    "icl_nuim": (S.Camera(640, 480, 481.2, -480.0, 320.0, 240.0), 5000.0),  # ICL-NUIM: negative fy
+    "odd": (S.Camera(333, 201, 290.0, 305.0, 171.3, 96.2), 5000.0),        # odd size, fx != fy, off-centre
+    "mm": (S.Camera.tum(320, 240), 1000.0),                                 # depth in millimetres
+}
+
+# case: (camera, IntegrateParams overrides). The first six are the TUM-camera variants; the parameter cases run
+# the odd camera, where every projection also has fx != fy and a width that is not a multiple of 16 (k_blend's
+# scalar loads and stores).
+LIVE_CASES = {
+    "default": ("tum", {}),
+    "no_blending": ("tum", {"do_blending": 0}),
+    "reg0": ("tum", {"regularization_iterations_per_integration_iteration": 0}),
+    "reg2": ("tum", {"regularization_iterations_per_integration_iteration": 2}),
+    "window20": ("tum", {"surfel_integration_active_window_size": 2, "regularization_frame_window_size": 2}),
+    "blend_radius5": ("tum", {"measurement_blending_radius": 5}),
+    "tum_fr1": ("tum_fr1", {}),
+    "icl_nuim": ("icl_nuim", {}),
+    "odd": ("odd", {}),
+    "mm": ("mm", {}),
+    "sensor_noise0.02": ("odd", {"sensor_noise_factor": 0.02}),
+    "max_confidence2": ("odd", {"max_surfel_confidence": 2.0}),
+    "normal_threshold20": ("odd", {"normal_compatibility_threshold_deg": 20.0}),
+    "weight2": ("odd", {"regularizer_weight": 2.0}),
+    "weight40": ("odd", {"regularizer_weight": 40.0}),
+    "radius_factor1.5": ("odd", {"radius_factor_for_regularization_neighbors": 1.5}),
+    "radius_factor3": ("odd", {"radius_factor_for_regularization_neighbors": 3.0}),
+    "blend_radius1": ("odd", {"measurement_blending_radius": 1}),     # <= 2: no iteration of the blending loop
+    "blend_radius2": ("odd", {"measurement_blending_radius": 2}),
+    "blend_radius24": ("odd", {"measurement_blending_radius": 24}),
+    "pitched": ("odd", {}),
+}
+
+
+def live_case(case):
+    """(camera, stream, PreprocessParams, IntegrateParams) of test_integrate_teacher_forced_live_oracle."""
+    cam_name, overrides = LIVE_CASES[case]
+    cam_, scale = LIVE_CAMERAS[cam_name]
+    st = S.make_stream(cam_, 13, stream_id=11, depth_scaling=scale, device="cuda")
     pp = PreprocessParams.defaults()
+    pp.depth_valid_region_radius = cam_.valid_region_radius()
+    pp.depth_scaling = scale
     ip = IntegrateParams.defaults()
-    if variant == "no_blending":
-        ip.do_blending = 0
-    elif variant == "reg0":
-        ip.regularization_iterations_per_integration_iteration = 0
-    elif variant == "reg2":
-        ip.regularization_iterations_per_integration_iteration = 2
-    elif variant == "window20":
-        ip.surfel_integration_active_window_size = 2
-        ip.regularization_frame_window_size = 2
-    elif variant == "blend_radius5":
-        ip.measurement_blending_radius = 5
-    rec_p = R.CUDASurfelReconstruction(600_000, W, H, cam_.fx, cam_.fy, cam_.cx, cam_.cy)
-    rec_r = R.CUDASurfelReconstruction(600_000, W, H, cam_.fx, cam_.fy, cam_.cx, cam_.cy, lib=reference)
-    rec_b = R.CUDASurfelReconstruction(600_000, W, H, cam_.fx, cam_.fy, cam_.cx, cam_.cy, lib=reference)  # envelope
+    ip.depth_scaling = scale
+    for k, v in overrides.items():
+        setattr(ip, k, v)
+    return cam_, st, pp, ip
+
+
+CANARY16 = 0xBEEF
+
+
+def pitched_inputs(d, n, r, c):
+    """Views of copies of the four Integrate() inputs inside wider buffers: the depth view starts 2 bytes into its
+    row (not 16-byte aligned: k_blend's scalar path), the others one or more pixels in. Returns (views, wide depth)."""
+    H, W = d.shape
+    wide_d = torch.full((H, W + 24), CANARY16, dtype=torch.int32, device="cuda").to(torch.uint16)
+    wide_n = torch.full((H, W + 8, 2), float("nan"), device="cuda")
+    wide_r = torch.full((H, W + 16), float("nan"), device="cuda")
+    wide_c = torch.full((H, W + 5, 3), 77, dtype=torch.uint8, device="cuda")
+    views = (wide_d[:, 1:1 + W], wide_n[:, 1:1 + W], wide_r[:, 3:3 + W], wide_c[:, 2:2 + W])
+    for v, src in zip(views, (d, n, r, c)):
+        v.copy_(src)
+    assert views[0].data_ptr() % 16 == 2
+    return views, wide_d
+
+
+def preprocess_outputs(rec, pp, st, frame, H, W):
+    """rec.preprocess of one stream frame into fresh buffers (radius pre-filled with NaN, so that the pixels the call
+    writes can be told apart)."""
+    others = [st.depth[f] for f in other_frames(frame, pp.outlier_filtering_frame_count)]
+    d, n = u16(H, W), torch.zeros((H, W, 2), device="cuda")
+    r = torch.full((H, W), float("nan"), device="cuda")
+    rec.preprocess(None, pp, st.depth[frame], others, st.others_TR_reference[frame], d, n, r)
+    return d, n, r
+
+
+@pytest.mark.parametrize("case", list(LIVE_CASES))
+def test_integrate_teacher_forced_live_oracle(product, reference, case):
+    """Several frames, product re-synchronised to the oracle's state before every frame, on the cameras of real
+    datasets (anisotropic, negative fy, odd size, millimetre depth) and non-default Integrate() parameters. The
+    product's own pre-processing of the same frame is held to the oracle's bit for bit on the way."""
+    cam_, st, pp, ip = live_case(case)
+    W, H = cam_.width, cam_.height
+    make = lambda lib=None: R.CUDASurfelReconstruction(600_000, W, H, cam_.fx, cam_.fy, cam_.cx, cam_.cy, lib=lib)
+    rec_p, rec_r = make(), make(reference)
+    recs_b = [make(reference) for _ in range(ORACLE_B_RUNS)]      # the oracle's own envelope
+    rec_q = make() if case == "pitched" else None                  # packed inputs, against the pitched ones
     first, last = st.integrated_range()
     for frame in range(first, last):
-        others = [st.depth[f] for f in other_frames(frame, 8)]
-        d0, n0, r0 = u16(H, W), torch.zeros((H, W, 2), device="cuda"), torch.zeros((H, W), device="cuda")
-        rec_r.preprocess(None, pp, st.depth[frame], others, st.others_TR_reference[frame], d0, n0, r0)
+        d0, n0, r0 = preprocess_outputs(rec_r, pp, st, frame, H, W)
+        dq, nq, rq = preprocess_outputs(rec_p, pp, st, frame, H, W)
+        torch.cuda.synchronize()
+        assert count_mismatch(dq.cpu().numpy(), d0.cpu().numpy()) == 0, "pre-processed depth"
+        assert count_mismatch(nq.cpu().numpy(), n0.cpu().numpy()) == 0, "normals"
+        written = ~np.isnan(r0.cpu().numpy())
+        assert written.any() and count_mismatch(rq.cpu().numpy(), r0.cpu().numpy(), written) == 0, "radius"
+        r0 = torch.nan_to_num(r0, nan=0.0)
         rows, n_before, merges = rec_r.dump_state()
-        rec_p.load_state(rows, merges)
-        rec_b.load_state(rows, merges)
+        for rec in [rec_p] + recs_b + ([rec_q] if rec_q else []):
+            rec.load_state(rows, merges)
         dp, dr = d0.clone(), d0.clone()
-        for rec, d in ((rec_p, dp), (rec_r, dr), (rec_b, d0.clone())):
+        inputs_p = (dp, n0, r0, st.color[frame])
+        if rec_q is not None:
+            inputs_p, wide_d = pitched_inputs(dp, n0, r0, st.color[frame])
+            dq = d0.clone()
+            rec_q.integrate(None, frame, ip, dq, n0, r0, st.color[frame], st.global_T_frame[frame],
+                            st.frame_T_global[frame])
+        rec_p.integrate(None, frame, ip, *inputs_p, st.global_T_frame[frame], st.frame_T_global[frame])
+        for rec, d in [(rec_r, dr)] + [(rec_b, d0.clone()) for rec_b in recs_b]:
             rec.integrate(None, frame, ip, d, n0, r0, st.color[frame], st.global_T_frame[frame], st.frame_T_global[frame])
         torch.cuda.synchronize()
-        state_r = rec_r.dump_state()
-        compare_integrate(rec_p.download_rasters(), dp.cpu().numpy(), rec_p.dump_state(), rec_r.download_rasters(),
-                          dr.cpu().numpy(), state_r, n_before, envelope=race_envelope(rec_b.dump_state(), state_r, n_before))
-        assert rec_p.surfel_count() == rec_p.surfels_size() - rec_p.dump_state()[2]
+        if rec_q is not None:
+            wide = wide_d.cpu().numpy()
+            assert (wide[:, 0] == CANARY16).all() and (wide[:, W + 1:] == CANARY16).all(), "padding written"
+            dp = inputs_p[0]
+            compare_product_runs(rec_p, dp.cpu().numpy(), rec_q, dq.cpu().numpy())
+        state_p, state_r = rec_p.dump_state(), rec_r.dump_state()
+        compare_integrate(rec_p.download_rasters(), dp.cpu().numpy(), state_p, rec_r.download_rasters(),
+                          dr.cpu().numpy(), state_r, n_before, states_b=[rec.dump_state() for rec in recs_b], ip=ip,
+                          frame_index=frame, walk=frame_walk(rows, frame, cam_, st, d0, n0, ip))
+        assert rec_p.surfel_count() == rec_p.surfels_size() - state_p[2]
+    if case == "max_confidence2":
+        assert state_p[0][6].max() == 2.0, "the confidence clamp was reached"
+
+
+def frame_walk(rows, frame_index, cam_, st, depth, normals, ip, stream_frame=None):
+    """The inputs link_attribution recomputes a frame's supporter sets from (`depth`, `normals`: pre-blend tensors)."""
+    f = frame_index if stream_frame is None else stream_frame
+    return {"rows": rows, "frame_index": frame_index, "camera": (cam_.fx, cam_.fy, cam_.cx, cam_.cy),
+            "frame_T_global": st.frame_T_global[f], "depth": depth.cpu().numpy(), "normals": normals.cpu().numpy(),
+            "ip": ip}
+
+
+def compare_product_runs(rec_a, depth_a, rec_b, depth_b):
+    """Two product runs of one Integrate() on the same state and inputs. Everything but the float-atomic depth sums
+    is deterministic in the product: rasters bit-equal, blended depth and the integrated rows bit-equal up to the
+    pixels whose depth sum rounds differently (as compare_integrate)."""
+    ras_a, ras_b = rec_a.download_rasters(), rec_b.download_rasters()
+    for k in DETERMINISTIC_RASTERS + ("supporting_surfels",):
+        assert count_mismatch(ras_a[k], ras_b[k]) == 0, k
+    depth_diff = np.abs(depth_a.astype(np.int32) - depth_b.astype(np.int32))
+    assert (depth_diff != 0).sum() <= 5 and depth_diff.max() <= 1, "blended depth"
+    (rows_a, n_a, m_a), (rows_b, n_b, m_b) = rec_a.dump_state(), rec_b.dump_state()
+    assert (n_a, m_a) == (n_b, m_b)
+    for row in INTEGRATE_ROWS + NEIGHBOR_ROWS:
+        assert count_mismatch(rows_a[row], rows_b[row]) <= 4 * int((depth_diff != 0).sum()), f"row {row}"
 
 
 def test_smooth_positions_close_to_oracle(golden, product):

@@ -22,6 +22,9 @@ IDENTITY = np.eye(4, dtype=np.float32)[:3]
 # an output camera unlike the handle's: non-square, odd sizes, fx != fy, off-centre principal point
 ODD = dict(width=333, height=197, fx=300.0, fy=310.0, cx=170.3, cy=95.6)
 VGA = dict(width=CAM.width, height=CAM.height, fx=CAM.fx, fy=CAM.fy, cx=CAM.cx, cy=CAM.cy)
+# an ICL-NUIM-like output camera: negative fy (the image is flipped vertically; axis_range swaps the bounds for f < 0)
+FLIPPED = dict(width=CAM.width, height=CAM.height, fx=481.2, fy=-480.0, cx=320.0, cy=240.0)
+OUTPUT_CAMERAS = {"vga": VGA, "odd": ODD, "negative_fy": FLIPPED}
 
 
 def make(lib=None):
@@ -83,9 +86,9 @@ HAND_BUILT = {
 
 
 @pytest.mark.parametrize("case", sorted(HAND_BUILT))
-@pytest.mark.parametrize("cam", ["vga", "odd"])
+@pytest.mark.parametrize("cam", ["vga", "odd", "negative_fy"])
 def test_hand_built_clouds_bit_exact(case, cam):
-    cam = VGA if cam == "vga" else ODD
+    cam = OUTPUT_CAMERAS[cam]
     rows = make_rows(HAND_BUILT[case])
     rec = make()
     rec.load_state(rows, 0)
@@ -115,11 +118,11 @@ def integrated():
 
 
 @pytest.mark.parametrize("pose", ["input", "orbit", "behind"])
-@pytest.mark.parametrize("cam", ["vga", "odd"])
+@pytest.mark.parametrize("cam", ["vga", "odd", "negative_fy"])
 def test_integrated_cloud_bit_exact(integrated, pose, cam):
     st, rec, rows, n = integrated
     T = {"input": st.frame_T_global[30], "orbit": orbit_pose(st, 30, 35.0, 0.4), "behind": BEHIND}[pose]
-    cam = VGA if cam == "vga" else ODD
+    cam = OUTPUT_CAMERAS[cam]
     out = rec.render(T, near=NEAR, far=FAR, **cam)
     torch.cuda.synchronize()
     ref = walk(rows, T, **cam)

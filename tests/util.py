@@ -89,6 +89,35 @@ def other_frames(frame, K):
     return [frame - (i + 1) for i in range(half)] + [frame + (i + 1) for i in range(half)]
 
 
+def smooth_violations(rows_m, rows_r, slots):
+    """Slots of the bool mask `slots` whose smooth position (rows 3-5) breaks |delta| <= 1e-4 |p| + 1e-5 m in some
+    component: the bound of the golden smooth-position test (float atomics make the reference differ from itself at
+    a few ulp of the accumulated gradient, far below it)."""
+    sm, sr = rows_m[list(SMOOTH_ROWS)], rows_r[list(SMOOTH_ROWS)]
+    close = np.all(np.isclose(sm, sr, rtol=1e-4, atol=1e-5), axis=0)
+    return int((~close & slots).sum())
+
+
+def link_stable_slots(rows_m, rows_r):
+    """Slots whose merge flag and four neighbour links agree between the two states, and for which the same holds
+    for every slot they link to: the regularisation reads exactly these, so their smooth positions are comparable."""
+    own = (rows_m[7] < 0) == (rows_r[7] < 0)
+    links_m = rows_m[list(NEIGHBOR_ROWS)].view(np.uint32)
+    own &= np.all(links_m == rows_r[list(NEIGHBOR_ROWS)].view(np.uint32), axis=0)
+    stable = own.copy()
+    for links in links_m:
+        linked = links != INVALID
+        stable &= ~linked | own[np.where(linked, links, 0)]
+    return stable
+
+
+def regularization_threshold(frame_index, window):
+    """int(frame_index - window) with the subtraction in u32, as the regularisation sweeps evaluate it: slots with
+    int(last update stamp) below it are outside the window."""
+    t = (int(frame_index) - int(window)) & 0xFFFFFFFF
+    return t - (1 << 32) if t >= 1 << 31 else t
+
+
 def check_state_invariants(rows, n):
     """Size-independent properties of a surfel SoA (rows [25, n])."""
     r2 = rows[7]
