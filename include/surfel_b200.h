@@ -349,6 +349,102 @@ int sm_render_surfels(sm_reconstruction* r, void* stream, const sm_render_params
                       float* normal, size_t normal_pitch,
                       uint32_t* index, size_t index_pitch);
 
+/* ---- camera tracking against the cloud (DESIGN.md section 1 row f8, section 5.6) ----------------------------
+ * The reference reads every camera pose from a trajectory file (APP/main.cc:601-625) and has no tracker.
+ * sm_track_frame estimates the pose of a depth map by projective point-to-plane ICP against a model view,
+ * coarse to fine, with every Gauss-Newton iteration on the device. It only reads the surfel state.
+ *
+ * sm_track_frame, in order, on `stream`:
+ *  1. Live images. Level 0 is the raw depth (u16, the handle's camera size) through the bilateral filter and depth
+ *     cutoff of sm_bilateral_filter_and_depth_cutoff with pp's bilateral_filter_*, depth_scaling * max_depth and
+ *     depth_valid_region_radius (the first pre-processing stage of the stream loop). Level l = 1..levels-1 is level
+ *     0 downscaled as sm_downscale_using_median_while_excluding(0, ...) does, to the size of Camera.scaled(l):
+ *     int(W / 2^l + 0.5) x int(H / 2^l + 0.5), intrinsics fx / 2^l, fy / 2^l, cx / 2^l, cy / 2^l (pixel corner).
+ *  2. Model view at the handle's camera. SM_TRACK_CLOUD: sm_render_surfels from view_T_global = the fp64 inverse
+ *     of global_T_guess rounded to fp32, depth range [0.1, 100] m, depth and normal only; the model pose is the
+ *     guess. SM_TRACK_PREVIOUS_FRAME: the level-0 view (step 3) of this handle's previous sm_track_frame call;
+ *     the model pose is the pose that call returned. Every level associates into this one full-size view.
+ *     The starting model_T_live is inverse(model pose) * global_T_guess (fp64, rounded to fp32). Before that, the
+ *     3x3 parts of the guess and of the model pose are replaced by their nearest rotations (polar decomposition in
+ *     fp64), and so is the returned pose: fp32 poses are a few ulp off SO(3), and a chain of calls that feeds each
+ *     returned pose into the next guess would otherwise carry that scale and shear forward and amplify it.
+ *  3. The level-0 view of this frame is kept for the next call: per pixel z and n of rule L below (0 where L
+ *     rejects the pixel).
+ *  4. For level = levels-1 down to 0, iterations[level] times: linearise (rules L and M below), then solve.
+ *  5. One synchronisation; then global_T_out = model pose * model_T_live (fp64, rounded to fp32), or
+ *     global_T_guess if the frame is lost. Synchronous, like sm_knn_batch_host; every SM_OK call keeps its view
+ *     and its returned pose as the "previous frame".
+ *
+ * Per live pixel (x, y) of a level of size w x h and intrinsics fx, fy, cx, cy, in fp32 with every product, sum
+ * and quotient rounded on its own (no fma), IEEE division and square root; a.b = (a.x*b.x + a.y*b.y) + a.z*b.z:
+ *  L1. The pixel is skipped at the border (x = 0, y = 0, x = w-1, y = h-1) and if any of the depths at (x, y),
+ *      (x+-1, y), (x, y+-1) is 0. Otherwise valid_pixels counts it.
+ *  L2. P(u, v) = z * (((u + 0.5) - cx) / fx, ((v + 0.5) - cy) / fy, 1) with z = depth * (1 / depth_scaling)
+ *      (the reciprocal rounded once); p = P(x, y). a = P(x+1, y) - P(x-1, y), b = P(x, y+1) - P(x, y-1);
+ *      n = b x a (per component (b.y*a.z) - (b.z*a.y) etc.: faces the camera), then n = n * (1 / sqrt(n.n));
+ *      the pixel is skipped (and not counted) unless n.n is finite and > 0.
+ *  M1. With T = model_T_live (device memory, rows r): p' = ((r.x*p.x + r.y*p.y) + r.z*p.z) + r.w per row, n' the
+ *      same without r.w. The pixel is an outlier unless p'.z > 0.
+ *  M2. u = fmx * (p'.x / p'.z) + mcx, v likewise (the model camera = the handle's camera); outlier unless
+ *      0 <= u < W and 0 <= v < H; (ix, iy) = (int(u), int(v)).
+ *  M3. d = model depth at (ix, iy): outlier unless finite and > 0. m = model normal at (ix, iy) normalised as in
+ *      L2 (outlier if that fails); q = d * (((ix + 0.5) - mcx) / mfx, ((iy + 0.5) - mcy) / mfy, 1); m = -m if
+ *      m.q > 0 (the renderer draws both faces of a disk).
+ *  M4. e = p' - q. Inlier iff e.e <= max_point_distance^2 (fp32) and n'.m >= cos(max_normal_angle_deg)
+ *      (evaluated in double, rounded to fp32).
+ *  M5. r = m.e, J = (p' x m, m) (cross product as in L2) for the increment xi = (omega, v) applied as
+ *      T <- exp(xi) T in the model camera frame. The 21 products J_i J_j (i <= j, row by row), the 6 J_i r,
+ *      r^2 and the inlier and valid counts are formed and summed in fp64 (fixed per-thread, warp-shuffle and
+ *      block orders, one partial row per block, no atomics: a call reproduces bit for bit).
+ * Solve (one block, fp64): the partial rows are summed in block order. The frame is lost if inliers <
+ * min_inlier_fraction * valid_pixels, a Cholesky pivot of J^T J is <= 0 or the step is not finite; otherwise
+ * xi = -(J^T J)^-1 J^T r, T <- exp(xi) T (Rodrigues, the SE(3) left Jacobian for the translation), rounded to fp32.
+ * |omega| < convergence_rotation and |v| < convergence_translation end the level; the remaining iterations of a
+ * level that converged, and all after a loss, return at once (the launch count does not depend on the data).
+ * result: tracked (0 = lost, global_T_out = global_T_guess), iterations = steps applied, inliers / valid_pixels /
+ * rms_residual = sqrt(sum r^2 / inliers) of the last level-0 linearisation. A lost frame still returns SM_OK.
+ *
+ * sm_track_linearize runs one linearisation (rules L and M) on caller images, synchronously: live_depth is the
+ * filtered u16 image of Camera.scaled(level) of the handle's camera; model_depth (f32) and model_normal (f32x3)
+ * are at the handle's camera size. out_system = the 21 J^T J sums then the 6 J^T r sums; out_inliers = inliers.
+ *
+ * Scratch (the live pyramid, the model view, two level-0 views, one partial row per resident block of the
+ * linearisation, the state) is allocated by the first call; sm_create allocates nothing for tracking.
+ * SM_ERR_INVALID_ARGUMENT, with no launch, for NULL pointers, a pitch below the row size, levels outside [1, 4],
+ * a negative iterations entry, a non-finite pose, a guess whose 3x3 part has a determinant <= 0, a non-finite threshold (max_point_distance <= 0, max_normal_angle_deg
+ * outside [0, 180], min_inlier_fraction outside [0, 1], a negative convergence threshold, depth_scaling <= 0),
+ * SM_TRACK_PREVIOUS_FRAME without an earlier sm_track_frame call on the handle, or a level whose image is smaller
+ * than 3 x 3 pixels. */
+#define SM_TRACK_CLOUD 0
+#define SM_TRACK_PREVIOUS_FRAME 1
+typedef struct sm_track_params {
+  int32_t levels;                  /* live-depth pyramid levels, 1..4 (3) */
+  int32_t iterations[4];           /* Gauss-Newton iterations per level, finest first ({4, 5, 10, 0}) */
+  float max_point_distance;        /* metres, correspondence gate (0.05) */
+  float max_normal_angle_deg;      /* live vs model normal gate (20) */
+  float min_inlier_fraction;       /* of the level's valid live pixels; below it the frame is lost (0.1) */
+  float convergence_rotation;      /* rad (1e-5) */
+  float convergence_translation;   /* metres (1e-5) */
+  int32_t model_source;            /* SM_TRACK_CLOUD or SM_TRACK_PREVIOUS_FRAME (SM_TRACK_CLOUD) */
+} sm_track_params;
+typedef struct sm_track_result {
+  int32_t tracked;                 /* 0 = lost: global_T_out = global_T_guess */
+  int32_t iterations;              /* Gauss-Newton steps applied, all levels */
+  uint32_t inliers, valid_pixels;  /* level 0, last linearisation */
+  float rms_residual;              /* metres, level 0, last linearisation */
+} sm_track_result;
+/* Host only, no device needed. */
+void sm_default_track_params(sm_track_params* p);
+int sm_track_frame(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_preprocess_params* pp,
+                   const uint16_t* depth, size_t depth_pitch,   /* raw u16, device, the handle's camera size */
+                   const float global_T_guess[12], float global_T_out[12], sm_track_result* result);
+int sm_track_linearize(sm_reconstruction* r, void* stream, const sm_track_params* tp, int32_t level,
+                       float depth_scaling,
+                       const uint16_t* live_depth, size_t live_pitch,   /* filtered level image, device */
+                       const float* model_depth, size_t model_depth_pitch,
+                       const float* model_normal, size_t model_normal_pitch,
+                       const float model_T_live[12], double out_system[27], uint32_t* out_inliers);
+
 /* ---- radius-limited k-nearest-neighbour queries for the meshing thread (SURVEY section 8 f4) ----
  * Replaces CompressedOctree::FindNearestSurfelsWithinRadius<include_completed_surfels, include_free_surfels>
  * (octree.h:471, octree.cc:313-470; callers surfel_meshing.cc:421 <false, true> and :821 <true, false>) for a BATCH of
@@ -496,7 +592,8 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * Between pushes, calls on `stream` see the state after status.last_integrated_frame, and the next push's
  * work waits for them: the hand-off calls (sm_transfer_all_to_cpu, sm_transfer_delta_to_cpu,
  * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
- * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_surfel_count / sm_surfels_size) and
+ * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_track_frame, sm_track_linearize,
+ * sm_surfel_count / sm_surfels_size) and
  * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
  * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which
  * that frame's Integrate() applies in the next step. The device merge counter then already includes them, so

@@ -123,6 +123,29 @@ class RenderParams(C.Structure):
                 ("cx", C.c_float), ("cy", C.c_float), ("near_depth", C.c_float), ("far_depth", C.c_float)]
 
 
+TRACK_CLOUD = 0
+TRACK_PREVIOUS_FRAME = 1
+
+
+class TrackParams(C.Structure):
+    """sm_track_params: pyramid levels, Gauss-Newton iterations per level (finest first), correspondence gates,
+    the lost-frame threshold, convergence thresholds and the model source."""
+    _fields_ = [("levels", C.c_int32), ("iterations", C.c_int32 * 4), ("max_point_distance", C.c_float),
+                ("max_normal_angle_deg", C.c_float), ("min_inlier_fraction", C.c_float),
+                ("convergence_rotation", C.c_float), ("convergence_translation", C.c_float),
+                ("model_source", C.c_int32)]
+
+    @classmethod
+    def defaults(cls) -> "TrackParams":
+        return cls(3, (C.c_int32 * 4)(4, 5, 10, 0), 0.05, 20.0, 0.1, 1e-5, 1e-5, TRACK_CLOUD)
+
+
+class TrackResult(C.Structure):
+    """sm_track_result: tracked (0 = lost), steps applied, and the level-0 inliers, valid pixels and RMS residual."""
+    _fields_ = [("tracked", C.c_int32), ("iterations", C.c_int32), ("inliers", C.c_uint32),
+                ("valid_pixels", C.c_uint32), ("rms_residual", C.c_float)]
+
+
 _P = C.c_void_p
 _SZ = C.c_size_t
 _F = C.c_float
@@ -190,6 +213,11 @@ _PRODUCT_ONLY = {
     "session_push": (C.c_int, [_P, _P, _SZ, _P, _SZ, _I, _P, _P, C.POINTER(SessionStatus)]),
     "session_end": (C.c_int, [_P, C.POINTER(StreamStats)]),
     "render_surfels": (C.c_int, [_P, _P, C.POINTER(RenderParams), _P, _P, _SZ, _P, _SZ, _P, _SZ, _P, _SZ]),
+    "default_track_params": (None, [C.POINTER(TrackParams)]),
+    "track_frame": (C.c_int, [_P, _P, C.POINTER(TrackParams), C.POINTER(PreprocessParams), _P, _SZ, _P, _P,
+                              C.POINTER(TrackResult)]),
+    "track_linearize": (C.c_int, [_P, _P, C.POINTER(TrackParams), _I, _F, _P, _SZ, _P, _SZ, _P, _SZ, _P, _P,
+                                  C.POINTER(_U32)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

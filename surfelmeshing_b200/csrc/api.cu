@@ -154,7 +154,8 @@ const char* KernelName(int id) {
       "k_normals", "k_radii", "k_project", "k_associate", "k_merge", "k_blend", "k_integrate", "k_update_neighbors",
       "k_new_surfel_scan", "k_create_surfels", "k_reg_accumulate", "k_reg_step", "k_reg_copy_only",
       "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_downscale_depth_median",
-      "k_downscale_color", "k_reg_mirror", "k_reg_pack", "k_render_splat", "k_render_large", "k_render_resolve"};
+      "k_downscale_color", "k_reg_mirror", "k_reg_pack", "k_render_splat", "k_render_large", "k_render_resolve",
+      "k_track_live_view", "k_track_linearize", "k_track_solve"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -519,6 +520,7 @@ int sm_destroy(sm_reconstruction* r) {
   cudaFree(r->pyramid_depth_stage); cudaFree(r->pyramid_color_stage);
   FreeTransferBuffers(r);
   FreeRenderBuffers(r);
+  FreeTrackBuffers(r);
   for (cudaStream_t st : {r->upload_stream, r->graph_stream})
     if (st) cudaStreamDestroy(st);
   for (cudaEvent_t e : {r->entry_event, r->upload_done, r->graph_exit})
@@ -700,6 +702,37 @@ int sm_render_surfels(sm_reconstruction* r, void* stream, const sm_render_params
   if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_surfels: null argument");
   return RenderSurfels(r, static_cast<cudaStream_t>(stream), *p, view_T_global, depth, depth_pitch, color, color_pitch,
                        normal, normal_pitch, index, index_pitch);
+}
+
+void sm_default_track_params(sm_track_params* p) {
+  p->levels = 3;
+  p->iterations[0] = 4; p->iterations[1] = 5; p->iterations[2] = 10; p->iterations[3] = 0;
+  p->max_point_distance = 0.05f;
+  p->max_normal_angle_deg = 20.0f;
+  p->min_inlier_fraction = 0.1f;
+  p->convergence_rotation = 1e-5f;
+  p->convergence_translation = 1e-5f;
+  p->model_source = SM_TRACK_CLOUD;
+}
+
+int sm_track_frame(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_preprocess_params* pp,
+                   const uint16_t* depth, size_t depth_pitch, const float global_T_guess[12], float global_T_out[12],
+                   sm_track_result* result) {
+  if (!r || !tp || !pp || !depth || !global_T_guess || !global_T_out || !result)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_frame: null argument");
+  return TrackFrame(r, static_cast<cudaStream_t>(stream), *tp, *pp, depth, depth_pitch, global_T_guess, global_T_out,
+                    result);
+}
+
+int sm_track_linearize(sm_reconstruction* r, void* stream, const sm_track_params* tp, int32_t level,
+                       float depth_scaling, const uint16_t* live_depth, size_t live_pitch, const float* model_depth,
+                       size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
+                       const float model_T_live[12], double out_system[27], uint32_t* out_inliers) {
+  if (!r || !tp || !live_depth || !model_depth || !model_normal || !model_T_live || !out_system || !out_inliers)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_linearize: null argument");
+  return TrackLinearize(r, static_cast<cudaStream_t>(stream), *tp, level, depth_scaling, live_depth, live_pitch,
+                        model_depth, model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system,
+                        out_inliers);
 }
 
 int sm_export_vertices(sm_reconstruction* r, void* stream, float* position_buffer, uint8_t* color_buffer) {

@@ -48,6 +48,7 @@ struct FrameGraph;  // pipeline.cu
 void DestroyFrameGraph(FrameGraph* g);
 struct StreamSession;  // pipeline.cu: an open sm_session_begin
 void DestroySession(StreamSession* s);
+struct TrackState;     // track.cu
 
 }  // namespace smb
 
@@ -132,6 +133,22 @@ struct sm_reconstruction {
   smb::u32* render_large_list = nullptr;
   smb::u32* render_large_count = nullptr;
   int render_splat_blocks = 0, render_large_blocks = 0;
+  // sm_track_frame / sm_track_linearize scratch (track.cu), allocated by the first call: the filtered live pyramid,
+  // the rendered model view, two level-0 views of tracked frames (depth, normals) of which track_previous is the
+  // newest, the pose that call returned, the per-block partial rows and the device / pinned tracker state (allocated
+  // last: non-null means every buffer exists).
+  smb::u16* track_level[4] = {}; size_t track_level_pitch[4] = {};
+  float* track_model_depth = nullptr; size_t track_model_depth_pitch = 0;
+  float* track_model_normal = nullptr; size_t track_model_normal_pitch = 0;
+  float* track_view_depth[2] = {}; size_t track_view_depth_pitch[2] = {};
+  float* track_view_normal[2] = {}; size_t track_view_normal_pitch[2] = {};
+  int track_previous = 0;
+  bool track_has_previous = false;
+  float track_previous_pose[12] = {};
+  double* track_partials = nullptr;
+  int track_blocks = 0;
+  smb::TrackState* track_state = nullptr;
+  smb::TrackState* track_host_state = nullptr;
 };
 
 namespace smb {
@@ -161,6 +178,14 @@ int RenderSurfels(sm_reconstruction* r, cudaStream_t stream, const sm_render_par
                   float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch, float* normal,
                   size_t normal_pitch, uint32_t* index, size_t index_pitch);
 void FreeRenderBuffers(sm_reconstruction* r);
+// track.cu
+int TrackFrame(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const sm_preprocess_params& pp,
+               const u16* depth, size_t depth_pitch, const float* guess, float* pose_out, sm_track_result* result);
+int TrackLinearize(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, int level, float depth_scaling,
+                   const u16* live, size_t live_pitch, const float* model_depth, size_t model_depth_pitch,
+                   const float* model_normal, size_t model_normal_pitch, const float* model_T_live, double* out_system,
+                   uint32_t* out_inliers);
+void FreeTrackBuffers(sm_reconstruction* r);
 // pipeline.cu
 int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
               const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats);

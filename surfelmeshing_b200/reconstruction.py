@@ -20,7 +20,7 @@ import torch
 
 from . import _lib
 from ._lib import (IntegrateParams, Library, PreprocessParams, RenderParams, SessionStatus, StreamDesc, StreamStats,
-                   TransferStats, TransferToken, VisualizationParams)
+                   TrackParams, TrackResult, TransferStats, TransferToken, VisualizationParams)
 
 RENDER_OUTPUTS = ("depth", "color", "normal", "index")
 
@@ -354,6 +354,56 @@ class CUDASurfelReconstruction:
                       *args)
         return out
 
+    def track(self, depth, guess, params: Optional[TrackParams] = None, pp: Optional[PreprocessParams] = None,
+              source: str = "cloud", stream=None):
+        """sm_track_frame: the camera-to-world pose of a raw depth map ([H, W] uint16 CUDA tensor at the handle's
+        camera size) by point-to-plane ICP, starting from `guess` (3x4 camera-to-world). source="cloud" tracks
+        against the cloud rendered from the guess, source="previous" against the previous track() call's frame.
+        Synchronous. Returns (pose [3, 4] float32, TrackResult); a lost frame returns the guess with tracked = 0."""
+        if source not in ("cloud", "previous"):
+            raise ValueError(f"source must be 'cloud' or 'previous', got {source!r}")
+        tp = TrackParams.defaults() if params is None else TrackParams.from_buffer_copy(params)
+        tp.model_source = _lib.TRACK_CLOUD if source == "cloud" else _lib.TRACK_PREVIOUS_FRAME
+        pp = pp if pp is not None else PreprocessParams.defaults()
+        dp, dpitch = _raster(depth)
+        if tuple(depth.shape) != (self.height, self.width) or depth.dtype != torch.uint16:
+            raise ValueError(f"depth must be uint16 [{self.height}, {self.width}]")
+        g = _mat12(guess)
+        out = np.zeros(12, np.float32)
+        result = TrackResult()
+        self.lib.call("track_frame", self._h, _stream_handle(stream), C.byref(tp), C.byref(pp), dp, dpitch,
+                      g.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p), C.byref(result))
+        return out.reshape(3, 4), result
+
+    def track_linearize(self, level: int, live_depth, model_depth, model_normal, model_T_live,
+                        params: Optional[TrackParams] = None, depth_scaling: float = 5000.0, stream=None):
+        """sm_track_linearize: one point-to-plane linearisation of a filtered live level image against caller model
+        images (depth [H, W] float32, normal [H, W, 3] float32 at the handle's camera). Synchronous. Returns
+        (system float64 [27]: the 21 upper-triangle J^T J sums then the 6 J^T r sums, inlier count)."""
+        tp = TrackParams.defaults() if params is None else params
+        level = int(level)
+        if not 0 <= level <= 3:
+            raise ValueError(f"level must be in [0, 3], got {level}")
+        factor = float(np.float32(1.0) / np.float32(2.0 ** level))   # Camera.scaled(level) sizes
+        live_shape = (int(factor * self.height + 0.5), int(factor * self.width + 0.5))
+        H, W = self.height, self.width
+        for name, t, shape, dtype in (("live_depth", live_depth, live_shape, torch.uint16),
+                                      ("model_depth", model_depth, (H, W), torch.float32),
+                                      ("model_normal", model_normal, (H, W, 3), torch.float32)):
+            if not isinstance(t, torch.Tensor) or tuple(t.shape) != shape or t.dtype != dtype:
+                got = (tuple(t.shape), t.dtype) if isinstance(t, torch.Tensor) else type(t).__name__
+                raise ValueError(f"{name} must be a {dtype} tensor of shape {shape}, got {got}")
+        lp, lpitch = _raster(live_depth)
+        mp, mpitch = _raster(model_depth)
+        np_, npitch = _raster(model_normal, 3)
+        T = _mat12(model_T_live)
+        system = np.zeros(27, np.float64)
+        inliers = C.c_uint32()
+        self.lib.call("track_linearize", self._h, _stream_handle(stream), C.byref(tp), int(level), float(depth_scaling),
+                      lp, lpitch, mp, mpitch, np_, npitch, T.ctypes.data_as(C.c_void_p),
+                      system.ctypes.data_as(C.c_void_p), C.byref(inliers))
+        return system, int(inliers.value)
+
     def ExportVertices(self, stream, position_buffer: torch.Tensor, color_buffer: torch.Tensor):
         """cuda_surfel_reconstruction.cc:405-410."""
         self.lib.call("export_vertices", self._h, _stream_handle(stream), C.c_void_p(position_buffer.data_ptr()),
@@ -542,6 +592,68 @@ class StreamSession:
             self.open = False
             self.rec.lib.fn["session_end"](self.rec._h, None)
         return False
+
+
+def _to4(m) -> np.ndarray:
+    return np.concatenate([np.asarray(m, np.float64).reshape(3, 4), [[0.0, 0.0, 0.0, 1.0]]], axis=0)
+
+
+class TrackedSession:
+    """A pose-free stream: every frame is tracked (sm_track_frame) and then pushed into a StreamSession with the pose
+    it tracked. Only the first frame's camera-to-world pose is given. Frames are at the handle's camera size.
+
+    Each frame after the first starts from a constant-velocity guess, T_{k-1} (T_{k-2}^-1 T_{k-1}). It is tracked
+    against the previous frame until the session has integrated a frame, and against the cloud after that. A lost
+    frame keeps its guess. `trajectory` holds the [3, 4] float32 poses pushed, `results` the TrackResults::
+
+        with TrackedSession(rec, pp, ip, first_pose) as s:
+            for depth, color in frames:
+                s.push(depth, color)
+        s.trajectory
+    """
+
+    def __init__(self, rec: CUDASurfelReconstruction, pp: PreprocessParams, ip: IntegrateParams, first_pose,
+                 params: Optional[TrackParams] = None, first_frame_index: int = 0, stream=None):
+        self.rec, self.pp = rec, pp
+        self.params = TrackParams.defaults() if params is None else params
+        self.first_pose = np.asarray(first_pose, np.float32).reshape(3, 4)
+        self.session = StreamSession(rec, pp, ip, (rec.width, rec.height), first_frame_index, stream)
+        self.trajectory: list = []
+        self.results: list = []
+        self.integrated = False
+
+    def guess(self) -> np.ndarray:
+        if len(self.trajectory) < 2:
+            return self.trajectory[-1]
+        a, b = _to4(self.trajectory[-2]), _to4(self.trajectory[-1])
+        return (b @ np.linalg.inv(a) @ b)[:3].astype(np.float32)
+
+    def push(self, depth, color) -> SessionStatus:
+        d = depth if isinstance(depth, torch.Tensor) and depth.is_cuda else torch.as_tensor(np.asarray(depth)).cuda()
+        stream = self.session.stream
+        if not self.trajectory:
+            # the first frame's view is kept as the model of the second: no Gauss-Newton steps, the given pose
+            seed = TrackParams.from_buffer_copy(self.params)
+            seed.levels = 1
+            seed.iterations = (C.c_int32 * 4)(0, 0, 0, 0)
+            pose, result = self.rec.track(d, self.first_pose, seed, self.pp, "cloud", stream)
+        else:
+            pose, result = self.rec.track(d, self.guess(), self.params, self.pp,
+                                          "cloud" if self.integrated else "previous", stream)
+        self.trajectory.append(pose)
+        self.results.append(result)
+        status = self.session.push(depth, color, pose, invert_rigid(pose))
+        self.integrated = status.last_integrated_frame >= 0
+        return status
+
+    def end(self) -> StreamStats:
+        return self.session.end()
+
+    def __enter__(self) -> "TrackedSession":
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        return self.session.__exit__(exc_type, exc, tb)
 
 
 def outlier_filter_transforms(global_T_frame, frame_T_global, frame: int, other_count: int, depth_scaling: float,
