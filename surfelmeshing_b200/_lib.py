@@ -268,7 +268,8 @@ _shimref: Library | None = None
 
 def load_product() -> Library:
     """The product library. SM_B200_LIB=<path> loads another BUILD OF THE PRODUCT instead (A/B
-    measurements of kernel variants, e.g. variants/lib_r2base.so); it exports the same ABI."""
+    measurements of kernel variants, e.g. variants/lib_x.so from
+    `python -m surfelmeshing_b200.build --out variants/lib_x.so -- <nvcc flags>`); it exports the same ABI."""
     global _product
     if _product is None:
         import os

@@ -5,6 +5,11 @@ sm_90a (H100) only (no fallback architectures) and links them in-tree into
 surfelmeshing_b200/libsurfel_b200.so, so that the package is importable from the
 repository tree.
 
+`python -m surfelmeshing_b200.build --out variants/lib_x.so -- -DFOO` builds a variant of the
+library for an A/B run (tools/ab_probe.py --lib x=variants/lib_x.so): the same recipe with extra
+nvcc flags, its objects in a directory of their own next to the output (variants/lib_x.objs/), so
+the product's incremental build is left alone.
+
 Flags: -ftz=true -fmad=false. The kernels spell out every fp32 operation (csrc/sm_math.cuh)
 in the order of the reference's -use_fast_math SASS; -fmad=false guarantees the compiler
 contracts nothing on its own. -ffp-contract=off does the same for the host compiler, whose default
@@ -50,32 +55,48 @@ def _stale(target: Path, deps) -> bool:
     return any(Path(d).stat().st_mtime > t for d in deps)
 
 
-def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile csrc/*.cu -> libsurfel_b200.so (incremental). Returns the library path."""
+def build(force: bool = False, verbose: bool = False, out: Path = LIB_PATH, extra_flags=()) -> Path:
+    """Compile csrc/*.cu -> `out` (incremental) with NVCC_FLAGS + `extra_flags`. Returns the library path."""
     nvcc = _nvcc()
-    obj_dir = PKG_DIR / "build"
-    obj_dir.mkdir(exist_ok=True)
+    out = Path(out).resolve()
+    obj_dir = PKG_DIR / "build" if out == LIB_PATH else out.with_suffix(".objs")
+    obj_dir.mkdir(parents=True, exist_ok=True)
+    flags = [*NVCC_FLAGS, *extra_flags]
+    flags_stamp = obj_dir / "nvcc_flags"
+    force = force or not flags_stamp.exists() or flags_stamp.read_text() != " ".join(flags)
     headers = [CSRC / h for h in HEADERS] + [Path(__file__)]
     objects = []
     for src in SOURCES:
         obj = obj_dir / (src.replace(".cu", ".o"))
         objects.append(obj)
         if force or _stale(obj, [CSRC / src] + headers):
-            cmd = [nvcc, *NVCC_FLAGS, "-c", str(CSRC / src), "-o", str(obj)]
+            cmd = [nvcc, *flags, "-c", str(CSRC / src), "-o", str(obj)]
             res = subprocess.run(cmd, capture_output=True, text=True)
             if verbose or res.returncode != 0:
                 sys.stderr.write(" ".join(cmd) + "\n" + res.stdout + res.stderr)
             if res.returncode != 0:
                 raise RuntimeError(f"nvcc failed on {src}")
             (obj_dir / (src + ".ptxas.log")).write_text(res.stderr)
-    if force or _stale(LIB_PATH, objects):
-        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", str(LIB_PATH), *map(str, objects)]
+    flags_stamp.write_text(" ".join(flags))
+    if force or _stale(out, objects):
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", str(out), *map(str, objects)]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:
             sys.stderr.write(" ".join(cmd) + "\n" + res.stdout + res.stderr)
             raise RuntimeError("link failed")
-    return LIB_PATH
+    return out
+
+
+def main(argv) -> None:
+    import argparse
+    split = argv.index("--") if "--" in argv else len(argv)
+    ap = argparse.ArgumentParser(prog="python -m surfelmeshing_b200.build",
+                                 usage="%(prog)s [--force] [--out LIB] [-- extra nvcc flags...]")
+    ap.add_argument("--force", action="store_true", help="recompile every source")
+    ap.add_argument("--out", type=Path, default=LIB_PATH, help="library to build (default: the product, in-tree)")
+    args = ap.parse_args(argv[:split])
+    print(build(force=args.force, verbose=True, out=args.out, extra_flags=argv[split + 1:]))
 
 
 if __name__ == "__main__":
-    print(build(force="--force" in sys.argv, verbose=True))
+    main(sys.argv[1:])

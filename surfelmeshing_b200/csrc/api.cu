@@ -6,8 +6,6 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <limits>
 #include <mutex>
@@ -59,18 +57,7 @@ unsigned long long LaunchCount() { return g_launches.load(); }
 // Launch of a described kernel (KernelLaunch, sm_kernels.cuh) on a stream.
 void LaunchOnStream(cudaStream_t stream, const KernelLaunch& k, bool dependent) {
   LaunchScope scope(stream, static_cast<KernelId>(k.kernel_id));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = k.grid;
-  cfg.blockDim = k.block;
-  cfg.dynamicSmemBytes = k.smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  const int mode = PdlMode();
-  cfg.numAttrs = (mode == 2 || (mode == 1 && dependent)) ? 1 : 0;
-  cudaLaunchKernelExC(&cfg, k.func, const_cast<void**>(k.args));
+  cudaLaunchKernelExC(LaunchConfig(k.grid, k.block, k.smem, stream, dependent).get(), k.func, const_cast<void**>(k.args));
 }
 
 // ---- supporting-surfel tie-break (sm_kernels.cuh, kSecondaryBit) ---------------------------------
@@ -131,21 +118,6 @@ TieBreak MakeTieBreak(const TieBreakConfig& cfg, u32 frame_index) {
   t.early_threshold_second = threshold(cfg.early_fraction_second >= 0 ? cfg.early_fraction_second : later);
   t.index_order_threshold_later = threshold(cfg.index_order_fraction_later >= 0 ? cfg.index_order_fraction_later : cfg.index_order_fraction);
   return t;
-}
-
-// SM_B200_GRID_PERCENT (measurement hook): percentage of the resident block count to launch.
-int ScaleGrid(int blocks) {
-  static const int percent = [] { const char* e = std::getenv("SM_B200_GRID_PERCENT"); return e ? std::atoi(e) : 100; }();
-  const int scaled = static_cast<int>(static_cast<long long>(blocks) * percent / 100);
-  return scaled > 0 ? scaled : 1;
-}
-
-int PdlMode() {
-  static const int mode = [] {
-    const char* e = std::getenv("SM_B200_PDL");
-    return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
-  }();
-  return mode;
 }
 
 const char* KernelName(int id) {
@@ -310,18 +282,13 @@ int CreateImpl(sm_reconstruction* r, uint64_t max_surfel_count, int32_t width, i
   r->sm_count = prop.multiProcessorCount;
   r->plan.sm_count = r->sm_count;
   {
-    // One shared-memory carve-out for every kernel of the library (SM_B200_CARVEOUT, percent of
-    // the 228 KB; -1 = leave it to the driver). k_blend needs ~100 KB per block and everything else
-    // a few KB; left to the driver, the SMs keep switching between configurations and the gather
-    // kernels (integrate, update_neighbors, regularisation) slow down after a blend. 47 % selects
-    // the 132 KB configuration (an H100 SM offers 0, 8, 16, 32, 64, 100, 132, 164, 196
-    // and 228 KB), the smallest that holds a blend block, and leaves 124 KB of L1 to the gathers.
-    // Function attributes and occupancy are per device: configured for every handle.
-    const char* e = std::getenv("SM_B200_CARVEOUT");
-    const int percent = e ? std::atoi(e) : 47;
-    int status = ConfigurePreprocessKernels(percent);
-    if (status == SM_OK) status = ConfigureIntegrateKernels(percent, &r->plan);
-    if (status == SM_OK) status = ConfigureRegularizeKernels(percent, &r->plan);
+    // The shared-memory carve-out (kSharedMemoryCarveoutPercent) of the pre-processing, Integrate() and
+    // regularisation kernels, k_blend's shared memory limit and the resident grids. The render, tracking,
+    // k-NN and transfer kernels keep the driver's carve-out. Function attributes and occupancy are per
+    // device: configured for every handle.
+    int status = ConfigurePreprocessKernels();
+    if (status == SM_OK) status = ConfigureIntegrateKernels(&r->plan);
+    if (status == SM_OK) status = ConfigureRegularizeKernels(&r->plan);
     if (status != SM_OK) return status;
   }
   r->fx = fx; r->fy = fy; r->cx = cx; r->cy = cy;
@@ -369,40 +336,23 @@ int CreateImpl(sm_reconstruction* r, uint64_t max_surfel_count, int32_t width, i
   SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->scratch_B), &r->scratch_B_pitch, width * sizeof(u16), height));
   SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->blend_src), &r->blend_src_pitch, width * sizeof(u16), height));
   {
-    // Tile fill of the pre-processing tail: "tma" (default) = one cp.async.bulk.tensor per block through a
-    // descriptor of scratch_B, "vector" = cooperative 128-bit loads (SM_B200_TAIL_FILL, A/B hook).
-    const char* e = std::getenv("SM_B200_TAIL_FILL");
-    const bool want_tma = !(e && std::string(e) == "vector");
-    if (want_tma) {
-      const int status = MakeDepthTensorMap(&r->scratch_B_map, r->scratch_B, r->scratch_B_pitch, width, height);
-      if (status != SM_OK) return status;
-      r->scratch_B_map_valid = true;
-    }
+    // The pre-processing tail fills its input tile with one cp.async.bulk.tensor per block through this descriptor.
+    const int status = MakeDepthTensorMap(&r->scratch_B_map, r->scratch_B, r->scratch_B_pitch, width, height);
+    if (status != SM_OK) return status;
   }
   for (int i = 0; i < 14; ++i) SM_CUDA(cudaEventCreate(&r->events.ev[i]));
   r->events.enabled = false;
-  // Supporting-surfel tie-break defaults (DESIGN.md section 4); SM_B200_TIEBREAK="wave,early_fraction" overrides.
+  // Supporting-surfel tie-break defaults (DESIGN.md section 4); sm_configure("tiebreak_*") changes them.
   {
-    u32 wave = kDefaultTieBreakWave, lanes = 1u << kDefaultTieBreakLaneShift;
-    double early = kDefaultTieBreakEarlyFraction, index_order = kDefaultTieBreakIndexOrderFraction;
-    u32 offset = kDefaultTieBreakWaveOffset;
-    if (const char* e = std::getenv("SM_B200_TIEBREAK")) {   // "wave,early[,index_order[,lanes[,wave_offset]]]"
-      unsigned w = 0, l = 0, o = 0; double q = 0, b = 0;
-      const int got = std::sscanf(e, "%u,%lf,%lf,%u,%u", &w, &q, &b, &l, &o);
-      if (got >= 2) { wave = w; early = q; }
-      if (got >= 3) index_order = b;
-      if (got >= 4) lanes = l;
-      if (got >= 5) offset = o ? 1u : 0u;
-    }
-    r->tiebreak.wave_offset = offset;
-    u32 lane_shift = 0;
-    while ((1u << lane_shift) < lanes && lane_shift < 10) ++lane_shift;
-    if (wave != 0 && (static_cast<unsigned long long>(d.capacity) / wave + 2) * 2ull * wave >= 0xFFFFFFFFull) wave = 0;
-    r->tiebreak.lane_request = lane_shift;
+    u32 wave = kDefaultTieBreakWave;
+    // the keys of the default wave would not fit in 32 bits at this surfel cap: plain rule
+    if ((static_cast<unsigned long long>(d.capacity) / wave + 2) * 2ull * wave >= 0xFFFFFFFFull) wave = 0;
+    r->tiebreak.wave_offset = kDefaultTieBreakWaveOffset;
+    r->tiebreak.lane_request = kDefaultTieBreakLaneShift;
     const int status = SetTieBreakWave(&r->tiebreak, wave, d.capacity);
     if (status != SM_OK) return status;
-    r->tiebreak.early_fraction = early;
-    r->tiebreak.index_order_fraction = index_order;
+    r->tiebreak.early_fraction = kDefaultTieBreakEarlyFraction;
+    r->tiebreak.index_order_fraction = kDefaultTieBreakIndexOrderFraction;
     r->tiebreak.early_fraction_later = kDefaultTieBreakEarlyFractionLater;
     r->tiebreak.index_order_fraction_later = kDefaultTieBreakIndexOrderFractionLater;
     r->tiebreak.early_fraction_second = kDefaultTieBreakEarlyFractionSecond;
@@ -556,7 +506,7 @@ int sm_preprocess(sm_reconstruction* r, void* stream, const sm_preprocess_params
                                      others_TR_reference, r->scratch_B, r->scratch_B_pitch, out_depth,
                                      out_depth_pitch, reinterpret_cast<float2*>(out_normals), out_normals_pitch,
                                      out_radius, out_radius_pitch, r->d.assoc, r->d.first_depth, r->d.supported, nullptr, 0,
-                                     nullptr, nullptr, r->ScratchBMap());
+                                     nullptr, nullptr, r->scratch_B_map);
   if (status == SM_OK) r->rasters_cleared = true;
   return status;
 }

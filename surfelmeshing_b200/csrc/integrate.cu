@@ -1533,50 +1533,32 @@ int ExportVertices(cudaStream_t stream, const DeviceState& d, int count_slot, in
 }
 
 // Per-device configuration of the kernels of this file for the CURRENT device (called by
-// sm_create for every handle: function attributes and occupancy are per device):
-//  - one shared-memory carve-out for all kernels (see sm_create in api.cu),
-//  - k_blend's dynamic shared memory limit,
-//  - grids of the list kernels = exactly the blocks that are resident at once (occupancy x SMs), so
-//    that every block is scheduled in the first wave and the per-block loops (which fetch the next
-//    item ahead) take care of longer lists. SM_B200_RESIDENT_GRIDS=0 restores fixed 8 blocks/SM.
-int ConfigureIntegrateKernels(int carveout_percent, LaunchPlan* plan) {
-  if (carveout_percent >= 0) {
-    cudaFuncSetAttribute(k_clear, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_project, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_associate, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_merge, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_blend, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_integrate, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_update_neighbors, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_new_surfel_scan, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_create_surfels, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_export_vertices, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaGetLastError();
-  }
+// sm_create for every handle: function attributes and occupancy are per device): the shared-memory
+// carve-out (kSharedMemoryCarveoutPercent), k_blend's dynamic shared memory limit and the resident
+// grids of the list kernels (ResidentBlocks).
+int ConfigureIntegrateKernels(LaunchPlan* plan) {
+  const int carveout_percent = kSharedMemoryCarveoutPercent;
+  cudaFuncSetAttribute(k_clear, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_project, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_associate, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_merge, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_blend, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_integrate, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_update_neighbors, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_new_surfel_scan, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_create_surfels, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_export_vertices, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaGetLastError();
   if (cudaFuncSetAttribute(k_blend, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kBlendSmemLimit)) != cudaSuccess) {
     return SetError(SM_ERR_CUDA, "cudaFuncSetAttribute(k_blend, MaxDynamicSharedMemorySize)");
   }
   const int sm_count = plan->sm_count;
-  const char* e = std::getenv("SM_B200_RESIDENT_GRIDS");
-  if (e && e[0] == '0') {
-    plan->project = sm_count * 4;
-    plan->associate = plan->merge = plan->integrate = plan->update_neighbors = sm_count * 8;
-    return SM_OK;
-  }
-  auto resident = [&](auto kernel, int block, int fallback_per_sm) {
-    int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0) != cudaSuccess || per_sm < 1) {
-      cudaGetLastError();
-      per_sm = fallback_per_sm;
-    }
-    return ScaleGrid(sm_count * per_sm);
-  };
-  plan->project = resident(k_project, kProjectBlock, 2);
-  plan->associate = resident(k_associate, kBlock, 8);
-  plan->merge = resident(k_merge, kBlock, 4);
-  plan->integrate = resident(k_integrate, kBlock, 3);
-  plan->update_neighbors = resident(k_update_neighbors, kBlock, 3);
-  return SM_OK;
+  int status = ResidentBlocks(k_project, kProjectBlock, sm_count, &plan->project);
+  if (status == SM_OK) status = ResidentBlocks(k_associate, kBlock, sm_count, &plan->associate);
+  if (status == SM_OK) status = ResidentBlocks(k_merge, kBlock, sm_count, &plan->merge);
+  if (status == SM_OK) status = ResidentBlocks(k_integrate, kBlock, sm_count, &plan->integrate);
+  if (status == SM_OK) status = ResidentBlocks(k_update_neighbors, kBlock, sm_count, &plan->update_neighbors);
+  return status;
 }
 
 }  // namespace smb

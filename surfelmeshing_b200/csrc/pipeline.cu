@@ -485,7 +485,7 @@ int GraphStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
                                 r->run_radius[set], r->run_radius_pitch, r->assoc_set[set], r->first_depth_set[set],
                                 r->supported_set[set], r->run_depth_pre[set], r->run_depth_pitch,
                                 TimelineSlot(r->d, static_cast<u32>(frame), KID_BILATERAL_OUTLIER),
-                                TimelineSlot(r->d, static_cast<u32>(frame), KID_ERODE_NORMALS_RADII), r->ScratchBMap());
+                                TimelineSlot(r->d, static_cast<u32>(frame), KID_ERODE_NORMALS_RADII), r->scratch_B_map);
     if (status != SM_OK) return status;
   }
 
@@ -527,7 +527,7 @@ int SerialStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
                                r->run_depth_pitch, r->run_normals[set], r->run_normals_pitch, r->run_radius[set],
                                r->run_radius_pitch, r->assoc_set[set], r->first_depth_set[set], r->supported_set[set],
                                nullptr, 0, TimelineSlot(r->d, static_cast<u32>(it), KID_BILATERAL_OUTLIER),
-                               TimelineSlot(r->d, static_cast<u32>(it), KID_ERODE_NORMALS_RADII), r->ScratchBMap());
+                               TimelineSlot(r->d, static_cast<u32>(it), KID_ERODE_NORMALS_RADII), r->scratch_B_map);
   if (status != SM_OK) return status;
   UseSet(r->d, r, set);
   r->rasters_cleared = true;

@@ -20,7 +20,6 @@
 // rows cost one sector per value.
 
 #include <algorithm>
-#include <cstdlib>
 
 #include "sm_kernels.cuh"
 
@@ -321,28 +320,18 @@ int RegularizeSurfels(cudaStream_t stream, DeviceState& d, bool disable_denoisin
   return CheckLaunch("regularize");
 }
 
-// Per-device configuration: one shared-memory carve-out for every kernel of the file (see
-// sm_create in api.cu) and grids = the blocks resident at once (see ConfigureIntegrateKernels).
-int ConfigureRegularizeKernels(int carveout_percent, LaunchPlan* plan) {
-  if (carveout_percent >= 0) {
-    cudaFuncSetAttribute(k_reg_accumulate, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_reg_step, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaFuncSetAttribute(k_reg_copy_only, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
-    cudaGetLastError();
-  }
-  const char* e = std::getenv("SM_B200_RESIDENT_GRIDS");
-  auto resident = [&](auto kernel) {
-    int per_sm = 0;
-    if ((e && e[0] == '0') || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kBlock, 0) != cudaSuccess || per_sm < 1) {
-      cudaGetLastError();
-      per_sm = 8;
-    }
-    return ScaleGrid(plan->sm_count * per_sm);
-  };
-  plan->reg_accumulate = resident(k_reg_accumulate);
-  plan->reg_step = resident(k_reg_step);
-  plan->reg_copy = resident(k_reg_copy_only);
-  return SM_OK;
+// Per-device configuration: the shared-memory carve-out of every kernel of the file
+// (kSharedMemoryCarveoutPercent) and grids = the blocks resident at once (ResidentBlocks).
+int ConfigureRegularizeKernels(LaunchPlan* plan) {
+  const int carveout_percent = kSharedMemoryCarveoutPercent;
+  cudaFuncSetAttribute(k_reg_accumulate, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_reg_step, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaFuncSetAttribute(k_reg_copy_only, cudaFuncAttributePreferredSharedMemoryCarveout, carveout_percent);
+  cudaGetLastError();
+  int status = ResidentBlocks(k_reg_accumulate, kBlock, plan->sm_count, &plan->reg_accumulate);
+  if (status == SM_OK) status = ResidentBlocks(k_reg_step, kBlock, plan->sm_count, &plan->reg_step);
+  if (status == SM_OK) status = ResidentBlocks(k_reg_copy_only, kBlock, plan->sm_count, &plan->reg_copy);
+  return status;
 }
 
 }  // namespace smb

@@ -206,11 +206,9 @@ int EnsureRenderBuffers(sm_reconstruction* r, cudaStream_t stream, size_t pixels
     SM_CUDA(cudaMalloc(&r->render_large_list, sizeof(u32) * r->d.stride));
     SM_CUDA(cudaMalloc(&r->render_large_count, sizeof(u32)));
     SM_CUDA(cudaMemsetAsync(r->render_large_count, 0, sizeof(u32), stream));
-    int per_sm = 0;
-    SM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_render_splat, kSplatBlock, 0));
-    r->render_splat_blocks = (per_sm > 0 ? per_sm : 1) * r->sm_count;
-    SM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_render_large, kLargeBlock, 0));
-    r->render_large_blocks = (per_sm > 0 ? per_sm : 1) * r->sm_count;
+    int status = ResidentBlocks(k_render_splat, kSplatBlock, r->sm_count, &r->render_splat_blocks);
+    if (status == SM_OK) status = ResidentBlocks(k_render_large, kLargeBlock, r->sm_count, &r->render_large_blocks);
+    if (status != SM_OK) return status;
   }
   if (pixels > r->render_key_capacity) {
     cudaFree(r->render_keys);   // synchronises the device: an earlier render may still use it

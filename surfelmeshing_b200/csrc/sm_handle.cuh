@@ -71,8 +71,6 @@ struct sm_reconstruction {
   // pre-processing scratch (APP/main.cc filtered_depth_buffer_B)
   smb::u16* scratch_B = nullptr; size_t scratch_B_pitch = 0;
   smb::TensorMapStorage scratch_B_map{};   // TMA descriptor of scratch_B (tile fill of the pre-processing tail)
-  bool scratch_B_map_valid = false;
-  const smb::TensorMapStorage* ScratchBMap() const { return scratch_B_map_valid ? &scratch_B_map : nullptr; }
   // sm_integrate: snapshot of the depth before the measurement blending (k_blend reads the snapshot and
   // writes the caller's buffer: see the kernel)
   smb::u16* blend_src = nullptr; size_t blend_src_pitch = 0;

@@ -7,6 +7,8 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <string>
+
 #include "../../include/surfel_b200.h"
 #include "sm_math.cuh"
 
@@ -278,7 +280,7 @@ struct FrameParams {
 // Programmatic dependent launch (sm_90+): every kernel starts with pdl_prologue(): it lets the NEXT
 // kernel of the stream be scheduled early (launch_dependents) and then waits until the PREVIOUS
 // kernel has completed and flushed its memory (wait). With the launch attribute set
-// (LaunchKernel below) this overlaps launch latency / block scheduling of dependent kernels with
+// (LaunchConfig below) this overlaps launch latency / block scheduling of dependent kernels with
 // the tail of their predecessor; without the attribute both instructions are no-ops.
 __device__ __forceinline__ void pdl_prologue() {
 #if defined(__CUDA_ARCH__)
@@ -312,38 +314,35 @@ inline unsigned long long* TimelineSlot(const DeviceState& d, u32 frame, int ker
   return d.timeline ? d.timeline + (static_cast<size_t>(frame % d.timeline_frames) * KID_TIMELINE_COUNT + kernel_id) * 2 : nullptr;
 }
 
-// SM_B200_PDL: 0 = never, 1 (default) = only launches marked as dependents (LaunchDependent: the
-// kernel follows its producer on the same stream), 2 = every launch. Applies to stream launches
-// (sm_preprocess, sm_integrate, the serial mode of sm_stream_run), not to the nodes of the frame graph.
-int PdlMode();
-int ScaleGrid(int blocks);  // SM_B200_GRID_PERCENT measurement hook (integrate.cu)
+// Configuration of one stream launch. `dependent`: the kernel's producer is the previous kernel of the same stream,
+// and the launch carries the programmatic-serialization attribute (sm_preprocess, sm_integrate and the serial mode
+// of sm_stream_run; the nodes of the frame graph are not stream launches).
+class LaunchConfig {
+ public:
+  LaunchConfig(dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool dependent) {
+    attr_.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr_.val.programmaticStreamSerializationAllowed = 1;
+    cfg_ = {};
+    cfg_.gridDim = grid;
+    cfg_.blockDim = block;
+    cfg_.dynamicSmemBytes = smem;
+    cfg_.stream = stream;
+    cfg_.attrs = &attr_;
+    cfg_.numAttrs = dependent ? 1 : 0;
+  }
+  LaunchConfig(const LaunchConfig&) = delete;
+  LaunchConfig& operator=(const LaunchConfig&) = delete;
+  const cudaLaunchConfig_t* get() const { return &cfg_; }
 
-template <typename... KArgs, typename... Args>
-inline void LaunchKernelImpl(bool dependent, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                             cudaStream_t stream, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  const int mode = PdlMode();
-  cfg.numAttrs = (mode == 2 || (mode == 1 && dependent)) ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
+ private:
+  cudaLaunchAttribute attr_;
+  cudaLaunchConfig_t cfg_;
+};
+
 template <typename... KArgs, typename... Args>
 inline void LaunchKernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                          Args&&... args) {
-  LaunchKernelImpl(false, kernel, grid, block, smem, stream, static_cast<Args&&>(args)...);
-}
-// For a kernel whose producer is the previous kernel of the same stream.
-template <typename... KArgs, typename... Args>
-inline void LaunchDependent(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                            Args&&... args) {
-  LaunchKernelImpl(true, kernel, grid, block, smem, stream, static_cast<Args&&>(args)...);
+  cudaLaunchKernelEx(LaunchConfig(grid, block, smem, stream, false).get(), kernel, static_cast<KArgs>(args)...);
 }
 
 // One kernel launch with its by-value arguments packed into `storage`: what a stream launch and
@@ -374,32 +373,53 @@ struct KernelLaunch {
 // Launches a described kernel on a stream (counts it, profiles it like LaunchKernel).
 void LaunchOnStream(cudaStream_t stream, const KernelLaunch& k, bool dependent);
 
-// Grid sizes of the list / sweep kernels: exactly the blocks that are resident at once
-// (occupancy x SMs) so that every block is scheduled in the first wave. Occupancy and function
-// attributes are per device, so the plan lives in the handle (sm_create), not in statics.
+// Grid of a resident sweep: exactly the blocks of `kernel` that are resident at once (occupancy x SMs), so that
+// every block is scheduled in the first wave and the per-block loops take care of longer lists.
+template <typename Kernel>
+inline int ResidentBlocks(Kernel kernel, int block, int sm_count, int* out) {
+  int per_sm = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return SetError(SM_ERR_CUDA, (std::string("cudaOccupancyMaxActiveBlocksPerMultiprocessor: ") + cudaGetErrorString(e)).c_str());
+  }
+  *out = (per_sm > 0 ? per_sm : 1) * sm_count;
+  return SM_OK;
+}
+
+// Grid sizes of the list / sweep kernels (ResidentBlocks). Occupancy and function attributes are per
+// device, so the plan lives in the handle (sm_create), not in statics.
 struct LaunchPlan {
   int sm_count;
   int project, associate, merge, integrate, update_neighbors;
   int reg_accumulate, reg_step, reg_copy;
 };
-// Per-device kernel configuration of the current device: shared-memory carve-out (percent, < 0:
-// driver default), k_blend's dynamic shared memory limit, the resident grids.
-int ConfigurePreprocessKernels(int carveout_percent);
-int ConfigureIntegrateKernels(int carveout_percent, LaunchPlan* plan);
-int ConfigureRegularizeKernels(int carveout_percent, LaunchPlan* plan);
+// Shared-memory carve-out of the pre-processing, Integrate() and regularisation kernels, in percent of the
+// 228 KB of an SM. k_blend needs ~100 KB per block and everything else a few KB; left to the driver, the
+// SMs keep switching between configurations and the gather kernels (integrate, update_neighbors,
+// regularisation) slow down after a blend. 47 % selects the 132 KB configuration (an H100 SM offers 0, 8,
+// 16, 32, 64, 100, 132, 164, 196 and 228 KB), the smallest that holds a blend block, and leaves 124 KB of
+// L1 to the gathers.
+constexpr int kSharedMemoryCarveoutPercent = 47;
+// Per-device kernel configuration of the current device: the carve-out, k_blend's dynamic shared memory
+// limit, the resident grids.
+int ConfigurePreprocessKernels();
+int ConfigureIntegrateKernels(LaunchPlan* plan);
+int ConfigureRegularizeKernels(LaunchPlan* plan);
 
 // ---- preprocess.cu --------------------------------------------------------------------------
 // Opaque storage of a CUtensorMap (TMA descriptor; cuda.h stays out of this header).
 struct alignas(64) TensorMapStorage { unsigned char bytes[128]; };
 int MakeDepthTensorMap(TensorMapStorage* out, const u16* base, size_t pitch_bytes, int width, int height);
+// `scratch_B_map`: TMA descriptor of scratch_B (MakeDepthTensorMap), the tail's input tile.
 int PreprocessFused(cudaStream_t stream, const sm_preprocess_params& p, int width, int height, float fx, float fy,
                     float cx, float cy, const u16* raw, size_t raw_pitch, const u16* const* other_depths,
                     const size_t* other_pitches, const float* others_TR_reference, u16* scratch_B,
                     size_t scratch_B_pitch, u16* out_depth, size_t out_depth_pitch, float2* out_normals,
                     size_t out_normals_pitch, float* out_radius, size_t out_radius_pitch, uint4* clear_assoc,
-                    float* clear_first_depth, u8* clear_supported, u16* out_depth_copy = nullptr,
-                    size_t out_depth_copy_pitch = 0, unsigned long long* timeline_bilateral = nullptr,
-                    unsigned long long* timeline_tail = nullptr, const TensorMapStorage* scratch_B_map = nullptr);
+                    float* clear_first_depth, u8* clear_supported, u16* out_depth_copy,
+                    size_t out_depth_copy_pitch, unsigned long long* timeline_bilateral,
+                    unsigned long long* timeline_tail, const TensorMapStorage& scratch_B_map);
 // Bilateral filter radius (cuda_depth_processing.cu:135). Radius 6 has the fused bilateral + outlier kernel.
 inline int BilateralRadius(const sm_preprocess_params& p) {
   return static_cast<int>(p.bilateral_filter_radius_factor * p.bilateral_filter_sigma_xy + 0.5f);
@@ -413,7 +433,7 @@ int DescribePreprocess(KernelLaunch* bilateral, KernelLaunch* outlier, KernelLau
                        size_t out_depth_pitch, float2* out_normals, size_t out_normals_pitch, float* out_radius,
                        size_t out_radius_pitch, uint4* clear_assoc, float* clear_first_depth, u8* clear_supported,
                        u16* out_depth_copy, size_t out_depth_copy_pitch, unsigned long long* timeline_bilateral,
-                       unsigned long long* timeline_tail, const TensorMapStorage* scratch_B_map);
+                       unsigned long long* timeline_tail, const TensorMapStorage& scratch_B_map);
 int StageBilateral(cudaStream_t stream, float sigma_xy, float sigma_value_factor, u16 value_to_ignore,
                    float radius_factor, u16 max_depth, float depth_valid_region_radius, int width, int height,
                    const u16* in, size_t in_pitch, u16* out, size_t out_pitch);

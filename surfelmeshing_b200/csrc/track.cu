@@ -426,9 +426,8 @@ void ComposeRigid(const double* a, const double* b, double* out) {
 // All scratch, the device state last: a non-null track_state means every buffer exists. A failed allocation frees
 // what was allocated, so the next call starts over.
 int AllocateTrackBuffers(sm_reconstruction* r) {
-  int per_sm = 0;
-  SM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_track_linearize, kLinearizeBlock, 0));
-  r->track_blocks = (per_sm > 0 ? per_sm : 1) * r->sm_count;
+  const int status = ResidentBlocks(k_track_linearize, kLinearizeBlock, r->sm_count, &r->track_blocks);
+  if (status != SM_OK) return status;
   SM_CUDA(cudaMalloc(&r->track_partials, sizeof(double) * kTerms * r->track_blocks));
   SM_CUDA(cudaMallocHost(&r->track_host_state, sizeof(TrackState)));
   const size_t W = static_cast<size_t>(r->d.width), H = static_cast<size_t>(r->d.height);

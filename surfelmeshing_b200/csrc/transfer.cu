@@ -21,9 +21,6 @@
 // This is a superset of the changed slots, so the arrays end up identical to a full transfer.
 
 #include <algorithm>
-#include <chrono>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <exception>
 #include <string>
@@ -230,13 +227,6 @@ void FreeTransferBuffers(sm_reconstruction* r) {
   r->delta_capacity = 0; r->delta_host_capacity = 0;
 }
 
-namespace {
-bool DeltaTimingEnabled() {
-  static const bool enabled = [] { const char* e = std::getenv("SM_B200_DELTA_TIMING"); return e && e[0] == '1'; }();
-  return enabled;
-}
-}  // namespace
-
 int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_index, sm_transfer_token* token, float* x,
                   float* y, float* z, float* radius_squared, float* nx, float* ny, float* nz,
                   uint32_t* last_update_stamp, sm_transfer_stats* stats) {
@@ -308,7 +298,6 @@ int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_inde
       st.d2h_bytes += sizeof(u32) * words;
       // scatter into the CUDASurfelBuffersCPU arrays: the eight arrays are independent, four host threads take two
       // each once the list is long enough to pay for starting them
-      const auto t_scatter = std::chrono::steady_clock::now();
       u32* const dst_rows[8] = {reinterpret_cast<u32*>(x), reinterpret_cast<u32*>(y), reinterpret_cast<u32*>(z),
                                 reinterpret_cast<u32*>(radius_squared), reinterpret_cast<u32*>(nx),
                                 reinterpret_cast<u32*>(ny), reinterpret_cast<u32*>(nz), last_update_stamp};
@@ -335,10 +324,6 @@ int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_inde
         scattered = true;
       }
       if (!scattered) scatter_rows(0, 8);
-      if (DeltaTimingEnabled()) {
-        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_scatter).count();
-        fprintf(stderr, "[surfel_b200] delta transfer: %u of %u slots, host scatter %.3f ms\n", changed, n, ms);
-      }
     }
     st.changed_count = changed;
   }

@@ -71,6 +71,15 @@ def test_missing_library_fails_loudly(tmp_path):
         _lib.Library(tmp_path / "libsurfel_b200.so", "sm_", product=True)
 
 
+def test_library_reads_no_environment():
+    """The library has one configuration: tuning goes through sm_configure or a separate build, never through
+    environment variables that only some processes see."""
+    csrc = ROOT / "surfelmeshing_b200" / "csrc"
+    readers = [f"{p.name}:{i}" for p in sorted(csrc.iterdir()) if p.is_file()
+               for i, line in enumerate(p.read_text().splitlines(), 1) if "getenv" in line]
+    assert not readers, readers
+
+
 def test_every_configure_key_is_documented():
     """sm_configure accepts named knobs: each key the library tests for appears in the header's description."""
     source = (ROOT / "surfelmeshing_b200" / "csrc" / "api.cu").read_text()

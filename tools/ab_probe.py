@@ -1,11 +1,10 @@
 #!/usr/bin/env python
-"""Same-box A/B of pipeline / kernel variants (run on a GPU): one synthetic stream, one process,
-every configuration = environment knobs (read per call / per handle) and optionally another build of
-the product library (--lib name=path). Prints frames/s (best and median of --reps passes, CUDA events)
-and the surfel counts; writes probe_out/ab_probe.json."""
+"""Same-box A/B of builds of the product library (run on a GPU): one synthetic stream, one process, the
+product first and last and every --lib name=path build in between (a variant is built with
+`python -m surfelmeshing_b200.build --out variants/lib_<name>.so -- <nvcc flags>`). Prints frames/s (best and
+median of --reps passes, CUDA events) and the surfel counts; writes probe_out/ab_probe.json."""
 import argparse
 import json
-import os
 import sys
 from pathlib import Path
 
@@ -16,8 +15,6 @@ sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 from surfelmeshing_b200 import _lib, synthetic as S  # noqa: E402
 from surfelmeshing_b200 import reconstruction as R  # noqa: E402
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams  # noqa: E402
-
-KNOBS = ("SM_B200_TAIL_FILL", "SM_B200_PDL", "SM_B200_CARVEOUT", "SM_B200_GRID_PERCENT", "SM_B200_TIEBREAK")
 
 
 def main():
@@ -30,28 +27,17 @@ def main():
     ap.add_argument("--host", action="store_true", help="pinned host frames (e2e path)")
     ap.add_argument("--sigma-xy", type=float, default=None,
                     help="bilateral_filter_sigma_xy (default 3: radius 6, the fused kernel; 2 gives radius 4)")
-    ap.add_argument("--lib", action="append", default=[], help="name=path of another product build")
-    ap.add_argument("--config", action="append", default=[],
-                    help="name:KEY=VAL+KEY=VAL[+lib=name]; 'default' is always run first and last")
+    ap.add_argument("--lib", action="append", default=[],
+                    help="name=path of another product build; the product itself runs first and last")
     ap.add_argument("--out", default="probe_out/ab_probe.json")
     args = ap.parse_args()
 
-    libs = {"product": _lib.load_product()}
+    product = _lib.load_product()
+    arms = [("default", product)]
     for item in args.lib:
         name, path = item.split("=", 1)
-        libs[name] = _lib.Library(Path(path).resolve(), "sm_", product=True)
-    configs = [("default", {}, "product")]
-    for item in args.config:
-        name, _, rest = item.partition(":")
-        env, lib = {}, "product"
-        for kv in filter(None, rest.split("+")):
-            k, v = kv.split("=", 1)
-            if k == "lib":
-                lib = v
-            else:
-                env[k] = v
-        configs.append((name, env, lib))
-    configs.append(("default_again", {}, "product"))
+        arms.append((name, _lib.Library(Path(path).resolve(), "sm_", product=True)))
+    arms.append(("default_again", product))
 
     cam = S.Camera.tum(args.width, args.height)
     st = S.make_stream(cam, args.frames, device="cuda")
@@ -66,11 +52,8 @@ def main():
     f0, f1 = st.integrated_range()
     torch.cuda.synchronize()
     results = []
-    for name, env, lib in configs:
-        for k in KNOBS:
-            os.environ.pop(k, None)
-        os.environ.update(env)
-        rec = R.CUDASurfelReconstruction(args.cap, cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy, lib=libs[lib])
+    for name, lib in arms:
+        rec = R.CUDASurfelReconstruction(args.cap, cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy, lib=lib)
         rates, host_ms = [], []
         stats = None
         for rep in range(args.reps + 1):  # first pass = warm-up (graph instantiation, buffers)
@@ -86,7 +69,7 @@ def main():
                 rates.append(stats.frames_integrated / e0.elapsed_time(e1) * 1e3)
                 host_ms.append(stats.host_enqueue_ms)
         rec.close()
-        entry = {"config": name, "env": env, "lib": lib, "fps_best": max(rates), "fps_median": float(np.median(rates)),
+        entry = {"config": name, "lib": str(lib.path), "fps_best": max(rates), "fps_median": float(np.median(rates)),
                  "host_enqueue_ms": float(np.median(host_ms)), "surfels_size": int(stats.surfels_size),
                  "surfel_count": int(stats.surfel_count), "launches": int(stats.kernel_launches)}
         results.append(entry)
