@@ -207,7 +207,14 @@ int sm_compute_point_radii_and_remove_isolated_pixels(
  * Unlike the reference the call does NOT block the host (the reference
  * synchronises twice, cuda_surfel_reconstruction_kernels.cc:509 and
  * cuda_surfel_reconstruction.cc:290): counts stay device-resident and are
- * fetched by sm_surfel_count()/sm_surfels_size() on demand. */
+ * fetched by sm_surfel_count()/sm_surfels_size() on demand.
+ *
+ * Frame indices, and so last-update stamps, must stay below 2^31: the
+ * window test int(stamp) >= int(frame_index - window) compares them as int,
+ * and the regularisation records keep the detach flag in bit 31 of the
+ * stamp. sm_integrate and sm_regularize return SM_ERR_INVALID_ARGUMENT, and
+ * launch nothing, for frame_index >= 2^31; sm_load_state does the same for a
+ * state with a last-update stamp >= 2^31. */
 int sm_integrate(sm_reconstruction* r, void* stream, uint32_t frame_index,
                  const sm_integrate_params* p,
                  uint16_t* depth, size_t depth_pitch,

@@ -580,12 +580,14 @@ int sm_integrate(sm_reconstruction* r, void* stream, uint32_t frame_index, const
                  size_t radius_pitch, const uint8_t* color, size_t color_pitch, const float global_T_local[12],
                  const float local_T_global[12]) {
   if (r->session) return RejectInSession("sm_integrate");
+  if (frame_index >= kFrameIndexLimit) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_integrate: frame_index must be below 2^31");
   return IntegrateImpl(r, static_cast<cudaStream_t>(stream), frame_index, *p, depth, depth_pitch, normals,
                        normals_pitch, radius, radius_pitch, color, color_pitch, global_T_local, local_T_global);
 }
 
 int sm_regularize(sm_reconstruction* r, void* stream, uint32_t frame_index, float regularizer_weight,
                   float radius_factor_for_regularization_neighbors, int32_t regularization_frame_window_size) {
+  if (frame_index >= kFrameIndexLimit) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_regularize: frame_index must be below 2^31");
   r->last_stream = static_cast<cudaStream_t>(stream);
   RecordOperation(r, static_cast<int>(frame_index - static_cast<u32>(regularization_frame_window_size)));
   return RegularizeSurfels(static_cast<cudaStream_t>(stream), r->d, /*disable_denoising*/ false, frame_index,
@@ -728,6 +730,12 @@ int sm_load_state(sm_reconstruction* r, void* stream_v, const float* host_rows, 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   if (r->session) return RejectInSession("sm_load_state");
   if (surfels_size > r->d.capacity) return SetError(SM_ERR_CAPACITY, "sm_load_state: state larger than the surfel cap");
+  {
+    const u32* stamps = reinterpret_cast<const u32*>(host_rows) + SM_ROW_LAST_UPDATE_STAMP * host_row_stride_elems;
+    for (u32 i = 0; i < surfels_size; ++i) {
+      if (stamps[i] >= kFrameIndexLimit) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_load_state: a last-update stamp is 2^31 or above");
+    }
+  }
   r->d.reg_full_sweep = 1;  // as after sm_create (both record buffers are packed below)
   if (surfels_size > 0) {
     SM_CUDA(cudaMemcpy2DAsync(r->d.surfels, r->d.stride * sizeof(float), host_rows,

@@ -62,10 +62,13 @@ constexpr u32 kInvalidIndex = 0xFFFFFFFFu;   // APP/surfel.h:63, kernels.cu:74
 //   row 14  operation epoch at which the surfel was merged (delta transfer, transfer.cu)
 //   row 15  export mirror of the "meta" word of the regularisation record (DeviceState::smooth):
 //           last-update stamp | detach flag << 31. Written only by MirrorRegRecords before a dump,
-//           transfer or k-NN build; scratch otherwise. Stamps are frame indices < 2^31.
+//           transfer or k-NN build; scratch otherwise.
+// Stamps are frame indices < kFrameIndexLimit, which the entry points enforce: bit 31 of the meta word is free for
+// the detach flag, and k_reg_accumulate's window test on the meta word equals the reference's on the whole stamp.
 constexpr int kRowMergeEpoch = SM_ROW_ACCUM_X;
 constexpr int kRowMeta = SM_ROW_ACCUM_Y;
 constexpr u32 kMetaDetachBit = 0x80000000u;
+constexpr u32 kFrameIndexLimit = 0x80000000u;
 
 // The meta word (.w) of a regularisation record, stored on its own (4 bytes at offset 12 of the record).
 __device__ __forceinline__ void store_reg_meta(float4* records, u32 i, u32 meta) {
