@@ -452,6 +452,74 @@ int sm_track_linearize(sm_reconstruction* r, void* stream, const sm_track_params
                        const float* model_normal, size_t model_normal_pitch,
                        const float model_T_live[12], double out_system[27], uint32_t* out_inliers);
 
+/* ---- triangulating the surfel cloud (DESIGN.md section 1 row f9, section 5.7) ---------------------------------
+ * The reference's meshing thread grows its mesh by advancing triangle fronts one surfel at a time
+ * (APP/surfel_meshing.cc:667-752), which is sequential by construction. sm_triangulate meshes the whole current
+ * cloud at once with a different, local rule: every slot proposes the triangles of its umbrella, and a triangle is
+ * output when its three corners propose it alike. Only reads the surfel state.
+ *
+ * Slots i in [0, surfels_size()) with radius_squared (row 7) > 0 take part ("present"). Slot i has position p_i =
+ * its current SMOOTH position, radius^2 r_i^2 and normal n_i = rows 8-10 times 1 / sqrt(n.n) (IEEE square root and
+ * division); a slot whose n.n is not finite and > 0 has no umbrella and is nobody's neighbour. In fp32 with
+ * denormals flushed to zero and no contraction, a.b = (a.x*b.x + a.y*b.y) + a.z*b.z, 2D a.b = a.x*b.x + a.y*b.y,
+ * cross(a, b) = a.x*b.y - a.y*b.x, each product, sum and quotient rounded on its own; f2 = f * f with
+ * f = neighbor_radius_factor, cos_n and cos_t = cos(angle in radians) of the two angle parameters, evaluated in
+ * double and rounded to float:
+ *  1. Neighbours. The <= 64 nearest present slots j with (d^2, j) ascending, d^2 = ((dx*dx + dy*dy) + dz*dz) <=
+ *     r_i^2 * f2 (what sm_knn_query returns), i itself dropped wherever it ranks; then every j with n_i.n_j < cos_n.
+ *  2. Tangent plane. sign = copysign(1, n.z), a = -1 / (sign + n.z), b = (n.x * n.y) * a,
+ *     u = (1 + ((sign * n.x) * n.x) * a, sign * b, -(sign * n.x)), v = (b, sign + (n.y * n.y) * a, -n.y)
+ *     (Duff et al. 2017: u x v = n). q_j = ((p_j - p_i).u, (p_j - p_i).v). A neighbour with q_j = (0, 0), or with
+ *     the same q as a neighbour of lower rank, is dropped.
+ *  3. Umbrella. On the bisector of j, parametrised by s (the point q_j / 2 + (s / 2) (-q_j.y, q_j.x)), every
+ *     other neighbour k sets c = cross(q_j, q_k), b = q_k.q_k - q_j.q_k. c == 0: j is dropped if b < 0, else k sets
+ *     nothing. c > 0: an upper end t = b / c; c < 0: a lower end t = b / c. hi = the smallest upper end, lo = the
+ *     largest lower end, each with the smallest slot index among the neighbours that set it (hi_min, lo_min).
+ *     j is kept iff it has no lower or no upper end, or lo < hi, or lo == hi (bisectors through one point:
+ *     cocircular neighbours) and min(i, j) < min(lo_min, hi_min), so that the four slots of a cocircular quad
+ *     agree on its diagonal. next(j) = among the kept k with c > 0 and b / c == hi, the first counter-clockwise
+ *     from j (k replaces the current choice m iff cross(q_k, q_m) > 0, k in rank order); none if j has no upper
+ *     end (an open cell: a boundary). A slot that is next(j) of two or more j is nobody's next. U(i) = the pairs
+ *     {j, next(j)} in the rank order of j. A slot with more than SM_MESH_MAX_UMBRELLA pairs has an empty umbrella
+ *     and counts as an umbrella overflow.
+ *  4. Triangles. For {a, b} in U(i), the triangle (i, a, b) is output iff {b, i} is in U(a), {i, a} is in U(b),
+ *     and, in the rotation (o, x, y) that starts at o = min(i, a, b): with e1 = p_x - p_o, e2 = p_y - p_o, the
+ *     geometric normal (e1.y*e2.z - e1.z*e2.y, e1.z*e2.x - e1.x*e2.z, e1.x*e2.y - e1.y*e2.x) has g.n_o > 0, and
+ *     at each corner (o: e1, e2; x: p_y - p_x, p_o - p_x; y: p_o - p_y, p_x - p_y) with edges (g, h) it is not
+ *     true that g.h < cos_t * sqrt((g.g) * (h.h)). It is written once, by o, as (o, x, y): counter-clockwise
+ *     about n_o. A directed edge lies in at most one output triangle, so the mesh is edge-manifold and
+ *     consistently oriented.
+ *  5. Order: by owner slot, then by the owner's umbrella order.
+ * stats: triangle_count (set also when the capacity is too small), vertices_meshed = present slots that are a
+ * corner of an output triangle, boundary_edges = edges in exactly one output triangle, umbrella_overflows.
+ *
+ * triangles is a DEVICE buffer of 3 x capacity uint32 (may be NULL with capacity 0: a count query). If capacity <
+ * triangle_count the call returns SM_ERR_CAPACITY with stats filled and nothing written. The call synchronises
+ * `stream` three times (surfels_size(), the largest radius, the triangle count); on return the triangles are
+ * written by work enqueued on `stream`, ordered before anything the caller enqueues there next. The k-NN index uses
+ * cells of 2 * sqrt(max r_i^2 * f2) (a query touches at most 3 cells per axis; one slot with a huge radius makes
+ * every query walk more records, never a different answer). Scratch (the index, SM_MESH_MAX_UMBRELLA pairs and a
+ * few words per slot) belongs to the handle, is allocated by the first call and grows to surfels_size(); sm_create
+ * allocates nothing for meshing. SM_ERR_INVALID_ARGUMENT, with no launch, for NULL params or stats, triangles NULL
+ * with capacity > 0, a neighbor_radius_factor that is not finite and > 0 (or whose square overflows), or an angle
+ * that is not in (0, 180]. */
+#define SM_MESH_MAX_UMBRELLA 16
+typedef struct sm_mesh_params {
+  float neighbor_radius_factor;          /* 2   (main.cc max_neighbor_search_range_increase_factor) */
+  float max_angle_between_normals_deg;   /* 90  (main.cc default) */
+  float max_triangle_angle_deg;          /* 170 (main.cc default) */
+} sm_mesh_params;
+typedef struct sm_mesh_stats {
+  uint64_t triangle_count;    /* always set, also when capacity was too small */
+  uint64_t vertices_meshed;   /* present slots with >= 1 output triangle */
+  uint64_t boundary_edges;    /* edges in exactly one output triangle */
+  uint64_t umbrella_overflows;
+} sm_mesh_stats;
+/* Host only, no device needed. */
+void sm_default_mesh_params(sm_mesh_params* p);
+int sm_triangulate(sm_reconstruction* r, void* stream, const sm_mesh_params* p,
+                   uint32_t* triangles /* device, 3 x capacity */, uint64_t capacity, sm_mesh_stats* stats);
+
 /* ---- radius-limited k-nearest-neighbour queries for the meshing thread (SURVEY section 8 f4) ----
  * Replaces CompressedOctree::FindNearestSurfelsWithinRadius<include_completed_surfels, include_free_surfels>
  * (octree.h:471, octree.cc:313-470; callers surfel_meshing.cc:421 <false, true> and :821 <true, false>) for a BATCH of
@@ -600,7 +668,7 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * work waits for them: the hand-off calls (sm_transfer_all_to_cpu, sm_transfer_delta_to_cpu,
  * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
  * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_track_frame, sm_track_linearize,
- * sm_surfel_count / sm_surfels_size) and
+ * sm_triangulate, sm_surfel_count / sm_surfels_size) and
  * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
  * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which
  * that frame's Integrate() applies in the next step. The device merge counter then already includes them, so

@@ -146,6 +146,24 @@ class TrackResult(C.Structure):
                 ("valid_pixels", C.c_uint32), ("rms_residual", C.c_float)]
 
 
+class MeshParams(C.Structure):
+    """sm_mesh_params: k-NN radius factor, normal gate and largest triangle angle (main.cc's meshing defaults)."""
+    _fields_ = [("neighbor_radius_factor", C.c_float), ("max_angle_between_normals_deg", C.c_float),
+                ("max_triangle_angle_deg", C.c_float)]
+
+    @classmethod
+    def defaults(cls) -> "MeshParams":
+        return cls(2.0, 90.0, 170.0)
+
+
+class MeshStats(C.Structure):
+    """sm_mesh_stats: triangles (also when the capacity was too small), meshed slots, boundary edges, overflows."""
+    _fields_ = [("triangle_count", C.c_uint64), ("vertices_meshed", C.c_uint64), ("boundary_edges", C.c_uint64),
+                ("umbrella_overflows", C.c_uint64)]
+
+
+MESH_MAX_UMBRELLA = 16
+
 _P = C.c_void_p
 _SZ = C.c_size_t
 _F = C.c_float
@@ -218,6 +236,8 @@ _PRODUCT_ONLY = {
                               C.POINTER(TrackResult)]),
     "track_linearize": (C.c_int, [_P, _P, C.POINTER(TrackParams), _I, _F, _P, _SZ, _P, _SZ, _P, _SZ, _P, _P,
                                   C.POINTER(_U32)]),
+    "default_mesh_params": (None, [C.POINTER(MeshParams)]),
+    "triangulate": (C.c_int, [_P, _P, C.POINTER(MeshParams), _P, C.c_uint64, C.POINTER(MeshStats)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

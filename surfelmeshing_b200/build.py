@@ -27,8 +27,8 @@ PKG_DIR = Path(__file__).resolve().parent
 CSRC = PKG_DIR / "csrc"
 LIB_PATH = PKG_DIR / "libsurfel_b200.so"
 SOURCES = ["api.cu", "pipeline.cu", "transfer.cu", "preprocess.cu", "integrate.cu", "regularize.cu", "knn.cu",
-           "render.cu", "track.cu"]
-HEADERS = ["sm_math.cuh", "sm_kernels.cuh", "sm_handle.cuh", "../../include/surfel_b200.h"]
+           "render.cu", "track.cu", "mesh.cu"]
+HEADERS = ["sm_math.cuh", "sm_kernels.cuh", "sm_handle.cuh", "sm_knn.cuh", "../../include/surfel_b200.h"]
 
 NVCC_FLAGS = [
     "-std=c++17",

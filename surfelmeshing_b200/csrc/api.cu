@@ -127,7 +127,8 @@ const char* KernelName(int id) {
       "k_new_surfel_scan", "k_create_surfels", "k_reg_accumulate", "k_reg_step", "k_reg_copy_only",
       "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_downscale_depth_median",
       "k_downscale_color", "k_reg_mirror", "k_reg_pack", "k_render_splat", "k_render_large", "k_render_resolve",
-      "k_track_live_view", "k_track_linearize", "k_track_solve"};
+      "k_track_live_view", "k_track_linearize", "k_track_solve", "k_mesh_bound", "k_mesh_umbrella", "k_mesh_count",
+      "k_mesh_scan", "k_mesh_write"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -471,6 +472,7 @@ int sm_destroy(sm_reconstruction* r) {
   FreeTransferBuffers(r);
   FreeRenderBuffers(r);
   FreeTrackBuffers(r);
+  FreeMeshBuffers(r);
   for (cudaStream_t st : {r->upload_stream, r->graph_stream})
     if (st) cudaStreamDestroy(st);
   for (cudaEvent_t e : {r->entry_event, r->upload_done, r->graph_exit})
@@ -685,6 +687,18 @@ int sm_track_linearize(sm_reconstruction* r, void* stream, const sm_track_params
   return TrackLinearize(r, static_cast<cudaStream_t>(stream), *tp, level, depth_scaling, live_depth, live_pitch,
                         model_depth, model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system,
                         out_inliers);
+}
+
+void sm_default_mesh_params(sm_mesh_params* p) {
+  p->neighbor_radius_factor = 2.0f;
+  p->max_angle_between_normals_deg = 90.0f;
+  p->max_triangle_angle_deg = 170.0f;
+}
+
+int sm_triangulate(sm_reconstruction* r, void* stream, const sm_mesh_params* p, uint32_t* triangles, uint64_t capacity,
+                   sm_mesh_stats* stats) {
+  if (!r || !p || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_triangulate: null argument");
+  return Triangulate(r, static_cast<cudaStream_t>(stream), *p, triangles, capacity, stats);
 }
 
 int sm_export_vertices(sm_reconstruction* r, void* stream, float* position_buffer, uint8_t* color_buffer) {

@@ -49,6 +49,7 @@ void DestroyFrameGraph(FrameGraph* g);
 struct StreamSession;  // pipeline.cu: an open sm_session_begin
 void DestroySession(StreamSession* s);
 struct TrackState;     // track.cu
+struct MeshCounters;   // mesh.cu
 
 }  // namespace smb
 
@@ -147,6 +148,19 @@ struct sm_reconstruction {
   int track_blocks = 0;
   smb::TrackState* track_state = nullptr;
   smb::TrackState* track_host_state = nullptr;
+  // sm_triangulate scratch (mesh.cu), allocated by the first call and grown to surfels_size(): the k-NN index over
+  // the smooth positions, the umbrellas ([mesh_slots][SM_MESH_MAX_UMBRELLA] pairs) and their lengths, the per-slot
+  // triangle counts (scanned in place into offsets) and the scan's tile sums; the device counters and their
+  // pinned mirror; resident grids.
+  sm_knn_index* mesh_index = nullptr;
+  uint2* mesh_umbrella = nullptr;
+  smb::u32* mesh_umbrella_count = nullptr;
+  smb::u32* mesh_counts = nullptr;
+  smb::u32* mesh_scan_sums = nullptr;
+  smb::u32 mesh_slots = 0;
+  smb::MeshCounters* mesh_counters = nullptr;
+  smb::MeshCounters* mesh_host_counters = nullptr;
+  int mesh_umbrella_blocks = 0, mesh_emit_blocks = 0;
 };
 
 namespace smb {
@@ -184,6 +198,10 @@ int TrackLinearize(sm_reconstruction* r, cudaStream_t stream, const sm_track_par
                    const float* model_normal, size_t model_normal_pitch, const float* model_T_live, double* out_system,
                    uint32_t* out_inliers);
 void FreeTrackBuffers(sm_reconstruction* r);
+// mesh.cu
+int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, uint32_t* triangles,
+                uint64_t capacity, sm_mesh_stats* stats);
+void FreeMeshBuffers(sm_reconstruction* r);
 // pipeline.cu
 int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
               const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats);

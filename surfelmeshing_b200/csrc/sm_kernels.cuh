@@ -29,10 +29,12 @@ enum KernelId {
   KID_EXPORT_VERTICES, KID_MEDIAN_DENSIFY, KID_DELTA_SELECT, KID_VIZ_BUFFERS, KID_DOWNSCALE_DEPTH, KID_DOWNSCALE_COLOR,
   KID_REG_MIRROR, KID_REG_PACK,
   // The kernels below this id have a column in the device timeline (DeviceState::timeline, [frame][column]); the
-  // render kernels (render.cu) and the tracking kernels (track.cu) run outside the frame pipeline and have none.
+  // render kernels (render.cu), the tracking kernels (track.cu) and the meshing kernels (mesh.cu) run outside the
+  // frame pipeline and have none.
   KID_TIMELINE_COUNT,
   KID_RENDER_SPLAT = KID_TIMELINE_COUNT, KID_RENDER_LARGE, KID_RENDER_RESOLVE,
-  KID_TRACK_LIVE_VIEW, KID_TRACK_LINEARIZE, KID_TRACK_SOLVE, KID_COUNT
+  KID_TRACK_LIVE_VIEW, KID_TRACK_LINEARIZE, KID_TRACK_SOLVE,
+  KID_MESH_BOUND, KID_MESH_UMBRELLA, KID_MESH_COUNT, KID_MESH_SCAN, KID_MESH_WRITE, KID_COUNT
 };
 const char* KernelName(int id);
 bool ProfilingEnabled();

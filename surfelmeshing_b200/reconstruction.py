@@ -19,8 +19,10 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import (IntegrateParams, Library, PreprocessParams, RenderParams, SessionStatus, StreamDesc, StreamStats,
-                   TrackParams, TrackResult, TransferStats, TransferToken, VisualizationParams)
+from . import mesh_io
+from ._lib import (IntegrateParams, Library, MeshParams, MeshStats, PreprocessParams, RenderParams, SessionStatus,
+                   StreamDesc, StreamStats, TrackParams, TrackResult, TransferStats, TransferToken,
+                   VisualizationParams)
 
 RENDER_OUTPUTS = ("depth", "color", "normal", "index")
 
@@ -403,6 +405,55 @@ class CUDASurfelReconstruction:
                       lp, lpitch, mp, mpitch, np_, npitch, T.ctypes.data_as(C.c_void_p),
                       system.ctypes.data_as(C.c_void_p), C.byref(inliers))
         return system, int(inliers.value)
+
+    def triangulate(self, params: Optional[MeshParams] = None, stream=None):
+        """sm_triangulate: the current cloud as a triangle mesh over its slots (include/surfel_b200.h gives the
+        rules). Synchronous. Returns (triangles int32 CUDA tensor [T, 3] of slot indices, counter-clockwise about
+        the owner's normal, MeshStats). Tries a capacity of 2 x surfels_size() first and retries once with the
+        reported count."""
+        p = MeshParams.defaults() if params is None else params
+        handle = _stream_handle(stream)
+        stats = MeshStats()
+        capacity = max(2 * self.surfels_size(), 1)
+        for attempt in range(2):
+            out = torch.empty((capacity, 3), dtype=torch.int32, device="cuda")
+            if isinstance(stream, torch.cuda.Stream):
+                out.record_stream(stream)
+            status = self.lib.fn["triangulate"](self._h, handle, C.byref(p), C.c_void_p(out.data_ptr()), capacity,
+                                                C.byref(stats))
+            if status == _lib.SM_ERR_CAPACITY and attempt == 0:
+                capacity = max(int(stats.triangle_count), 1)
+                continue
+            if status != _lib.SM_OK:
+                raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+            return out[:int(stats.triangle_count)], stats
+        raise AssertionError("unreachable")
+
+    def export_vertices_host(self, stream=None):
+        """sm_export_vertices into host arrays: positions [n, 3] float32 (NaN rows for merged slots), colours
+        [n, 3] uint8, n = surfels_size()."""
+        n = self.surfels_size()
+        pos = torch.empty(max(3 * n, 3), dtype=torch.float32, device="cuda")
+        col = torch.empty(max(3 * n, 3), dtype=torch.uint8, device="cuda")
+        if n:
+            self.ExportVertices(stream, pos, col)
+        torch.cuda.synchronize()
+        return pos[:3 * n].cpu().numpy().reshape(n, 3), col[:3 * n].cpu().numpy().reshape(n, 3)
+
+    def save_mesh_obj(self, path, params: Optional[MeshParams] = None, stream=None) -> MeshStats:
+        """The reference's SaveMeshAsOBJ (main.cc:128-175): the non-merged slots in slot order with their colour,
+        and the triangles of triangulate() over them (1-based, remapped to that order)."""
+        tri, stats = self.triangulate(params, stream)
+        positions, colors = self.export_vertices_host(stream)
+        mesh_io.write_obj(path, positions, colors, tri.cpu().numpy())
+        return stats
+
+    def save_point_cloud_ply(self, path, stream=None) -> int:
+        """The reference's SavePointCloudAsPLY (main.cc:180-203): position and normal of every non-merged slot,
+        with its real colour (the reference writes white there). Returns the number of points written."""
+        positions, colors = self.export_vertices_host(stream)
+        rows, n, _ = self.dump_state(stream)
+        return mesh_io.write_ply(path, positions, rows[8:11].T, colors)
 
     def ExportVertices(self, stream, position_buffer: torch.Tensor, color_buffer: torch.Tensor):
         """cuda_surfel_reconstruction.cc:405-410."""
