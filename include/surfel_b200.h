@@ -520,6 +520,66 @@ void sm_default_mesh_params(sm_mesh_params* p);
 int sm_triangulate(sm_reconstruction* r, void* stream, const sm_mesh_params* p,
                    uint32_t* triangles /* device, 3 x capacity */, uint64_t capacity, sm_mesh_stats* stats);
 
+/* ---- keeping the mesh up to date (DESIGN.md section 1 row f10, section 5.8) ----------------------------------
+ * The reference's meshing thread remeshes only the surfels that changed (APP/surfel_meshing.cc:189-288).
+ * sm_mesh_update keeps a persistent mesh in the handle and brings it up to date with the current cloud, rebuilding
+ * only the umbrellas a change can reach. Afterwards:
+ *  1. Full mesh. sm_mesh_read(SM_MESH_ALL) gives exactly what sm_triangulate with the same params returns on this
+ *     state (triangles, their order, and stats->mesh == its four stats), after any sequence of calls between
+ *     updates (sm_integrate, sm_regularize, session pushes, sm_stream_run, sm_load_state, sm_reset).
+ *  2. Delta. As sets of ordered triples (o, x, y): removed = previous mesh - new mesh, added = new - previous,
+ *     where the previous mesh is that of this handle's last completed update (empty before the first one, and
+ *     after an update that failed). Each list is ordered by owner slot, then by that owner's umbrella order (the
+ *     old umbrella for removed, the new one for added).
+ *  3. Read-only: only reads the surfel state (apart from the smooth-position mirror into rows 3-5 that
+ *     sm_triangulate also writes).
+ *  4. Independent of sm_triangulate, which has buffers of its own (both rebuild the one k-NN index object).
+ * What is recomputed, step by step (n = surfels_size(), n_prev = surfels_size() at the previous update; a slot's
+ * inputs are the bits of its smooth x y z, radius^2 and normal x y z, kept as a snapshot of 28 bytes per slot):
+ *  a. C (changed): the slots that are or were present and whose inputs differ from the snapshot; every present
+ *     slot of [n_prev, n) is in C. C does not depend on what caused the change.
+ *  b. A (umbrellas rebuilt): C, plus every present slot i whose ball holds the old position (of a slot present
+ *     then) or the new position (of a slot present now) of some slot of C, by rule 1's own fp32 test
+ *     ((dx*dx + dy*dy) + dz*dz) <= r_i^2 * f2. A slot outside A has the same ball with the same slots inside it,
+ *     so the same umbrella.
+ *  c. R (owners rechecked): A, plus every slot whose umbrella names a slot of A in either place of a pair. A slot
+ *     outside R owns the same triangles and has the same share of the stats (meshed, boundary edges of its
+ *     triangles, overflow), all of which read only its umbrella, the umbrellas it names and their inputs.
+ *  d. Everything: every slot is in A and in R when the params differ from the previous update's, when n < n_prev
+ *     (after sm_reset), before the first update, after a failed one, and when C holds more than 1/16 of the slots
+ *     (marking A would then cost more than it saves). Slots of [n, n_prev) then own nothing.
+ *  e. The umbrellas of A are rebuilt from a list of A, or by a sweep over all slots when A holds more than three
+ *     quarters of them (stats->full_sweep); both give the same umbrellas. The stats are kept as sums of per-slot
+ *     shares.
+ * stats: mesh = the whole mesh after the update; slots_changed = |C|, umbrellas_rebuilt = |A| (n when everything
+ * is rebuilt), owners_rechecked = |R|, triangles_added / triangles_removed = the lengths of the two lists.
+ * The call synchronises `stream` three times (surfels_size(), the largest radius and |C|, the mesh and delta
+ * sizes), plus once, with cudaFree's device synchronisations, in a call whose buffers grow (by x 1.5). Memory (allocated by the first update, grown with surfels_size() and the mesh, freed by sm_destroy;
+ * sm_create allocates nothing for meshing): 173 bytes per slot kept between updates (snapshot 28, umbrella
+ * SM_MESH_MAX_UMBRELLA x 8 + 4, 5 bytes of per-slot stats, 8 of offsets), 46 bytes per slot of scratch, 24 bytes per
+ * triangle (the previous and the current mesh), 12 per added or removed triangle, and an index over the changed
+ * positions. SM_ERR_INVALID_ARGUMENT, with no launch, for NULL arguments and for params sm_triangulate rejects.
+ *
+ * sm_mesh_read copies one of the lists of the last completed update into `triangles` (DEVICE, 3 x capacity
+ * uint32; may be NULL with capacity 0: a count query) with work enqueued on `stream`, and sets *count. If capacity
+ * < *count it returns SM_ERR_CAPACITY and writes nothing; SM_ERR_INVALID_ARGUMENT for an unknown `which`, NULL
+ * count, or when no update has completed on this handle. */
+typedef struct sm_mesh_update_stats {
+  sm_mesh_stats mesh;            /* the whole mesh after the update (== sm_triangulate's stats) */
+  uint64_t slots_changed;        /* |C| */
+  uint64_t umbrellas_rebuilt;    /* |A| */
+  uint64_t owners_rechecked;     /* |R| */
+  uint64_t triangles_added, triangles_removed;
+  int32_t full_sweep;            /* 1 when the umbrellas were rebuilt by the plain sweep */
+  int32_t reserved;
+} sm_mesh_update_stats;
+int sm_mesh_update(sm_reconstruction* r, void* stream, const sm_mesh_params* p, sm_mesh_update_stats* stats);
+#define SM_MESH_ALL 0
+#define SM_MESH_ADDED 1
+#define SM_MESH_REMOVED 2
+int sm_mesh_read(sm_reconstruction* r, void* stream, int32_t which, uint32_t* triangles /* device, 3 x capacity */,
+                 uint64_t capacity, uint64_t* count);
+
 /* ---- radius-limited k-nearest-neighbour queries for the meshing thread (SURVEY section 8 f4) ----
  * Replaces CompressedOctree::FindNearestSurfelsWithinRadius<include_completed_surfels, include_free_surfels>
  * (octree.h:471, octree.cc:313-470; callers surfel_meshing.cc:421 <false, true> and :821 <true, false>) for a BATCH of
@@ -668,7 +728,7 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * work waits for them: the hand-off calls (sm_transfer_all_to_cpu, sm_transfer_delta_to_cpu,
  * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
  * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_track_frame, sm_track_linearize,
- * sm_triangulate, sm_surfel_count / sm_surfels_size) and
+ * sm_mesh_update, sm_mesh_read, sm_triangulate, sm_surfel_count / sm_surfels_size) and
  * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
  * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which
  * that frame's Integrate() applies in the next step. The device merge counter then already includes them, so

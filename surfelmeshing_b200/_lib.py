@@ -162,7 +162,16 @@ class MeshStats(C.Structure):
                 ("umbrella_overflows", C.c_uint64)]
 
 
+class MeshUpdateStats(C.Structure):
+    """sm_mesh_update_stats: the whole mesh after the update, |C|, |A|, |R|, the delta sizes, and whether the
+    umbrellas were rebuilt by the plain sweep."""
+    _fields_ = [("mesh", MeshStats), ("slots_changed", C.c_uint64), ("umbrellas_rebuilt", C.c_uint64),
+                ("owners_rechecked", C.c_uint64), ("triangles_added", C.c_uint64),
+                ("triangles_removed", C.c_uint64), ("full_sweep", C.c_int32), ("reserved", C.c_int32)]
+
+
 MESH_MAX_UMBRELLA = 16
+MESH_ALL, MESH_ADDED, MESH_REMOVED = 0, 1, 2
 
 _P = C.c_void_p
 _SZ = C.c_size_t
@@ -238,6 +247,8 @@ _PRODUCT_ONLY = {
                                   C.POINTER(_U32)]),
     "default_mesh_params": (None, [C.POINTER(MeshParams)]),
     "triangulate": (C.c_int, [_P, _P, C.POINTER(MeshParams), _P, C.c_uint64, C.POINTER(MeshStats)]),
+    "mesh_update": (C.c_int, [_P, _P, C.POINTER(MeshParams), C.POINTER(MeshUpdateStats)]),
+    "mesh_read": (C.c_int, [_P, _P, _I, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

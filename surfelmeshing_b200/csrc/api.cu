@@ -128,7 +128,8 @@ const char* KernelName(int id) {
       "k_export_vertices", "k_median_densify", "k_delta_select", "k_viz_buffers", "k_downscale_depth_median",
       "k_downscale_color", "k_reg_mirror", "k_reg_pack", "k_render_splat", "k_render_large", "k_render_resolve",
       "k_track_live_view", "k_track_linearize", "k_track_solve", "k_mesh_bound", "k_mesh_umbrella", "k_mesh_count",
-      "k_mesh_scan", "k_mesh_write"};
+      "k_mesh_scan", "k_mesh_write", "k_mesh_changes", "k_mesh_mark", "k_mesh_owners", "k_mesh_umbrella_update",
+      "k_mesh_recheck", "k_mesh_recheck_write"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -699,6 +700,17 @@ int sm_triangulate(sm_reconstruction* r, void* stream, const sm_mesh_params* p, 
                    sm_mesh_stats* stats) {
   if (!r || !p || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_triangulate: null argument");
   return Triangulate(r, static_cast<cudaStream_t>(stream), *p, triangles, capacity, stats);
+}
+
+int sm_mesh_update(sm_reconstruction* r, void* stream, const sm_mesh_params* p, sm_mesh_update_stats* stats) {
+  if (!r || !p || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_update: null argument");
+  return MeshUpdate(r, static_cast<cudaStream_t>(stream), *p, stats);
+}
+
+int sm_mesh_read(sm_reconstruction* r, void* stream, int32_t which, uint32_t* triangles, uint64_t capacity,
+                 uint64_t* count) {
+  if (!r || !count) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_read: null argument");
+  return MeshRead(r, static_cast<cudaStream_t>(stream), which, triangles, capacity, count);
 }
 
 int sm_export_vertices(sm_reconstruction* r, void* stream, float* position_buffer, uint8_t* color_buffer) {

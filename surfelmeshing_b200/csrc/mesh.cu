@@ -14,9 +14,12 @@
 //   (the three-launch exclusive scan of knn.cu over the counts)
 //   k_mesh_write     one thread per slot: writes its triangles at its scanned offset.
 
+#include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstring>
 #include <string>
+#include <vector>
 
 #include "sm_handle.cuh"
 #include "sm_knn.cuh"
@@ -107,19 +110,23 @@ struct Candidate {
 
 __device__ __forceinline__ float pick(int reg, float v0, float v1) { return reg ? v1 : v0; }
 
-__global__ void __launch_bounds__(kUmbrellaBlock) k_mesh_umbrella(MeshArgs a) {
-  __shared__ unsigned long long s_stage[kUmbrellaBlock / 32][kMaxResults];
-  const int lane = threadIdx.x & 31;
-  const u32 warps_per_grid = gridDim.x * (kUmbrellaBlock / 32);
-  for (u32 i = blockIdx.x * (kUmbrellaBlock / 32) + (threadIdx.x >> 5); i < a.n; i += warps_per_grid) {
+// Rules 1-3 for slot i, by one warp (`stage`: the warp's 64-key row in shared memory): writes U(i) and its length,
+// 0 when U(i) overflowed. An overflow is counted in a.counters (sm_triangulate) or, with kSlotFlag, flagged in
+// overflow[i], which is cleared otherwise (sm_mesh_update).
+template <bool kSlotFlag>
+__device__ __forceinline__ void build_umbrella(const MeshArgs& a, u32 i, int lane, unsigned long long* stage, u8* overflow) {
+  {
     const float r2 = SM_S(SM_ROW_RADIUS_SQUARED, i);
     float3 ni;
     if (!(r2 > 0.f) || !unit_normal(a, i, &ni)) {   // warp-uniform
-      if (lane == 0) a.umbrella_count[i] = 0;
-      continue;
+      if (lane == 0) {
+        a.umbrella_count[i] = 0;
+        if (kSlotFlag) overflow[i] = 0;
+      }
+      return;
     }
     const float3 pi = position(a, i);
-    QueryState s{{kEmptyKey, kEmptyKey}, 0, true, kEmptyKey, s_stage[threadIdx.x >> 5]};
+    QueryState s{{kEmptyKey, kEmptyKey}, 0, true, kEmptyKey, stage};
     warp_query(a.q, s, pi.x, pi.y, pi.z, fmul(r2, a.radius_factor_squared), lane);
     const int found = min(s.count, kMaxResults);
 
@@ -236,15 +243,28 @@ __global__ void __launch_bounds__(kUmbrellaBlock) k_mesh_umbrella(MeshArgs a) {
     if (total > kUmbrella) {
       if (lane == 0) {
         a.umbrella_count[i] = 0;
-        atomicAdd(&a.counters->umbrella_overflows, 1ull);
+        if (kSlotFlag) overflow[i] = 1;
+        else atomicAdd(&a.counters->umbrella_overflows, 1ull);
       }
-      continue;
+      return;
     }
     const unsigned below = (1u << lane) - 1u;
     uint2* row = a.umbrella + static_cast<size_t>(i) * kUmbrella;
     if (pair0) row[__popc(b0 & below)] = make_uint2(c[0].index, next[0]);
     if (pair1) row[__popc(b0) + __popc(b1 & below)] = make_uint2(c[1].index, next[1]);
-    if (lane == 0) a.umbrella_count[i] = total;
+    if (lane == 0) {
+      a.umbrella_count[i] = total;
+      if (kSlotFlag) overflow[i] = 0;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kUmbrellaBlock) k_mesh_umbrella(MeshArgs a) {
+  __shared__ unsigned long long s_stage[kUmbrellaBlock / 32][kMaxResults];
+  const int lane = threadIdx.x & 31;
+  const u32 warps_per_grid = gridDim.x * (kUmbrellaBlock / 32);
+  for (u32 i = blockIdx.x * (kUmbrellaBlock / 32) + (threadIdx.x >> 5); i < a.n; i += warps_per_grid) {
+    build_umbrella<false>(a, i, lane, s_stage[threadIdx.x >> 5], nullptr);
   }
 }
 
@@ -338,6 +358,292 @@ __global__ void __launch_bounds__(kEmitBlock) k_mesh_write(MeshArgs a) {
   }
 }
 
+// ---- sm_mesh_update (DESIGN.md section 5.8): the persistent mesh, brought up to date from what changed ----------
+
+constexpr int kSnapshotWords = 7;   // bits of smooth x y z, radius^2, normal x y z at the previous update
+// The rebuild walks the whole cloud, as k_mesh_umbrella does, once A holds more than this share of surfels_size().
+// On an H100 (tools/mesh_update_probe.py, DESIGN.md 5.8) the list costs ~24.5 us per 1 000 umbrellas and the sweep
+// ~19.2 us per 1 000 slots of the final bench cloud: they cross at |A| / n ~ 0.78.
+constexpr u32 kSweepNumerator = 3, kSweepDenominator = 4;
+// Every slot is in A and R, without marking, once |C| exceeds this share of surfels_size(). In a live session the
+// regularisation window changes 28-66 % of the slots per frame, far past it; marking then cost 2-4 ms on top of an
+// umbrella rebuild of most slots. Below it the marking costs <= ~0.5 ms on the bench cloud (DESIGN.md 5.8).
+constexpr u32 kMarkNumerator = 1, kMarkDenominator = 16;
+
+struct UpdateCounters {
+  // sums of the per-slot words over the current mesh, kept from call to call
+  unsigned long long vertices_meshed, boundary_edges, umbrella_overflows;
+  // per call (cleared at its start)
+  MeshCounters bound;   // k_mesh_bound's largest radius^2
+  u32 changed, rebuilt, rechecked, full_sweep;
+  u32 triangle_count, added, removed, unused;
+};
+
+struct UpdateArgs {
+  u32 n_prev;                  // surfels_size() at the previous update (0 before the first)
+  u32 n_max;                   // max(n, n_prev)
+  int everything;              // every slot is in A and in R
+  u32* snapshot;               // [slots][kSnapshotWords]
+  u8* overflow;                // [slots] U(i) overflowed
+  u32* word;                   // [slots] the slot's share of the stats: boundary edges | meshed << 16 | overflow << 17
+  u8* in_a;                    // [slots]
+  u8* in_r;                    // [slots]
+  u32* rebuild_list;           // [slots] the slots of A, in no particular order
+  float* points;               // [4][point_stride]: x, y, z, 1 (present) or -1 of the old and new position of C's slots
+  u32 point_stride;
+  QueryArgs changed;           // the index over `points`
+  const u32* old_offsets;      // [n_prev + 1] the previous mesh, by owner
+  const uint3* old_triangles;
+  u32* new_offsets;            // [n_max + 1] owned triangles, then (scanned) offsets
+  u32* added_offsets;          // [n_max + 1]
+  u32* removed_offsets;        // [n_max + 1]
+  uint3* new_triangles;
+  uint3* added;
+  uint3* removed;
+  UpdateCounters* counters;
+};
+
+// The lane's place in a warp-aggregated append to *counter.
+__device__ __forceinline__ u32 warp_append(bool take, u32* counter, int lane) {
+  const unsigned m = __ballot_sync(kFullMask, take);
+  u32 base = 0;
+  if (lane == 0 && m) base = atomicAdd(counter, static_cast<u32>(__popc(m)));
+  return __shfl_sync(kFullMask, base, 0) + __popc(m & ((1u << lane) - 1u));
+}
+
+// C: a slot that is or was present and whose inputs differ from the snapshot (every slot of [n_prev, n) differs).
+// Refreshes the snapshot, flags C in in_a and appends the old and new position of each slot of C to `points`.
+// A slot of [n_prev, n) that is not present gets an empty umbrella and a zero share of the stats here: neither
+// the rebuild nor the recheck visits it.
+__global__ void __launch_bounds__(kEmitBlock) k_mesh_changes(MeshArgs a, UpdateArgs u) {
+  const int lane = threadIdx.x & 31;
+  const int rows[kSnapshotWords] = {SM_ROW_SMOOTH_X, SM_ROW_SMOOTH_Y, SM_ROW_SMOOTH_Z, SM_ROW_RADIUS_SQUARED,
+                                    SM_ROW_NORMAL_X, SM_ROW_NORMAL_Y, SM_ROW_NORMAL_Z};
+  for (u32 base = blockIdx.x * blockDim.x; base < u.n_max; base += gridDim.x * blockDim.x) {
+    const u32 i = base + threadIdx.x;
+    bool changed = false, was = false, is = false;
+    u32 cur[kSnapshotWords] = {}, old[kSnapshotWords] = {};
+    if (i < u.n_max) {
+      const bool now = i < a.n, then = i < u.n_prev;
+      u32* snap = u.snapshot + static_cast<size_t>(i) * kSnapshotWords;
+#pragma unroll
+      for (int k = 0; k < kSnapshotWords; ++k) {
+        if (now) cur[k] = __float_as_uint(SM_S(rows[k], i));
+        if (then) old[k] = snap[k];
+      }
+      bool differ = !then || !now;
+#pragma unroll
+      for (int k = 0; k < kSnapshotWords; ++k) differ = differ || cur[k] != old[k];
+      was = then && __uint_as_float(old[3]) > 0.f;
+      is = now && __uint_as_float(cur[3]) > 0.f;
+      changed = (was || is) && differ;
+      if (now && differ) {
+#pragma unroll
+        for (int k = 0; k < kSnapshotWords; ++k) snap[k] = cur[k];
+      }
+      if (now && !then && !is) {
+        a.umbrella_count[i] = 0;
+        u.overflow[i] = 0;
+        u.word[i] = 0;
+      }
+      if (now) u.in_a[i] = changed;
+    }
+    const u32 slot = warp_append(changed, &u.counters->changed, lane);
+    if (changed && !u.everything) {
+      const size_t st = u.point_stride;
+      float* pt = u.points + 2 * static_cast<size_t>(slot);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        pt[k * st] = __uint_as_float(old[k]);
+        pt[k * st + 1] = __uint_as_float(cur[k]);
+      }
+      pt[3 * st] = was ? 1.f : -1.f;
+      pt[3 * st + 1] = is ? 1.f : -1.f;
+    }
+  }
+}
+
+// Whether some record of the index lies within radius_squared of p, by the test and the cell walk of warp_query.
+__device__ __forceinline__ bool near_record(const QueryArgs& q, float px, float py, float pz, float radius_squared) {
+  auto within = [&](const float4 record) {
+    const float dx = fsub(record.x, px), dy = fsub(record.y, py), dz = fsub(record.z, pz);
+    return fadd(fadd(fmul(dx, dx), fmul(dy, dy)), fmul(dz, dz)) <= radius_squared;
+  };
+  const float reach = __fmul_ru(__fsqrt_ru(radius_squared), 1.00001f);
+  const int x0 = cell_of(__fsub_rd(px, reach), q.inverse_cell_size), x1 = cell_of(__fadd_ru(px, reach), q.inverse_cell_size);
+  const int y0 = cell_of(__fsub_rd(py, reach), q.inverse_cell_size), y1 = cell_of(__fadd_ru(py, reach), q.inverse_cell_size);
+  const int z0 = cell_of(__fsub_rd(pz, reach), q.inverse_cell_size), z1 = cell_of(__fadd_ru(pz, reach), q.inverse_cell_size);
+  const long long nx = static_cast<long long>(x1) - x0 + 1, ny = static_cast<long long>(y1) - y0 + 1,
+                  nz = static_cast<long long>(z1) - z0 + 1;
+  if (nx > kMaxCellsPerQuery || ny > kMaxCellsPerQuery || nz > kMaxCellsPerQuery || nx * ny * nz > kMaxCellsPerQuery ||
+      x1 == INT_MAX || y1 == INT_MAX || z1 == INT_MAX) {
+    const u32 end = q.bucket_start[q.mask + 1];
+    for (u32 e = 0; e < end; ++e)
+      if (within(q.records[e])) return true;
+    return false;
+  }
+  for (int cz = z0; cz <= z1; ++cz) {
+    for (int cy = y0; cy <= y1; ++cy) {
+      for (int cx = x0; cx <= x1; ++cx) {
+        const u32 bucket = bucket_of(cx, cy, cz, q.mask);
+        for (u32 e = q.bucket_start[bucket]; e < q.bucket_start[bucket + 1]; ++e) {
+          const float4 record = q.records[e];
+          if (cell_of(record.x, q.inverse_cell_size) == cx && cell_of(record.y, q.inverse_cell_size) == cy &&
+              cell_of(record.z, q.inverse_cell_size) == cz && within(record))
+            return true;
+        }
+      }
+    }
+  }
+  return false;
+}
+
+// A: C, plus every present slot whose ball (the query of rule 1) holds an old or new position of a slot of C.
+__global__ void __launch_bounds__(kEmitBlock) k_mesh_mark(MeshArgs a, UpdateArgs u) {
+  const int lane = threadIdx.x & 31;
+  for (u32 base = blockIdx.x * blockDim.x; base < a.n; base += gridDim.x * blockDim.x) {
+    const u32 i = base + threadIdx.x;
+    bool in = false;
+    if (i < a.n) {
+      in = u.in_a[i] != 0;
+      const float r2 = SM_S(SM_ROW_RADIUS_SQUARED, i);
+      if (!in && r2 > 0.f) {
+        const float3 p = position(a, i);
+        in = near_record(u.changed, p.x, p.y, p.z, fmul(r2, a.radius_factor_squared));
+        if (in) u.in_a[i] = 1;
+      }
+    }
+    const u32 slot = warp_append(in, &u.counters->rebuilt, lane);
+    if (in) u.rebuild_list[slot] = i;
+  }
+}
+
+// R: A, plus every slot whose umbrella names a slot of A (a slot outside A has the same umbrella before and after).
+__global__ void __launch_bounds__(kEmitBlock) k_mesh_owners(MeshArgs a, UpdateArgs u) {
+  const int lane = threadIdx.x & 31;
+  for (u32 base = blockIdx.x * blockDim.x; base < u.n_max; base += gridDim.x * blockDim.x) {
+    const u32 o = base + threadIdx.x;
+    bool in = false;
+    if (o < u.n_max) {
+      in = u.everything || u.in_a[o];
+      if (!in) {
+        const u32 count = a.umbrella_count[o];
+        const uint2* row = a.umbrella + static_cast<size_t>(o) * kUmbrella;
+        for (u32 t = 0; t < count && !in; ++t) {
+          const uint2 e = row[t];
+          in = u.in_a[e.x] || u.in_a[e.y];
+        }
+      }
+      u.in_r[o] = in;
+    }
+    const unsigned m = __ballot_sync(kFullMask, in);
+    if (lane == 0 && m) atomicAdd(&u.counters->rechecked, static_cast<u32>(__popc(m)));
+  }
+}
+
+// The umbrellas of A from the list, or of every slot by the sweep once A is a large share of the cloud.
+__global__ void __launch_bounds__(kUmbrellaBlock) k_mesh_umbrella_update(MeshArgs a, UpdateArgs u) {
+  __shared__ unsigned long long s_stage[kUmbrellaBlock / 32][kMaxResults];
+  const int lane = threadIdx.x & 31;
+  const u32 listed = u.counters->rebuilt;
+  const bool sweep = u.everything || static_cast<unsigned long long>(listed) * kSweepDenominator >
+                                         static_cast<unsigned long long>(a.n) * kSweepNumerator;
+  if (blockIdx.x == 0 && threadIdx.x == 0) u.counters->full_sweep = sweep;
+  const u32 items = sweep ? a.n : listed;
+  const u32 warps_per_grid = gridDim.x * (kUmbrellaBlock / 32);
+  for (u32 k = blockIdx.x * (kUmbrellaBlock / 32) + (threadIdx.x >> 5); k < items; k += warps_per_grid)
+    build_umbrella<true>(a, sweep ? k : u.rebuild_list[k], lane, s_stage[threadIdx.x >> 5], u.overflow);
+}
+
+// (o, t.y, t.z) of the previous mesh is in the new one.
+__device__ __forceinline__ bool in_new_mesh(const MeshArgs& a, u32 o, uint3 t) {
+  return o < a.n && successor(a, o, t.y) == t.z && triangle_ok(a, o, t.y, t.z);
+}
+
+// (o, x, y) is among the previous mesh's triangles of o, old_triangles[begin, end).
+__device__ __forceinline__ bool in_old_mesh(const UpdateArgs& u, u32 begin, u32 end, u32 x, u32 y) {
+  for (u32 t = begin; t < end; ++t) {
+    const uint3 v = u.old_triangles[t];
+    if (v.y == x && v.z == y) return true;
+  }
+  return false;
+}
+
+// One thread per owner o < n_max. Outside R, o keeps its triangles (counted, then copied). In R, the first pass
+// counts o's new triangles, its added and removed ones and its share of the stats exactly as k_mesh_count does,
+// and adds the change of that share to the totals; the second writes them at the scanned offsets.
+template <bool kWrite>
+__global__ void __launch_bounds__(kEmitBlock) k_mesh_recheck(MeshArgs a, UpdateArgs u) {
+  const int lane = threadIdx.x & 31;
+  for (u32 base = blockIdx.x * blockDim.x; base < u.n_max; base += gridDim.x * blockDim.x) {
+    const u32 o = base + threadIdx.x;
+    int d_meshed = 0, d_boundary = 0, d_overflow = 0;
+    if (o < u.n_max) {
+      const u32 begin = o < u.n_prev ? u.old_offsets[o] : 0u, end = o < u.n_prev ? u.old_offsets[o + 1] : 0u;
+      const u32 count = o < a.n ? a.umbrella_count[o] : 0u;
+      const uint2* row = a.umbrella + static_cast<size_t>(o) * kUmbrella;
+      if (!u.in_r[o]) {
+        if (!kWrite) {
+          u.new_offsets[o] = end - begin;
+          u.added_offsets[o] = 0;
+          u.removed_offsets[o] = 0;
+        } else {
+          u32 out = u.new_offsets[o];
+          for (u32 t = begin; t < end; ++t) u.new_triangles[out++] = u.old_triangles[t];
+        }
+      } else if (!kWrite) {
+        u32 owned = 0, boundary = 0, added = 0, removed = 0;
+        bool meshed = false;
+        for (u32 t = 0; t < count; ++t) {
+          const uint2 e = row[t];
+          if (!triangle_ok(a, o, e.x, e.y)) continue;
+          meshed = true;
+          if (o < e.x && o < e.y) {
+            ++owned;
+            if (!in_old_mesh(u, begin, end, e.x, e.y)) ++added;
+          }
+          const u32 w = successor(a, e.x, o);
+          if (w == kNone || !triangle_ok(a, e.x, o, w)) ++boundary;
+        }
+        for (u32 t = begin; t < end; ++t) removed += in_new_mesh(a, o, u.old_triangles[t]) ? 0u : 1u;
+        const u32 word = boundary | (meshed ? 1u << 16 : 0u) | (o < a.n && u.overflow[o] ? 1u << 17 : 0u);
+        const u32 before = o < u.n_prev ? u.word[o] : 0u;
+        d_meshed = static_cast<int>((word >> 16) & 1u) - static_cast<int>((before >> 16) & 1u);
+        d_boundary = static_cast<int>(word & 0xFFFFu) - static_cast<int>(before & 0xFFFFu);
+        d_overflow = static_cast<int>(word >> 17) - static_cast<int>(before >> 17);
+        u.word[o] = word;
+        u.new_offsets[o] = owned;
+        u.added_offsets[o] = added;
+        u.removed_offsets[o] = removed;
+      } else {
+        u32 out = u.new_offsets[o], add = u.added_offsets[o], rem = u.removed_offsets[o];
+        for (u32 t = 0; t < count; ++t) {
+          const uint2 e = row[t];
+          if (!(o < e.x && o < e.y) || !triangle_ok(a, o, e.x, e.y)) continue;
+          const uint3 tri = make_uint3(o, e.x, e.y);
+          u.new_triangles[out++] = tri;
+          if (!in_old_mesh(u, begin, end, e.x, e.y)) u.added[add++] = tri;
+        }
+        for (u32 t = begin; t < end; ++t) {
+          const uint3 v = u.old_triangles[t];
+          if (!in_new_mesh(a, o, v)) u.removed[rem++] = v;
+        }
+      }
+    }
+    if (!kWrite) {
+      d_meshed = __reduce_add_sync(kFullMask, d_meshed);
+      d_boundary = __reduce_add_sync(kFullMask, d_boundary);
+      d_overflow = __reduce_add_sync(kFullMask, d_overflow);
+      if (lane == 0) {
+        // two's complement: adding the sign-extended difference subtracts modulo 2^64
+        if (d_meshed) atomicAdd(&u.counters->vertices_meshed, static_cast<unsigned long long>(static_cast<long long>(d_meshed)));
+        if (d_boundary) atomicAdd(&u.counters->boundary_edges, static_cast<unsigned long long>(static_cast<long long>(d_boundary)));
+        if (d_overflow) atomicAdd(&u.counters->umbrella_overflows, static_cast<unsigned long long>(static_cast<long long>(d_overflow)));
+      }
+    }
+  }
+}
+
 void FreeMeshScratch(sm_reconstruction* r) {
   KnnDestroy(r->mesh_index);
   cudaFree(r->mesh_umbrella);
@@ -374,26 +680,30 @@ int EnsureMeshScratch(sm_reconstruction* r, u32 n) {
   return SM_OK;
 }
 
-}  // namespace
 
-void FreeMeshBuffers(sm_reconstruction* r) {
-  FreeMeshScratch(r);
-  cudaFree(r->mesh_counters);
-  if (r->mesh_host_counters) cudaFreeHost(r->mesh_host_counters);
-  r->mesh_counters = nullptr;
-  r->mesh_host_counters = nullptr;
-}
-
-int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, uint32_t* triangles,
-                uint64_t capacity, sm_mesh_stats* stats) {
-  auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_triangulate: ") + why).c_str()); };
+// SM_OK, or SM_ERR_INVALID_ARGUMENT for parameters outside their documented ranges.
+int CheckMeshParams(const sm_mesh_params& p, const char* who) {
+  auto bad = [who](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string(who) + ": " + why).c_str()); };
   const float f = p.neighbor_radius_factor;
   const float f2 = f * f;
   if (!std::isfinite(f) || !(f > 0.f) || !std::isfinite(f2)) return bad("neighbor_radius_factor must be finite and > 0");
   auto angle_ok = [](float deg) { return std::isfinite(deg) && deg > 0.f && deg <= 180.f; };
   if (!angle_ok(p.max_angle_between_normals_deg) || !angle_ok(p.max_triangle_angle_deg))
     return bad("angles must be in (0, 180] degrees");
-  if (!triangles && capacity > 0) return bad("triangles is NULL with a capacity > 0");
+  return SM_OK;
+}
+
+float CosDegrees(float deg) { return static_cast<float>(std::cos(static_cast<double>(deg) * (M_PI / 180.0))); }
+
+}  // namespace
+
+int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, uint32_t* triangles,
+                uint64_t capacity, sm_mesh_stats* stats) {
+  const int checked = CheckMeshParams(p, "sm_triangulate");
+  if (checked != SM_OK) return checked;
+  if (!triangles && capacity > 0)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_triangulate: triangles is NULL with a capacity > 0");
+  const float f2 = p.neighbor_radius_factor * p.neighbor_radius_factor;
   *stats = sm_mesh_stats{};
   r->last_stream = stream;
   int status = FetchCounters(r, stream);
@@ -408,8 +718,8 @@ int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params&
   a.rows = r->d.surfels;
   a.stride = r->d.stride;
   a.radius_factor_squared = f2;
-  a.cos_normal = static_cast<float>(std::cos(static_cast<double>(p.max_angle_between_normals_deg) * (M_PI / 180.0)));
-  a.cos_triangle = static_cast<float>(std::cos(static_cast<double>(p.max_triangle_angle_deg) * (M_PI / 180.0)));
+  a.cos_normal = CosDegrees(p.max_angle_between_normals_deg);
+  a.cos_triangle = CosDegrees(p.max_triangle_angle_deg);
   a.umbrella = r->mesh_umbrella;
   a.umbrella_count = r->mesh_umbrella_count;
   a.counts = r->mesh_counts;
@@ -470,6 +780,367 @@ int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params&
     LaunchKernel(k_mesh_write, dim3(emit_blocks), dim3(kEmitBlock), 0, stream, a);
   }
   return CheckLaunch("triangulate");
+}
+
+// The persistent mesh of sm_mesh_update. Per-slot arrays hold `slots` entries and grow (keeping what the previous
+// update left) with surfels_size(); the triangle arrays grow with the mesh and its deltas.
+struct MeshLive {
+  bool valid = false;          // an update completed and everything below describes its mesh
+  u32 n_prev = 0;              // surfels_size() at that update
+  sm_mesh_params params{};
+  int current = 0;             // which of offsets[] / triangles[] holds that mesh
+  u64 triangle_count = 0, added_count = 0, removed_count = 0;
+  u32 slots = 0;
+  // kept from one update to the next
+  u32* snapshot = nullptr;                  // [slots][kSnapshotWords]
+  uint2* umbrella = nullptr;                // [slots][SM_MESH_MAX_UMBRELLA]
+  u32* umbrella_count = nullptr;            // [slots]
+  u8* overflow = nullptr;                   // [slots]
+  u32* word = nullptr;                      // [slots]
+  u32* offsets[2] = {nullptr, nullptr};     // [slots + 1]
+  uint3* triangles[2] = {nullptr, nullptr};
+  u64 triangle_capacity[2] = {0, 0};
+  uint3* added = nullptr; u64 added_capacity = 0;
+  uint3* removed = nullptr; u64 removed_capacity = 0;
+  UpdateCounters* counters = nullptr;
+  UpdateCounters* host_counters = nullptr;  // pinned
+  // scratch of one update
+  u8* in_a = nullptr;
+  u8* in_r = nullptr;
+  u32* rebuild_list = nullptr;
+  u32* added_offsets = nullptr;             // [slots + 1]
+  u32* removed_offsets = nullptr;           // [slots + 1]
+  u32* scan_sums = nullptr;
+  float* points = nullptr;                  // [4][2 slots]
+  sm_knn_index* changed_index = nullptr;
+  int umbrella_blocks = 0, emit_blocks = 0;
+};
+
+namespace {
+
+void FreeLive(MeshLive* L) {
+  if (!L) return;
+  for (void* q : {static_cast<void*>(L->snapshot), static_cast<void*>(L->umbrella), static_cast<void*>(L->umbrella_count),
+                  static_cast<void*>(L->overflow), static_cast<void*>(L->word), static_cast<void*>(L->offsets[0]),
+                  static_cast<void*>(L->offsets[1]), static_cast<void*>(L->triangles[0]),
+                  static_cast<void*>(L->triangles[1]), static_cast<void*>(L->added), static_cast<void*>(L->removed),
+                  static_cast<void*>(L->counters), static_cast<void*>(L->in_a), static_cast<void*>(L->in_r),
+                  static_cast<void*>(L->rebuild_list), static_cast<void*>(L->added_offsets),
+                  static_cast<void*>(L->removed_offsets), static_cast<void*>(L->scan_sums), static_cast<void*>(L->points)})
+    cudaFree(q);
+  if (L->host_counters) cudaFreeHost(L->host_counters);
+  KnnDestroy(L->changed_index);
+  delete L;
+}
+
+// Grows a set of buffers behind one synchronisation: each new buffer gets the first `keep` elements of the old one
+// and zeros after them; the old buffers are freed (and the new ones take their place) only when every step
+// succeeded, otherwise the new ones are freed and the old ones stay.
+class Growth {
+ public:
+  explicit Growth(cudaStream_t stream) : stream_(stream) {}
+  ~Growth() { for (const Item& it : items_) cudaFree(status_ == SM_OK && done_ ? it.old_buffer : it.buffer); }
+  template <class T>
+  void grow(T** target, size_t count, size_t keep) {
+    if (status_ != SM_OK) return;
+    void* q = nullptr;
+    const size_t bytes = sizeof(T) * count, kept = *target ? sizeof(T) * keep : 0;
+    cudaError_t e = cudaMalloc(&q, bytes);
+    if (e == cudaSuccess && kept) e = cudaMemcpyAsync(q, *target, kept, cudaMemcpyDeviceToDevice, stream_);
+    if (e == cudaSuccess && bytes > kept) e = cudaMemsetAsync(static_cast<char*>(q) + kept, 0, bytes - kept, stream_);
+    if (q) items_.push_back({reinterpret_cast<void**>(target), q, *target});
+    if (e != cudaSuccess) status_ = SetError(SM_ERR_CUDA, (std::string("growing the mesh buffers: ") + cudaGetErrorString(e)).c_str());
+  }
+  int finish() {
+    if (status_ == SM_OK) {
+      const cudaError_t e = cudaStreamSynchronize(stream_);
+      if (e != cudaSuccess) status_ = SetError(SM_ERR_CUDA, (std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e)).c_str());
+    }
+    if (status_ == SM_OK) {
+      for (const Item& it : items_) *it.target = it.buffer;
+      done_ = true;
+    }
+    return status_;
+  }
+
+ private:
+  struct Item { void** target; void* buffer; void* old_buffer; };
+  cudaStream_t stream_;
+  std::vector<Item> items_;
+  int status_ = SM_OK;
+  bool done_ = false;
+};
+
+// The counters and grids on the first call; per-slot arrays for `slots` slots (x 1.5 when they grow, behind one
+// synchronisation).
+int EnsureLive(MeshLive& L, cudaStream_t stream, u32 slots, int sm_count) {
+  if (!L.counters) {
+    SM_CUDA(cudaMalloc(&L.counters, sizeof(UpdateCounters)));
+    SM_CUDA(cudaMemset(L.counters, 0, sizeof(UpdateCounters)));
+    SM_CUDA(cudaMallocHost(&L.host_counters, sizeof(UpdateCounters)));
+    int status = ResidentBlocks(k_mesh_umbrella_update, kUmbrellaBlock, sm_count, &L.umbrella_blocks);
+    if (status == SM_OK) status = ResidentBlocks(k_mesh_recheck<false>, kEmitBlock, sm_count, &L.emit_blocks);
+    if (status != SM_OK) return status;
+  }
+  if (slots <= L.slots) return SM_OK;
+  const size_t cap = std::max<size_t>(slots, static_cast<size_t>(L.slots) * 3 / 2);
+  const size_t keep = L.n_prev;   // (0 unless the previous update completed)
+  const size_t tiles = (cap + 1 + kScanTile - 1) / kScanTile;
+  Growth g(stream);
+  g.grow(&L.snapshot, cap * kSnapshotWords, keep * kSnapshotWords);
+  g.grow(&L.umbrella, cap * kUmbrella, keep * kUmbrella);
+  g.grow(&L.umbrella_count, cap, keep);
+  g.grow(&L.overflow, cap, keep);
+  g.grow(&L.word, cap, keep);
+  g.grow(&L.offsets[L.current], cap + 1, keep ? keep + 1 : 0);
+  g.grow(&L.offsets[L.current ^ 1], cap + 1, 0);
+  g.grow(&L.in_a, cap, 0);
+  g.grow(&L.in_r, cap, 0);
+  g.grow(&L.rebuild_list, cap, 0);
+  g.grow(&L.added_offsets, cap + 1, 0);
+  g.grow(&L.removed_offsets, cap + 1, 0);
+  g.grow(&L.scan_sums, tiles, 0);
+  g.grow(&L.points, 4 * 2 * cap, 0);
+  const int status = g.finish();
+  if (status != SM_OK) return status;
+  L.slots = static_cast<u32>(cap);
+  return SM_OK;
+}
+
+// A triangle buffer of at least `count` (x 1.5 when it grows); its content is not kept.
+int EnsureTriangles(uint3** p, u64* capacity, u64 count) {
+  if (count <= *capacity) return SM_OK;
+  const u64 grown = std::max<u64>(count + count / 2, 1024);
+  cudaFree(*p);
+  *p = nullptr;
+  *capacity = 0;
+  SM_CUDA(cudaMalloc(p, sizeof(uint3) * grown));
+  *capacity = grown;
+  return SM_OK;
+}
+
+void ScanCounts(cudaStream_t stream, u32* values, u32 count, u32* sums) {
+  const u32 tiles = (count + kScanTile - 1) / kScanTile;
+  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(values, count, sums); }
+  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(sums, tiles); }
+  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(values, count, sums); }
+}
+
+QueryArgs IndexQuery(const sm_knn_index* k) {
+  QueryArgs q{};
+  q.max_result_count = kMaxResults;
+  q.radius_scale = 1.f;
+  q.include_completed = 1;
+  q.include_free = 1;
+  q.inverse_cell_size = k->inverse_cell_size;
+  q.mask = k->table_size - 1;
+  q.bucket_start = k->bucket_start;
+  q.records = k->records;
+  return q;
+}
+
+int Grid(u32 items, int block, int resident) {
+  return static_cast<int>(std::max<u32>(1u, std::min<u32>((items + block - 1) / block, static_cast<u32>(resident))));
+}
+
+}  // namespace
+
+void FreeMeshBuffers(sm_reconstruction* r) {
+  FreeMeshScratch(r);
+  cudaFree(r->mesh_counters);
+  if (r->mesh_host_counters) cudaFreeHost(r->mesh_host_counters);
+  r->mesh_counters = nullptr;
+  r->mesh_host_counters = nullptr;
+  FreeLive(r->mesh_live);
+  r->mesh_live = nullptr;
+}
+
+int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, sm_mesh_update_stats* stats) {
+  int status = CheckMeshParams(p, "sm_mesh_update");
+  if (status != SM_OK) return status;
+  *stats = sm_mesh_update_stats{};
+  r->last_stream = stream;
+  status = FetchCounters(r, stream);
+  if (status == SM_ERR_CUDA) return status;   // (a surfel-cap overflow of an earlier frame does not matter here)
+  const u32 n = r->host_counters->surfel_count[r->count_slot];
+  if (!r->mesh_live) r->mesh_live = new MeshLive{};
+  MeshLive& L = *r->mesh_live;
+  const bool was_valid = L.valid;
+  L.valid = false;   // until this update completes; a failed one is followed by a rebuild from an empty mesh
+  if (!was_valid) L.n_prev = 0;
+  const u32 n_prev = L.n_prev, n_max = std::max(n, n_prev);
+  status = EnsureLive(L, stream, std::max(n_max, 1u), r->sm_count);
+  if (status != SM_OK) return status;
+  if (!was_valid) SM_CUDA(cudaMemsetAsync(L.counters, 0, sizeof(UpdateCounters), stream));
+  bool everything = !was_valid || n < n_prev || std::memcmp(&p, &L.params, sizeof(p)) != 0;
+  const int previous = L.current, next = previous ^ 1;
+
+  const float f2 = p.neighbor_radius_factor * p.neighbor_radius_factor;
+  MeshArgs a{};
+  a.n = n;
+  a.rows = r->d.surfels;
+  a.stride = r->d.stride;
+  a.radius_factor_squared = f2;
+  a.cos_normal = CosDegrees(p.max_angle_between_normals_deg);
+  a.cos_triangle = CosDegrees(p.max_triangle_angle_deg);
+  a.umbrella = L.umbrella;
+  a.umbrella_count = L.umbrella_count;
+  a.counters = &L.counters->bound;
+  UpdateArgs u{};
+  u.n_prev = n_prev;
+  u.n_max = n_max;
+  u.everything = everything;
+  u.snapshot = L.snapshot;
+  u.overflow = L.overflow;
+  u.word = L.word;
+  u.in_a = L.in_a;
+  u.in_r = L.in_r;
+  u.rebuild_list = L.rebuild_list;
+  u.points = L.points;
+  u.point_stride = 2 * L.slots;
+  u.old_offsets = L.offsets[previous];
+  u.old_triangles = L.triangles[previous];
+  u.new_offsets = L.offsets[next];
+  u.added_offsets = L.added_offsets;
+  u.removed_offsets = L.removed_offsets;
+  u.counters = L.counters;
+
+  const size_t per_call = offsetof(UpdateCounters, bound);
+  SM_CUDA(cudaMemsetAsync(reinterpret_cast<char*>(L.counters) + per_call, 0, sizeof(UpdateCounters) - per_call, stream));
+  if (n > 0) {
+    status = MirrorRegRecords(stream, r->d, n, r->sm_count);   // rows 3-5 <- the current smooth positions
+    if (status != SM_OK) return status;
+    const int bound_blocks = static_cast<int>(std::min<u32>((n + kBoundBlock - 1) / kBoundBlock, 4u * r->sm_count));
+    LaunchScope scope(stream, KID_MESH_BOUND);
+    LaunchKernel(k_mesh_bound, dim3(bound_blocks), dim3(kBoundBlock), 0, stream, a);
+  }
+  if (n_max > 0) {
+    LaunchScope scope(stream, KID_MESH_CHANGES);
+    LaunchKernel(k_mesh_changes, dim3(Grid(n_max, kEmitBlock, L.emit_blocks)), dim3(kEmitBlock), 0, stream, a, u);
+  }
+  SM_CUDA(cudaMemcpyAsync(L.host_counters, L.counters, sizeof(UpdateCounters), cudaMemcpyDeviceToHost, stream));
+  SM_CUDA(cudaStreamSynchronize(stream));
+  const u32 changed = L.host_counters->changed;
+  float max_r2;
+  std::memcpy(&max_r2, &L.host_counters->bound.max_radius_squared_bits, sizeof(float));
+  if (!(max_r2 > 0.f)) everything = true;   // no present slot: every umbrella is empty, no query runs
+  // Past this share of changed slots, marking A (an index over 2 |C| points and a query per slot) costs more than
+  // the list can save: every slot is rebuilt, as sm_triangulate does.
+  if (static_cast<unsigned long long>(changed) * kMarkDenominator > static_cast<unsigned long long>(n) * kMarkNumerator)
+    everything = true;
+  u.everything = everything;
+
+  if (max_r2 > 0.f) {
+    // The index of rule 1, as sm_triangulate builds it (the index object is shared: both calls rebuild it).
+    if (!r->mesh_index || r->mesh_index->capacity < n) {
+      KnnDestroy(r->mesh_index);
+      r->mesh_index = nullptr;
+      status = KnnCreate(&r->mesh_index, std::max(n + n / 2, r->mesh_slots));   // x 1.5: a session grows n
+      if (status != SM_OK) return status;
+    }
+    const float cell_size = 2.f * std::sqrt(max_r2 * f2);
+    const size_t st = r->d.stride;
+    const float* rows = r->d.surfels;
+    status = KnnBuild(r->mesh_index, stream, n, rows + SM_ROW_SMOOTH_X * st, rows + SM_ROW_SMOOTH_Y * st,
+                      rows + SM_ROW_SMOOTH_Z * st, rows + SM_ROW_RADIUS_SQUARED * st, nullptr, cell_size);
+    if (status != SM_OK) return status;
+    a.q = IndexQuery(r->mesh_index);
+    if (!everything && changed > 0) {
+      // A from the small side: an index over the <= 2 |C| old and new positions, one existence query per present
+      // slot with its own radius. A slot's work is bounded by the changed points near it, however large the
+      // largest radius (which sets the cell size) is.
+      const u32 points = 2 * changed;
+      if (!L.changed_index || L.changed_index->capacity < points) {
+        KnnDestroy(L.changed_index);
+        L.changed_index = nullptr;
+        status = KnnCreate(&L.changed_index, std::max(points, std::min(2 * L.slots, points * 2)));
+        if (status != SM_OK) return status;
+      }
+      const size_t ps = u.point_stride;
+      status = KnnBuild(L.changed_index, stream, points, L.points, L.points + ps, L.points + 2 * ps, L.points + 3 * ps,
+                        nullptr, cell_size);
+      if (status != SM_OK) return status;
+      u.changed = IndexQuery(L.changed_index);
+      LaunchScope scope(stream, KID_MESH_MARK);
+      LaunchKernel(k_mesh_mark, dim3(Grid(n, kEmitBlock, L.emit_blocks)), dim3(kEmitBlock), 0, stream, a, u);
+    }
+  }
+  const int emit_blocks = Grid(n_max, kEmitBlock, L.emit_blocks);
+  {
+    LaunchScope scope(stream, KID_MESH_OWNERS);
+    LaunchKernel(k_mesh_owners, dim3(emit_blocks), dim3(kEmitBlock), 0, stream, a, u);
+  }
+  if (n > 0) {
+    LaunchScope scope(stream, KID_MESH_UMBRELLA_UPDATE);
+    LaunchKernel(k_mesh_umbrella_update, dim3(Grid(n, kUmbrellaBlock / 32, L.umbrella_blocks)), dim3(kUmbrellaBlock), 0,
+                 stream, a, u);
+  }
+  for (u32* v : {u.new_offsets, u.added_offsets, u.removed_offsets})
+    SM_CUDA(cudaMemsetAsync(v + n_max, 0, sizeof(u32), stream));
+  {
+    LaunchScope scope(stream, KID_MESH_RECHECK);
+    LaunchKernel(k_mesh_recheck<false>, dim3(emit_blocks), dim3(kEmitBlock), 0, stream, a, u);
+  }
+  ScanCounts(stream, u.new_offsets, n_max + 1, L.scan_sums);
+  ScanCounts(stream, u.added_offsets, n_max + 1, L.scan_sums);
+  ScanCounts(stream, u.removed_offsets, n_max + 1, L.scan_sums);
+  SM_CUDA(cudaMemcpyAsync(&L.counters->triangle_count, u.new_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  SM_CUDA(cudaMemcpyAsync(&L.counters->added, u.added_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  SM_CUDA(cudaMemcpyAsync(&L.counters->removed, u.removed_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  SM_CUDA(cudaMemcpyAsync(L.host_counters, L.counters, sizeof(UpdateCounters), cudaMemcpyDeviceToHost, stream));
+  SM_CUDA(cudaStreamSynchronize(stream));
+  const UpdateCounters h = *L.host_counters;
+  status = EnsureTriangles(&L.triangles[next], &L.triangle_capacity[next], h.triangle_count);
+  if (status == SM_OK) status = EnsureTriangles(&L.added, &L.added_capacity, h.added);
+  if (status == SM_OK) status = EnsureTriangles(&L.removed, &L.removed_capacity, h.removed);
+  if (status != SM_OK) return status;
+  u.new_triangles = L.triangles[next];
+  u.added = L.added;
+  u.removed = L.removed;
+  if (n_max > 0) {
+    LaunchScope scope(stream, KID_MESH_RECHECK_WRITE);
+    LaunchKernel(k_mesh_recheck<true>, dim3(emit_blocks), dim3(kEmitBlock), 0, stream, a, u);
+  }
+  status = CheckLaunch("mesh_update");
+  if (status != SM_OK) return status;
+
+  L.current = next;
+  L.n_prev = n;
+  L.params = p;
+  L.triangle_count = h.triangle_count;
+  L.added_count = h.added;
+  L.removed_count = h.removed;
+  L.valid = true;
+  stats->mesh.triangle_count = h.triangle_count;
+  stats->mesh.vertices_meshed = h.vertices_meshed;
+  stats->mesh.boundary_edges = h.boundary_edges;
+  stats->mesh.umbrella_overflows = h.umbrella_overflows;
+  stats->slots_changed = h.changed;
+  stats->umbrellas_rebuilt = everything ? n : h.rebuilt;
+  stats->owners_rechecked = h.rechecked;
+  stats->triangles_added = h.added;
+  stats->triangles_removed = h.removed;
+  stats->full_sweep = everything || h.full_sweep ? 1 : 0;
+  return SM_OK;
+}
+
+int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t* triangles, uint64_t capacity,
+             uint64_t* count) {
+  auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_mesh_read: ") + why).c_str()); };
+  if (which != SM_MESH_ALL && which != SM_MESH_ADDED && which != SM_MESH_REMOVED) return bad("unknown `which`");
+  if (!triangles && capacity > 0) return bad("triangles is NULL with a capacity > 0");
+  const MeshLive* L = r->mesh_live;
+  if (!L || !L->valid) return bad("no sm_mesh_update has completed on this handle");
+  const uint3* src = which == SM_MESH_ALL ? L->triangles[L->current] : (which == SM_MESH_ADDED ? L->added : L->removed);
+  const u64 size = which == SM_MESH_ALL ? L->triangle_count : (which == SM_MESH_ADDED ? L->added_count : L->removed_count);
+  *count = size;
+  if (capacity < size) {
+    return SetError(SM_ERR_CAPACITY, ("sm_mesh_read: " + std::to_string(size) + " triangles do not fit the capacity of " +
+                                      std::to_string(capacity)).c_str());
+  }
+  r->last_stream = stream;
+  if (size > 0) SM_CUDA(cudaMemcpyAsync(triangles, src, sizeof(uint3) * size, cudaMemcpyDeviceToDevice, stream));
+  return SM_OK;
 }
 
 }  // namespace smb

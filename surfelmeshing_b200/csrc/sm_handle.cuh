@@ -50,6 +50,7 @@ struct StreamSession;  // pipeline.cu: an open sm_session_begin
 void DestroySession(StreamSession* s);
 struct TrackState;     // track.cu
 struct MeshCounters;   // mesh.cu
+struct MeshLive;       // mesh.cu: the persistent mesh of sm_mesh_update
 
 }  // namespace smb
 
@@ -161,6 +162,8 @@ struct sm_reconstruction {
   smb::MeshCounters* mesh_counters = nullptr;
   smb::MeshCounters* mesh_host_counters = nullptr;
   int mesh_umbrella_blocks = 0, mesh_emit_blocks = 0;
+  // sm_mesh_update's persistent mesh (mesh.cu), created by the first update; it shares only mesh_index.
+  smb::MeshLive* mesh_live = nullptr;
 };
 
 namespace smb {
@@ -202,6 +205,9 @@ void FreeTrackBuffers(sm_reconstruction* r);
 int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, uint32_t* triangles,
                 uint64_t capacity, sm_mesh_stats* stats);
 void FreeMeshBuffers(sm_reconstruction* r);
+int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, sm_mesh_update_stats* stats);
+int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t* triangles, uint64_t capacity,
+             uint64_t* count);
 // pipeline.cu
 int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
               const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats);

@@ -20,8 +20,8 @@ import torch
 
 from . import _lib
 from . import mesh_io
-from ._lib import (IntegrateParams, Library, MeshParams, MeshStats, PreprocessParams, RenderParams, SessionStatus,
-                   StreamDesc, StreamStats, TrackParams, TrackResult, TransferStats, TransferToken,
+from ._lib import (IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats, PreprocessParams, RenderParams,
+                   SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult, TransferStats, TransferToken,
                    VisualizationParams)
 
 RENDER_OUTPUTS = ("depth", "color", "normal", "index")
@@ -427,6 +427,43 @@ class CUDASurfelReconstruction:
             if status != _lib.SM_OK:
                 raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
             return out[:int(stats.triangle_count)], stats
+        raise AssertionError("unreachable")
+
+    def mesh_update(self, params: Optional[MeshParams] = None, stream=None) -> MeshUpdateStats:
+        """sm_mesh_update: brings the handle's persistent mesh up to date with the current cloud, rebuilding only
+        the umbrellas a change can reach (include/surfel_b200.h gives the rules). Synchronous. Afterwards
+        mesh_triangles("all") equals triangulate(params) on this state, and mesh_triangles("added" / "removed")
+        are the triangles the update added and removed."""
+        p = MeshParams.defaults() if params is None else params
+        stats = MeshUpdateStats()
+        self.lib.call("mesh_update", self._h, _stream_handle(stream), C.byref(p), C.byref(stats))
+        return stats
+
+    _MESH_LISTS = {"all": _lib.MESH_ALL, "added": _lib.MESH_ADDED, "removed": _lib.MESH_REMOVED}
+
+    def mesh_triangles(self, which: str = "all", stream=None):
+        """sm_mesh_read: one list of the last mesh_update() as an int32 CUDA tensor [T, 3] of slot indices, ordered
+        by owner slot, then the owner's umbrella order. Asks for the count first (capacity 0), so a delta of a few
+        triangles allocates only that much; retries once should the count change in between."""
+        code = self._MESH_LISTS[which]
+        handle = _stream_handle(stream)
+        count = C.c_uint64()
+        status = self.lib.fn["mesh_read"](self._h, handle, code, None, 0, C.byref(count))
+        if status not in (_lib.SM_OK, _lib.SM_ERR_CAPACITY):
+            raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+        capacity = max(int(count.value), 1)
+        for attempt in range(2):
+            out = torch.empty((capacity, 3), dtype=torch.int32, device="cuda")
+            if isinstance(stream, torch.cuda.Stream):
+                out.record_stream(stream)
+            status = self.lib.fn["mesh_read"](self._h, handle, code, C.c_void_p(out.data_ptr()), capacity,
+                                              C.byref(count))
+            if status == _lib.SM_ERR_CAPACITY and attempt == 0:
+                capacity = max(int(count.value), 1)
+                continue
+            if status != _lib.SM_OK:
+                raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+            return out[:int(count.value)]
         raise AssertionError("unreachable")
 
     def export_vertices_host(self, stream=None):
