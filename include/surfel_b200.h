@@ -356,6 +356,66 @@ int sm_render_surfels(sm_reconstruction* r, void* stream, const sm_render_params
                       float* normal, size_t normal_pitch,
                       uint32_t* index, size_t index_pitch);
 
+/* ---- rendering the triangle mesh into any pinhole camera (DESIGN.md section 1 row f11, section 5.9) ----------
+ * The reference's viewer draws its mesh over the visualisation vertex buffer with per-vertex colours, and keeps
+ * drawing the surfels the mesh does not cover yet as splats (APP/surfel_meshing_render_window.cc:239-359,
+ * --hide_new_surfel_splats off by default). sm_render_mesh draws a caller's triangle list over the handle's current
+ * cloud without a display, into the deterministic z-buffer of sm_render_surfels: same params, camera convention,
+ * output layouts and argument checks. triangles (DEVICE, 3 x triangle_count slot indices) may come from
+ * sm_triangulate or sm_mesh_read(SM_MESH_ALL), or be any list: it may be stale against the cloud.
+ *
+ * n = surfels_size(). In fp32 with denormals flushed to zero and no contraction, every product, sum and quotient
+ * rounded on its own (IEEE division and square root), for triangle t = (a, b, c):
+ *  T1. Corners. t is drawn only if a, b and c are all < n and have radius^2 (row 7) > 0; a triangle naming a merged
+ *      slot or a slot past the end is skipped (not an error). Its corners s_0 < s_1 < s_2 are a, b, c sorted by
+ *      slot, so nothing below depends on the winding or the rotation of t. A corner's vertex is its current SMOOTH
+ *      position, its colour the low three bytes (r, g, b) of row 24.
+ *  T2. Camera. c_k = view_T_global * vertex_k as in rule 1 of sm_render_surfels. t is skipped unless every corner
+ *      has near_depth <= c_k.z <= far_depth. There is no clipping: a triangle crossing the near plane is dropped.
+ *  T3. Screen. (u_k, v_k) = (fx * (c_k.x / c_k.z) + cx, fy * (c_k.y / c_k.z) + cy): the pixel-corner convention,
+ *      pixel (px, py) has its centre at (float(px) + 0.5, float(py) + 0.5). One function computes it, so a
+ *      corner shared by several triangles has the same bits in each. With the edge function of corners j < k
+ *        E_jk(x, y) = (u_k - u_j) * (y - v_j) - (v_k - v_j) * (x - u_j)
+ *      (always evaluated from the lower slot), D = E_01(u_2, v_2) is twice the signed screen area; t is skipped
+ *      if D == 0 or D is not finite.
+ *  T4. Coverage. At a pixel centre (x, y): w_0 = E_12(x, y), w_1 = -E_02(x, y), w_2 = E_01(x, y) (w_k belongs to
+ *      the edge opposite corner k; a triangle that runs an edge the other way negates its value, which is exact).
+ *      The pixel is covered iff w_0, w_1, w_2 >= 0 (D > 0) or all <= 0 (D < 0): edges are inclusive and there is
+ *      no back-face culling. Two triangles that share an edge compute its value alike, so no pixel centre between
+ *      them is left uncovered; a centre on the shared edge is proposed by both, and the key decides.
+ *  T5. Depth. q_k = (w_k / D) / c_k.z and z = 1 / ((q_0 + q_1) + q_2) (perspective-correct); the pixel is skipped
+ *      unless z is finite and > 0. It proposes the key (bits(z) << 32) | t, and the smallest key wins.
+ *  T6. Surfels the mesh leaves out (flags & SM_RENDER_UNMESHED_SURFELS, what the reference's viewer shows by
+ *      default). A slot < n that is a corner of no T1-valid triangle of the list is drawn as a disk by rules 1-4
+ *      of sm_render_surfels, with (bits(t) << 32) | (0x80000000 | slot) as its key: at equal depth a triangle
+ *      beats a disk.
+ *  T7. Outputs of the winning key. Triangle: depth = z, index = t, and with q_k and z of T5 at that pixel,
+ *      colour channel ch = the u8 of (((q_0 * C_0 + q_1 * C_1) + q_2 * C_2) * z) + 0.5, truncated, 255 if that
+ *      sum is >= 255 (C_k = float(channel ch of corner k)); normal = g * (1 / sqrt(g.g)) with e1 = c_1 - c_0,
+ *      e2 = c_2 - c_0, g = (e1.y*e2.z - e1.z*e2.y, e1.z*e2.x - e1.x*e2.z, e1.x*e2.y - e1.y*e2.x) negated if
+ *      g.c_0 > 0 (so it faces the camera), a.b = (a.x*b.x + a.y*b.y) + a.z*b.z, and (0, 0, 0) unless g.g is finite
+ *      and > 0. Disk: depth, colour and normal as sm_render_surfels gives them, index = 0x80000000 | slot. Empty
+ *      pixel: 0 / 0 / 0 / SM_INVALID_SURFEL_INDEX.
+ * Each triangle tests the pixels of its screen rectangle (the bounds of its corners, rounded outwards by at least
+ * one pixel); which pixels are covered is decided by T4 alone.
+ *
+ * Asynchronous on `stream`, no host synchronisation; surfels_size() is read on the device. Only reads the surfel
+ * state and the triangles. Scratch: the key raster of sm_render_surfels, a list of large triangles grown to
+ * triangle_count (4 bytes per triangle; growing it synchronises the device once) and one bit per slot of the
+ * handle's capacity, allocated by the first call (sm_create allocates nothing for rendering) and freed by
+ * sm_destroy. SM_ERR_INVALID_ARGUMENT, with no launch, for everything sm_render_surfels rejects, triangles NULL
+ * with triangle_count > 0, triangle_count >= 2^31 and flag bits other than SM_RENDER_UNMESHED_SURFELS. A count of 0
+ * is legal: with the flag it gives sm_render_surfels' image, the index with its high bit set. */
+#define SM_RENDER_UNMESHED_SURFELS 1
+int sm_render_mesh(sm_reconstruction* r, void* stream, const sm_render_params* p,
+                   const float view_T_global[12],      /* 3x4 row-major, global -> camera */
+                   const uint32_t* triangles /* device, 3 x triangle_count slot indices */, uint64_t triangle_count,
+                   int32_t flags,
+                   float* depth, size_t depth_pitch,
+                   uint8_t* color, size_t color_pitch,
+                   float* normal, size_t normal_pitch,
+                   uint32_t* index, size_t index_pitch);
+
 /* ---- camera tracking against the cloud (DESIGN.md section 1 row f8, section 5.6) ----------------------------
  * The reference reads every camera pose from a trajectory file (APP/main.cc:601-625) and has no tracker.
  * sm_track_frame estimates the pose of a depth map by projective point-to-plane ICP against a model view,
@@ -727,8 +787,8 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * Between pushes, calls on `stream` see the state after status.last_integrated_frame, and the next push's
  * work waits for them: the hand-off calls (sm_transfer_all_to_cpu, sm_transfer_delta_to_cpu,
  * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
- * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_track_frame, sm_track_linearize,
- * sm_mesh_update, sm_mesh_read, sm_triangulate, sm_surfel_count / sm_surfels_size) and
+ * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_render_mesh, sm_track_frame,
+ * sm_track_linearize, sm_mesh_update, sm_mesh_read, sm_triangulate, sm_surfel_count / sm_surfels_size) and
  * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
  * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which
  * that frame's Integrate() applies in the next step. The device merge counter then already includes them, so

@@ -123,6 +123,9 @@ class RenderParams(C.Structure):
                 ("cx", C.c_float), ("cy", C.c_float), ("near_depth", C.c_float), ("far_depth", C.c_float)]
 
 
+RENDER_UNMESHED_SURFELS = 1
+DISK_INDEX_FLAG = 0x80000000   # sm_render_mesh: the index of a pixel drawn by a disk
+
 TRACK_CLOUD = 0
 TRACK_PREVIOUS_FRAME = 1
 
@@ -240,6 +243,8 @@ _PRODUCT_ONLY = {
     "session_push": (C.c_int, [_P, _P, _SZ, _P, _SZ, _I, _P, _P, C.POINTER(SessionStatus)]),
     "session_end": (C.c_int, [_P, C.POINTER(StreamStats)]),
     "render_surfels": (C.c_int, [_P, _P, C.POINTER(RenderParams), _P, _P, _SZ, _P, _SZ, _P, _SZ, _P, _SZ]),
+    "render_mesh": (C.c_int, [_P, _P, C.POINTER(RenderParams), _P, _P, C.c_uint64, _I, _P, _SZ, _P, _SZ, _P, _SZ, _P,
+                              _SZ]),
     "default_track_params": (None, [C.POINTER(TrackParams)]),
     "track_frame": (C.c_int, [_P, _P, C.POINTER(TrackParams), C.POINTER(PreprocessParams), _P, _SZ, _P, _P,
                               C.POINTER(TrackResult)]),

@@ -129,7 +129,8 @@ const char* KernelName(int id) {
       "k_downscale_color", "k_reg_mirror", "k_reg_pack", "k_render_splat", "k_render_large", "k_render_resolve",
       "k_track_live_view", "k_track_linearize", "k_track_solve", "k_mesh_bound", "k_mesh_umbrella", "k_mesh_count",
       "k_mesh_scan", "k_mesh_write", "k_mesh_changes", "k_mesh_mark", "k_mesh_owners", "k_mesh_umbrella_update",
-      "k_mesh_recheck", "k_mesh_recheck_write"};
+      "k_mesh_recheck", "k_mesh_recheck_write", "k_mesh_render_mark", "k_mesh_render_tri", "k_mesh_render_large",
+      "k_mesh_render_splat", "k_mesh_render_splat_large", "k_mesh_render_resolve"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -657,6 +658,15 @@ int sm_render_surfels(sm_reconstruction* r, void* stream, const sm_render_params
   if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_surfels: null argument");
   return RenderSurfels(r, static_cast<cudaStream_t>(stream), *p, view_T_global, depth, depth_pitch, color, color_pitch,
                        normal, normal_pitch, index, index_pitch);
+}
+
+int sm_render_mesh(sm_reconstruction* r, void* stream, const sm_render_params* p, const float view_T_global[12],
+                   const uint32_t* triangles, uint64_t triangle_count, int32_t flags, float* depth, size_t depth_pitch,
+                   uint8_t* color, size_t color_pitch, float* normal, size_t normal_pitch, uint32_t* index,
+                   size_t index_pitch) {
+  if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_mesh: null argument");
+  return RenderMesh(r, static_cast<cudaStream_t>(stream), *p, view_T_global, triangles, triangle_count, flags, depth,
+                    depth_pitch, color, color_pitch, normal, normal_pitch, index, index_pitch);
 }
 
 void sm_default_track_params(sm_track_params* p) {

@@ -133,6 +133,14 @@ struct sm_reconstruction {
   smb::u32* render_large_list = nullptr;
   smb::u32* render_large_count = nullptr;
   int render_splat_blocks = 0, render_large_blocks = 0;
+  // sm_render_mesh scratch (render.cu) beyond the above, allocated by the first mesh render: one bit per slot of
+  // capacity (corners of the triangles drawn), the large-triangle list (grown to the triangle count) and its count
+  // (zero between calls), resident grids.
+  smb::u32* mesh_render_marks = nullptr;
+  smb::u32* mesh_render_large_list = nullptr; smb::u32 mesh_render_large_capacity = 0;   // in triangles
+  smb::u32* mesh_render_large_count = nullptr;
+  int mesh_render_mark_blocks = 0, mesh_render_tri_blocks = 0, mesh_render_large_blocks = 0;
+  int mesh_render_splat_blocks = 0, mesh_render_splat_large_blocks = 0;
   // sm_track_frame / sm_track_linearize scratch (track.cu), allocated by the first call: the filtered live pyramid,
   // the rendered model view, two level-0 views of tracked frames (depth, normals) of which track_previous is the
   // newest, the pose that call returned, the per-block partial rows and the device / pinned tracker state (allocated
@@ -192,6 +200,10 @@ int UpdateVisualizationBuffers(sm_reconstruction* r, cudaStream_t stream, const 
 int RenderSurfels(sm_reconstruction* r, cudaStream_t stream, const sm_render_params& p, const float* view_T_global,
                   float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch, float* normal,
                   size_t normal_pitch, uint32_t* index, size_t index_pitch);
+int RenderMesh(sm_reconstruction* r, cudaStream_t stream, const sm_render_params& p, const float* view_T_global,
+               const uint32_t* triangles, uint64_t triangle_count, int32_t flags, float* depth, size_t depth_pitch,
+               uint8_t* color, size_t color_pitch, float* normal, size_t normal_pitch, uint32_t* index,
+               size_t index_pitch);
 void FreeRenderBuffers(sm_reconstruction* r);
 // track.cu
 int TrackFrame(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const sm_preprocess_params& pp,

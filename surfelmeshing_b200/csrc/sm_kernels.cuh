@@ -36,6 +36,8 @@ enum KernelId {
   KID_TRACK_LIVE_VIEW, KID_TRACK_LINEARIZE, KID_TRACK_SOLVE,
   KID_MESH_BOUND, KID_MESH_UMBRELLA, KID_MESH_COUNT, KID_MESH_SCAN, KID_MESH_WRITE,
   KID_MESH_CHANGES, KID_MESH_MARK, KID_MESH_OWNERS, KID_MESH_UMBRELLA_UPDATE, KID_MESH_RECHECK, KID_MESH_RECHECK_WRITE,
+  KID_MESH_RENDER_MARK, KID_MESH_RENDER_TRI, KID_MESH_RENDER_LARGE, KID_MESH_RENDER_SPLAT, KID_MESH_RENDER_SPLAT_LARGE,
+  KID_MESH_RENDER_RESOLVE,
   KID_COUNT
 };
 const char* KernelName(int id);

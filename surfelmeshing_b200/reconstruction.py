@@ -87,6 +87,18 @@ def invert_rigid(m) -> np.ndarray:
     return np.concatenate([R.T, (-R.T @ t)[:, None]], axis=1).astype(np.float32)
 
 
+def shade_normals(normal: torch.Tensor) -> torch.Tensor:
+    """The reference viewer's triangle-normal shading (--triangle_normal_shading, light = the viewing direction) of a
+    camera-frame normal image [H, W, 3] from render_mesh(): intensity = clamp(0.8 * (-n.z) + 0.2, 0, 1) as uint8
+    [H, W] (x 255, rounded); pixels whose normal is zero (empty) are 0."""
+    if normal.dim() != 3 or normal.shape[2] != 3:
+        raise ValueError("normal must be [H, W, 3]")
+    n = normal.float()
+    intensity = (0.8 * (-n[..., 2]) + 0.2).clamp(0.0, 1.0)
+    value = torch.round(intensity * 255.0).to(torch.uint8)
+    return torch.where((n != 0).any(dim=2), value, torch.zeros_like(value))
+
+
 # ---------------------------------------------------------------------------------------
 # depth pre-processing (names of cuda_depth_processing.cuh)
 # ---------------------------------------------------------------------------------------
@@ -354,6 +366,44 @@ class CUDASurfelReconstruction:
         T = _mat12(view_T_global)
         self.lib.call("render_surfels", self._h, _stream_handle(stream), C.byref(p), T.ctypes.data_as(C.c_void_p),
                       *args)
+        return out
+
+    def render_mesh(self, triangles, view_T_global, width: int, height: int, fx: float, fy: float, cx: float,
+                    cy: float, near: float = 0.1, far: float = 100.0, unmeshed_surfels: bool = True, stream=None,
+                    outputs=RENDER_OUTPUTS) -> dict:
+        """sm_render_mesh: a triangle list over the current cloud (the int32 CUDA tensor [T, 3] of slot indices that
+        triangulate() and mesh_triangles() return) drawn into a pinhole camera of any size, with perspective-correct
+        depth and colour; unmeshed_surfels=True also draws the slots no triangle names as disks, as render() does.
+        Triangles naming merged or out-of-range slots, or with a corner outside [near, far], are not drawn.
+
+        Returns the dict of render(): "depth", "color", "normal" (the unit triangle normal facing the camera) and
+        "index" (the triangle's row in `triangles`; a disk's slot with bit 31 set, so negative in int32; -1 = empty),
+        enqueued on `stream` (not synchronised)."""
+        outputs = tuple(outputs)
+        unknown = [o for o in outputs if o not in RENDER_OUTPUTS]
+        if unknown or not outputs:
+            raise ValueError(f"outputs must be a non-empty subset of {RENDER_OUTPUTS}, got {outputs}")
+        if not isinstance(triangles, torch.Tensor) or triangles.dim() != 2 or triangles.shape[1] != 3 or \
+                triangles.dtype != torch.int32 or not triangles.is_cuda:
+            raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+        triangles = triangles.contiguous()
+        H, W = int(height), int(width)
+        shapes = {"depth": ((H, W), torch.float32), "color": ((H, W, 3), torch.uint8),
+                  "normal": ((H, W, 3), torch.float32), "index": ((H, W), torch.int32)}
+        out = {k: torch.empty(shapes[k][0], dtype=shapes[k][1], device="cuda") for k in outputs}
+        if isinstance(stream, torch.cuda.Stream):
+            for t in (*out.values(), triangles):
+                t.record_stream(stream)   # allocated on the current stream, used on `stream`
+        args = []
+        for k in RENDER_OUTPUTS:
+            t = out.get(k)
+            args += [C.c_void_p(t.data_ptr()), t.stride(0) * t.element_size()] if t is not None else [None, 0]
+        p = RenderParams(W, H, float(fx), float(fy), float(cx), float(cy), float(near), float(far))
+        T = _mat12(view_T_global)
+        count = int(triangles.shape[0])
+        self.lib.call("render_mesh", self._h, _stream_handle(stream), C.byref(p), T.ctypes.data_as(C.c_void_p),
+                      C.c_void_p(triangles.data_ptr()) if count else None, count,
+                      _lib.RENDER_UNMESHED_SURFELS if unmeshed_surfels else 0, *args)
         return out
 
     def track(self, depth, guess, params: Optional[TrackParams] = None, pp: Optional[PreprocessParams] = None,
