@@ -512,6 +512,90 @@ int sm_track_linearize(sm_reconstruction* r, void* stream, const sm_track_params
                        const float* model_normal, size_t model_normal_pitch,
                        const float model_T_live[12], double out_system[27], uint32_t* out_inliers);
 
+/* ---- camera tracking with colour (DESIGN.md section 1 row f12, section 5.10) ----------------------------------
+ * Point-to-plane ICP cannot see motion that slides along the surfaces in view: a single plane fixes 3 of the 6
+ * degrees of freedom, two planes or a corridor leave one translation free, and J^T J is then singular up to
+ * rounding. sm_track_frame_rgbd tracks a depth map and its registered colour image by minimising
+ *     E(T) = sum_icp r^2 + lambda^2 sum_photo r_c^2,
+ * the residual r_c aligning the model's intensity to the live intensity through the live depth (as ElasticFusion's
+ * joint ICP + RGB tracker and DVO do). Everything not written below is sm_track_frame: steps 1-5, rules L and M,
+ * the solve, the loss rule (depth inliers against min_inlier_fraction of the valid pixels), the convergence test,
+ * the pose bookkeeping and every argument check. Only reads the surfel state.
+ *
+ * Per-pixel rules, fp32 with every product, sum and quotient rounded on its own (no fma, IEEE division):
+ *  P1. Intensity of a u8x3 pixel (r, g, b): I = ((0.299f * r) + (0.587f * g)) + (0.114f * b).
+ *  P2. Live pyramid. Level 0 is P1 of the raw colour. Level l has the size w x h of Camera.scaled(l) and is built
+ *      from level l-1 of size w' x h': with a = (2x, 2y), b = (min(2x+1, w'-1), 2y), c = (2x, min(2y+1, h'-1)),
+ *      d = (min(2x+1, w'-1), min(2y+1, h'-1)), I_l(x, y) = ((I(a) + I(b)) + (I(c) + I(d))) * 0.25f.
+ *      (2x <= w'-1 and 2y <= h'-1 hold for every size Camera.scaled produces.)
+ *  P3. Model pyramid, at the model camera Camera.scaled(l) of the handle's camera. Level 0: P1 of the model colour
+ *      where the model depth is finite and > 0, NaN elsewhere; levels >= 1 as in P2 (a NaN child makes its parent
+ *      NaN). Model colour: SM_TRACK_CLOUD: the colour output of the sm_render_surfels call of step 2 (rendered
+ *      together with depth and normal); SM_TRACK_PREVIOUS_FRAME: the level-0 live intensity kept by this handle's
+ *      previous sm_track_frame_rgbd call, with that call's kept depth (step 3) as the model depth.
+ *  P4. Photometric sample, only for a pixel that is a depth inlier (passes M1-M4), with p' = T p of M1 and the
+ *      level-l model camera (fx_l, fy_l, cx_l, cy_l, size w_l x h_l):
+ *        u = fx_l * (p'.x / p'.z) + cx_l, v likewise; s = u - 0.5, t = v - 0.5; a photometric outlier unless
+ *        0 <= s < w_l - 1 and 0 <= t < h_l - 1 (the right-hand sides exact small integers);
+ *        i = int(s), j = int(t), a = s - i, b = t - j; I00, I10, I01, I11 = model level l at (i, j), (i+1, j),
+ *        (i, j+1), (i+1, j+1), all four finite or the pixel is a photometric outlier;
+ *        Im = ((1-a)*I00 + a*I10) * (1-b) + ((1-a)*I01 + a*I11) * b;
+ *        gx = (1-b)*(I10-I00) + b*(I11-I01), gy = (1-a)*(I01-I00) + a*(I11-I10)  (the analytic gradient of the
+ *        bilinear patch, so the Jacobian is the exact derivative inside a cell);
+ *        r_c = Im - I_live_l(x, y). A photometric inlier needs |r_c| <= max_intensity_residual and
+ *        gx*gx + gy*gy >= g2, g2 = min_gradient * min_gradient rounded to fp32.
+ *  P5. Jacobian for the increment of M5 (T <- exp(xi) T, xi = (omega, v)): ga = gx * fx_l, gb = gy * fy_l,
+ *      iz = 1 / p'.z, w = (ga * iz, gb * iz, -(((ga * p'.x + gb * p'.y) * iz) * iz)), J_c = (p' x w, w) with the
+ *      cross product of L2.
+ *  P6. Sums. With L2 = double(lambda) * double(lambda), the 21 L2 * (J_ci * J_cj) and the 6 L2 * (J_ci * r_c) are
+ *      formed in fp64 and added, after the pixel's depth terms, into the same per-thread sums as M5's; r_c^2 and the
+ *      photometric inlier count are two more sums. The solve and everything after it are those of sm_track_frame.
+ *  P7. photometric_weight == 0 runs sm_track_frame's own linearisation and solve: pose and result.depth are
+ *      sm_track_frame's bit for bit. The call still renders the model colour, builds the pyramids and keeps the
+ *      level-0 intensity, so a following SM_TRACK_PREVIOUS_FRAME call has its model.
+ * result: depth exactly as sm_track_frame reports it; photometric_inliers and rms_intensity = sqrt(sum r_c^2 /
+ * photometric_inliers) (0 without inliers) of the last level-0 linearisation (both 0 when the frame was lost
+ * before level 0, and with photometric_weight == 0).
+ *
+ * sm_track_linearize_rgbd runs one linearisation on caller images, synchronously: sm_track_linearize's arguments,
+ * plus rp, the raw live colour and the model colour (packed u8x3, both at the handle's camera size); it builds
+ * levels 0..level of both pyramids from them (P2, P3 with model_depth as the model depth) and returns the 27
+ * combined sums (P6), out_sum_rc2 = sum r_c^2, out_inliers = the depth inliers and out_photometric_inliers.
+ *
+ * Scratch (the render's colour image, both intensity pyramids in fp32 and one kept level-0 intensity) is allocated
+ * by the first RGB-D call; sm_create allocates nothing for it and sm_destroy frees it. A depth-only sm_track_frame
+ * between RGB-D calls keeps working as before; it leaves no kept intensity, so the next RGB-D call may not use
+ * SM_TRACK_PREVIOUS_FRAME. SM_ERR_INVALID_ARGUMENT, with no launch, for everything sm_track_frame (or
+ * sm_track_linearize) rejects, plus a NULL colour or rp, a colour pitch below 3 x width, a negative or non-finite
+ * photometric_weight, max_intensity_residual or min_gradient, and SM_TRACK_PREVIOUS_FRAME when the handle's
+ * previous sm_track_frame / sm_track_frame_rgbd call was not an RGB-D call. */
+typedef struct sm_track_rgbd_params {
+  float photometric_weight;        /* lambda, metres per intensity unit; 0 = the depth-only system (1e-4) */
+  float max_intensity_residual;    /* |r_c| gate, intensity units on the 0..255 scale (40) */
+  float min_gradient;              /* |grad I| gate, intensity units per pixel (2) */
+} sm_track_rgbd_params;
+typedef struct sm_track_rgbd_result {
+  sm_track_result depth;           /* exactly as sm_track_frame reports it */
+  uint32_t photometric_inliers;    /* level 0, last linearisation */
+  float rms_intensity;             /* sqrt(sum r_c^2 / photometric_inliers), level 0, last linearisation */
+} sm_track_rgbd_result;
+/* Host only, no device needed. */
+void sm_default_track_rgbd_params(sm_track_rgbd_params* p);
+int sm_track_frame_rgbd(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_preprocess_params* pp,
+                        const sm_track_rgbd_params* rp,
+                        const uint16_t* depth, size_t depth_pitch,   /* raw u16, device, the handle's camera size */
+                        const uint8_t* color, size_t color_pitch,    /* packed u8x3 (r, g, b), registered to depth */
+                        const float global_T_guess[12], float global_T_out[12], sm_track_rgbd_result* result);
+int sm_track_linearize_rgbd(sm_reconstruction* r, void* stream, const sm_track_params* tp,
+                            const sm_track_rgbd_params* rp, int32_t level, float depth_scaling,
+                            const uint16_t* live_depth, size_t live_pitch,   /* filtered level image, device */
+                            const uint8_t* live_color, size_t live_color_pitch,   /* raw u8x3, handle size */
+                            const float* model_depth, size_t model_depth_pitch,
+                            const float* model_normal, size_t model_normal_pitch,
+                            const uint8_t* model_color, size_t model_color_pitch,   /* u8x3, handle size */
+                            const float model_T_live[12], double out_system[27], double* out_sum_rc2,
+                            uint32_t* out_inliers, uint32_t* out_photometric_inliers);
+
 /* ---- triangulating the surfel cloud (DESIGN.md section 1 row f9, section 5.7) ---------------------------------
  * The reference's meshing thread grows its mesh by advancing triangle fronts one surfel at a time
  * (APP/surfel_meshing.cc:667-752), which is sequential by construction. sm_triangulate meshes the whole current
@@ -788,7 +872,8 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * work waits for them: the hand-off calls (sm_transfer_all_to_cpu, sm_transfer_delta_to_cpu,
  * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
  * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_render_mesh, sm_track_frame,
- * sm_track_linearize, sm_mesh_update, sm_mesh_read, sm_triangulate, sm_surfel_count / sm_surfels_size) and
+ * sm_track_linearize, sm_track_frame_rgbd, sm_track_linearize_rgbd,
+ * sm_mesh_update, sm_mesh_read, sm_triangulate, sm_surfel_count / sm_surfels_size) and
  * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
  * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which
  * that frame's Integrate() applies in the next step. The device merge counter then already includes them, so

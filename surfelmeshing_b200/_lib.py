@@ -149,6 +149,22 @@ class TrackResult(C.Structure):
                 ("valid_pixels", C.c_uint32), ("rms_residual", C.c_float)]
 
 
+class TrackRGBDParams(C.Structure):
+    """sm_track_rgbd_params: the photometric weight lambda (metres per intensity unit; 0 = the depth-only system), the
+    |r_c| gate (intensity units, 0..255 scale) and the |grad I| gate (intensity units per pixel)."""
+    _fields_ = [("photometric_weight", C.c_float), ("max_intensity_residual", C.c_float), ("min_gradient", C.c_float)]
+
+    @classmethod
+    def defaults(cls) -> "TrackRGBDParams":
+        return cls(1e-4, 40.0, 2.0)
+
+
+class TrackRGBDResult(C.Structure):
+    """sm_track_rgbd_result: the depth-only TrackResult, and the level-0 photometric inliers and RMS intensity
+    residual."""
+    _fields_ = [("depth", TrackResult), ("photometric_inliers", C.c_uint32), ("rms_intensity", C.c_float)]
+
+
 class MeshParams(C.Structure):
     """sm_mesh_params: k-NN radius factor, normal gate and largest triangle angle (main.cc's meshing defaults)."""
     _fields_ = [("neighbor_radius_factor", C.c_float), ("max_angle_between_normals_deg", C.c_float),
@@ -250,6 +266,12 @@ _PRODUCT_ONLY = {
                               C.POINTER(TrackResult)]),
     "track_linearize": (C.c_int, [_P, _P, C.POINTER(TrackParams), _I, _F, _P, _SZ, _P, _SZ, _P, _SZ, _P, _P,
                                   C.POINTER(_U32)]),
+    "default_track_rgbd_params": (None, [C.POINTER(TrackRGBDParams)]),
+    "track_frame_rgbd": (C.c_int, [_P, _P, C.POINTER(TrackParams), C.POINTER(PreprocessParams),
+                                   C.POINTER(TrackRGBDParams), _P, _SZ, _P, _SZ, _P, _P, C.POINTER(TrackRGBDResult)]),
+    "track_linearize_rgbd": (C.c_int, [_P, _P, C.POINTER(TrackParams), C.POINTER(TrackRGBDParams), _I, _F, _P, _SZ,
+                                       _P, _SZ, _P, _SZ, _P, _SZ, _P, _SZ, _P, _P, C.POINTER(C.c_double),
+                                       C.POINTER(_U32), C.POINTER(_U32)]),
     "default_mesh_params": (None, [C.POINTER(MeshParams)]),
     "triangulate": (C.c_int, [_P, _P, C.POINTER(MeshParams), _P, C.c_uint64, C.POINTER(MeshStats)]),
     "mesh_update": (C.c_int, [_P, _P, C.POINTER(MeshParams), C.POINTER(MeshUpdateStats)]),

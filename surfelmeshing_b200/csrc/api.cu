@@ -130,7 +130,8 @@ const char* KernelName(int id) {
       "k_track_live_view", "k_track_linearize", "k_track_solve", "k_mesh_bound", "k_mesh_umbrella", "k_mesh_count",
       "k_mesh_scan", "k_mesh_write", "k_mesh_changes", "k_mesh_mark", "k_mesh_owners", "k_mesh_umbrella_update",
       "k_mesh_recheck", "k_mesh_recheck_write", "k_mesh_render_mark", "k_mesh_render_tri", "k_mesh_render_large",
-      "k_mesh_render_splat", "k_mesh_render_splat_large", "k_mesh_render_resolve"};
+      "k_mesh_render_splat", "k_mesh_render_splat_large", "k_mesh_render_resolve",
+      "k_track_intensity_base", "k_track_intensity_down", "k_track_linearize_rgbd", "k_track_solve_rgbd"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -698,6 +699,39 @@ int sm_track_linearize(sm_reconstruction* r, void* stream, const sm_track_params
   return TrackLinearize(r, static_cast<cudaStream_t>(stream), *tp, level, depth_scaling, live_depth, live_pitch,
                         model_depth, model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system,
                         out_inliers);
+}
+
+void sm_default_track_rgbd_params(sm_track_rgbd_params* p) {
+  p->photometric_weight = 1e-4f;
+  p->max_intensity_residual = 40.0f;
+  p->min_gradient = 2.0f;
+}
+
+int sm_track_frame_rgbd(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_preprocess_params* pp,
+                        const sm_track_rgbd_params* rp, const uint16_t* depth, size_t depth_pitch, const uint8_t* color,
+                        size_t color_pitch, const float global_T_guess[12], float global_T_out[12],
+                        sm_track_rgbd_result* result) {
+  if (!r || !tp || !pp || !rp || !depth || !color || !global_T_guess || !global_T_out || !result)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_frame_rgbd: null argument");
+  const TrackColor c{rp, color, color_pitch, nullptr, 0};
+  return TrackFrameRGBD(r, static_cast<cudaStream_t>(stream), *tp, *pp, c, depth, depth_pitch, global_T_guess,
+                        global_T_out, result);
+}
+
+int sm_track_linearize_rgbd(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_track_rgbd_params* rp,
+                            int32_t level, float depth_scaling, const uint16_t* live_depth, size_t live_pitch,
+                            const uint8_t* live_color, size_t live_color_pitch, const float* model_depth,
+                            size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
+                            const uint8_t* model_color, size_t model_color_pitch, const float model_T_live[12],
+                            double out_system[27], double* out_sum_rc2, uint32_t* out_inliers,
+                            uint32_t* out_photometric_inliers) {
+  if (!r || !tp || !rp || !live_depth || !live_color || !model_depth || !model_normal || !model_color || !model_T_live ||
+      !out_system || !out_sum_rc2 || !out_inliers || !out_photometric_inliers)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_linearize_rgbd: null argument");
+  const TrackColor c{rp, live_color, live_color_pitch, model_color, model_color_pitch};
+  return TrackLinearizeRGBD(r, static_cast<cudaStream_t>(stream), *tp, c, level, depth_scaling, live_depth, live_pitch,
+                            model_depth, model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system,
+                            out_sum_rc2, out_inliers, out_photometric_inliers);
 }
 
 void sm_default_mesh_params(sm_mesh_params* p) {

@@ -157,6 +157,17 @@ struct sm_reconstruction {
   int track_blocks = 0;
   smb::TrackState* track_state = nullptr;
   smb::TrackState* track_host_state = nullptr;
+  // sm_track_frame_rgbd / sm_track_linearize_rgbd scratch (track.cu), allocated by the first RGB-D call: the model
+  // colour the render writes, the live and model intensity pyramids, the level-0 live intensity kept for the next
+  // SM_TRACK_PREVIOUS_FRAME call (allocated last: non-null means every buffer exists), the partial rows of the RGB-D
+  // linearisation's resident grid, and whether the previous tracking call was an RGB-D call.
+  smb::u8* track_model_color = nullptr; size_t track_model_color_pitch = 0;
+  float* track_live_intensity[4] = {}; size_t track_live_intensity_pitch[4] = {};
+  float* track_model_intensity[4] = {}; size_t track_model_intensity_pitch[4] = {};
+  double* track_rgbd_partials = nullptr;
+  int track_rgbd_blocks = 0;
+  float* track_kept_intensity = nullptr; size_t track_kept_intensity_pitch = 0;
+  bool track_previous_rgbd = false;
   // sm_triangulate scratch (mesh.cu), allocated by the first call and grown to surfels_size(): the k-NN index over
   // the smooth positions, the umbrellas ([mesh_slots][SM_MESH_MAX_UMBRELLA] pairs) and their lengths, the per-slot
   // triangle counts (scanned in place into offsets) and the scan's tile sums; the device counters and their
@@ -212,6 +223,21 @@ int TrackLinearize(sm_reconstruction* r, cudaStream_t stream, const sm_track_par
                    const u16* live, size_t live_pitch, const float* model_depth, size_t model_depth_pitch,
                    const float* model_normal, size_t model_normal_pitch, const float* model_T_live, double* out_system,
                    uint32_t* out_inliers);
+// The photometric part of an RGB-D call (sm_track_frame_rgbd / sm_track_linearize_rgbd): the parameters, the raw
+// live colour and, for the linearisation alone, the caller's model colour.
+struct TrackColor {
+  const sm_track_rgbd_params* params;
+  const uint8_t* live; size_t live_pitch;
+  const uint8_t* model; size_t model_pitch;
+};
+int TrackFrameRGBD(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const sm_preprocess_params& pp,
+                   const TrackColor& color, const u16* depth, size_t depth_pitch, const float* guess, float* pose_out,
+                   sm_track_rgbd_result* result);
+int TrackLinearizeRGBD(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const TrackColor& color,
+                       int level, float depth_scaling, const u16* live, size_t live_pitch, const float* model_depth,
+                       size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
+                       const float* model_T_live, double* out_system, double* out_sum_rc2, uint32_t* out_inliers,
+                       uint32_t* out_photometric_inliers);
 void FreeTrackBuffers(sm_reconstruction* r);
 // mesh.cu
 int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, uint32_t* triangles,

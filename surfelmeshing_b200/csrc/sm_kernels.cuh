@@ -38,6 +38,7 @@ enum KernelId {
   KID_MESH_CHANGES, KID_MESH_MARK, KID_MESH_OWNERS, KID_MESH_UMBRELLA_UPDATE, KID_MESH_RECHECK, KID_MESH_RECHECK_WRITE,
   KID_MESH_RENDER_MARK, KID_MESH_RENDER_TRI, KID_MESH_RENDER_LARGE, KID_MESH_RENDER_SPLAT, KID_MESH_RENDER_SPLAT_LARGE,
   KID_MESH_RENDER_RESOLVE,
+  KID_TRACK_INTENSITY_BASE, KID_TRACK_INTENSITY_DOWN, KID_TRACK_LINEARIZE_RGBD, KID_TRACK_SOLVE_RGBD,
   KID_COUNT
 };
 const char* KernelName(int id);

@@ -21,8 +21,8 @@ import torch
 from . import _lib
 from . import mesh_io
 from ._lib import (IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats, PreprocessParams, RenderParams,
-                   SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult, TransferStats, TransferToken,
-                   VisualizationParams)
+                   SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult, TrackRGBDParams, TrackRGBDResult,
+                   TransferStats, TransferToken, VisualizationParams)
 
 RENDER_OUTPUTS = ("depth", "color", "normal", "index")
 
@@ -456,6 +456,72 @@ class CUDASurfelReconstruction:
                       system.ctypes.data_as(C.c_void_p), C.byref(inliers))
         return system, int(inliers.value)
 
+    def _check_raster(self, name, t, shape, dtype):
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != shape or t.dtype != dtype:
+            got = (tuple(t.shape), t.dtype) if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"{name} must be a {dtype} tensor of shape {shape}, got {got}")
+
+    def track_rgbd(self, depth, color, guess, params: Optional[TrackParams] = None,
+                   rgbd: Optional[TrackRGBDParams] = None, pp: Optional[PreprocessParams] = None, source: str = "cloud",
+                   stream=None):
+        """sm_track_frame_rgbd: track() with the registered colour image as well (colour [H, W, 3] uint8 CUDA tensor,
+        r, g, b): joint point-to-plane and photometric Gauss-Newton, which also pins down the motions a single plane or
+        a corridor leaves free wherever the surface has texture. source="previous" needs the previous tracking call
+        on this handle to have been a track_rgbd() call. Synchronous. Returns (pose [3, 4] float32,
+        TrackRGBDResult); a lost frame returns the guess with depth.tracked = 0."""
+        if source not in ("cloud", "previous"):
+            raise ValueError(f"source must be 'cloud' or 'previous', got {source!r}")
+        tp = TrackParams.defaults() if params is None else TrackParams.from_buffer_copy(params)
+        tp.model_source = _lib.TRACK_CLOUD if source == "cloud" else _lib.TRACK_PREVIOUS_FRAME
+        rp = TrackRGBDParams.defaults() if rgbd is None else rgbd
+        pp = pp if pp is not None else PreprocessParams.defaults()
+        self._check_raster("depth", depth, (self.height, self.width), torch.uint16)
+        self._check_raster("color", color, (self.height, self.width, 3), torch.uint8)
+        dp, dpitch = _raster(depth)
+        cp, cpitch = _raster(color, 3)
+        g = _mat12(guess)
+        out = np.zeros(12, np.float32)
+        result = TrackRGBDResult()
+        self.lib.call("track_frame_rgbd", self._h, _stream_handle(stream), C.byref(tp), C.byref(pp), C.byref(rp), dp,
+                      dpitch, cp, cpitch, g.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p),
+                      C.byref(result))
+        return out.reshape(3, 4), result
+
+    def track_linearize_rgbd(self, level: int, live_depth, live_color, model_depth, model_normal, model_color,
+                             model_T_live, params: Optional[TrackParams] = None,
+                             rgbd: Optional[TrackRGBDParams] = None, depth_scaling: float = 5000.0, stream=None):
+        """sm_track_linearize_rgbd: one joint linearisation of a filtered live level image with the raw live colour
+        (uint8 [H, W, 3] at the handle's camera) against caller model images (depth, normal, colour at the handle's
+        camera). Synchronous. Returns (system float64 [27], sum r_c^2, depth inliers, photometric inliers)."""
+        tp = TrackParams.defaults() if params is None else params
+        rp = TrackRGBDParams.defaults() if rgbd is None else rgbd
+        level = int(level)
+        if not 0 <= level <= 3:
+            raise ValueError(f"level must be in [0, 3], got {level}")
+        factor = float(np.float32(1.0) / np.float32(2.0 ** level))   # Camera.scaled(level) sizes
+        live_shape = (int(factor * self.height + 0.5), int(factor * self.width + 0.5))
+        H, W = self.height, self.width
+        for name, t, shape, dtype in (("live_depth", live_depth, live_shape, torch.uint16),
+                                      ("live_color", live_color, (H, W, 3), torch.uint8),
+                                      ("model_depth", model_depth, (H, W), torch.float32),
+                                      ("model_normal", model_normal, (H, W, 3), torch.float32),
+                                      ("model_color", model_color, (H, W, 3), torch.uint8)):
+            self._check_raster(name, t, shape, dtype)
+        lp, lpitch = _raster(live_depth)
+        lc, lcpitch = _raster(live_color, 3)
+        mp, mpitch = _raster(model_depth)
+        np_, npitch = _raster(model_normal, 3)
+        mc, mcpitch = _raster(model_color, 3)
+        T = _mat12(model_T_live)
+        system = np.zeros(27, np.float64)
+        rc2 = C.c_double()
+        inliers, photometric = C.c_uint32(), C.c_uint32()
+        self.lib.call("track_linearize_rgbd", self._h, _stream_handle(stream), C.byref(tp), C.byref(rp), level,
+                      float(depth_scaling), lp, lpitch, lc, lcpitch, mp, mpitch, np_, npitch, mc, mcpitch,
+                      T.ctypes.data_as(C.c_void_p), system.ctypes.data_as(C.c_void_p), C.byref(rc2), C.byref(inliers),
+                      C.byref(photometric))
+        return system, float(rc2.value), int(inliers.value), int(photometric.value)
+
     def triangulate(self, params: Optional[MeshParams] = None, stream=None):
         """sm_triangulate: the current cloud as a triangle mesh over its slots (include/surfel_b200.h gives the
         rules). Synchronous. Returns (triangles int32 CUDA tensor [T, 3] of slot indices, counter-clockwise about
@@ -738,11 +804,14 @@ def _to4(m) -> np.ndarray:
 
 class TrackedSession:
     """A pose-free stream: every frame is tracked (sm_track_frame) and then pushed into a StreamSession with the pose
-    it tracked. Only the first frame's camera-to-world pose is given. Frames are at the handle's camera size.
+    it tracked. Only the first frame's camera-to-world pose is given. Frames are at the handle's camera size. With
+    `rgbd` set, every frame is tracked with its own colour as well (sm_track_frame_rgbd), the first one included, so
+    that its intensity is kept as the model of the second.
 
     Each frame after the first starts from a constant-velocity guess, T_{k-1} (T_{k-2}^-1 T_{k-1}). It is tracked
     against the previous frame until the session has integrated a frame, and against the cloud after that. A lost
-    frame keeps its guess. `trajectory` holds the [3, 4] float32 poses pushed, `results` the TrackResults::
+    frame keeps its guess. `trajectory` holds the [3, 4] float32 poses pushed, `results` the TrackResults
+    (TrackRGBDResults with `rgbd`)::
 
         with TrackedSession(rec, pp, ip, first_pose) as s:
             for depth, color in frames:
@@ -751,9 +820,11 @@ class TrackedSession:
     """
 
     def __init__(self, rec: CUDASurfelReconstruction, pp: PreprocessParams, ip: IntegrateParams, first_pose,
-                 params: Optional[TrackParams] = None, first_frame_index: int = 0, stream=None):
+                 params: Optional[TrackParams] = None, first_frame_index: int = 0, stream=None,
+                 rgbd: Optional[TrackRGBDParams] = None):
         self.rec, self.pp = rec, pp
         self.params = TrackParams.defaults() if params is None else params
+        self.rgbd = rgbd
         self.first_pose = np.asarray(first_pose, np.float32).reshape(3, 4)
         self.session = StreamSession(rec, pp, ip, (rec.width, rec.height), first_frame_index, stream)
         self.trajectory: list = []
@@ -769,15 +840,21 @@ class TrackedSession:
     def push(self, depth, color) -> SessionStatus:
         d = depth if isinstance(depth, torch.Tensor) and depth.is_cuda else torch.as_tensor(np.asarray(depth)).cuda()
         stream = self.session.stream
+        if self.rgbd is None:
+            track = lambda *args: self.rec.track(d, *args)
+        else:
+            c = color if isinstance(color, torch.Tensor) and color.is_cuda else torch.as_tensor(np.asarray(color)).cuda()
+            track = lambda guess, params, pp, source, stream: self.rec.track_rgbd(d, c, guess, params, self.rgbd, pp,
+                                                                                  source, stream)
         if not self.trajectory:
             # the first frame's view is kept as the model of the second: no Gauss-Newton steps, the given pose
             seed = TrackParams.from_buffer_copy(self.params)
             seed.levels = 1
             seed.iterations = (C.c_int32 * 4)(0, 0, 0, 0)
-            pose, result = self.rec.track(d, self.first_pose, seed, self.pp, "cloud", stream)
+            pose, result = track(self.first_pose, seed, self.pp, "cloud", stream)
         else:
-            pose, result = self.rec.track(d, self.guess(), self.params, self.pp,
-                                          "cloud" if self.integrated else "previous", stream)
+            pose, result = track(self.guess(), self.params, self.pp, "cloud" if self.integrated else "previous",
+                                 stream)
         self.trajectory.append(pose)
         self.results.append(result)
         status = self.session.push(depth, color, pose, invert_rigid(pose))
