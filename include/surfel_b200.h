@@ -596,6 +596,110 @@ int sm_track_linearize_rgbd(sm_reconstruction* r, void* stream, const sm_track_p
                             const float model_T_live[12], double out_system[27], double* out_sum_rc2,
                             uint32_t* out_inliers, uint32_t* out_photometric_inliers);
 
+/* ---- relocalisation: a keyframe database of random-fern codes (DESIGN.md section 1 row f13, section 5.11) --------
+ * A tracker that tracks against its own model has a small basin: a lost camera does not come back by itself. As in
+ * ElasticFusion (Glocker et al., "Real-Time RGB-D Camera Relocalization via Randomized Ferns for Keyframe Encoding",
+ * TVCG 2015), a frame is reduced to `ferns` 4-bit codes, keyframes are stored by code, a lost frame is matched to
+ * its nearest keyframes by block Hamming distance and tracking is restarted from their poses. The database is an
+ * object of its own (like sm_knn_index), bound to the device and the camera size of the handle it was created from;
+ * it is created on the current device, which must be the handle's.
+ * Every rule below is integer or fp64 arithmetic, so codes, distances and decisions are exact.
+ *  F1. Fern image. L = level in [1, 4]; w = int(W / 2^L + 0.5), h = int(H / 2^L + 0.5) (Camera.scaled(L) of the
+ *      handle's W x H camera). Depth D: the raw u16 depth downscaled to w x h by sm_downscale_using_median_while_excluding
+ *      (0, ...). Colour: the input block of pixel (x, y) is [W x / w, W (x + 1) / w) x [H y / h, H (y + 1) / h) (integer
+ *      division, the median's block); each channel is (S + n / 2) / n in integers, S the sum over the block's n pixels
+ *      of the raw packed u8x3 colour. sm_keyframe_db_create rejects a level whose blocks exceed 16 x 16 pixels.
+ *  F2. Fern tables, drawn once at creation by splitmix64 from `seed` (state += 0x9E3779B97F4A7C15; z = state;
+ *      z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9; z = (z ^ (z >> 27)) * 0x94D049BB133111EB; next = z ^ (z >> 31)),
+ *      for f = 0 .. ferns-1 in order, six draws per fern: x = (next >> 32) % w, y = (next >> 32) % h, then the
+ *      thresholds t_R, t_G, t_B = next >> 56 each, then t_D = min_depth + (max_depth - min_depth) *
+ *      ((next >> 11) * 2^-53) in fp64 (metres; min_depth and max_depth converted to double first). ferns is a multiple
+ *      of 8 in [8, 2048].
+ *  F3. Code. Nibble f: bit0 = R >= t_R, bit1 = G >= t_G, bit2 = B >= t_B, bit3 = (D > 0 and double(D) >= t_D *
+ *      double(depth_scaling)), with (R, G, B, D) the fern image at (x_f, y_f). Fern f is the nibble at bits
+ *      4 (f % 8) of 32-bit word f / 8; a code is ferns / 8 words.
+ *  F4. Distance between two codes: the number of ferns whose nibbles differ (block Hamming distance).
+ *  F5. Query: the distances to every stored keyframe; the keys (distance << 32 | index) in ascending order, the first
+ *      `candidates` (at most 8) of them, without those with double(distance) > double(max_query_fraction) * ferns.
+ *  F6. Add: the frame's code and its global_T_frame are appended as keyframe `count` when the database is empty, when
+ *      force != 0, or when its smallest distance to a stored keyframe d satisfies double(d) > double(add_fraction) *
+ *      ferns. A frame that would be appended to a database holding `capacity` keyframes is not, and `full` is set.
+ *      Nothing is ever evicted.
+ *  F7. Relocalise: the query (F5) with the call's params; then, for each candidate in order, sm_track_frame (or
+ *      sm_track_frame_rgbd when rp != NULL) against the cloud (params.track with model_source = SM_TRACK_CLOUD)
+ *      from the keyframe's pose, with the call's pp (and rp). The first candidate whose call reports tracked,
+ *      double(inliers) >= double(accept_inlier_fraction) * double(valid_pixels) and rms_residual <= accept_rms is
+ *      accepted: global_T_out is that call's pose bit for bit, result.relocalised = 1 and result.keyframe / rank /
+ *      distance / track name the candidate and that call's result. Otherwise relocalised = 0, keyframe = rank = -1,
+ *      global_T_out is NaN and result.track is the last attempt's (zero without attempts). attempts = the tracking
+ *      calls made (0 for an empty database or no candidate within the query bound).
+ *      The handle's "previous frame" (SM_TRACK_PREVIOUS_FRAME) afterwards is that of the last attempt, as for any
+ *      tracking call: this frame, with the accepted pose when one was accepted, otherwise the pose the last attempt
+ *      returned (its guess if it was lost). Without attempts it is left as it was. Only reads the surfel state.
+ *
+ * Kernels (one stream, a fixed launch count): a frame is encoded by the median downscale and k_reloc_encode; add and
+ * query run k_reloc_distance (one warp per keyframe) and k_reloc_select (one block: the top candidates, and for add
+ * the F6 decision and the append on the device), then one synchronisation. sm_relocalise adds one tracking call's
+ * launches per attempt. sm_keyframe_db_create uploads the tables and allocates every buffer (codes for `capacity`
+ * keyframes, the fern image, one code, the distances, the selection result); no later call allocates. Calls on one
+ * database are serialised by the caller.
+ *
+ * sm_keyframe_db_encode writes the code (F3) of a frame to out_codes (device, ferns / 8 words), asynchronously on
+ * `stream`. sm_keyframe_db_add (F6) and sm_keyframe_db_query (F5; out_index / out_distance hold `candidates`
+ * entries, *found are filled) are synchronous. sm_keyframe_db_read copies keyframe `index`'s pose (host, 12 floats)
+ * and / or code (host, ferns / 8 words); either may be NULL. sm_relocalise params: NULL uses the database's own;
+ * otherwise its level, ferns, seed, min_depth, max_depth and capacity must equal the database's.
+ * SM_ERR_INVALID_ARGUMENT, with no launch, for NULL pointers, a pitch below the row size, params outside their
+ * ranges (below), depth_scaling not finite and > 0, a non-finite global_T_frame, an index >= count, and a database
+ * created from a handle of another camera size or device than `r`. Everything is allowed while a stream session is
+ * open on `r` (like sm_track_frame; the database reads no surfel state except through the tracking calls).
+ * Ranges: level 1..4 with blocks <= 16 x 16, ferns % 8 == 0 in [8, 2048], 0 <= min_depth < max_depth finite,
+ * capacity in [1, 2^20], add_fraction and max_query_fraction finite in [0, 1], candidates 1..8,
+ * accept_inlier_fraction finite in [0, 1], accept_rms finite and >= 0, track as sm_track_frame checks it. */
+#define SM_RELOC_MAX_CANDIDATES 8
+typedef struct sm_reloc_params {
+  int32_t level;                   /* fern image level, 1..4 (3) */
+  int32_t ferns;                   /* multiple of 8 in [8, 2048] (512) */
+  uint64_t seed;                   /* splitmix64 seed of the fern tables (20150401) */
+  float min_depth, max_depth;      /* metres, range of the depth thresholds (0.3, 4.0) */
+  uint32_t capacity;               /* keyframes (4096) */
+  float add_fraction;              /* F6 (0.2) */
+  int32_t candidates;              /* F5, 1..8 (1) */
+  float max_query_fraction;        /* F5 (0.4) */
+  sm_track_params track;           /* F7: the tracking calls (sm_default_track_params, max_point_distance 0.1) */
+  float accept_inlier_fraction;    /* F7 (0.7) */
+  float accept_rms;                /* metres, F7 (0.01) */
+} sm_reloc_params;
+typedef struct sm_reloc_result {
+  int32_t relocalised;             /* 1 = global_T_out is the accepted pose; 0 = NaN */
+  int32_t attempts;                /* tracking calls made */
+  int32_t keyframe;                /* accepted keyframe, -1 */
+  int32_t rank;                    /* its rank among the candidates, -1 */
+  uint32_t distance;               /* its distance (F4), 0 */
+  sm_track_result track;           /* the accepted call's; the last attempt's when none was accepted */
+} sm_reloc_result;
+typedef struct sm_keyframe_db sm_keyframe_db;
+/* Host only, no device needed. */
+void sm_default_reloc_params(sm_reloc_params* p);
+int sm_keyframe_db_create(sm_keyframe_db** out, sm_reconstruction* r, const sm_reloc_params* params);
+void sm_keyframe_db_destroy(sm_keyframe_db* db);
+int sm_keyframe_db_reset(sm_keyframe_db* db);
+int sm_keyframe_db_count(sm_keyframe_db* db, uint32_t* out);
+int sm_keyframe_db_encode(sm_keyframe_db* db, void* stream, const uint16_t* depth, size_t depth_pitch,
+                          const uint8_t* color, size_t color_pitch, float depth_scaling, uint32_t* out_codes);
+int sm_keyframe_db_add(sm_keyframe_db* db, void* stream, const uint16_t* depth, size_t depth_pitch,
+                       const uint8_t* color, size_t color_pitch, float depth_scaling, const float global_T_frame[12],
+                       int32_t force, int32_t* out_index /* -1: not appended */, int32_t* out_full);
+int sm_keyframe_db_query(sm_keyframe_db* db, void* stream, const uint16_t* depth, size_t depth_pitch,
+                         const uint8_t* color, size_t color_pitch, float depth_scaling, int32_t* out_index,
+                         uint32_t* out_distance, int32_t* out_found);
+int sm_keyframe_db_read(sm_keyframe_db* db, uint32_t index, float pose[12] /* may be NULL */,
+                        uint32_t* codes /* may be NULL */);
+int sm_relocalise(sm_reconstruction* r, sm_keyframe_db* db, void* stream, const sm_reloc_params* params,
+                  const sm_preprocess_params* pp, const sm_track_rgbd_params* rp /* NULL: depth only */,
+                  const uint16_t* depth, size_t depth_pitch, const uint8_t* color, size_t color_pitch,
+                  float global_T_out[12], sm_reloc_result* result);
+
 /* ---- triangulating the surfel cloud (DESIGN.md section 1 row f9, section 5.7) ---------------------------------
  * The reference's meshing thread grows its mesh by advancing triangle fronts one surfel at a time
  * (APP/surfel_meshing.cc:667-752), which is sequential by construction. sm_triangulate meshes the whole current
@@ -872,7 +976,7 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * work waits for them: the hand-off calls (sm_transfer_all_to_cpu, sm_transfer_delta_to_cpu,
  * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
  * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_render_mesh, sm_track_frame,
- * sm_track_linearize, sm_track_frame_rgbd, sm_track_linearize_rgbd,
+ * sm_track_linearize, sm_track_frame_rgbd, sm_track_linearize_rgbd, sm_relocalise,
  * sm_mesh_update, sm_mesh_read, sm_triangulate, sm_surfel_count / sm_surfels_size) and
  * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
  * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which

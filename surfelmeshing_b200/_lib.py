@@ -189,6 +189,32 @@ class MeshUpdateStats(C.Structure):
                 ("triangles_removed", C.c_uint64), ("full_sweep", C.c_int32), ("reserved", C.c_int32)]
 
 
+RELOC_MAX_CANDIDATES = 8
+
+
+class RelocParams(C.Structure):
+    """sm_reloc_params: the fern image level, fern count, table seed and depth-threshold range (metres), the keyframe
+    capacity, the add and query bounds (fractions of the fern count), the candidates tried, the tracking parameters
+    of a relocalisation attempt and its acceptance thresholds (inlier fraction, RMS residual in metres)."""
+    _fields_ = [("level", C.c_int32), ("ferns", C.c_int32), ("seed", C.c_uint64), ("min_depth", C.c_float),
+                ("max_depth", C.c_float), ("capacity", C.c_uint32), ("add_fraction", C.c_float),
+                ("candidates", C.c_int32), ("max_query_fraction", C.c_float), ("track", TrackParams),
+                ("accept_inlier_fraction", C.c_float), ("accept_rms", C.c_float)]
+
+    @classmethod
+    def defaults(cls) -> "RelocParams":
+        track = TrackParams.defaults()
+        track.max_point_distance = 0.1
+        return cls(3, 512, 20150401, 0.3, 4.0, 4096, 0.2, 1, 0.4, track, 0.7, 0.01)
+
+
+class RelocResult(C.Structure):
+    """sm_reloc_result: relocalised (0 = the pose is NaN), tracking attempts, the accepted keyframe, its rank and
+    distance (-1 / -1 / 0 when none), and the accepted attempt's TrackResult (the last attempt's otherwise)."""
+    _fields_ = [("relocalised", C.c_int32), ("attempts", C.c_int32), ("keyframe", C.c_int32), ("rank", C.c_int32),
+                ("distance", C.c_uint32), ("track", TrackResult)]
+
+
 MESH_MAX_UMBRELLA = 16
 MESH_ALL, MESH_ADDED, MESH_REMOVED = 0, 1, 2
 
@@ -276,6 +302,17 @@ _PRODUCT_ONLY = {
     "triangulate": (C.c_int, [_P, _P, C.POINTER(MeshParams), _P, C.c_uint64, C.POINTER(MeshStats)]),
     "mesh_update": (C.c_int, [_P, _P, C.POINTER(MeshParams), C.POINTER(MeshUpdateStats)]),
     "mesh_read": (C.c_int, [_P, _P, _I, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "default_reloc_params": (None, [C.POINTER(RelocParams)]),
+    "keyframe_db_create": (C.c_int, [C.POINTER(_P), _P, C.POINTER(RelocParams)]),
+    "keyframe_db_destroy": (None, [_P]),
+    "keyframe_db_reset": (C.c_int, [_P]),
+    "keyframe_db_count": (C.c_int, [_P, C.POINTER(_U32)]),
+    "keyframe_db_encode": (C.c_int, [_P, _P, _P, _SZ, _P, _SZ, _F, _P]),
+    "keyframe_db_add": (C.c_int, [_P, _P, _P, _SZ, _P, _SZ, _F, _P, _I, C.POINTER(_I), C.POINTER(_I)]),
+    "keyframe_db_query": (C.c_int, [_P, _P, _P, _SZ, _P, _SZ, _F, _P, _P, C.POINTER(_I)]),
+    "keyframe_db_read": (C.c_int, [_P, _U32, _P, _P]),
+    "relocalise": (C.c_int, [_P, _P, _P, C.POINTER(RelocParams), C.POINTER(PreprocessParams),
+                             C.POINTER(TrackRGBDParams), _P, _SZ, _P, _SZ, _P, C.POINTER(RelocResult)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

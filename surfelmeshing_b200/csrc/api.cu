@@ -131,7 +131,8 @@ const char* KernelName(int id) {
       "k_mesh_scan", "k_mesh_write", "k_mesh_changes", "k_mesh_mark", "k_mesh_owners", "k_mesh_umbrella_update",
       "k_mesh_recheck", "k_mesh_recheck_write", "k_mesh_render_mark", "k_mesh_render_tri", "k_mesh_render_large",
       "k_mesh_render_splat", "k_mesh_render_splat_large", "k_mesh_render_resolve",
-      "k_track_intensity_base", "k_track_intensity_down", "k_track_linearize_rgbd", "k_track_solve_rgbd"};
+      "k_track_intensity_base", "k_track_intensity_down", "k_track_linearize_rgbd", "k_track_solve_rgbd",
+      "k_reloc_encode", "k_reloc_distance", "k_reloc_select"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 

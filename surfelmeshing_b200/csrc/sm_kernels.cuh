@@ -39,6 +39,7 @@ enum KernelId {
   KID_MESH_RENDER_MARK, KID_MESH_RENDER_TRI, KID_MESH_RENDER_LARGE, KID_MESH_RENDER_SPLAT, KID_MESH_RENDER_SPLAT_LARGE,
   KID_MESH_RENDER_RESOLVE,
   KID_TRACK_INTENSITY_BASE, KID_TRACK_INTENSITY_DOWN, KID_TRACK_LINEARIZE_RGBD, KID_TRACK_SOLVE_RGBD,
+  KID_RELOC_ENCODE, KID_RELOC_DISTANCE, KID_RELOC_SELECT,
   KID_COUNT
 };
 const char* KernelName(int id);

@@ -20,8 +20,9 @@ import torch
 
 from . import _lib
 from . import mesh_io
-from ._lib import (IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats, PreprocessParams, RenderParams,
-                   SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult, TrackRGBDParams, TrackRGBDResult,
+from ._lib import (IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats, PreprocessParams, RelocParams,
+                   RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult,
+                   TrackRGBDParams, TrackRGBDResult,
                    TransferStats, TransferToken, VisualizationParams)
 
 RENDER_OUTPUTS = ("depth", "color", "normal", "index")
@@ -522,6 +523,26 @@ class CUDASurfelReconstruction:
                       C.byref(photometric))
         return system, float(rc2.value), int(inliers.value), int(photometric.value)
 
+    def relocalise(self, db: "KeyframeDatabase", depth, color, params: Optional[RelocParams] = None,
+                   rgbd: Optional[TrackRGBDParams] = None, pp: Optional[PreprocessParams] = None, stream=None):
+        """sm_relocalise: the pose of a frame the tracker lost (raw depth [H, W] uint16 and colour [H, W, 3] uint8 CUDA
+        tensors at the handle's camera size), tracked against the cloud from the poses of `db`'s nearest keyframes in
+        turn (params: the query and acceptance fields; None = the database's own). With `rgbd` the attempts track with
+        colour (sm_track_frame_rgbd). Synchronous. Returns (pose [3, 4] float32, NaN when not relocalised,
+        RelocResult)."""
+        p = db.params if params is None else params
+        pp = pp if pp is not None else PreprocessParams.defaults()
+        self._check_raster("depth", depth, (self.height, self.width), torch.uint16)
+        self._check_raster("color", color, (self.height, self.width, 3), torch.uint8)
+        dp, dpitch = _raster(depth)
+        cp, cpitch = _raster(color, 3)
+        out = np.zeros(12, np.float32)
+        result = RelocResult()
+        self.lib.call("relocalise", self._h, db._h, _stream_handle(stream), C.byref(p), C.byref(pp),
+                      C.byref(rgbd) if rgbd is not None else None, dp, dpitch, cp, cpitch,
+                      out.ctypes.data_as(C.c_void_p), C.byref(result))
+        return out.reshape(3, 4), result
+
     def triangulate(self, params: Optional[MeshParams] = None, stream=None):
         """sm_triangulate: the current cloud as a triangle mesh over its slots (include/surfel_b200.h gives the
         rules). Synchronous. Returns (triangles int32 CUDA tensor [T, 3] of slot indices, counter-clockwise about
@@ -723,6 +744,89 @@ class CUDASurfelReconstruction:
         return StreamSession(self, pp, ip, frame_size, first_frame_index, stream)
 
 
+class KeyframeDatabase:
+    """A keyframe database of random-fern codes (sm_keyframe_db_create), bound to the device and camera size of
+    `rec`: add() stores frames that look new with their poses, query() finds the stored keyframes nearest to a frame,
+    and CUDASurfelReconstruction.relocalise() restarts tracking from them. Frames are raw depth [H, W] uint16 and
+    colour [H, W, 3] uint8 CUDA tensors at the handle's camera size."""
+
+    def __init__(self, rec: CUDASurfelReconstruction, params: Optional[RelocParams] = None):
+        self.lib = rec.lib
+        self.params = RelocParams.defaults() if params is None else RelocParams.from_buffer_copy(params)
+        self.width, self.height = rec.width, rec.height
+        self.words = self.params.ferns // 8
+        h = C.c_void_p()
+        self.lib.call("keyframe_db_create", C.byref(h), rec._h, C.byref(self.params))
+        self._h = h
+
+    def close(self):
+        if self._h:
+            self.lib.fn["keyframe_db_destroy"](self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _frame(self, depth, color):
+        for name, t, shape, dtype in (("depth", depth, (self.height, self.width), torch.uint16),
+                                      ("color", color, (self.height, self.width, 3), torch.uint8)):
+            if not isinstance(t, torch.Tensor) or tuple(t.shape) != shape or t.dtype != dtype:
+                raise ValueError(f"{name} must be a {dtype} tensor of shape {shape}")
+        return (*_raster(depth), *_raster(color, 3))
+
+    def __len__(self) -> int:
+        n = C.c_uint32()
+        self.lib.call("keyframe_db_count", self._h, C.byref(n))
+        return int(n.value)
+
+    def reset(self):
+        """Forgets every keyframe (the fern tables stay)."""
+        self.lib.call("keyframe_db_reset", self._h)
+
+    def encode(self, depth, color, depth_scaling: float = 5000.0, stream=None) -> torch.Tensor:
+        """sm_keyframe_db_encode: the frame's code, int32 CUDA tensor [ferns / 8] (the uint32 words' bits)."""
+        out = torch.empty(self.words, dtype=torch.int32, device=depth.device)
+        self.lib.call("keyframe_db_encode", self._h, _stream_handle(stream), *self._frame(depth, color),
+                      float(depth_scaling), C.c_void_p(out.data_ptr()))
+        return out
+
+    def add(self, depth, color, global_T_frame, force: bool = False, depth_scaling: float = 5000.0, stream=None):
+        """sm_keyframe_db_add: stores the frame as a keyframe if the database is empty, `force` is set, or it is far
+        enough from every stored one. Synchronous. Returns (index, or -1 when not stored, full)."""
+        g = _mat12(global_T_frame)
+        index, full = C.c_int32(), C.c_int32()
+        self.lib.call("keyframe_db_add", self._h, _stream_handle(stream), *self._frame(depth, color),
+                      float(depth_scaling), g.ctypes.data_as(C.c_void_p), 1 if force else 0, C.byref(index),
+                      C.byref(full))
+        return int(index.value), bool(full.value)
+
+    def query(self, depth, color, depth_scaling: float = 5000.0, stream=None):
+        """sm_keyframe_db_query: the nearest keyframes in (distance, index) order within the query bound. Synchronous.
+        Returns (indices int32 [found], distances uint32 [found])."""
+        index = np.zeros(_lib.RELOC_MAX_CANDIDATES, np.int32)
+        distance = np.zeros(_lib.RELOC_MAX_CANDIDATES, np.uint32)
+        found = C.c_int32()
+        self.lib.call("keyframe_db_query", self._h, _stream_handle(stream), *self._frame(depth, color),
+                      float(depth_scaling), index.ctypes.data_as(C.c_void_p), distance.ctypes.data_as(C.c_void_p),
+                      C.byref(found))
+        return index[:found.value].copy(), distance[:found.value].copy()
+
+    def pose(self, i: int) -> np.ndarray:
+        """The [3, 4] float32 global_T_frame keyframe `i` was stored with."""
+        out = np.zeros(12, np.float32)
+        self.lib.call("keyframe_db_read", self._h, int(i), out.ctypes.data_as(C.c_void_p), None)
+        return out.reshape(3, 4)
+
+    def code(self, i: int) -> np.ndarray:
+        """Keyframe `i`'s code, uint32 [ferns / 8]."""
+        out = np.zeros(self.words, np.uint32)
+        self.lib.call("keyframe_db_read", self._h, int(i), None, out.ctypes.data_as(C.c_void_p))
+        return out
+
+
 def _dtype_name(a) -> str:
     """'uint16', 'uint8', ... of a torch tensor or a numpy-convertible array."""
     if isinstance(a, torch.Tensor):
@@ -817,36 +921,50 @@ class TrackedSession:
             for depth, color in frames:
                 s.push(depth, color)
         s.trajectory
-    """
+
+    With `reloc` set, the session keeps a KeyframeDatabase (`database`): every frame tracked or relocalised against
+    the cloud is offered to it (add()). A lost frame is relocalised (CUDASurfelReconstruction.relocalise, with colour
+    when `rgbd` is set): if that succeeds it is pushed with the relocalised pose and the constant-velocity guess
+    restarts from that pose; if not, the frame is held out of the session (not pushed, push() returns None) and the
+    next frame tries again. `trajectory` stays indexed by frame, with NaN poses for held-out frames. `states` holds
+    "tracked", "relocalised" or "lost" per frame (without `reloc` a "lost" frame is pushed with its guess, as
+    above) and `reloc_results` the RelocResult of each relocalisation (None where none was tried)."""
 
     def __init__(self, rec: CUDASurfelReconstruction, pp: PreprocessParams, ip: IntegrateParams, first_pose,
                  params: Optional[TrackParams] = None, first_frame_index: int = 0, stream=None,
-                 rgbd: Optional[TrackRGBDParams] = None):
+                 rgbd: Optional[TrackRGBDParams] = None, reloc: Optional[RelocParams] = None):
         self.rec, self.pp = rec, pp
         self.params = TrackParams.defaults() if params is None else params
         self.rgbd = rgbd
+        self.reloc = reloc
         self.first_pose = np.asarray(first_pose, np.float32).reshape(3, 4)
+        self.database = KeyframeDatabase(rec, reloc) if reloc is not None else None
         self.session = StreamSession(rec, pp, ip, (rec.width, rec.height), first_frame_index, stream)
         self.trajectory: list = []
         self.results: list = []
+        self.states: list = []
+        self.reloc_results: list = []
+        self.history: list = []   # the poses the constant-velocity guess extrapolates
         self.integrated = False
 
     def guess(self) -> np.ndarray:
-        if len(self.trajectory) < 2:
-            return self.trajectory[-1]
-        a, b = _to4(self.trajectory[-2]), _to4(self.trajectory[-1])
+        if len(self.history) < 2:
+            return self.history[-1]
+        a, b = _to4(self.history[-2]), _to4(self.history[-1])
         return (b @ np.linalg.inv(a) @ b)[:3].astype(np.float32)
 
-    def push(self, depth, color) -> SessionStatus:
+    def push(self, depth, color) -> Optional[SessionStatus]:
         d = depth if isinstance(depth, torch.Tensor) and depth.is_cuda else torch.as_tensor(np.asarray(depth)).cuda()
         stream = self.session.stream
+        c = None
+        if self.rgbd is not None or self.reloc is not None:
+            c = color if isinstance(color, torch.Tensor) and color.is_cuda else torch.as_tensor(np.asarray(color)).cuda()
         if self.rgbd is None:
             track = lambda *args: self.rec.track(d, *args)
         else:
-            c = color if isinstance(color, torch.Tensor) and color.is_cuda else torch.as_tensor(np.asarray(color)).cuda()
             track = lambda guess, params, pp, source, stream: self.rec.track_rgbd(d, c, guess, params, self.rgbd, pp,
                                                                                   source, stream)
-        if not self.trajectory:
+        if not self.history:
             # the first frame's view is kept as the model of the second: no Gauss-Newton steps, the given pose
             seed = TrackParams.from_buffer_copy(self.params)
             seed.levels = 1
@@ -855,8 +973,23 @@ class TrackedSession:
         else:
             pose, result = track(self.guess(), self.params, self.pp, "cloud" if self.integrated else "previous",
                                  stream)
-        self.trajectory.append(pose)
         self.results.append(result)
+        reloc_result = None
+        state = "tracked" if (result.tracked if self.rgbd is None else result.depth.tracked) else "lost"
+        if self.reloc is not None and self.history and state == "lost":
+            pose, reloc_result = self.rec.relocalise(self.database, d, c, self.reloc, self.rgbd, self.pp, stream)
+            state = "relocalised" if reloc_result.relocalised else "lost"
+        self.states.append(state)
+        self.reloc_results.append(reloc_result)
+        self.trajectory.append(pose)
+        if state == "lost" and self.reloc is not None:
+            return None   # held out: not pushed, the next frame tries again from the same history
+        if state == "relocalised":
+            self.history = [pose]
+        else:
+            self.history.append(pose)
+        if self.reloc is not None and (self.integrated or state == "relocalised"):
+            self.database.add(d, c, pose, depth_scaling=self.pp.depth_scaling, stream=stream)
         status = self.session.push(depth, color, pose, invert_rigid(pose))
         self.integrated = status.last_integrated_frame >= 0
         return status
