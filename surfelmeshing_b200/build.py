@@ -5,10 +5,10 @@ sm_90a (H100) only (no fallback architectures) and links them in-tree into
 surfelmeshing_b200/libsurfel_b200.so, so that the package is importable from the
 repository tree.
 
-`python -m surfelmeshing_b200.build --out variants/lib_x.so -- -DFOO` builds a variant of the
-library for an A/B run (tools/ab_probe.py --lib x=variants/lib_x.so): the same recipe with extra
-nvcc flags, its objects in a directory of their own next to the output (variants/lib_x.objs/), so
-the product's incremental build is left alone.
+`python -m surfelmeshing_b200.build --out variants/lib_x.so [-- extra nvcc flags]` builds a variant
+of the library for an A/B run (tools/ab_probe.py --lib x=variants/lib_x.so) from a patched source
+tree or with extra nvcc flags, its objects in a directory of their own next to the output
+(variants/lib_x.objs/), so the product's incremental build is left alone.
 
 Flags: -ftz=true -fmad=false. The kernels spell out every fp32 operation (csrc/sm_math.cuh)
 in the order of the reference's -use_fast_math SASS; -fmad=false guarantees the compiler

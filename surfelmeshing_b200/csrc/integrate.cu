@@ -258,52 +258,18 @@ __global__ void __launch_bounds__(kProjectBlock) k_project(DeviceState d, FrameP
 // a8 / a9: association and merge gates
 // ---------------------------------------------------------------------------------------
 
-// Everything a gate needs from one pixel, loaded up front so that all gathers of a list
-// entry are in flight together.
+// What the association gates read from one pixel.
 struct PixelGate {
   float measurement_depth;  // depth_correction_factor * depth
   float first;              // first_surfel_depth
   float2 normal;
 };
 
-__device__ __forceinline__ PixelGate load_pixel_gate(const DeviceState& d, const FrameParams& f, int x, int y) {
-  PixelGate g;
-  g.measurement_depth = fmul(u2f(row_ptr(f.depth_pre, f.depth_pre_pitch, y)[x]), f.inv_depth_scaling);
-  g.first = d.first_depth[y * d.width + x];
-  g.normal = row_ptr(f.normals, f.normals_pitch, y)[x];
-  return g;
-}
-
-// Gates shared by association and merge up to the normal-compatibility test
-// (kernels.cu:1603-1668 / :1875-1936). `dot_angle` / `ln`: facing test of this surfel (pixel
-// independent). Returns true if the measurement supports the surfel; writes the
-// conflicting-surfel entry like the reference does.
-__device__ __forceinline__ bool supports_surfel(const DeviceState& d, const FrameParams& f, const PixelGate& g, int p,
-                                                u32 idx, float cz_, float dot_angle, const float3& ln) {
-  if (!(g.measurement_depth > 0.f)) return false;
-  if (g.first < fmul(g.measurement_depth, fadd(-f.sensor_noise_factor, 1.0f))) {
-    if (g.first == cz_) d.assoc[p].y = idx;  // this surfel is conflicting
-    return false;
-  }
-  if (cz_ > fmul(fadd(f.sensor_noise_factor, 1.0f), g.measurement_depth)) return false;  // occluded
-  if (dot_angle > 0.f) return false;  // kSurfelNormalToViewingDirThreshold = 0
-  if (g.measurement_depth < cz_) {
-    const float s = normal_z_abs(g.normal.x, g.normal.y);
-    const float dot2 = ffma(-ln.z, s, ffma(ln.x, g.normal.x, fmul(ln.y, g.normal.y)));
-    if (dot2 < f.cos_normal_compatibility_threshold) return false;
-  }
-  return true;
-}
-
-// SM_ASSOCIATE_LEVELS (compile-time A/B hook): 1 = one batch of gathers per list entry (round 1); 2 = the
-// depth and min-depth of the (up to two) pixels first - five entries out of six stop at the measurement /
-// conflict / occlusion gates that only need those - and the surfel's normal and radius and the pixels'
-// normals only for the rest. Same decisions (pure predicates; the conflicting-surfel entry is written
-// where the reference writes it).
-#ifndef SM_ASSOCIATE_LEVELS
-#define SM_ASSOCIATE_LEVELS 2
-#endif
-
+// Association (kernels.cu:1603-1668) gathers in two levels. Level 1 loads the depth and min-depth of the
+// (up to two) pixels: five entries out of six stop at the measurement / conflict / occlusion gates, which
+// need nothing else. Level 2 loads the surfel's normal and radius and the pixels' normals only for the
+// rest. The gates are pure predicates, so the order decides nothing; the conflicting-surfel entry is
+// written where the reference writes it.
 __global__ void __launch_bounds__(kBlock) k_associate(DeviceState d, FrameParams f) {
   pdl_prologue();
   if (f.skip) return;
@@ -315,16 +281,6 @@ __global__ void __launch_bounds__(kBlock) k_associate(DeviceState d, FrameParams
     const Projection p = project(f, d.width, d.height, x, y, z);
     int ox = p.px, oy = p.py;
     const bool has2 = secondary_pixel(p, d.width, d.height, &ox, &oy);
-#if SM_ASSOCIATE_LEVELS == 1
-    // one batch of gathers
-    const PixelGate g0 = load_pixel_gate(d, f, p.px, p.py);
-    const PixelGate g1 = load_pixel_gate(d, f, ox, oy);
-    const float snx = SM_S(SM_ROW_NORMAL_X, idx), sny = SM_S(SM_ROW_NORMAL_Y, idx), snz = SM_S(SM_ROW_NORMAL_Z, idx);
-    const float surfel_radius_squared = SM_S(SM_ROW_RADIUS_SQUARED, idx);
-    float3 ln;
-    const float dot_angle = facing_dot(f, x, y, z, snx, sny, snz, &ln);
-    bool pass[2] = {true, has2};
-#else
     // level 1: measurement, conflict and occlusion gates (kernels.cu:1603-1632)
     PixelGate g0, g1;
     g0.measurement_depth = fmul(u2f(row_ptr(f.depth_pre, f.depth_pre_pitch, p.py)[p.px]), f.inv_depth_scaling);
@@ -353,24 +309,17 @@ __global__ void __launch_bounds__(kBlock) k_associate(DeviceState d, FrameParams
     g1.normal = row_ptr(f.normals, f.normals_pitch, pass[1] ? oy : p.py)[pass[1] ? ox : p.px];
     float3 ln;
     const float dot_angle = facing_dot(f, x, y, z, snx, sny, snz, &ln);
-#endif
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
       if (!pass[k]) continue;
       const int pp = k == 0 ? p.py * d.width + p.px : oy * d.width + ox;
-#if SM_ASSOCIATE_LEVELS == 1
-      if (!supports_surfel(d, f, k == 0 ? g0 : g1, pp, idx, z, dot_angle, ln)) continue;
-#else
-      {
-        const PixelGate& g = k == 0 ? g0 : g1;
-        if (dot_angle > 0.f) continue;  // kSurfelNormalToViewingDirThreshold = 0
-        if (g.measurement_depth < z) {
-          const float s = normal_z_abs(g.normal.x, g.normal.y);
-          const float dot2 = ffma(-ln.z, s, ffma(ln.x, g.normal.x, fmul(ln.y, g.normal.y)));
-          if (dot2 < f.cos_normal_compatibility_threshold) continue;
-        }
+      const PixelGate& g = k == 0 ? g0 : g1;
+      if (dot_angle > 0.f) continue;  // kSurfelNormalToViewingDirThreshold = 0
+      if (g.measurement_depth < z) {
+        const float s = normal_z_abs(g.normal.x, g.normal.y);
+        const float dot2 = ffma(-ln.z, s, ffma(ln.x, g.normal.x, fmul(ln.y, g.normal.y)));
+        if (dot2 < f.cos_normal_compatibility_threshold) continue;
       }
-#endif
       if (!(surfel_radius_squared > 0.f)) continue;
       PixelAssoc* a = &d.assoc[pp];
       // Reference: atomicCAS(INV -> idx), first come wins. Here: the minimum of a reproducible
@@ -389,17 +338,13 @@ __global__ void __launch_bounds__(kBlock) k_associate(DeviceState d, FrameParams
 // predicates (the one side effect, the conflicting-surfel entry, comes first in the reference too), so
 // they are evaluated cheapest first: level 1 gathers only the surfel's radius and the pixel's depth,
 // min-depth and association record (4 gathers); the 14 row gathers of the surfel and of its merge
-// partner are issued together as level 2, only for the candidates. (Round 1 gathered 11 values for
-// every entry: at BASELINE config 3 the kernel was the longest of the frame.)
-#ifndef SM_MERGE_LEVELS
-#define SM_MERGE_LEVELS 2   // compile-time A/B hook, 1 = round 1's gather order
-#endif
+// partner are issued together as level 2, only for the candidates. (Gathering 11 values for every entry
+// made this the longest kernel of the frame at BASELINE config 3.)
 __global__ void __launch_bounds__(kBlock) k_merge(DeviceState d, FrameParams f) {
   pdl_prologue();
   if (f.skip) return;
   const TimelineScope timeline_scope(d, f.frame_index, KID_MERGE);
   u32 merged_by_thread = 0;
-#if SM_MERGE_LEVELS == 2
   for_each_visible(d, &d.counters->surfel_count[f.count_slot], [&](size_t pos, const VisEntry& e) {
     const u32 idx = e.x & ~kActiveBit;  // no active-window test here (kernels.cu:2016)
     const float x = __uint_as_float(e.y), y = __uint_as_float(e.z), z = __uint_as_float(e.w);
@@ -445,40 +390,6 @@ __global__ void __launch_bounds__(kBlock) k_merge(DeviceState d, FrameParams f) 
     d.merge_flag[pos] = merged ? 1 : 0;
     merged_by_thread += merged ? 1u : 0u;
   });
-#else  // round 1: one batch of 11 gathers per entry, a second one for the candidates
-  for_each_visible(d, &d.counters->surfel_count[f.count_slot], [&](size_t pos, const VisEntry& e) {
-    const u32 idx = e.x & ~kActiveBit;  // no active-window test here (kernels.cu:2016)
-    const float x = __uint_as_float(e.y), y = __uint_as_float(e.z), z = __uint_as_float(e.w);
-    const Projection p = project(f, d.width, d.height, x, y, z);
-    const int pp = p.py * d.width + p.px;
-    // batch 1
-    const PixelGate g = load_pixel_gate(d, f, p.px, p.py);
-    const u32 supported_surfel = supporting_index(f.tb, d.assoc[pp].x, static_cast<u32>(pp));
-    const float surfel_radius_squared = SM_S(SM_ROW_RADIUS_SQUARED, idx);
-    const float snx = SM_S(SM_ROW_NORMAL_X, idx), sny = SM_S(SM_ROW_NORMAL_Y, idx), snz = SM_S(SM_ROW_NORMAL_Z, idx);
-    const float gx = SM_S(SM_ROW_X, idx), gy = SM_S(SM_ROW_Y, idx), gz = SM_S(SM_ROW_Z, idx);
-    bool merged = false;
-    if (surfel_radius_squared >= 0.f) {
-      float3 ln;
-      const float dot_angle = facing_dot(f, x, y, z, snx, sny, snz, &ln);
-      if (supports_surfel(d, f, g, pp, idx, z, dot_angle, ln) && supported_surfel != idx &&
-          supported_surfel != kInvalidIndex) {
-        // batch 2: the supporting surfel (kernels.cu:1955-1984)
-        const u32 q = supported_surfel;
-        const float other_radius_squared = SM_S(SM_ROW_RADIUS_SQUARED, q);
-        const float qx = SM_S(SM_ROW_X, q), qy = SM_S(SM_ROW_Y, q), qz = SM_S(SM_ROW_Z, q);
-        const float qnx = SM_S(SM_ROW_NORMAL_X, q), qny = SM_S(SM_ROW_NORMAL_Y, q), qnz = SM_S(SM_ROW_NORMAL_Z, q);
-        const float radius_diff = fmul(surfel_radius_squared, frcp(other_radius_squared));
-        const float distance_squared = squared_norm(fsub(gx, qx), fsub(gy, qy), fsub(gz, qz));
-        merged = !(radius_diff > 1.4400000572204589844f || radius_diff < 0.69444441795349121094f) &&
-                 !(distance_squared > fmul(fadd(surfel_radius_squared, other_radius_squared), 0.03125f)) &&
-                 !(dot3(snx, sny, snz, qnx, qny, qnz) < 0.93968999385833740234f);  // cos 20 deg
-      }
-    }
-    d.merge_flag[pos] = merged ? 1 : 0;
-    merged_by_thread += merged ? 1u : 0u;
-  });
-#endif
   // Block reduction of the merge count (reference: cub::BlockReduce + atomicAdd, :2045-2051).
   merged_by_thread = __reduce_add_sync(0xffffffffu, merged_by_thread);
   __shared__ u32 warp_sums[kBlock / 32];
@@ -519,12 +430,6 @@ constexpr int kMaxBlendRadius = 64;
 
 __host__ __device__ inline int blend_halo_y(int radius) { return radius - 1 > 1 ? radius - 1 : 1; }  // (radius - 2) iterations + the 3x3 start stencil
 __host__ __device__ inline int blend_halo_x(int radius) { return (blend_halo_y(radius) + 15) & ~15; }  // 16-pixel chunks stay aligned
-
-#ifdef SM_BLEND_CLOCKS
-#define SM_BLEND_CLOCK(i) blend_clock[i] = clock64()
-#else
-#define SM_BLEND_CLOCK(i)
-#endif
 
 // 3x3 dilation of a bit raster (rows of `wpr` words, bit b of word w = pixel 32 w + b) at word
 // (y, w); rows / words outside the raster read as 0.
@@ -567,13 +472,9 @@ __device__ __forceinline__ void append_word_pixels(u32 bits, int y, int w, u16* 
 }
 
 __global__ void __launch_bounds__(kBlendBlock) k_blend(DeviceState d, FrameParams f) {
-#ifdef SM_BLEND_CLOCKS
-  long long blend_clock[5] = {0, 0, 0, 0, 0};
-#endif
   pdl_prologue();
   if (f.skip) return;
   const TimelineScope timeline_scope(d, f.frame_index, KID_BLEND);
-  SM_BLEND_CLOCK(0);
   extern __shared__ __align__(16) unsigned char blend_smem[];
   __shared__ int s_count[kMaxBlendRadius + 1][2];  // pixels per level and ring
   const int radius = f.blend_radius;
@@ -646,7 +547,6 @@ __global__ void __launch_bounds__(kBlendBlock) k_blend(DeviceState d, FrameParam
     reinterpret_cast<u16*>(s_supported)[t] = static_cast<u16>(supported);
   }
   __syncthreads();
-  SM_BLEND_CLOCK(1);
 
   const float depth_scaling = f.depth_scaling;  // the reference passes 1 / depth_correction_factor (kernels.cc:179)
   const float rcp_scaling = frcp(depth_scaling);
@@ -682,7 +582,6 @@ __global__ void __launch_bounds__(kBlendBlock) k_blend(DeviceState d, FrameParam
     append_word_pixels(surfel_border, y, w, s_front + rn16, 0, &s_count[1][1], lane);
   }
   __syncthreads();
-  SM_BLEND_CLOCK(2);
   end0 = s_count[1][0];
   end1 = s_count[1][1];
   if (end0 == 0 && end1 == 0) return;  // no border ring reaches this tile: depth unchanged
@@ -734,7 +633,6 @@ __global__ void __launch_bounds__(kBlendBlock) k_blend(DeviceState d, FrameParam
     }
   }
   __syncthreads();
-  SM_BLEND_CLOCK(3);
   begin0 = end0; end0 += s_count[2][0];
   begin1 = end1; end1 += s_count[2][1];
 
@@ -784,7 +682,6 @@ __global__ void __launch_bounds__(kBlendBlock) k_blend(DeviceState d, FrameParam
     begin1 = end1; end1 += s_count[iteration + 1][1];
   }
 
-  SM_BLEND_CLOCK(4);
   // Write back the tile interior (f.depth holds the same values as f.depth_pre so far: tiles that no
   // ring reaches returned above and keep them).
   constexpr int kChunksPerTileRow = kBlendTileW / 8;
@@ -805,15 +702,6 @@ __global__ void __launch_bounds__(kBlendBlock) k_blend(DeviceState d, FrameParam
         if (gx + k < d.width) out_row[gx + k] = now.e[k];
     }
   }
-#ifdef SM_BLEND_CLOCKS
-  __syncthreads();
-  if (threadIdx.x == 0 && f.frame_index == 450u) {
-    const long long t5 = clock64();
-    printf("blend tile %d,%d load %lld startA %lld startB %lld iter %lld write %lld | final %d %d\n", blockIdx.x, blockIdx.y,
-           blend_clock[1] - blend_clock[0], blend_clock[2] - blend_clock[1], blend_clock[3] - blend_clock[2],
-           blend_clock[4] - blend_clock[3], t5 - blend_clock[4], end0, end1);
-  }
-#endif
 }
 
 // ---------------------------------------------------------------------------------------
@@ -835,22 +723,6 @@ struct PixelMeasurement {
   u32 conflicting, count;
   u32 r, g, b;
 };
-
-__device__ __forceinline__ PixelMeasurement load_pixel_measurement(const DeviceState& d, const FrameParams& f, int x,
-                                                                   int y) {
-  PixelMeasurement m;
-  const int p = y * d.width + x;
-  m.measurement_depth = fmul(u2f(row_ptr(f.depth, f.depth_pitch, y)[x]), f.inv_depth_scaling);
-  m.first = d.first_depth[p];
-  const PixelAssoc a = d.assoc[p];
-  m.conflicting = a.y;
-  m.count = a.z;
-  m.normal = row_ptr(f.normals, f.normals_pitch, y)[x];
-  m.radius_squared = row_ptr(f.radius, f.radius_pitch, y)[x];
-  const uchar3 c = row_ptr(f.color, f.color_pitch, y)[x];
-  m.r = c.x; m.g = c.y; m.b = c.z;
-  return m;
-}
 
 // IntegrateOrConflictSurfel (kernels.cu:741-982) for one (surfel, pixel) pair. The
 // reference serialises accesses to a surfel with a NaN spin-lock on its x coordinate; each
@@ -930,17 +802,6 @@ __device__ __forceinline__ void integrate_or_conflict(const FrameParams& f, cons
   }
 }
 
-// SM_INTEGRATE_LEVELS (compile-time A/B hook, tools/build_variant.sh): 1 = one batch of gathers per list
-// entry (everything the integration can need); 2 = a light first batch (merge flag, radius, and per pixel
-// the depth, the min-depth and the association record) decides whether either pixel can integrate into
-// or conflict with the surfel, and only then the heavy batch (normal / radius / colour rasters, nine
-// surfel rows) is gathered. Only ~10 % of the listed surfels are changed by a frame: with 2 the kernel
-// moves a third of the bytes (it is the longest kernel of BASELINE config 3), at the price of one more
-// dependent level for the surfels that do integrate.
-#ifndef SM_INTEGRATE_LEVELS
-#define SM_INTEGRATE_LEVELS 2
-#endif
-
 // The gates of integrate_or_conflict that only need the light per-pixel values (kernels.cu:757-800):
 // can this pixel integrate into or conflict with the surfel at all?
 __device__ __forceinline__ bool pixel_can_touch(const FrameParams& f, float measurement_depth, float first, u32 conflicting,
@@ -952,6 +813,12 @@ __device__ __forceinline__ bool pixel_can_touch(const FrameParams& f, float meas
 
 // One list entry of k_integrate. Returns whether the surfel goes on the neighbour-update list, with its
 // pixel after the integration in (*ux, *uy).
+// The entry is gathered in two levels. A light first batch (merge flag, radius, and per pixel the depth, the
+// min-depth and the association record) decides whether either pixel can integrate into or conflict with
+// the surfel; only then is the heavy batch (normal / radius / colour rasters, nine surfel rows) gathered.
+// Only ~10 % of the listed surfels are changed by a frame, so the kernel moves a third of the bytes that
+// one batch of everything the integration can need would (it was the longest kernel of BASELINE config 3),
+// at the price of one more dependent level for the surfels that do integrate.
 __device__ __forceinline__ bool integrate_entry(const DeviceState& d, const FrameParams& f, size_t pos, const VisEntry& e,
                                                 int* ux, int* uy) {
     const u32 idx = e.x & ~kActiveBit;
@@ -962,17 +829,6 @@ __device__ __forceinline__ bool integrate_entry(const DeviceState& d, const Fram
     const u8 merged = d.merge_flag[pos];
     SurfelState s;
     PixelMeasurement m0, m1;
-#if SM_INTEGRATE_LEVELS == 1
-    // one batch of gathers: the merge decision, both pixels and the surfel
-    m0 = load_pixel_measurement(d, f, p.px, p.py);
-    m1 = load_pixel_measurement(d, f, ox, oy);
-    s.x = SM_S(SM_ROW_X, idx); s.y = SM_S(SM_ROW_Y, idx); s.z = SM_S(SM_ROW_Z, idx);
-    s.confidence = SM_S(SM_ROW_CONFIDENCE, idx);
-    s.radius_squared = SM_S(SM_ROW_RADIUS_SQUARED, idx);
-    s.nx = SM_S(SM_ROW_NORMAL_X, idx); s.ny = SM_S(SM_ROW_NORMAL_Y, idx); s.nz = SM_S(SM_ROW_NORMAL_Z, idx);
-    s.color = SM_SU(SM_ROW_COLOR, idx);
-    s.creation_stamp = SM_SU(SM_ROW_CREATION_STAMP, idx);
-#else
     // level 1: the merge decision, the radius and the light per-pixel values
     const int p0 = p.py * d.width + p.px, p1 = oy * d.width + ox;
     m0.measurement_depth = fmul(u2f(row_ptr(f.depth, f.depth_pitch, p.py)[p.px]), f.inv_depth_scaling);
@@ -983,7 +839,6 @@ __device__ __forceinline__ bool integrate_entry(const DeviceState& d, const Fram
     m0.conflicting = a0.y; m0.count = a0.z;
     m1.conflicting = a1.y; m1.count = a1.z;
     s.radius_squared = SM_S(SM_ROW_RADIUS_SQUARED, idx);
-#endif
     s.last_update_stamp = 0;
     s.smooth_x = s.smooth_y = s.smooth_z = 0.f;
     s.replaced = false; s.dirty = false; s.stamped = false;
@@ -1003,7 +858,6 @@ __device__ __forceinline__ bool integrate_entry(const DeviceState& d, const Fram
     }
     if (!(e.x & kActiveBit)) return false;
     if (s.radius_squared < 0.f) return false;  // kernels.cu:1050
-#if SM_INTEGRATE_LEVELS != 1
     const bool touch0 = pixel_can_touch(f, m0.measurement_depth, m0.first, m0.conflicting, idx, z);
     const bool touch1 = has2 && pixel_can_touch(f, m1.measurement_depth, m1.first, m1.conflicting, idx, z);
     // level 2: the rest of the pixels that can touch the surfel, and the surfel
@@ -1026,10 +880,6 @@ __device__ __forceinline__ bool integrate_entry(const DeviceState& d, const Fram
       if (touch0) integrate_or_conflict(f, m0, p.px, p.py, idx, x, y, z, s);
       if (touch1) integrate_or_conflict(f, m1, ox, oy, idx, x, y, z, s);
     }
-#else
-    integrate_or_conflict(f, m0, p.px, p.py, idx, x, y, z, s);
-    if (has2) integrate_or_conflict(f, m1, ox, oy, idx, x, y, z, s);
-#endif
     if (s.dirty) {
       SM_S(SM_ROW_X, idx) = s.x; SM_S(SM_ROW_Y, idx) = s.y; SM_S(SM_ROW_Z, idx) = s.z;
       SM_S(SM_ROW_CONFIDENCE, idx) = s.confidence;

@@ -31,16 +31,10 @@ namespace {
 #define SM_SU(row, i) reinterpret_cast<u32*>(d.surfels)[static_cast<size_t>(row) * d.stride + (i)]
 
 constexpr int kBlock = 256;
-// Minimum resident blocks per SM of the two sweeps (1 = whatever the register count gives: 64 and 56 registers,
-// 4 blocks of 256 threads each). A/B hook (tools/build_variant.sh): more resident warps against spills. On an
-// H100 at 400 W (tools/ab_probe.py, VGA stream, median of 5 passes) 6 blocks (40 registers, spills in both
-// sweeps) ran 8 926 frames/s and 8 blocks (32 registers) 7 600, against 8 990-9 643 for the default.
-#ifndef SM_REG_ACCUMULATE_MIN_BLOCKS
-#define SM_REG_ACCUMULATE_MIN_BLOCKS 1
-#endif
-#ifndef SM_REG_STEP_MIN_BLOCKS
-#define SM_REG_STEP_MIN_BLOCKS 1
-#endif
+// The two sweeps ask for a minimum of 1 resident block per SM: 64 and 56 registers, 4 blocks of 256 threads
+// each. The explicit 1 is not the same as no minimum, which gives 60 and 46 registers. More resident warps
+// cost spills: on an H100 at 400 W (tools/ab_probe.py, VGA stream, median of 5 passes) 6 blocks (40 registers,
+// spills in both sweeps) ran 8 926 frames/s and 8 blocks (32 registers) 7 600, against 8 990-9 643 for 1.
 
 struct RegParams {
   u32 frame_index;
@@ -62,7 +56,7 @@ __device__ __forceinline__ bool outside_window(u32 stamp, const RegParams& p) {
   return static_cast<int>(stamp) < static_cast<int>(p.frame_index - static_cast<u32>(p.window));
 }
 
-__global__ void __launch_bounds__(kBlock, SM_REG_ACCUMULATE_MIN_BLOCKS) k_reg_accumulate(DeviceState d, RegParams p) {
+__global__ void __launch_bounds__(kBlock, 1) k_reg_accumulate(DeviceState d, RegParams p) {
   pdl_prologue();
   if (p.skip) return;
   const TimelineScope timeline_scope(d, p.frame_index, KID_REG_ACCUMULATE);
@@ -137,7 +131,7 @@ __global__ void __launch_bounds__(kBlock, SM_REG_ACCUMULATE_MIN_BLOCKS) k_reg_ac
   }
 }
 
-__global__ void __launch_bounds__(kBlock, SM_REG_STEP_MIN_BLOCKS) k_reg_step(DeviceState d, RegParams p) {
+__global__ void __launch_bounds__(kBlock, 1) k_reg_step(DeviceState d, RegParams p) {
   pdl_prologue();
   if (p.skip) return;
   const TimelineScope timeline_scope(d, p.frame_index, KID_REG_STEP);

@@ -62,9 +62,6 @@ struct Splat {
   int x0, y0, x1, y1;     // pixel rectangle (inclusive), inside the image
 };
 
-// Ray coordinate of pixel p: ((p + 0.5) - c) / f with IEEE division.
-__device__ __forceinline__ float ray_coord(int p, float c, float f) { return __fdiv_rn(fsub(fadd(i2f(p), 0.5f), c), f); }
-
 // Pixels [*p0, *p1] of one image axis whose ray coordinate can lie in [lo / z, hi / z] for z in [z_lo, z_hi]
 // (z_lo > 0), plus one pixel on each side for the rounding of the ray coordinate and of this bound, clamped to
 // [0, size - 1]. False if none is inside the image. A NaN bound clamps to the image edge.

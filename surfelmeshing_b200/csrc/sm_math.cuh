@@ -102,4 +102,8 @@ __device__ __forceinline__ const T* row_ptr(const T* base, size_t pitch, int y) 
   return reinterpret_cast<const T*>(reinterpret_cast<const char*>(base) + static_cast<size_t>(y) * pitch);
 }
 
+// Ray coordinate of pixel p: ((p + 0.5) - c) / f with IEEE division. sm_render_surfels casts its rays through the
+// pixel centres with it, and the tracker back-projects the live and the rendered model depth with the same rays.
+__device__ __forceinline__ float ray_coord(int p, float c, float f) { return __fdiv_rn(fsub(fadd(i2f(p), 0.5f), c), f); }
+
 }  // namespace smb

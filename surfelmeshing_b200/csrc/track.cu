@@ -131,9 +131,6 @@ struct SolveArgs {
   float convergence_rotation, convergence_translation;
 };
 
-// ((p + 0.5) - c) / f, IEEE division: the pixel-centre ray of sm_render_surfels.
-__device__ __forceinline__ float ray_coord(int p, float c, float f) { return __fdiv_rn(fsub(fadd(i2f(p), 0.5f), c), f); }
-
 // a.x*b.x + a.y*b.y + a.z*b.z as ((a.x*b.x + a.y*b.y) + a.z*b.z), every product and sum rounded.
 __device__ __forceinline__ float dot_rn(float3 a, float3 b) {
   return fadd(fadd(fmul(a.x, b.x), fmul(a.y, b.y)), fmul(a.z, b.z));
@@ -277,35 +274,11 @@ __global__ void __launch_bounds__(kLinearizeBlock) k_track_linearize(LinearizeAr
                            &n))
       continue;
     acc[kTermValid] += 1.0;
-    const float3 pm = rigid_point(T, p);
-    const float3 nl = rigid_vector(T, n);
-    if (!(pm.z > 0.f)) continue;
-    const float u = fadd(fmul(a.mfx, __fdiv_rn(pm.x, pm.z)), a.mcx);
-    const float v = fadd(fmul(a.mfy, __fdiv_rn(pm.y, pm.z)), a.mcy);
-    if (!(u >= 0.f && u < i2f(a.model_width) && v >= 0.f && v < i2f(a.model_height))) continue;
-    const int ix = static_cast<int>(u), iy = static_cast<int>(v);
-    const float dm = row_ptr(a.model_depth, a.model_depth_pitch, iy)[ix];
-    if (!(dm > 0.f) || !isfinite(dm)) continue;
-    const float* mn = row_ptr(a.model_normal, a.model_normal_pitch, iy) + 3 * static_cast<size_t>(ix);
-    float3 nm = make_float3(mn[0], mn[1], mn[2]);
-    if (!normalize_rn(&nm)) continue;
-    const float3 q = make_float3(fmul(dm, ray_coord(ix, a.mcx, a.mfx)), fmul(dm, ray_coord(iy, a.mcy, a.mfy)), dm);
-    if (dot_rn(nm, q) > 0.f) nm = make_float3(-nm.x, -nm.y, -nm.z);
-    const float3 e = sub_rn(pm, q);
-    if (!(dot_rn(e, e) <= a.max_distance_squared)) continue;
-    if (!(dot_rn(nl, nm) >= a.cos_max_angle)) continue;
+    float3 pm, nm, e;
+    if (!associate(a, T, p, n, &pm, &nm, &e)) continue;
     const float r = dot_rn(nm, e);
-    const float3 c = cross_rn(pm, nm);
-    const double J[6] = {c.x, c.y, c.z, nm.x, nm.y, nm.z};
-    int k = 0;
-#pragma unroll
-    for (int row = 0; row < 6; ++row) {
-#pragma unroll
-      for (int col = row; col < 6; ++col) acc[k++] += J[row] * J[col];
-    }
+    accumulate_row<false>(acc, cross_rn(pm, nm), nm, r, 1.0);
     const double rd = r;
-#pragma unroll
-    for (int row = 0; row < 6; ++row) acc[21 + row] += J[row] * rd;
     acc[kTermR2] += rd * rd;
     acc[kTermInliers] += 1.0;
   }

@@ -80,6 +80,24 @@ def test_library_reads_no_environment():
     assert not readers, readers
 
 
+def test_library_selects_no_compile_time_variant():
+    """The committed sources build one product: a preprocessor conditional may only tell device from host
+    compilation (__CUDA_ARCH__). A variant is a patched tree or extra nvcc flags in a separate build."""
+    csrc = ROOT / "surfelmeshing_b200" / "csrc"
+    switches = []
+    for p in sorted(csrc.iterdir()):
+        if not p.is_file():
+            continue
+        for i, line in enumerate(p.read_text().splitlines(), 1):
+            m = re.match(r"\s*#\s*(if|ifdef|ifndef|elif)\b(.*)", line)
+            if not m:
+                continue
+            names = set(re.findall(r"[A-Za-z_]\w*", m.group(2).split("//")[0])) - {"defined"}
+            if names != {"__CUDA_ARCH__"}:
+                switches.append(f"{p.name}:{i}: {line.strip()}")
+    assert not switches, switches
+
+
 def test_every_configure_key_is_documented():
     """sm_configure accepts named knobs: each key the library tests for appears in the header's description."""
     source = (ROOT / "surfelmeshing_b200" / "csrc" / "api.cu").read_text()
