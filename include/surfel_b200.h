@@ -828,6 +828,92 @@ int sm_mesh_update(sm_reconstruction* r, void* stream, const sm_mesh_params* p, 
 int sm_mesh_read(sm_reconstruction* r, void* stream, int32_t which, uint32_t* triangles /* device, 3 x capacity */,
                  uint64_t capacity, uint64_t* count);
 
+/* ---- closing the small holes of a triangle mesh (DESIGN.md section 1 row f14, section 5.12) -------------------
+ * sm_triangulate and sm_mesh_update output a triangle only when the umbrellas of its three corners agree on it;
+ * where neighbouring tangent planes disagree (usually about the diagonal of a quad) they leave a hole. The
+ * reference's front-advancing mesher closes such holes as it goes (APP/surfel_meshing.cc:368-393, 1870-1944).
+ * sm_mesh_fill_holes closes the small ones afterwards: it takes an edge-manifold, consistently oriented triangle
+ * list over the handle's slots (the output of either call, or any list a caller builds) and returns the triangles
+ * that fill its closable boundary loops. It writes only the new triangles; the caller appends them to its list.
+ * Positions are read from the rows 3-5 mirror of the smooth positions, which the call refreshes as sm_triangulate
+ * does; nothing else of the surfel state is written.
+ *
+ * p_i, n_i (rows 8-10 normalised), the fp32 conventions and rule 2's tangent basis are those of sm_triangulate;
+ * cos_n and cos_t come from the two angles of sm_hole_params the same way. An edge is an ordered pair (a, b) of
+ * slots; the triangle (o, x, y) has the edges (o, x), (x, y) and (y, o). K = max_hole_edges.
+ *  H1. Hole edges. For each input edge (a, b) whose reverse (b, a) is not an input edge, (b, a) is a hole edge: the
+ *      hole lies on its left, and a fill triangle contains it in that direction. Hole edges are ordered by
+ *      (tail, head).
+ *  H2. Successor. The successor of hole edge (u, v) is the hole edge leaving v if there is exactly one, none if
+ *      there is none. With several (v is a pinch vertex): q_x = ((p_x - p_v).t, (p_x - p_v).s) in v's tangent basis
+ *      (t, s) of rule 2, and each candidate (v, w) has the half h_w = 0 if cross(q_u, q_w) < 0, h_w = 1 if
+ *      cross(q_u, q_w) > 0 or (cross(q_u, q_w) == 0 and q_u.q_w < 0), no half otherwise (a NaN cross product
+ *      included). w comes before w' iff
+ *      h_w < h_w', or h_w == h_w' and cross(q_w, q_w') < 0: the order is clockwise from q_u, the side on which the
+ *      hole of (u, v) lies at v. The successor is the candidate that comes before every other one; there is none
+ *      if n_v is not a unit normal, if a candidate has no half, or if no candidate comes before all the others
+ *      (collinear candidates).
+ *  H3. Loops. Following successors from a hole edge, if it comes back to that edge after k <= K edges whose k tails
+ *      are distinct, those k edges form a loop (so every hole edge is in at most one loop). The owner of the loop
+ *      is its smallest edge; L[0..k-1] are the tails of its edges in order, from the owner's tail.
+ *      (L[i], L[i+1 mod k]) are its loop edges.
+ *  H4. Validity. The triangle (L[i], L[j], L[m]), i < j < m, is valid iff: every edge of it that is not a loop edge
+ *      is an input edge in neither direction; all three corners have unit normals with n_a.n_b >= cos_n for each
+ *      pair; in the rotation (o, x, y) that starts at the smallest slot, rule 4's geometric normal g has g.n_c > 0
+ *      at each corner c; and rule 4's angle test with cos_t holds at each corner. Its weight is w = sqrt(g.g).
+ *  H5. Triangulation (minimum area). W(i, i+1) = 0; for m - i >= 2, W(i, m) = the minimum over i < j < m of
+ *      ((W(i, j) + W(j, m)) + w(i, j, m)), an invalid triangle counting as +inf, and j*(i, m) = the smallest j that
+ *      reaches it. The loop is rejected if W(0, k-1) is +inf; otherwise its triangles are (L[i], L[j*], L[m]) for
+ *      the nodes (i, m) of the tree that starts at (0, k-1), where node (i, m) with m - i >= 2 has the children
+ *      (i, j*) and (j*, m). Its diagonals are the unordered pairs {L[i], L[m]} of the nodes other than (0, k-1)
+ *      with m - i >= 2.
+ *  H6. Conflicts. A loop that is not rejected and shares a diagonal with another such loop is dropped, and so is
+ *      that other loop (one symmetric round: loops_conflicting). The other loops are filled.
+ *  H7. Output. The filled loops by owner edge, ascending; the triangles of a loop in the tree's pre-order (node
+ *      (i, m), then the subtree of (i, j*), then that of (j*, m)); each triangle written in the rotation that
+ *      starts at its smallest slot. Input and output together are edge-manifold and consistently oriented.
+ * stats: boundary_edges = hole edges of the input; loops_found = loops of H3; loops_rejected, loops_conflicting,
+ * loops_filled (the three add up to loops_found); triangles_added (set also when the capacity is too small);
+ * boundary_edges_after = the boundary edges of input and fill together = boundary_edges minus the lengths of the
+ * filled loops. All zero when the call fails for any other reason.
+ *
+ * fill is a DEVICE buffer of 3 x capacity uint32 (may be NULL with capacity 0: a count query); if capacity <
+ * triangles_added the call returns SM_ERR_CAPACITY with the stats set and writes nothing. SM_ERR_INVALID_ARGUMENT,
+ * with no launch, for NULL params or stats, triangles NULL with count > 0, fill NULL with capacity > 0, count >=
+ * 2^28, max_hole_edges outside [3, SM_MESH_MAX_HOLE] or an angle outside (0, 180]; and, found on the device and
+ * reported after the call's second synchronisation with nothing written, for a corner >= surfels_size() or whose
+ * slot is not present (radius^2 > 0), a triangle with a repeated corner, or a directed edge that occurs twice.
+ * The call synchronises `stream` three times (surfels_size(); the hole edge count and the input checks; the
+ * triangle count), plus once, with cudaFree's device synchronisation, in a call whose buffers grow (by x 1.5); on
+ * return the fill is written by work enqueued on `stream`. Memory (allocated by the first call, grown with the
+ * input, freed by sm_destroy; sm_create allocates nothing for it): 72 to 120 bytes per triangle of capacity (a
+ * directed-edge hash table, of which a call uses and clears the power of two >= 6 x count, and the unsorted hole
+ * edges) and about 150 to 180 bytes per
+ * hole edge of capacity (the sorted edges and the sort's scratch, the loop and its triangles, the count, the
+ * diagonal table). */
+#define SM_MESH_MAX_HOLE 16
+typedef struct sm_hole_params {
+  int32_t max_hole_edges;                /* 8; in [3, SM_MESH_MAX_HOLE] */
+  float max_angle_between_normals_deg;   /* 90, as sm_mesh_params */
+  float max_triangle_angle_deg;          /* 180 = no angle filter (the reference closes holes with pi,
+                                            APP/surfel_meshing.cc:1874) */
+} sm_hole_params;
+typedef struct sm_hole_stats {
+  uint64_t boundary_edges;         /* of the input mesh */
+  uint64_t loops_found;            /* closed hole loops of <= max_hole_edges edges */
+  uint64_t loops_filled;
+  uint64_t loops_rejected;         /* no valid triangulation */
+  uint64_t loops_conflicting;      /* a diagonal proposed by another loop too */
+  uint64_t triangles_added;        /* always set, also when the capacity was too small */
+  uint64_t boundary_edges_after;
+} sm_hole_stats;
+/* Host only, no device needed. */
+void sm_default_hole_params(sm_hole_params* p);
+int sm_mesh_fill_holes(sm_reconstruction* r, void* stream, const sm_hole_params* p,
+                       const uint32_t* triangles /* device, 3 x count */, uint64_t count,
+                       uint32_t* fill /* device, 3 x capacity; may be NULL with capacity 0 */, uint64_t capacity,
+                       sm_hole_stats* stats);
+
 /* ---- radius-limited k-nearest-neighbour queries for the meshing thread (SURVEY section 8 f4) ----
  * Replaces CompressedOctree::FindNearestSurfelsWithinRadius<include_completed_surfels, include_free_surfels>
  * (octree.h:471, octree.cc:313-470; callers surfel_meshing.cc:421 <false, true> and :821 <true, false>) for a BATCH of

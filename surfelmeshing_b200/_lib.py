@@ -217,6 +217,25 @@ class RelocResult(C.Structure):
 
 MESH_MAX_UMBRELLA = 16
 MESH_ALL, MESH_ADDED, MESH_REMOVED = 0, 1, 2
+MESH_MAX_HOLE = 16
+
+
+class HoleParams(C.Structure):
+    """sm_hole_params: the longest boundary loop filled (edges), the normal gate and the largest triangle angle."""
+    _fields_ = [("max_hole_edges", C.c_int32), ("max_angle_between_normals_deg", C.c_float),
+                ("max_triangle_angle_deg", C.c_float)]
+
+    @classmethod
+    def defaults(cls) -> "HoleParams":
+        return cls(8, 90.0, 180.0)
+
+
+class HoleStats(C.Structure):
+    """sm_hole_stats: boundary edges of the input, loops found / filled / rejected / conflicting, triangles added
+    (also when the capacity was too small) and the boundary edges of input and fill together."""
+    _fields_ = [("boundary_edges", C.c_uint64), ("loops_found", C.c_uint64), ("loops_filled", C.c_uint64),
+                ("loops_rejected", C.c_uint64), ("loops_conflicting", C.c_uint64), ("triangles_added", C.c_uint64),
+                ("boundary_edges_after", C.c_uint64)]
 
 _P = C.c_void_p
 _SZ = C.c_size_t
@@ -302,6 +321,8 @@ _PRODUCT_ONLY = {
     "triangulate": (C.c_int, [_P, _P, C.POINTER(MeshParams), _P, C.c_uint64, C.POINTER(MeshStats)]),
     "mesh_update": (C.c_int, [_P, _P, C.POINTER(MeshParams), C.POINTER(MeshUpdateStats)]),
     "mesh_read": (C.c_int, [_P, _P, _I, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "default_hole_params": (None, [C.POINTER(HoleParams)]),
+    "mesh_fill_holes": (C.c_int, [_P, _P, C.POINTER(HoleParams), _P, C.c_uint64, _P, C.c_uint64, C.POINTER(HoleStats)]),
     "default_reloc_params": (None, [C.POINTER(RelocParams)]),
     "keyframe_db_create": (C.c_int, [C.POINTER(_P), _P, C.POINTER(RelocParams)]),
     "keyframe_db_destroy": (None, [_P]),

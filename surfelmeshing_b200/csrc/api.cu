@@ -132,7 +132,8 @@ const char* KernelName(int id) {
       "k_mesh_recheck", "k_mesh_recheck_write", "k_mesh_render_mark", "k_mesh_render_tri", "k_mesh_render_large",
       "k_mesh_render_splat", "k_mesh_render_splat_large", "k_mesh_render_resolve",
       "k_track_intensity_base", "k_track_intensity_down", "k_track_linearize_rgbd", "k_track_solve_rgbd",
-      "k_reloc_encode", "k_reloc_distance", "k_reloc_select"};
+      "k_reloc_encode", "k_reloc_distance", "k_reloc_select", "k_hole_edges", "k_hole_boundary", "k_hole_sort",
+      "k_hole_walk", "k_hole_conflict", "k_hole_scan", "k_hole_write"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -477,6 +478,7 @@ int sm_destroy(sm_reconstruction* r) {
   FreeRenderBuffers(r);
   FreeTrackBuffers(r);
   FreeMeshBuffers(r);
+  FreeHoleBuffers(r);
   for (cudaStream_t st : {r->upload_stream, r->graph_stream})
     if (st) cudaStreamDestroy(st);
   for (cudaEvent_t e : {r->entry_event, r->upload_done, r->graph_exit})
@@ -756,6 +758,18 @@ int sm_mesh_read(sm_reconstruction* r, void* stream, int32_t which, uint32_t* tr
                  uint64_t* count) {
   if (!r || !count) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_read: null argument");
   return MeshRead(r, static_cast<cudaStream_t>(stream), which, triangles, capacity, count);
+}
+
+void sm_default_hole_params(sm_hole_params* p) {
+  p->max_hole_edges = 8;
+  p->max_angle_between_normals_deg = 90.0f;
+  p->max_triangle_angle_deg = 180.0f;
+}
+
+int sm_mesh_fill_holes(sm_reconstruction* r, void* stream, const sm_hole_params* p, const uint32_t* triangles,
+                       uint64_t count, uint32_t* fill, uint64_t capacity, sm_hole_stats* stats) {
+  if (!r || !p || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_fill_holes: null argument");
+  return FillHoles(r, static_cast<cudaStream_t>(stream), *p, triangles, count, fill, capacity, stats);
 }
 
 int sm_export_vertices(sm_reconstruction* r, void* stream, float* position_buffer, uint8_t* color_buffer) {

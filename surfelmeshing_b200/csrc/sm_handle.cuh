@@ -51,6 +51,7 @@ void DestroySession(StreamSession* s);
 struct TrackState;     // track.cu
 struct MeshCounters;   // mesh.cu
 struct MeshLive;       // mesh.cu: the persistent mesh of sm_mesh_update
+struct HoleScratch;    // holes.cu: the buffers of sm_mesh_fill_holes
 
 }  // namespace smb
 
@@ -183,6 +184,8 @@ struct sm_reconstruction {
   int mesh_umbrella_blocks = 0, mesh_emit_blocks = 0;
   // sm_mesh_update's persistent mesh (mesh.cu), created by the first update; it shares only mesh_index.
   smb::MeshLive* mesh_live = nullptr;
+  // sm_mesh_fill_holes scratch (holes.cu), created by the first call with more than zero triangles.
+  smb::HoleScratch* holes = nullptr;
 };
 
 namespace smb {
@@ -246,6 +249,10 @@ void FreeMeshBuffers(sm_reconstruction* r);
 int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, sm_mesh_update_stats* stats);
 int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t* triangles, uint64_t capacity,
              uint64_t* count);
+// holes.cu
+int FillHoles(sm_reconstruction* r, cudaStream_t stream, const sm_hole_params& p, const uint32_t* triangles,
+              uint64_t count, uint32_t* fill, uint64_t capacity, sm_hole_stats* stats);
+void FreeHoleBuffers(sm_reconstruction* r);
 // pipeline.cu
 int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
               const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats);

@@ -20,8 +20,8 @@ import torch
 
 from . import _lib
 from . import mesh_io
-from ._lib import (IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats, PreprocessParams, RelocParams,
-                   RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult,
+from ._lib import (HoleParams, HoleStats, IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats,
+                   PreprocessParams, RelocParams, RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult,
                    TrackRGBDParams, TrackRGBDResult,
                    TransferStats, TransferToken, VisualizationParams)
 
@@ -603,6 +603,31 @@ class CUDASurfelReconstruction:
             return out[:int(count.value)]
         raise AssertionError("unreachable")
 
+    def fill_holes(self, triangles, params: Optional[HoleParams] = None, stream=None):
+        """sm_mesh_fill_holes: the triangles that close the small boundary loops of `triangles` (an int32 CUDA
+        tensor [T, 3] of slot indices, edge-manifold and consistently oriented, as triangulate() and
+        mesh_triangles() return it; include/surfel_b200.h gives the rules). Synchronous. Returns (fill int32 CUDA
+        tensor [F, 3], in the mesh's convention, to be appended to `triangles`; HoleStats). Asks for the count first
+        (capacity 0), then writes."""
+        p = HoleParams.defaults() if params is None else params
+        if not (isinstance(triangles, torch.Tensor) and triangles.is_cuda and triangles.dtype == torch.int32
+                and triangles.dim() == 2 and triangles.shape[1] == 3):
+            raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+        tri = triangles.contiguous()
+        handle = _stream_handle(stream)
+        stats = HoleStats()
+        fn = self.lib.fn["mesh_fill_holes"]
+        status = fn(self._h, handle, C.byref(p), C.c_void_p(tri.data_ptr()), len(tri), None, 0, C.byref(stats))
+        if status not in (_lib.SM_OK, _lib.SM_ERR_CAPACITY):
+            raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+        capacity = max(int(stats.triangles_added), 1)
+        out = torch.empty((capacity, 3), dtype=torch.int32, device="cuda")
+        if isinstance(stream, torch.cuda.Stream):
+            out.record_stream(stream)
+        self.lib.call("mesh_fill_holes", self._h, handle, C.byref(p), C.c_void_p(tri.data_ptr()), len(tri),
+                      C.c_void_p(out.data_ptr()), capacity, C.byref(stats))
+        return out[:int(stats.triangles_added)], stats
+
     def export_vertices_host(self, stream=None):
         """sm_export_vertices into host arrays: positions [n, 3] float32 (NaN rows for merged slots), colours
         [n, 3] uint8, n = surfels_size()."""
@@ -614,10 +639,15 @@ class CUDASurfelReconstruction:
         torch.cuda.synchronize()
         return pos[:3 * n].cpu().numpy().reshape(n, 3), col[:3 * n].cpu().numpy().reshape(n, 3)
 
-    def save_mesh_obj(self, path, params: Optional[MeshParams] = None, stream=None) -> MeshStats:
+    def save_mesh_obj(self, path, params: Optional[MeshParams] = None, stream=None,
+                      holes: Optional[HoleParams] = None) -> MeshStats:
         """The reference's SaveMeshAsOBJ (main.cc:128-175): the non-merged slots in slot order with their colour,
-        and the triangles of triangulate() over them (1-based, remapped to that order)."""
+        and the triangles of triangulate() over them (1-based, remapped to that order). With `holes`, the
+        triangles of fill_holes(holes) follow the mesh's."""
         tri, stats = self.triangulate(params, stream)
+        if holes is not None:
+            fill, _ = self.fill_holes(tri, holes, stream)
+            tri = torch.cat([tri, fill])
         positions, colors = self.export_vertices_host(stream)
         mesh_io.write_obj(path, positions, colors, tri.cpu().numpy())
         return stats
