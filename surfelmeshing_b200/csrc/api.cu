@@ -159,15 +159,6 @@ LaunchScope::~LaunchScope() {
 
 using namespace smb;
 
-#define SM_CUDA(call)                                                                        \
-  do {                                                                                       \
-    const cudaError_t e_ = (call);                                                           \
-    if (e_ != cudaSuccess) {                                                                 \
-      g_last_error = std::string(#call) + ": " + cudaGetErrorString(e_);                     \
-      return SM_ERR_CUDA;                                                                    \
-    }                                                                                        \
-  } while (0)
-
 namespace {
 // Calls that would change what an open session builds on (sm_session_begin, include/surfel_b200.h).
 int RejectInSession(const char* call) {
@@ -311,19 +302,17 @@ int CreateImpl(sm_reconstruction* r, uint64_t max_surfel_count, int32_t width, i
   d.smooth = r->reg_records;
   d.smooth_next = r->reg_records + d.stride;
   SM_CUDA(cudaMemset(d.gradient, 0, sizeof(float4) * d.stride));
-  for (int i = 0; i < kSets; ++i) {
-    SM_CUDA(cudaMalloc(&r->assoc_set[i], sizeof(PixelAssoc) * P));
-    SM_CUDA(cudaMalloc(&r->first_depth_set[i], sizeof(float) * P));
-    SM_CUDA(cudaMalloc(&r->supported_set[i], P));
-    SM_CUDA(cudaMalloc(&r->vis_set[i], sizeof(VisEntry) * padded));
-    SM_CUDA(cudaMalloc(&r->seg_count_set[i], sizeof(u32) * (padded / kSegment)));
-    SM_CUDA(cudaMalloc(&r->merge_flag_set[i], padded));
-    SM_CUDA(cudaMalloc(&r->upd_list_set[i], sizeof(uint2) * padded));
-    SM_CUDA(cudaMalloc(&r->upd_count_set[i], sizeof(u32)));
+  for (BufferSet& s : r->sets) {
+    SM_CUDA(cudaMalloc(&s.assoc, sizeof(PixelAssoc) * P));
+    SM_CUDA(cudaMalloc(&s.first_depth, sizeof(float) * P));
+    SM_CUDA(cudaMalloc(&s.supported, P));
+    SM_CUDA(cudaMalloc(&s.vis, sizeof(VisEntry) * padded));
+    SM_CUDA(cudaMalloc(&s.seg_count, sizeof(u32) * (padded / kSegment)));
+    SM_CUDA(cudaMalloc(&s.merge_flag, padded));
+    SM_CUDA(cudaMalloc(&s.upd_list, sizeof(uint2) * padded));
+    SM_CUDA(cudaMalloc(&s.upd_count, sizeof(u32)));
   }
-  d.assoc = r->assoc_set[0]; d.first_depth = r->first_depth_set[0]; d.supported = r->supported_set[0];
-  d.vis = r->vis_set[0]; d.seg_count = r->seg_count_set[0]; d.merge_flag = r->merge_flag_set[0];
-  d.upd_list = r->upd_list_set[0]; d.upd_count = r->upd_count_set[0];
+  UseSet(d, r->sets[0]);
   d.reg_t_prev = 0;
   d.reg_full_sweep = 1;  // smooth_next is undefined
   SM_CUDA(cudaMalloc(&d.new_list, sizeof(u32) * P));
@@ -458,35 +447,24 @@ int sm_destroy(sm_reconstruction* r) {
   if (r->session) SessionEnd(r, nullptr);   // drains the open session
   cudaDeviceSynchronize();
   cudaGetLastError();
-  DestroyFrameGraph(r->graph);
   DeviceState& d = r->d;
   cudaFree(d.surfels); cudaFree(d.gradient); cudaFree(r->reg_records); cudaFree(d.new_list);
-  for (int i = 0; i < kSets; ++i) {
-    cudaFree(r->vis_set[i]); cudaFree(r->seg_count_set[i]); cudaFree(r->merge_flag_set[i]);
-    cudaFree(r->upd_list_set[i]); cudaFree(r->upd_count_set[i]);
-    cudaFree(r->assoc_set[i]); cudaFree(r->first_depth_set[i]); cudaFree(r->supported_set[i]);
-    cudaFree(r->run_depth[i]); cudaFree(r->run_depth_pre[i]); cudaFree(r->run_normals[i]); cudaFree(r->run_radius[i]);
+  for (BufferSet& s : r->sets) {
+    cudaFree(s.vis); cudaFree(s.seg_count); cudaFree(s.merge_flag); cudaFree(s.upd_list); cudaFree(s.upd_count);
+    cudaFree(s.assoc); cudaFree(s.first_depth); cudaFree(s.supported);
   }
   cudaFree(d.new_flag); cudaFree(d.new_index); cudaFree(d.scan_state); cudaFree(d.counters);
   cudaFree(d.timeline);
   if (r->host_counters) cudaFreeHost(r->host_counters);
   cudaFree(r->scratch_B);
   cudaFree(r->blend_src);
-  cudaFree(r->median_stage[0]); cudaFree(r->median_stage[1]);
-  cudaFree(r->pyramid_depth_stage); cudaFree(r->pyramid_color_stage);
+  for (int i = 0; i < 14; ++i) if (r->events.ev[i]) cudaEventDestroy(r->events.ev[i]);
+  FreeRunBuffers(r);
   FreeTransferBuffers(r);
   FreeRenderBuffers(r);
   FreeTrackBuffers(r);
   FreeMeshBuffers(r);
   FreeHoleBuffers(r);
-  for (cudaStream_t st : {r->upload_stream, r->graph_stream})
-    if (st) cudaStreamDestroy(st);
-  for (cudaEvent_t e : {r->entry_event, r->upload_done, r->graph_exit})
-    if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : r->iteration_done) if (e) cudaEventDestroy(e);
-  for (u16* b : r->ring_depth) cudaFree(b);
-  for (uchar3* b : r->ring_color) cudaFree(b);
-  for (int i = 0; i < 14; ++i) if (r->events.ev[i]) cudaEventDestroy(r->events.ev[i]);
   delete r;
   cudaGetLastError();
   return SM_OK;

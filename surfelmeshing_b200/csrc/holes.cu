@@ -30,12 +30,6 @@ namespace smb {
 
 namespace {
 
-#define SM_CUDA(call)                                                                                   \
-  do {                                                                                                  \
-    const cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-  } while (0)
-
 constexpr int kBlock = 256;
 constexpr int kMaxHole = SM_MESH_MAX_HOLE;
 constexpr u32 kNone = 0xFFFFFFFFu;

@@ -30,12 +30,6 @@ namespace smb {
 
 namespace {
 
-#define SM_CUDA(call)                                                                                   \
-  do {                                                                                                  \
-    const cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-  } while (0)
-
 constexpr int kBuildBlock = 256;
 constexpr int kQueryBlock = 128;           // 4 queries per block, one warp each
 

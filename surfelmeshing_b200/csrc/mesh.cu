@@ -34,13 +34,26 @@ struct MeshCounters {
   u32 triangle_count;            // copied from the end of the scanned counts
 };
 
-namespace {
+struct MeshLive;
 
-#define SM_CUDA(call)                                                                                   \
-  do {                                                                                                  \
-    const cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-  } while (0)
+// The scratch of sm_triangulate, allocated by the first call and grown to surfels_size(): the k-NN index over the
+// smooth positions, the umbrellas ([slots][SM_MESH_MAX_UMBRELLA] pairs) and their lengths, the per-slot triangle
+// counts (scanned in place into offsets) and the scan's tile sums; the device counters and their pinned mirror;
+// resident grids. Also sm_mesh_update's persistent mesh, which shares only the index.
+struct MeshScratch {
+  sm_knn_index* index = nullptr;
+  uint2* umbrella = nullptr;
+  u32* umbrella_count = nullptr;
+  u32* counts = nullptr;
+  u32* scan_sums = nullptr;
+  u32 slots = 0;
+  MeshCounters* counters = nullptr;
+  MeshCounters* host_counters = nullptr;
+  int umbrella_blocks = 0, emit_blocks = 0;
+  MeshLive* live = nullptr;   // created by the first sm_mesh_update
+};
+
+namespace {
 
 constexpr int kUmbrellaBlock = 128;   // 4 slots per block, one warp each
 constexpr int kEmitBlock = 256;
@@ -644,39 +657,41 @@ __global__ void __launch_bounds__(kEmitBlock) k_mesh_recheck(MeshArgs a, UpdateA
   }
 }
 
-void FreeMeshScratch(sm_reconstruction* r) {
-  KnnDestroy(r->mesh_index);
-  cudaFree(r->mesh_umbrella);
-  cudaFree(r->mesh_umbrella_count);
-  cudaFree(r->mesh_counts);
-  cudaFree(r->mesh_scan_sums);
-  r->mesh_index = nullptr;
-  r->mesh_umbrella = nullptr;
-  r->mesh_umbrella_count = nullptr;
-  r->mesh_counts = nullptr;
-  r->mesh_scan_sums = nullptr;
-  r->mesh_slots = 0;
+void FreeSlotScratch(MeshScratch& m) {
+  KnnDestroy(m.index);
+  cudaFree(m.umbrella);
+  cudaFree(m.umbrella_count);
+  cudaFree(m.counts);
+  cudaFree(m.scan_sums);
+  m.index = nullptr;
+  m.umbrella = nullptr;
+  m.umbrella_count = nullptr;
+  m.counts = nullptr;
+  m.scan_sums = nullptr;
+  m.slots = 0;
 }
 
 // Scratch for n slots (grown, never shrunk); the counters and the grids are set up once.
 int EnsureMeshScratch(sm_reconstruction* r, u32 n) {
-  if (!r->mesh_counters) {
-    SM_CUDA(cudaMalloc(&r->mesh_counters, sizeof(MeshCounters)));
-    SM_CUDA(cudaMallocHost(&r->mesh_host_counters, sizeof(MeshCounters)));
-    int status = ResidentBlocks(k_mesh_umbrella, kUmbrellaBlock, r->sm_count, &r->mesh_umbrella_blocks);
-    if (status == SM_OK) status = ResidentBlocks(k_mesh_count, kEmitBlock, r->sm_count, &r->mesh_emit_blocks);
+  if (!r->mesh) r->mesh = new MeshScratch();
+  MeshScratch& m = *r->mesh;
+  if (!m.counters) {
+    SM_CUDA(cudaMalloc(&m.counters, sizeof(MeshCounters)));
+    SM_CUDA(cudaMallocHost(&m.host_counters, sizeof(MeshCounters)));
+    int status = ResidentBlocks(k_mesh_umbrella, kUmbrellaBlock, r->sm_count, &m.umbrella_blocks);
+    if (status == SM_OK) status = ResidentBlocks(k_mesh_count, kEmitBlock, r->sm_count, &m.emit_blocks);
     if (status != SM_OK) return status;
   }
-  if (n <= r->mesh_slots) return SM_OK;
-  FreeMeshScratch(r);   // cudaFree synchronises the device: an earlier call may still use the buffers
-  const int status = KnnCreate(&r->mesh_index, n);
+  if (n <= m.slots) return SM_OK;
+  FreeSlotScratch(m);   // cudaFree synchronises the device: an earlier call may still use the buffers
+  const int status = KnnCreate(&m.index, n);
   if (status != SM_OK) return status;
   const u32 tiles = (n + 1 + kScanTile - 1) / kScanTile;
-  SM_CUDA(cudaMalloc(&r->mesh_umbrella, sizeof(uint2) * kUmbrella * static_cast<size_t>(n)));
-  SM_CUDA(cudaMalloc(&r->mesh_umbrella_count, sizeof(u32) * static_cast<size_t>(n)));
-  SM_CUDA(cudaMalloc(&r->mesh_counts, sizeof(u32) * (static_cast<size_t>(n) + 1)));
-  SM_CUDA(cudaMalloc(&r->mesh_scan_sums, sizeof(u32) * tiles));
-  r->mesh_slots = n;
+  SM_CUDA(cudaMalloc(&m.umbrella, sizeof(uint2) * kUmbrella * static_cast<size_t>(n)));
+  SM_CUDA(cudaMalloc(&m.umbrella_count, sizeof(u32) * static_cast<size_t>(n)));
+  SM_CUDA(cudaMalloc(&m.counts, sizeof(u32) * (static_cast<size_t>(n) + 1)));
+  SM_CUDA(cudaMalloc(&m.scan_sums, sizeof(u32) * tiles));
+  m.slots = n;
   return SM_OK;
 }
 
@@ -712,6 +727,7 @@ int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params&
   if (n == 0) return SM_OK;
   status = EnsureMeshScratch(r, n);
   if (status != SM_OK) return status;
+  const MeshScratch& m = *r->mesh;
 
   MeshArgs a{};
   a.n = n;
@@ -720,29 +736,29 @@ int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params&
   a.radius_factor_squared = f2;
   a.cos_normal = CosDegrees(p.max_angle_between_normals_deg);
   a.cos_triangle = CosDegrees(p.max_triangle_angle_deg);
-  a.umbrella = r->mesh_umbrella;
-  a.umbrella_count = r->mesh_umbrella_count;
-  a.counts = r->mesh_counts;
+  a.umbrella = m.umbrella;
+  a.umbrella_count = m.umbrella_count;
+  a.counts = m.counts;
   a.triangles = reinterpret_cast<uint3*>(triangles);
-  a.counters = r->mesh_counters;
+  a.counters = m.counters;
   status = MirrorRegRecords(stream, r->d, n, r->sm_count);   // rows 3-5 <- the current smooth positions
   if (status != SM_OK) return status;
-  SM_CUDA(cudaMemsetAsync(r->mesh_counters, 0, sizeof(MeshCounters), stream));
+  SM_CUDA(cudaMemsetAsync(m.counters, 0, sizeof(MeshCounters), stream));
   const int bound_blocks = static_cast<int>(std::min<u32>((n + kBoundBlock - 1) / kBoundBlock, 4u * r->sm_count));
   { LaunchScope scope(stream, KID_MESH_BOUND); LaunchKernel(k_mesh_bound, dim3(bound_blocks), dim3(kBoundBlock), 0, stream, a); }
-  SM_CUDA(cudaMemcpyAsync(r->mesh_host_counters, r->mesh_counters, sizeof(MeshCounters), cudaMemcpyDeviceToHost, stream));
+  SM_CUDA(cudaMemcpyAsync(m.host_counters, m.counters, sizeof(MeshCounters), cudaMemcpyDeviceToHost, stream));
   SM_CUDA(cudaStreamSynchronize(stream));
   float max_r2;
-  std::memcpy(&max_r2, &r->mesh_host_counters->max_radius_squared_bits, sizeof(float));
+  std::memcpy(&max_r2, &m.host_counters->max_radius_squared_bits, sizeof(float));
   if (!(max_r2 > 0.f)) return SM_OK;   // no present slot
   // Cell size: twice the largest query radius, so that a query touches at most 3 cells per axis.
   const float cell_size = 2.f * std::sqrt(max_r2 * f2);
   const size_t st = r->d.stride;
   const float* s = r->d.surfels;
-  status = KnnBuild(r->mesh_index, stream, n, s + SM_ROW_SMOOTH_X * st, s + SM_ROW_SMOOTH_Y * st,
+  status = KnnBuild(m.index, stream, n, s + SM_ROW_SMOOTH_X * st, s + SM_ROW_SMOOTH_Y * st,
                     s + SM_ROW_SMOOTH_Z * st, s + SM_ROW_RADIUS_SQUARED * st, nullptr, cell_size);
   if (status != SM_OK) return status;
-  sm_knn_index* k = r->mesh_index;
+  sm_knn_index* k = m.index;
   a.q = QueryArgs{};
   a.q.max_result_count = kMaxResults;
   a.q.radius_scale = 1.f;
@@ -753,20 +769,20 @@ int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params&
   a.q.bucket_start = k->bucket_start;
   a.q.records = k->records;
   const int umbrella_blocks =
-      static_cast<int>(std::min<u32>((n + kUmbrellaBlock / 32 - 1) / (kUmbrellaBlock / 32), r->mesh_umbrella_blocks));
-  const int emit_blocks = static_cast<int>(std::min<u32>((n + kEmitBlock - 1) / kEmitBlock, r->mesh_emit_blocks));
+      static_cast<int>(std::min<u32>((n + kUmbrellaBlock / 32 - 1) / (kUmbrellaBlock / 32), m.umbrella_blocks));
+  const int emit_blocks = static_cast<int>(std::min<u32>((n + kEmitBlock - 1) / kEmitBlock, m.emit_blocks));
   { LaunchScope scope(stream, KID_MESH_UMBRELLA); LaunchKernel(k_mesh_umbrella, dim3(umbrella_blocks), dim3(kUmbrellaBlock), 0, stream, a); }
-  SM_CUDA(cudaMemsetAsync(r->mesh_counts + n, 0, sizeof(u32), stream));
+  SM_CUDA(cudaMemsetAsync(m.counts + n, 0, sizeof(u32), stream));
   { LaunchScope scope(stream, KID_MESH_COUNT); LaunchKernel(k_mesh_count, dim3(emit_blocks), dim3(kEmitBlock), 0, stream, a); }
   const u32 scan_n = n + 1;
   const u32 tiles = (scan_n + kScanTile - 1) / kScanTile;
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(r->mesh_counts, scan_n, r->mesh_scan_sums); }
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(r->mesh_scan_sums, tiles); }
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(r->mesh_counts, scan_n, r->mesh_scan_sums); }
-  SM_CUDA(cudaMemcpyAsync(&r->mesh_counters->triangle_count, r->mesh_counts + n, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
-  SM_CUDA(cudaMemcpyAsync(r->mesh_host_counters, r->mesh_counters, sizeof(MeshCounters), cudaMemcpyDeviceToHost, stream));
+  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(m.counts, scan_n, m.scan_sums); }
+  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(m.scan_sums, tiles); }
+  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(m.counts, scan_n, m.scan_sums); }
+  SM_CUDA(cudaMemcpyAsync(&m.counters->triangle_count, m.counts + n, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  SM_CUDA(cudaMemcpyAsync(m.host_counters, m.counters, sizeof(MeshCounters), cudaMemcpyDeviceToHost, stream));
   SM_CUDA(cudaStreamSynchronize(stream));
-  const MeshCounters& h = *r->mesh_host_counters;
+  const MeshCounters& h = *m.host_counters;
   stats->triangle_count = h.triangle_count;
   stats->vertices_meshed = h.vertices_meshed;
   stats->boundary_edges = h.boundary_edges;
@@ -946,13 +962,14 @@ int Grid(u32 items, int block, int resident) {
 }  // namespace
 
 void FreeMeshBuffers(sm_reconstruction* r) {
-  FreeMeshScratch(r);
-  cudaFree(r->mesh_counters);
-  if (r->mesh_host_counters) cudaFreeHost(r->mesh_host_counters);
-  r->mesh_counters = nullptr;
-  r->mesh_host_counters = nullptr;
-  FreeLive(r->mesh_live);
-  r->mesh_live = nullptr;
+  MeshScratch* m = r->mesh;
+  if (!m) return;
+  FreeSlotScratch(*m);
+  cudaFree(m->counters);
+  if (m->host_counters) cudaFreeHost(m->host_counters);
+  FreeLive(m->live);
+  delete m;
+  r->mesh = nullptr;
 }
 
 int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, sm_mesh_update_stats* stats) {
@@ -963,8 +980,10 @@ int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& 
   status = FetchCounters(r, stream);
   if (status == SM_ERR_CUDA) return status;   // (a surfel-cap overflow of an earlier frame does not matter here)
   const u32 n = r->host_counters->surfel_count[r->count_slot];
-  if (!r->mesh_live) r->mesh_live = new MeshLive{};
-  MeshLive& L = *r->mesh_live;
+  if (!r->mesh) r->mesh = new MeshScratch();
+  MeshScratch& m = *r->mesh;
+  if (!m.live) m.live = new MeshLive{};
+  MeshLive& L = *m.live;
   const bool was_valid = L.valid;
   L.valid = false;   // until this update completes; a failed one is followed by a rebuild from an empty mesh
   if (!was_valid) L.n_prev = 0;
@@ -1032,19 +1051,19 @@ int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& 
 
   if (max_r2 > 0.f) {
     // The index of rule 1, as sm_triangulate builds it (the index object is shared: both calls rebuild it).
-    if (!r->mesh_index || r->mesh_index->capacity < n) {
-      KnnDestroy(r->mesh_index);
-      r->mesh_index = nullptr;
-      status = KnnCreate(&r->mesh_index, std::max(n + n / 2, r->mesh_slots));   // x 1.5: a session grows n
+    if (!m.index || m.index->capacity < n) {
+      KnnDestroy(m.index);
+      m.index = nullptr;
+      status = KnnCreate(&m.index, std::max(n + n / 2, m.slots));   // x 1.5: a session grows n
       if (status != SM_OK) return status;
     }
     const float cell_size = 2.f * std::sqrt(max_r2 * f2);
     const size_t st = r->d.stride;
     const float* rows = r->d.surfels;
-    status = KnnBuild(r->mesh_index, stream, n, rows + SM_ROW_SMOOTH_X * st, rows + SM_ROW_SMOOTH_Y * st,
+    status = KnnBuild(m.index, stream, n, rows + SM_ROW_SMOOTH_X * st, rows + SM_ROW_SMOOTH_Y * st,
                       rows + SM_ROW_SMOOTH_Z * st, rows + SM_ROW_RADIUS_SQUARED * st, nullptr, cell_size);
     if (status != SM_OK) return status;
-    a.q = IndexQuery(r->mesh_index);
+    a.q = IndexQuery(m.index);
     if (!everything && changed > 0) {
       // A from the small side: an index over the <= 2 |C| old and new positions, one existence query per present
       // slot with its own radius. A slot's work is bounded by the changed points near it, however large the
@@ -1129,7 +1148,7 @@ int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t*
   auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_mesh_read: ") + why).c_str()); };
   if (which != SM_MESH_ALL && which != SM_MESH_ADDED && which != SM_MESH_REMOVED) return bad("unknown `which`");
   if (!triangles && capacity > 0) return bad("triangles is NULL with a capacity > 0");
-  const MeshLive* L = r->mesh_live;
+  const MeshLive* L = r->mesh ? r->mesh->live : nullptr;
   if (!L || !L->valid) return bad("no sm_mesh_update has completed on this handle");
   const uint3* src = which == SM_MESH_ALL ? L->triangles[L->current] : (which == SM_MESH_ADDED ? L->added : L->removed);
   const u64 size = which == SM_MESH_ALL ? L->triangle_count : (which == SM_MESH_ADDED ? L->added_count : L->removed_count);

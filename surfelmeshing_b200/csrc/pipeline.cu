@@ -36,13 +36,34 @@
 
 namespace smb {
 
-namespace {
+struct FrameGraph;
 
-#define SM_CUDA(call)                                                                                   \
-  do {                                                                                                  \
-    const cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-  } while (0)
+// The frame loop's buffers, streams and events (sm_stream_run, sessions), created by the first call.
+struct RunBuffers {
+  // pre-processing outputs per buffer set
+  u16* depth[kSets] = {}; size_t depth_pitch = 0;
+  u16* depth_pre[kSets] = {};   // pre-blend copy of depth (merge runs next to blend)
+  float2* normals[kSets] = {}; size_t normals_pitch = 0;
+  float* radius[kSets] = {}; size_t radius_pitch = 0;
+  cudaEvent_t entry_event = nullptr;   // the start of the frame loop on the caller's stream
+  cudaStream_t graph_stream = nullptr;
+  cudaEvent_t graph_exit = nullptr;
+  FrameGraph* graph = nullptr;
+  // host-resident streams: raw-depth / colour rings filled by the upload stream
+  std::vector<u16*> ring_depth; size_t ring_depth_pitch = 0;
+  std::vector<uchar3*> ring_color; size_t ring_color_pitch = 0;
+  cudaStream_t upload_stream = nullptr;
+  cudaEvent_t upload_done = nullptr;
+  std::vector<cudaEvent_t> iteration_done;   // one event per step slot (ring reuse)
+  // staging of the MedianFilterAndDensifyDepthMap passes (sm_reconstruction::median_iterations)
+  u16* median_stage[2] = {nullptr, nullptr}; size_t median_stage_pitch = 0;
+  // full-size staging of host frames at a pyramid level
+  u16* pyramid_depth_stage = nullptr; size_t pyramid_depth_stage_pitch = 0;
+  u8* pyramid_color_stage = nullptr; size_t pyramid_color_stage_pitch = 0;
+  int pyramid_stage_width = 0, pyramid_stage_height = 0;
+};
+
+namespace {
 
 constexpr int kDepthRing = 16;      // raw-depth frames resident at once (host-resident streams); >= K + 2 + slack
 // Colour images resident at once. A session uploads frame p's image when p is pushed; the frame graph integrates
@@ -67,64 +88,59 @@ struct SessionFrames {
 int EnsureRunBuffers(sm_reconstruction* r, bool on_host, bool depth_ring, bool color_ring, int source_width,
                      int source_height) {
   const int W = r->d.width, H = r->d.height;
-  if (!r->run_depth[0]) {
+  if (!r->run) r->run = new RunBuffers();
+  RunBuffers& b = *r->run;
+  if (!b.depth[0]) {
     for (int i = 0; i < kSets; ++i) {
-      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->run_depth[i]), &r->run_depth_pitch, W * sizeof(u16), H));
-      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->run_depth_pre[i]), &r->run_depth_pitch, W * sizeof(u16), H));
-      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->run_normals[i]), &r->run_normals_pitch, W * sizeof(float2), H));
-      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->run_radius[i]), &r->run_radius_pitch, W * sizeof(float), H));
-      SM_CUDA(cudaMemset2D(r->run_radius[i], r->run_radius_pitch, 0, W * sizeof(float), H));
+      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b.depth[i]), &b.depth_pitch, W * sizeof(u16), H));
+      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b.depth_pre[i]), &b.depth_pitch, W * sizeof(u16), H));
+      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b.normals[i]), &b.normals_pitch, W * sizeof(float2), H));
+      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b.radius[i]), &b.radius_pitch, W * sizeof(float), H));
+      SM_CUDA(cudaMemset2D(b.radius[i], b.radius_pitch, 0, W * sizeof(float), H));
     }
-    SM_CUDA(cudaStreamCreateWithFlags(&r->graph_stream, cudaStreamNonBlocking));
-    SM_CUDA(cudaEventCreateWithFlags(&r->entry_event, cudaEventDisableTiming));
-    SM_CUDA(cudaEventCreateWithFlags(&r->graph_exit, cudaEventDisableTiming));
+    SM_CUDA(cudaStreamCreateWithFlags(&b.graph_stream, cudaStreamNonBlocking));
+    SM_CUDA(cudaEventCreateWithFlags(&b.entry_event, cudaEventDisableTiming));
+    SM_CUDA(cudaEventCreateWithFlags(&b.graph_exit, cudaEventDisableTiming));
   }
-  if ((on_host || depth_ring) && !r->upload_stream) {
-    SM_CUDA(cudaStreamCreateWithFlags(&r->upload_stream, cudaStreamNonBlocking));
-    SM_CUDA(cudaEventCreateWithFlags(&r->upload_done, cudaEventDisableTiming));
-    r->iteration_done.assign(kIterationEvents, nullptr);
-    for (auto& e : r->iteration_done) SM_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  if ((on_host || depth_ring) && !b.upload_stream) {
+    SM_CUDA(cudaStreamCreateWithFlags(&b.upload_stream, cudaStreamNonBlocking));
+    SM_CUDA(cudaEventCreateWithFlags(&b.upload_done, cudaEventDisableTiming));
+    b.iteration_done.assign(kIterationEvents, nullptr);
+    for (auto& e : b.iteration_done) SM_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   }
-  if (depth_ring && r->ring_depth.empty()) {
-    r->ring_depth.assign(kDepthRing, nullptr);
-    for (auto& b : r->ring_depth) {
-      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b), &r->ring_depth_pitch, W * sizeof(u16), H));
+  if (depth_ring && b.ring_depth.empty()) {
+    b.ring_depth.assign(kDepthRing, nullptr);
+    for (auto& p : b.ring_depth) {
+      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&p), &b.ring_depth_pitch, W * sizeof(u16), H));
     }
   }
-  if (color_ring && r->ring_color.empty()) {
-    r->ring_color.assign(kColorRing, nullptr);
-    for (auto& b : r->ring_color) {
-      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b), &r->ring_color_pitch, W * 3, H));
+  if (color_ring && b.ring_color.empty()) {
+    b.ring_color.assign(kColorRing, nullptr);
+    for (auto& p : b.ring_color) {
+      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&p), &b.ring_color_pitch, W * 3, H));
     }
   }
   // host frames at a pyramid level: full-size staging on the upload stream (one frame at a time)
   if (on_host && r->pyramid_level > 0 &&
-      (r->pyramid_stage_width != source_width || r->pyramid_stage_height != source_height)) {
-    SM_CUDA(cudaFree(r->pyramid_depth_stage));
-    SM_CUDA(cudaFree(r->pyramid_color_stage));
-    r->pyramid_depth_stage = nullptr;
-    r->pyramid_color_stage = nullptr;
-    r->pyramid_stage_width = r->pyramid_stage_height = 0;
-    SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->pyramid_depth_stage), &r->pyramid_depth_stage_pitch,
+      (b.pyramid_stage_width != source_width || b.pyramid_stage_height != source_height)) {
+    SM_CUDA(cudaFree(b.pyramid_depth_stage));
+    SM_CUDA(cudaFree(b.pyramid_color_stage));
+    b.pyramid_depth_stage = nullptr;
+    b.pyramid_color_stage = nullptr;
+    b.pyramid_stage_width = b.pyramid_stage_height = 0;
+    SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b.pyramid_depth_stage), &b.pyramid_depth_stage_pitch,
                             source_width * sizeof(u16), source_height));
-    SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->pyramid_color_stage), &r->pyramid_color_stage_pitch,
+    SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b.pyramid_color_stage), &b.pyramid_color_stage_pitch,
                             static_cast<size_t>(source_width) * 3, source_height));
-    r->pyramid_stage_width = source_width;
-    r->pyramid_stage_height = source_height;
+    b.pyramid_stage_width = source_width;
+    b.pyramid_stage_height = source_height;
   }
-  if (r->median_iterations > 0 && !r->median_stage[0]) {
+  if (r->median_iterations > 0 && !b.median_stage[0]) {
     for (int i = 0; i < 2; ++i) {
-      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&r->median_stage[i]), &r->median_stage_pitch, W * sizeof(u16), H));
+      SM_CUDA(cudaMallocPitch(reinterpret_cast<void**>(&b.median_stage[i]), &b.median_stage_pitch, W * sizeof(u16), H));
     }
   }
   return SM_OK;
-}
-
-// Points `d` at buffer set `set` (association rasters, visible list, merge flags, neighbour-update list).
-void UseSet(DeviceState& d, const sm_reconstruction* r, int set) {
-  d.assoc = r->assoc_set[set]; d.first_depth = r->first_depth_set[set]; d.supported = r->supported_set[set];
-  d.vis = r->vis_set[set]; d.seg_count = r->seg_count_set[set]; d.merge_flag = r->merge_flag_set[set];
-  d.upd_list = r->upd_list_set[set]; d.upd_count = r->upd_count_set[set];
 }
 
 // Everything both modes share about one call (or one session).
@@ -149,7 +165,7 @@ struct RunContext {
   uint64_t h2d = 0;
 
   int CountSlot(int frame) const { return (base_slot + (frame - first)) % kCountSlots; }
-  cudaStream_t Upload() const { return upload_override ? upload_override : r->upload_stream; }
+  cudaStream_t Upload() const { return upload_override ? upload_override : r->run->upload_stream; }
   bool Active(int frame) const { return frame >= first && frame < last; }
   const float* GlobalT(int frame) const { return ring ? ring->global_T_frame[frame % kPoseRing] : s->global_T_frame + 12 * frame; }
   const float* FrameT(int frame) const { return ring ? ring->frame_T_global[frame % kPoseRing] : s->frame_T_global + 12 * frame; }
@@ -168,27 +184,29 @@ struct RunContext {
     return s->color + 3 * source_elems * frame;
   }
   const u16* Raw(int frame, size_t* pitch) const {
-    if (depth_ring) { *pitch = r->ring_depth_pitch; return r->ring_depth[frame % kDepthRing]; }
+    if (depth_ring) { *pitch = r->run->ring_depth_pitch; return r->run->ring_depth[frame % kDepthRing]; }
     *pitch = W * sizeof(u16);
     return s->depth + frame_elems * frame;
   }
   const uint8_t* Color(int frame, size_t* pitch) const {
-    if (color_ring) { *pitch = r->ring_color_pitch; return reinterpret_cast<const uint8_t*>(r->ring_color[frame % kColorRing]); }
+    if (color_ring) { *pitch = r->run->ring_color_pitch; return reinterpret_cast<const uint8_t*>(r->run->ring_color[frame % kColorRing]); }
     *pitch = static_cast<size_t>(W) * 3;
     return s->color + 3 * frame_elems * frame;
   }
   FrameParams Params(int frame, int set) const {
     size_t color_pitch;
     const uint8_t* color = Color(frame, &color_pitch);
-    return MakeFrameParams(r, static_cast<u32>(frame), CountSlot(frame), *ip, r->run_depth[set], r->run_depth_pitch,
-                           r->run_depth_pre[set], r->run_depth_pitch,
-                           reinterpret_cast<const float*>(r->run_normals[set]), r->run_normals_pitch,
-                           r->run_radius[set], r->run_radius_pitch, color, color_pitch, GlobalT(frame), FrameT(frame));
+    const RunBuffers& b = *r->run;
+    return MakeFrameParams(r, static_cast<u32>(frame), CountSlot(frame), *ip, b.depth[set], b.depth_pitch,
+                           b.depth_pre[set], b.depth_pitch, reinterpret_cast<const float*>(b.normals[set]),
+                           b.normals_pitch, b.radius[set], b.radius_pitch, color, color_pitch, GlobalT(frame),
+                           FrameT(frame));
   }
   // Upload stream: raw depth map `frame` into its ring slot (main.cc:902-965), through the
   // MedianFilterAndDensifyDepthMap passes when configured (main.cc:927-939, there on the CPU).
   int EnqueueRawFrame(int frame) {
-    u16* const slot = r->ring_depth[frame % kDepthRing];
+    RunBuffers& b = *r->run;
+    u16* const slot = b.ring_depth[frame % kDepthRing];
     size_t src_pitch;
     const u16* const src = SourceDepth(frame, &src_pitch);
     if (pyramid > 0) {
@@ -197,27 +215,28 @@ struct RunContext {
       const u16* full = src;
       size_t full_pitch = src_pitch;
       if (on_host) {
-        SM_CUDA(cudaMemcpy2DAsync(r->pyramid_depth_stage, r->pyramid_depth_stage_pitch, src, src_pitch,
+        SM_CUDA(cudaMemcpy2DAsync(b.pyramid_depth_stage, b.pyramid_depth_stage_pitch, src, src_pitch,
                                   source_W * sizeof(u16), source_H, cudaMemcpyHostToDevice, Upload()));
         h2d += source_elems * sizeof(u16);
-        full = r->pyramid_depth_stage;
-        full_pitch = r->pyramid_depth_stage_pitch;
+        full = b.pyramid_depth_stage;
+        full_pitch = b.pyramid_depth_stage_pitch;
       }
       return StageDownscaleMedian(Upload(), 0, source_W, source_H, full, full_pitch, W, H, slot,
-                                  r->ring_depth_pitch);
+                                  b.ring_depth_pitch);
     }
     const int n = r->median_iterations;
-    u16* const target = n > 0 ? r->median_stage[0] : slot;
-    const size_t target_pitch = n > 0 ? r->median_stage_pitch : r->ring_depth_pitch;
+    u16* const target = n > 0 ? b.median_stage[0] : slot;
+    const size_t target_pitch = n > 0 ? b.median_stage_pitch : b.ring_depth_pitch;
     SM_CUDA(cudaMemcpy2DAsync(target, target_pitch, src, src_pitch, W * sizeof(u16), H, cudaMemcpyDefault, Upload()));
     if (on_host) h2d += frame_elems * sizeof(u16);
     if (n > 0) {
-      return StageMedianDensify(Upload(), n, W, H, r->median_stage[0], r->median_stage_pitch, slot,
-                                r->ring_depth_pitch, r->median_stage[1], r->median_stage_pitch);
+      return StageMedianDensify(Upload(), n, W, H, b.median_stage[0], b.median_stage_pitch, slot,
+                                b.ring_depth_pitch, b.median_stage[1], b.median_stage_pitch);
     }
     return SM_OK;
   }
   int EnqueueColorFrame(int frame) {
+    RunBuffers& b = *r->run;
     size_t src_pitch;
     const uint8_t* const src = SourceColor(frame, &src_pitch);
     if (pyramid > 0) {
@@ -225,16 +244,16 @@ struct RunContext {
       const uint8_t* full = src;
       size_t full_pitch = src_pitch;
       if (on_host) {
-        SM_CUDA(cudaMemcpy2DAsync(r->pyramid_color_stage, r->pyramid_color_stage_pitch, src, src_pitch,
+        SM_CUDA(cudaMemcpy2DAsync(b.pyramid_color_stage, b.pyramid_color_stage_pitch, src, src_pitch,
                                   static_cast<size_t>(source_W) * 3, source_H, cudaMemcpyHostToDevice, Upload()));
         h2d += source_elems * 3;
-        full = r->pyramid_color_stage;
-        full_pitch = r->pyramid_color_stage_pitch;
+        full = b.pyramid_color_stage;
+        full_pitch = b.pyramid_color_stage_pitch;
       }
       return StageColorPyramid(Upload(), pyramid, source_W, source_H, full, full_pitch,
-                               reinterpret_cast<u8*>(r->ring_color[frame % kColorRing]), r->ring_color_pitch);
+                               reinterpret_cast<u8*>(b.ring_color[frame % kColorRing]), b.ring_color_pitch);
     }
-    SM_CUDA(cudaMemcpy2DAsync(r->ring_color[frame % kColorRing], r->ring_color_pitch, src, src_pitch,
+    SM_CUDA(cudaMemcpy2DAsync(b.ring_color[frame % kColorRing], b.ring_color_pitch, src, src_pitch,
                               static_cast<size_t>(W) * 3, H, cudaMemcpyDefault, Upload()));
     if (on_host) h2d += frame_elems * 3;
     return SM_OK;
@@ -358,10 +377,10 @@ struct FrameLoop {
 };
 
 int BeginLoop(RunContext& c, cudaStream_t stream, bool graph, FrameLoop* g) {
-  sm_reconstruction* r = c.r;
+  const RunBuffers& b = *c.r->run;
   g->graph = graph;
   g->ahead = graph ? 2 : 0;
-  g->work = graph ? r->graph_stream : stream;
+  g->work = graph ? b.graph_stream : stream;
   if (graph) {
     g->blending = c.ip->do_blending != 0;
     g->iterations = c.ip->regularization_iterations_per_integration_iteration;
@@ -372,16 +391,16 @@ int BeginLoop(RunContext& c, cudaStream_t stream, bool graph, FrameLoop* g) {
   }
   g->it0 = c.first - g->ahead;
   g->uploaded_until = c.first - c.half - 1;
-  SM_CUDA(cudaEventRecord(r->entry_event, stream));
-  if (g->work != stream) SM_CUDA(cudaStreamWaitEvent(g->work, r->entry_event, 0));
-  if (c.depth_ring) SM_CUDA(cudaStreamWaitEvent(r->upload_stream, r->entry_event, 0));
+  SM_CUDA(cudaEventRecord(b.entry_event, stream));
+  if (g->work != stream) SM_CUDA(cudaStreamWaitEvent(g->work, b.entry_event, 0));
+  if (c.depth_ring) SM_CUDA(cudaStreamWaitEvent(b.upload_stream, b.entry_event, 0));
   return SM_OK;
 }
 
 // The ring uploads of both modes: a slot is rewritten once the step that last read it has finished
 // (iteration_done, recorded on the loop's stream after every step).
 int WaitForStep(RunContext& c, const FrameLoop& g, int step) {
-  if (step >= g.it0) SM_CUDA(cudaStreamWaitEvent(c.Upload(), c.r->iteration_done[(step - g.it0) % kIterationEvents], 0));
+  if (step >= g.it0) SM_CUDA(cudaStreamWaitEvent(c.Upload(), c.r->run->iteration_done[(step - g.it0) % kIterationEvents], 0));
   return SM_OK;
 }
 
@@ -407,6 +426,7 @@ int UploadColor(RunContext& c, FrameLoop& g, int frame) {
 // Frame graph: crit = it, front = it + 1, pre = it + 2.
 int GraphStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
   sm_reconstruction* r = c.r;
+  RunBuffers& b = *r->run;
   const int W = c.W, H = c.H;
   const StepLayout& l = g.l;
   std::vector<KernelLaunch>& launches = g.launches;
@@ -419,7 +439,7 @@ int GraphStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
   {  // crit: frame `crit`
     const int frame = clamp_frame(crit), set = frame % kSets;
     DeviceState d = r->d;   // smooth / smooth_next as the handle holds them (a Regularize() swaps them)
-    UseSet(d, r, set);
+    UseSet(d, r->sets[set]);
     if (c.Active(crit)) RecordOperation(r, static_cast<int>(static_cast<u32>(frame) - static_cast<u32>(c.ip->regularization_frame_window_size)));
     FrameParams f = c.Params(frame, set);  // carries the operation epoch just recorded
     f.skip = c.Active(crit) ? 0 : 1;
@@ -453,14 +473,14 @@ int GraphStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
       ++*integrated;
       // the handle's rasters / lists / count are those of the newest integrated frame (sm_download_rasters,
       // sm_frame_counters, sm_surfel_count, the hand-off calls between the pushes of a session)
-      UseSet(r->d, r, set);
+      UseSet(r->d, r->sets[set]);
       r->count_slot = new_slot;
     }
   }
   {  // front: frame `front`
     const int frame = clamp_frame(front), set = frame % kSets;
     DeviceState d = r->d;
-    UseSet(d, r, set);
+    UseSet(d, r->sets[set]);
     FrameParams f = c.Params(frame, set);
     f.skip = c.Active(front) ? 0 : 1;
     const FrameKernel kernels[4] = {FK_PROJECT, FK_ASSOCIATE, FK_MERGE, FK_BLEND};
@@ -478,28 +498,28 @@ int GraphStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
     c.Others(frame, others, other_pitches);
     size_t raw_pitch;
     const u16* raw = c.Raw(frame, &raw_pitch);
+    const BufferSet& s = r->sets[set];
     status = DescribePreprocess(&launches[l.bilateral], l.outlier >= 0 ? &launches[l.outlier] : nullptr,
                                 &launches[l.tail], !c.Active(pre), *c.pp, W, H, r->fx, r->fy, r->cx, r->cy, raw,
                                 raw_pitch, others, other_pitches, c.OthersTR(frame), r->scratch_B, r->scratch_B_pitch,
-                                r->run_depth[set], r->run_depth_pitch, r->run_normals[set], r->run_normals_pitch,
-                                r->run_radius[set], r->run_radius_pitch, r->assoc_set[set], r->first_depth_set[set],
-                                r->supported_set[set], r->run_depth_pre[set], r->run_depth_pitch,
+                                b.depth[set], b.depth_pitch, b.normals[set], b.normals_pitch, b.radius[set],
+                                b.radius_pitch, s.assoc, s.first_depth, s.supported, b.depth_pre[set], b.depth_pitch,
                                 TimelineSlot(r->d, static_cast<u32>(frame), KID_BILATERAL_OUTLIER),
                                 TimelineSlot(r->d, static_cast<u32>(frame), KID_ERODE_NORMALS_RADII), r->scratch_B_map);
     if (status != SM_OK) return status;
   }
 
   // ---- (re)build on the first step or when the layout changed, else update the node arguments ----
-  FrameGraph* fg = r->graph;
+  FrameGraph* fg = b.graph;
   bool rebuild = fg == nullptr || static_cast<int>(fg->nodes.size()) != l.count;
   if (!rebuild) {
     for (int i = 0; i < l.count && !rebuild; ++i) rebuild = fg->funcs[i] != launches[i].func;
     if (l.blend >= 0) rebuild = rebuild || fg->blend_smem != launches[l.blend].smem;
   }
   if (rebuild) {
-    if (fg) { SM_CUDA(cudaStreamSynchronize(g.work)); DestroyFrameGraph(fg); r->graph = nullptr; }
+    if (fg) { SM_CUDA(cudaStreamSynchronize(g.work)); DestroyFrameGraph(fg); b.graph = nullptr; }
     fg = new FrameGraph();
-    r->graph = fg;
+    b.graph = fg;
     status = BuildFrameGraph(fg, l, launches);
     if (status != SM_OK) return status;
   } else {
@@ -516,26 +536,27 @@ int GraphStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
 // Serial mode: pre-processing and Integrate() of frame `it`, one kernel after the other.
 int SerialStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
   sm_reconstruction* r = c.r;
+  const RunBuffers& b = *r->run;
   const int set = it % kSets;
+  const BufferSet& s = r->sets[set];
   const u16* others[8];
   size_t other_pitches[8];
   c.Others(it, others, other_pitches);
   size_t raw_pitch;
   const u16* raw = c.Raw(it, &raw_pitch);
   int status = PreprocessFused(g.work, *c.pp, c.W, c.H, r->fx, r->fy, r->cx, r->cy, raw, raw_pitch, others,
-                               other_pitches, c.OthersTR(it), r->scratch_B, r->scratch_B_pitch, r->run_depth[set],
-                               r->run_depth_pitch, r->run_normals[set], r->run_normals_pitch, r->run_radius[set],
-                               r->run_radius_pitch, r->assoc_set[set], r->first_depth_set[set], r->supported_set[set],
-                               nullptr, 0, TimelineSlot(r->d, static_cast<u32>(it), KID_BILATERAL_OUTLIER),
+                               other_pitches, c.OthersTR(it), r->scratch_B, r->scratch_B_pitch, b.depth[set],
+                               b.depth_pitch, b.normals[set], b.normals_pitch, b.radius[set], b.radius_pitch, s.assoc,
+                               s.first_depth, s.supported, nullptr, 0, TimelineSlot(r->d, static_cast<u32>(it), KID_BILATERAL_OUTLIER),
                                TimelineSlot(r->d, static_cast<u32>(it), KID_ERODE_NORMALS_RADII), r->scratch_B_map);
   if (status != SM_OK) return status;
-  UseSet(r->d, r, set);
+  UseSet(r->d, s);
   r->rasters_cleared = true;
   size_t color_pitch;
   const uint8_t* color = c.Color(it, &color_pitch);
-  status = IntegrateImpl(r, g.work, static_cast<u32>(it), *c.ip, r->run_depth[set], r->run_depth_pitch,
-                         reinterpret_cast<const float*>(r->run_normals[set]), r->run_normals_pitch, r->run_radius[set],
-                         r->run_radius_pitch, color, color_pitch, c.GlobalT(it), c.FrameT(it));
+  status = IntegrateImpl(r, g.work, static_cast<u32>(it), *c.ip, b.depth[set], b.depth_pitch,
+                         reinterpret_cast<const float*>(b.normals[set]), b.normals_pitch, b.radius[set],
+                         b.radius_pitch, color, color_pitch, c.GlobalT(it), c.FrameT(it));
   if (status != SM_OK) return status;
   ++*integrated;
   return SM_OK;
@@ -544,28 +565,28 @@ int SerialStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
 // One step of the loop. Afterwards the handle's state (smooth record buffers, count slot, rasters, regularisation
 // window) is that after frame `it` when it was integrated.
 int Step(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
-  sm_reconstruction* r = c.r;
+  const RunBuffers& b = *c.r->run;
   const int pre = it + g.ahead;
   if (c.depth_ring && c.Active(pre)) {  // the frames the pre-processing of this step reads
     int st = UploadDepth(c, g, pre + c.half);
     if (st == SM_OK && c.color_ring && !g.color_at_push) st = UploadColor(c, g, pre);
     if (st != SM_OK) return st;
     if (c.Upload() != g.work) {
-      SM_CUDA(cudaEventRecord(r->upload_done, c.Upload()));
-      SM_CUDA(cudaStreamWaitEvent(g.work, r->upload_done, 0));  // main.cc:995
+      SM_CUDA(cudaEventRecord(b.upload_done, c.Upload()));
+      SM_CUDA(cudaStreamWaitEvent(g.work, b.upload_done, 0));  // main.cc:995
     }
   }
   const int status = g.graph ? GraphStep(c, g, it, integrated) : SerialStep(c, g, it, integrated);
   if (status != SM_OK) return status;
-  if (c.depth_ring) SM_CUDA(cudaEventRecord(r->iteration_done[(it - g.it0) % kIterationEvents], g.work));
+  if (c.depth_ring) SM_CUDA(cudaEventRecord(b.iteration_done[(it - g.it0) % kIterationEvents], g.work));
   return SM_OK;
 }
 
 // `stream` waits for everything the loop has launched so far.
 int JoinLoop(sm_reconstruction* r, const FrameLoop& g, cudaStream_t stream) {
   if (g.work == stream) return SM_OK;
-  SM_CUDA(cudaEventRecord(r->graph_exit, g.work));
-  SM_CUDA(cudaStreamWaitEvent(stream, r->graph_exit, 0));
+  SM_CUDA(cudaEventRecord(r->run->graph_exit, g.work));
+  SM_CUDA(cudaStreamWaitEvent(stream, r->run->graph_exit, 0));
   return SM_OK;
 }
 
@@ -849,7 +870,7 @@ int SessionPush(sm_reconstruction* r, const u16* depth, size_t depth_pitch, cons
   if (status == SM_OK) status = UploadColor(c, loop, p);
   cuda(cudaEventRecord(ss->uploaded, c.Upload()), "cudaEventRecord");
   if (on_host) {
-    cuda(cudaEventRecord(ss->staging_free[slot], r->upload_stream), "cudaEventRecord");
+    cuda(cudaEventRecord(ss->staging_free[slot], r->run->upload_stream), "cudaEventRecord");
   } else {
     cuda(cudaStreamWaitEvent(stream, ss->uploaded, 0), "cudaStreamWaitEvent");   // the caller may overwrite the frame now
   }
@@ -898,12 +919,28 @@ int SessionEnd(sm_reconstruction* r, sm_stream_stats* stats) {
   ss->host_ms += MillisecondsSince(host_t0);
   status = FetchCounters(r, stream);
   FillStats(r, ss->integrated, ss->launches_before, c.h2d, ss->host_ms, stats);
-  cudaStreamSynchronize(r->upload_stream);   // the staging buffers are no longer read
+  cudaStreamSynchronize(r->run->upload_stream);   // the staging buffers are no longer read
   FreeSession(ss);
   r->session = nullptr;
   return status;
 }
 
-void DestroySession(StreamSession* ss) { FreeSession(ss); }
+void FreeRunBuffers(sm_reconstruction* r) {
+  RunBuffers* b = r->run;
+  if (!b) return;
+  DestroyFrameGraph(b->graph);
+  for (int i = 0; i < kSets; ++i) { cudaFree(b->depth[i]); cudaFree(b->depth_pre[i]); cudaFree(b->normals[i]); cudaFree(b->radius[i]); }
+  for (u16* p : b->ring_depth) cudaFree(p);
+  for (uchar3* p : b->ring_color) cudaFree(p);
+  cudaFree(b->median_stage[0]); cudaFree(b->median_stage[1]);
+  cudaFree(b->pyramid_depth_stage); cudaFree(b->pyramid_color_stage);
+  for (cudaStream_t st : {b->upload_stream, b->graph_stream})
+    if (st) cudaStreamDestroy(st);
+  for (cudaEvent_t e : {b->entry_event, b->upload_done, b->graph_exit})
+    if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : b->iteration_done) if (e) cudaEventDestroy(e);
+  delete b;
+  r->run = nullptr;
+}
 
 }  // namespace smb

@@ -21,12 +21,6 @@ namespace smb {
 
 namespace {
 
-#define SM_CUDA(call)                                                                                   \
-  do {                                                                                                  \
-    const cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-  } while (0)
-
 constexpr int kEncodeBlock = 256;
 constexpr int kDistanceBlock = 256;
 constexpr int kDistanceWarps = kDistanceBlock / 32;

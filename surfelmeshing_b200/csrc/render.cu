@@ -20,13 +20,24 @@
 
 namespace smb {
 
-namespace {
+// The scratch of sm_render_surfels and sm_render_mesh, created by the first render.
+struct RenderScratch {
+  // sm_render_surfels: the key raster (all keys "empty" between calls), the large-splat list (capacity slots) and
+  // its count (zero between calls), resident grids
+  unsigned long long* keys = nullptr; size_t key_capacity = 0;   // in pixels
+  u32* large_list = nullptr;
+  u32* large_count = nullptr;
+  int splat_blocks = 0, large_blocks = 0;
+  // sm_render_mesh, from the first mesh render: one bit per slot (the corners of the triangles drawn), the
+  // large-triangle list (grown to the triangle count) and its count (zero between calls), resident grids
+  u32* mesh_marks = nullptr;
+  u32* mesh_large_list = nullptr; u32 mesh_large_capacity = 0;   // in triangles
+  u32* mesh_large_count = nullptr;
+  int mesh_mark_blocks = 0, mesh_tri_blocks = 0, mesh_large_blocks = 0;
+  int mesh_splat_blocks = 0, mesh_splat_large_blocks = 0;
+};
 
-#define SM_CUDA(call)                                                                                   \
-  do {                                                                                                  \
-    const cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-  } while (0)
+namespace {
 
 #define SM_S(row, i) d.surfels[static_cast<size_t>(row) * d.stride + (i)]
 #define SM_SU(row, i) reinterpret_cast<const u32*>(d.surfels)[static_cast<size_t>(row) * d.stride + (i)]
@@ -470,21 +481,23 @@ bool Finite(float v) { return std::isfinite(v); }
 
 // The key raster grows to `pixels`; the list, its count and the grids are set up once.
 int EnsureRenderBuffers(sm_reconstruction* r, cudaStream_t stream, size_t pixels) {
-  if (r->render_large_list == nullptr) {
-    SM_CUDA(cudaMalloc(&r->render_large_list, sizeof(u32) * r->d.stride));
-    SM_CUDA(cudaMalloc(&r->render_large_count, sizeof(u32)));
-    SM_CUDA(cudaMemsetAsync(r->render_large_count, 0, sizeof(u32), stream));
-    int status = ResidentBlocks(k_render_splat, kSplatBlock, r->sm_count, &r->render_splat_blocks);
-    if (status == SM_OK) status = ResidentBlocks(k_render_large, kLargeBlock, r->sm_count, &r->render_large_blocks);
+  if (!r->render) r->render = new RenderScratch();
+  RenderScratch& s = *r->render;
+  if (s.large_list == nullptr) {
+    SM_CUDA(cudaMalloc(&s.large_list, sizeof(u32) * r->d.stride));
+    SM_CUDA(cudaMalloc(&s.large_count, sizeof(u32)));
+    SM_CUDA(cudaMemsetAsync(s.large_count, 0, sizeof(u32), stream));
+    int status = ResidentBlocks(k_render_splat, kSplatBlock, r->sm_count, &s.splat_blocks);
+    if (status == SM_OK) status = ResidentBlocks(k_render_large, kLargeBlock, r->sm_count, &s.large_blocks);
     if (status != SM_OK) return status;
   }
-  if (pixels > r->render_key_capacity) {
-    cudaFree(r->render_keys);   // synchronises the device: an earlier render may still use it
-    r->render_keys = nullptr;
-    r->render_key_capacity = 0;
-    SM_CUDA(cudaMalloc(&r->render_keys, sizeof(unsigned long long) * pixels));
-    SM_CUDA(cudaMemsetAsync(r->render_keys, 0xFF, sizeof(unsigned long long) * pixels, stream));
-    r->render_key_capacity = pixels;
+  if (pixels > s.key_capacity) {
+    cudaFree(s.keys);   // synchronises the device: an earlier render may still use it
+    s.keys = nullptr;
+    s.key_capacity = 0;
+    SM_CUDA(cudaMalloc(&s.keys, sizeof(unsigned long long) * pixels));
+    SM_CUDA(cudaMemsetAsync(s.keys, 0xFF, sizeof(unsigned long long) * pixels, stream));
+    s.key_capacity = pixels;
   }
   return SM_OK;
 }
@@ -520,24 +533,25 @@ int MakeRenderArgs(sm_reconstruction* r, cudaStream_t stream, const char* name, 
 // sm_render_mesh's scratch beyond EnsureRenderBuffers': the triangle list grows to `triangles` entries; the slot
 // bitmap (capacity bits), the list count and the grids are set up once.
 int EnsureMeshRenderBuffers(sm_reconstruction* r, cudaStream_t stream, u32 triangles) {
-  if (r->mesh_render_large_count == nullptr) {
-    SM_CUDA(cudaMalloc(&r->mesh_render_marks, sizeof(u32) * ((r->d.stride + 31) / 32)));
-    SM_CUDA(cudaMalloc(&r->mesh_render_large_count, sizeof(u32)));
-    SM_CUDA(cudaMemsetAsync(r->mesh_render_large_count, 0, sizeof(u32), stream));
-    int status = ResidentBlocks(k_mesh_render_mark, kMarkBlock, r->sm_count, &r->mesh_render_mark_blocks);
-    if (status == SM_OK) status = ResidentBlocks(k_mesh_render_tri, kTriBlock, r->sm_count, &r->mesh_render_tri_blocks);
-    if (status == SM_OK) status = ResidentBlocks(k_mesh_render_large, kLargeBlock, r->sm_count, &r->mesh_render_large_blocks);
-    if (status == SM_OK) status = ResidentBlocks(k_mesh_render_splat, kSplatBlock, r->sm_count, &r->mesh_render_splat_blocks);
+  RenderScratch& s = *r->render;
+  if (s.mesh_large_count == nullptr) {
+    SM_CUDA(cudaMalloc(&s.mesh_marks, sizeof(u32) * ((r->d.stride + 31) / 32)));
+    SM_CUDA(cudaMalloc(&s.mesh_large_count, sizeof(u32)));
+    SM_CUDA(cudaMemsetAsync(s.mesh_large_count, 0, sizeof(u32), stream));
+    int status = ResidentBlocks(k_mesh_render_mark, kMarkBlock, r->sm_count, &s.mesh_mark_blocks);
+    if (status == SM_OK) status = ResidentBlocks(k_mesh_render_tri, kTriBlock, r->sm_count, &s.mesh_tri_blocks);
+    if (status == SM_OK) status = ResidentBlocks(k_mesh_render_large, kLargeBlock, r->sm_count, &s.mesh_large_blocks);
+    if (status == SM_OK) status = ResidentBlocks(k_mesh_render_splat, kSplatBlock, r->sm_count, &s.mesh_splat_blocks);
     if (status == SM_OK)
-      status = ResidentBlocks(k_mesh_render_splat_large, kLargeBlock, r->sm_count, &r->mesh_render_splat_large_blocks);
+      status = ResidentBlocks(k_mesh_render_splat_large, kLargeBlock, r->sm_count, &s.mesh_splat_large_blocks);
     if (status != SM_OK) return status;
   }
-  if (triangles > r->mesh_render_large_capacity) {
-    cudaFree(r->mesh_render_large_list);   // synchronises the device: an earlier render may still use it
-    r->mesh_render_large_list = nullptr;
-    r->mesh_render_large_capacity = 0;
-    SM_CUDA(cudaMalloc(&r->mesh_render_large_list, sizeof(u32) * triangles));
-    r->mesh_render_large_capacity = triangles;
+  if (triangles > s.mesh_large_capacity) {
+    cudaFree(s.mesh_large_list);   // synchronises the device: an earlier render may still use it
+    s.mesh_large_list = nullptr;
+    s.mesh_large_capacity = 0;
+    SM_CUDA(cudaMalloc(&s.mesh_large_list, sizeof(u32) * triangles));
+    s.mesh_large_capacity = triangles;
   }
   return SM_OK;
 }
@@ -552,12 +566,13 @@ int RenderSurfels(sm_reconstruction* r, cudaStream_t stream, const sm_render_par
                               normal, normal_pitch, index, index_pitch, &a);
   if (status == SM_OK) status = EnsureRenderBuffers(r, stream, static_cast<size_t>(p.width) * static_cast<size_t>(p.height));
   if (status != SM_OK) return status;
-  a.keys = r->render_keys;
-  a.large_list = r->render_large_list;
-  a.large_count = r->render_large_count;
+  const RenderScratch& s = *r->render;
+  a.keys = s.keys;
+  a.large_list = s.large_list;
+  a.large_count = s.large_count;
   r->last_stream = stream;
-  { LaunchScope scope(stream, KID_RENDER_SPLAT); LaunchKernel(k_render_splat, dim3(r->render_splat_blocks), dim3(kSplatBlock), 0, stream, r->d, a); }
-  { LaunchScope scope(stream, KID_RENDER_LARGE); LaunchKernel(k_render_large, dim3(r->render_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a); }
+  { LaunchScope scope(stream, KID_RENDER_SPLAT); LaunchKernel(k_render_splat, dim3(s.splat_blocks), dim3(kSplatBlock), 0, stream, r->d, a); }
+  { LaunchScope scope(stream, KID_RENDER_LARGE); LaunchKernel(k_render_large, dim3(s.large_blocks), dim3(kLargeBlock), 0, stream, r->d, a); }
   const dim3 resolve_grid((p.width + kResolveBlock - 1) / kResolveBlock, p.height < 65535 ? p.height : 65535);
   { LaunchScope scope(stream, KID_RENDER_RESOLVE); LaunchKernel(k_render_resolve, resolve_grid, dim3(kResolveBlock), 0, stream, r->d, a); }
   return CheckLaunch("render surfels");
@@ -579,31 +594,32 @@ int RenderMesh(sm_reconstruction* r, cudaStream_t stream, const sm_render_params
   status = EnsureRenderBuffers(r, stream, static_cast<size_t>(p.width) * static_cast<size_t>(p.height));
   if (status == SM_OK) status = EnsureMeshRenderBuffers(r, stream, static_cast<u32>(triangle_count));
   if (status != SM_OK) return status;
-  a.keys = r->render_keys;
-  a.large_list = r->render_large_list;
-  a.large_count = r->render_large_count;
+  const RenderScratch& s = *r->render;
+  a.keys = s.keys;
+  a.large_list = s.large_list;
+  a.large_count = s.large_count;
   MeshArgs m;
   m.triangles = triangles;
   m.triangle_count = static_cast<u32>(triangle_count);
-  m.marks = r->mesh_render_marks;
-  m.large_list = r->mesh_render_large_list;
-  m.large_count = r->mesh_render_large_count;
+  m.marks = s.mesh_marks;
+  m.large_list = s.mesh_large_list;
+  m.large_count = s.mesh_large_count;
   r->last_stream = stream;
   auto grid = [](u32 items, int block, int resident) {
     const u32 blocks = (items + block - 1) / block;
     return dim3(blocks == 0 ? 1u : (blocks < static_cast<u32>(resident) ? blocks : static_cast<u32>(resident)));
   };
   if (disks) {
-    SM_CUDA(cudaMemsetAsync(r->mesh_render_marks, 0, sizeof(u32) * ((r->d.stride + 31) / 32), stream));
+    SM_CUDA(cudaMemsetAsync(s.mesh_marks, 0, sizeof(u32) * ((r->d.stride + 31) / 32), stream));
     LaunchScope scope(stream, KID_MESH_RENDER_MARK);
-    LaunchKernel(k_mesh_render_mark, grid(m.triangle_count, kMarkBlock, r->mesh_render_mark_blocks), dim3(kMarkBlock), 0,
+    LaunchKernel(k_mesh_render_mark, grid(m.triangle_count, kMarkBlock, s.mesh_mark_blocks), dim3(kMarkBlock), 0,
                  stream, r->d, a, m);
   }
-  { LaunchScope scope(stream, KID_MESH_RENDER_TRI); LaunchKernel(k_mesh_render_tri, grid(m.triangle_count, kTriBlock, r->mesh_render_tri_blocks), dim3(kTriBlock), 0, stream, r->d, a, m); }
-  { LaunchScope scope(stream, KID_MESH_RENDER_LARGE); LaunchKernel(k_mesh_render_large, dim3(r->mesh_render_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a, m); }
+  { LaunchScope scope(stream, KID_MESH_RENDER_TRI); LaunchKernel(k_mesh_render_tri, grid(m.triangle_count, kTriBlock, s.mesh_tri_blocks), dim3(kTriBlock), 0, stream, r->d, a, m); }
+  { LaunchScope scope(stream, KID_MESH_RENDER_LARGE); LaunchKernel(k_mesh_render_large, dim3(s.mesh_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a, m); }
   if (disks) {
-    { LaunchScope scope(stream, KID_MESH_RENDER_SPLAT); LaunchKernel(k_mesh_render_splat, dim3(r->mesh_render_splat_blocks), dim3(kSplatBlock), 0, stream, r->d, a, m); }
-    { LaunchScope scope(stream, KID_MESH_RENDER_SPLAT_LARGE); LaunchKernel(k_mesh_render_splat_large, dim3(r->mesh_render_splat_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a); }
+    { LaunchScope scope(stream, KID_MESH_RENDER_SPLAT); LaunchKernel(k_mesh_render_splat, dim3(s.mesh_splat_blocks), dim3(kSplatBlock), 0, stream, r->d, a, m); }
+    { LaunchScope scope(stream, KID_MESH_RENDER_SPLAT_LARGE); LaunchKernel(k_mesh_render_splat_large, dim3(s.mesh_splat_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a); }
   }
   const dim3 resolve_grid((p.width + kResolveBlock - 1) / kResolveBlock, p.height < 65535 ? p.height : 65535);
   { LaunchScope scope(stream, KID_MESH_RENDER_RESOLVE); LaunchKernel(k_mesh_render_resolve, resolve_grid, dim3(kResolveBlock), 0, stream, r->d, a, m); }
@@ -611,20 +627,12 @@ int RenderMesh(sm_reconstruction* r, cudaStream_t stream, const sm_render_params
 }
 
 void FreeRenderBuffers(sm_reconstruction* r) {
-  cudaFree(r->render_keys);
-  cudaFree(r->render_large_list);
-  cudaFree(r->render_large_count);
-  r->render_keys = nullptr;
-  r->render_large_list = nullptr;
-  r->render_large_count = nullptr;
-  r->render_key_capacity = 0;
-  cudaFree(r->mesh_render_marks);
-  cudaFree(r->mesh_render_large_list);
-  cudaFree(r->mesh_render_large_count);
-  r->mesh_render_marks = nullptr;
-  r->mesh_render_large_list = nullptr;
-  r->mesh_render_large_count = nullptr;
-  r->mesh_render_large_capacity = 0;
+  RenderScratch* s = r->render;
+  if (!s) return;
+  cudaFree(s->keys); cudaFree(s->large_list); cudaFree(s->large_count);
+  cudaFree(s->mesh_marks); cudaFree(s->mesh_large_list); cudaFree(s->mesh_large_count);
+  delete s;
+  r->render = nullptr;
 }
 
 }  // namespace smb

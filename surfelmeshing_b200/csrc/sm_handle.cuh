@@ -44,14 +44,32 @@ constexpr double kDefaultTieBreakEarlyFractionSecond = 0.02;
 TieBreak MakeTieBreak(const TieBreakConfig& cfg, u32 frame_index);
 int SetTieBreakWave(TieBreakConfig* cfg, u32 wave, u32 capacity);   // uses cfg->lane_request
 
-struct FrameGraph;  // pipeline.cu
-void DestroyFrameGraph(FrameGraph* g);
-struct StreamSession;  // pipeline.cu: an open sm_session_begin
-void DestroySession(StreamSession* s);
-struct TrackState;     // track.cu
-struct MeshCounters;   // mesh.cu
-struct MeshLive;       // mesh.cu: the persistent mesh of sm_mesh_update
-struct HoleScratch;    // holes.cu: the buffers of sm_mesh_fill_holes
+// One buffer set of the frame pipeline: association rasters, visible list, merge flags, neighbour-update list.
+struct BufferSet {
+  PixelAssoc* assoc = nullptr;
+  float* first_depth = nullptr;
+  u8* supported = nullptr;
+  VisEntry* vis = nullptr;
+  u32* seg_count = nullptr;
+  u8* merge_flag = nullptr;
+  uint2* upd_list = nullptr;
+  u32* upd_count = nullptr;
+};
+
+// Points `d` at buffer set `s`.
+inline void UseSet(DeviceState& d, const BufferSet& s) {
+  d.assoc = s.assoc; d.first_depth = s.first_depth; d.supported = s.supported;
+  d.vis = s.vis; d.seg_count = s.seg_count; d.merge_flag = s.merge_flag;
+  d.upd_list = s.upd_list; d.upd_count = s.upd_count;
+}
+
+struct RunBuffers;       // pipeline.cu: the frame loop of sm_stream_run and of sessions
+struct StreamSession;    // pipeline.cu: an open sm_session_begin
+struct TransferScratch;  // transfer.cu: the staging of sm_transfer_delta_to_cpu
+struct RenderScratch;    // render.cu: sm_render_surfels / sm_render_mesh
+struct TrackScratch;     // track.cu: sm_track_frame* / sm_track_linearize*
+struct MeshScratch;      // mesh.cu: sm_triangulate, and the persistent mesh of sm_mesh_update
+struct HoleScratch;      // holes.cu: the buffers of sm_mesh_fill_holes
 
 }  // namespace smb
 
@@ -79,112 +97,30 @@ struct sm_reconstruction {
   smb::u16* blend_src = nullptr; size_t blend_src_pitch = 0;
   // Association rasters / lists per buffer set: the pre-processing tail of a later frame resets one set
   // while Integrate() of an earlier frame still works on another (sm_stream_run).
-  smb::PixelAssoc* assoc_set[smb::kSets] = {};
-  float* first_depth_set[smb::kSets] = {};
-  smb::u8* supported_set[smb::kSets] = {};
-  smb::VisEntry* vis_set[smb::kSets] = {};
-  smb::u32* seg_count_set[smb::kSets] = {};
-  smb::u8* merge_flag_set[smb::kSets] = {};
-  uint2* upd_list_set[smb::kSets] = {};
-  smb::u32* upd_count_set[smb::kSets] = {};
-  // stream-runner buffers (pre-processing outputs per buffer set)
-  smb::u16* run_depth[smb::kSets] = {}; size_t run_depth_pitch = 0;
-  float2* run_normals[smb::kSets] = {}; size_t run_normals_pitch = 0;
-  float* run_radius[smb::kSets] = {}; size_t run_radius_pitch = 0;
-  smb::u16* run_depth_pre[smb::kSets] = {};   // pre-blend copy of run_depth (merge runs next to blend)
+  smb::BufferSet sets[smb::kSets];
   float4* reg_records = nullptr;  // [2][stride]: both regularisation record buffers (DeviceState::smooth / smooth_next)
-  cudaEvent_t entry_event = nullptr;   // sm_stream_run / sm_session_begin: the start of the frame loop on the caller's stream
-  // host-resident streams: raw-depth / colour rings filled by the upload stream
-  std::vector<smb::u16*> ring_depth; size_t ring_depth_pitch = 0;
-  std::vector<uchar3*> ring_color; size_t ring_color_pitch = 0;
-  cudaStream_t upload_stream = nullptr;
-  cudaEvent_t upload_done = nullptr;
-  // MedianFilterAndDensifyDepthMap passes applied to every raw depth map entering the ring
-  // (APP/main.cc:435 --median_filter_and_densify_iterations, default 0) and their staging buffers
+  // MedianFilterAndDensifyDepthMap passes applied to every raw depth map entering the frame ring
+  // (APP/main.cc:435 --median_filter_and_densify_iterations, default 0)
   int median_iterations = 0;
-  smb::u16* median_stage[2] = {nullptr, nullptr}; size_t median_stage_pitch = 0;
   // Input pyramid level (APP/main.cc:299-303 --pyramid_level, default 0): sm_stream_run takes frames of
-  // 2^L times the handle's size and downscales them on the upload stream; host frames pass through
-  // full-size staging buffers of pyramid_stage_width x pyramid_stage_height pixels.
+  // 2^L times the handle's size and downscales them on the upload stream.
   int pyramid_level = 0;
-  smb::u16* pyramid_depth_stage = nullptr; size_t pyramid_depth_stage_pitch = 0;
-  smb::u8* pyramid_color_stage = nullptr; size_t pyramid_color_stage_pitch = 0;
-  int pyramid_stage_width = 0, pyramid_stage_height = 0;
-  std::vector<cudaEvent_t> iteration_done;   // frame loop: one event per step slot (ring reuse)
-  // delta transfer (transfer.cu): operation counter, per-operation regularisation thresholds, staging
+  // delta transfer (transfer.cu): operation counter, per-operation regularisation thresholds
   smb::u32 op_epoch = 0;
   uint64_t state_generation = 1;   // bumped by sm_reset / sm_load_state
   struct Operation { smb::u32 epoch; int stamp_threshold; };
   std::vector<Operation> op_history;
-  smb::u32* delta_index = nullptr; float* delta_values = nullptr; smb::u32* delta_cursor = nullptr;
-  smb::u32 delta_capacity = 0;
-  smb::u32* delta_host = nullptr; size_t delta_host_capacity = 0;   // pinned, in 32-bit words
-  // frame graph (pipeline.cu)
-  cudaStream_t graph_stream = nullptr;
-  cudaEvent_t graph_exit = nullptr;
-  smb::FrameGraph* graph = nullptr;
   // incremental session (sm_session_begin .. sm_session_end); nullptr = none open
   smb::StreamSession* session = nullptr;
   // Set while a frame-graph session is open: a device copy of Counters::merge_count as of the newest integrated
   // frame, which FetchCounters reports instead (the front half of a step already counted the next frame's merges).
   const smb::u32* reported_merge_count = nullptr;
-  // sm_render_surfels scratch (render.cu), allocated by the first render: the key raster (all keys "empty"
-  // between calls), the large-splat list (capacity slots) and its count (zero between calls), resident grids.
-  unsigned long long* render_keys = nullptr; size_t render_key_capacity = 0;   // in pixels
-  smb::u32* render_large_list = nullptr;
-  smb::u32* render_large_count = nullptr;
-  int render_splat_blocks = 0, render_large_blocks = 0;
-  // sm_render_mesh scratch (render.cu) beyond the above, allocated by the first mesh render: one bit per slot of
-  // capacity (corners of the triangles drawn), the large-triangle list (grown to the triangle count) and its count
-  // (zero between calls), resident grids.
-  smb::u32* mesh_render_marks = nullptr;
-  smb::u32* mesh_render_large_list = nullptr; smb::u32 mesh_render_large_capacity = 0;   // in triangles
-  smb::u32* mesh_render_large_count = nullptr;
-  int mesh_render_mark_blocks = 0, mesh_render_tri_blocks = 0, mesh_render_large_blocks = 0;
-  int mesh_render_splat_blocks = 0, mesh_render_splat_large_blocks = 0;
-  // sm_track_frame / sm_track_linearize scratch (track.cu), allocated by the first call: the filtered live pyramid,
-  // the rendered model view, two level-0 views of tracked frames (depth, normals) of which track_previous is the
-  // newest, the pose that call returned, the per-block partial rows and the device / pinned tracker state (allocated
-  // last: non-null means every buffer exists).
-  smb::u16* track_level[4] = {}; size_t track_level_pitch[4] = {};
-  float* track_model_depth = nullptr; size_t track_model_depth_pitch = 0;
-  float* track_model_normal = nullptr; size_t track_model_normal_pitch = 0;
-  float* track_view_depth[2] = {}; size_t track_view_depth_pitch[2] = {};
-  float* track_view_normal[2] = {}; size_t track_view_normal_pitch[2] = {};
-  int track_previous = 0;
-  bool track_has_previous = false;
-  float track_previous_pose[12] = {};
-  double* track_partials = nullptr;
-  int track_blocks = 0;
-  smb::TrackState* track_state = nullptr;
-  smb::TrackState* track_host_state = nullptr;
-  // sm_track_frame_rgbd / sm_track_linearize_rgbd scratch (track.cu), allocated by the first RGB-D call: the model
-  // colour the render writes, the live and model intensity pyramids, the level-0 live intensity kept for the next
-  // SM_TRACK_PREVIOUS_FRAME call (allocated last: non-null means every buffer exists), the partial rows of the RGB-D
-  // linearisation's resident grid, and whether the previous tracking call was an RGB-D call.
-  smb::u8* track_model_color = nullptr; size_t track_model_color_pitch = 0;
-  float* track_live_intensity[4] = {}; size_t track_live_intensity_pitch[4] = {};
-  float* track_model_intensity[4] = {}; size_t track_model_intensity_pitch[4] = {};
-  double* track_rgbd_partials = nullptr;
-  int track_rgbd_blocks = 0;
-  float* track_kept_intensity = nullptr; size_t track_kept_intensity_pitch = 0;
-  bool track_previous_rgbd = false;
-  // sm_triangulate scratch (mesh.cu), allocated by the first call and grown to surfels_size(): the k-NN index over
-  // the smooth positions, the umbrellas ([mesh_slots][SM_MESH_MAX_UMBRELLA] pairs) and their lengths, the per-slot
-  // triangle counts (scanned in place into offsets) and the scan's tile sums; the device counters and their
-  // pinned mirror; resident grids.
-  sm_knn_index* mesh_index = nullptr;
-  uint2* mesh_umbrella = nullptr;
-  smb::u32* mesh_umbrella_count = nullptr;
-  smb::u32* mesh_counts = nullptr;
-  smb::u32* mesh_scan_sums = nullptr;
-  smb::u32 mesh_slots = 0;
-  smb::MeshCounters* mesh_counters = nullptr;
-  smb::MeshCounters* mesh_host_counters = nullptr;
-  int mesh_umbrella_blocks = 0, mesh_emit_blocks = 0;
-  // sm_mesh_update's persistent mesh (mesh.cu), created by the first update; it shares only mesh_index.
-  smb::MeshLive* mesh_live = nullptr;
-  // sm_mesh_fill_holes scratch (holes.cu), created by the first call with more than zero triangles.
+  // The scratch of each feature, created by its first call; nullptr = not yet. Its Free... releases it.
+  smb::RunBuffers* run = nullptr;
+  smb::TransferScratch* transfer = nullptr;
+  smb::RenderScratch* render = nullptr;
+  smb::TrackScratch* track = nullptr;
+  smb::MeshScratch* mesh = nullptr;
   smb::HoleScratch* holes = nullptr;
 };
 
@@ -261,6 +197,7 @@ int SessionBegin(sm_reconstruction* r, cudaStream_t stream, const sm_preprocess_
 int SessionPush(sm_reconstruction* r, const u16* depth, size_t depth_pitch, const uint8_t* color, size_t color_pitch,
                 bool on_host, const float* global_T_frame, const float* frame_T_global, sm_session_status* status);
 int SessionEnd(sm_reconstruction* r, sm_stream_stats* stats);
+void FreeRunBuffers(sm_reconstruction* r);
 // out (3x4) = scale(other_T_global) . scale(global_T_ref) (sm_outlier_filter_transforms)
 void OutlierFilterTransform(float depth_scaling, const float* global_T_ref, const float* other_T_global, float* out);
 }  // namespace smb

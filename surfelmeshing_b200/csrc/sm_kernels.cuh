@@ -17,6 +17,12 @@ namespace smb {
 // ---- error / bookkeeping (api.cu) ---------------------------------------------------------
 int SetError(int code, const char* message);
 int CheckLaunch(const char* what);   // cudaGetLastError() -> SM_OK / SM_ERR_CUDA
+// A failed CUDA call returns SM_ERR_CUDA from the enclosing function, "<call>: <CUDA's message>" in sm_last_error().
+#define SM_CUDA(call)                                                                                   \
+  do {                                                                                                  \
+    const cudaError_t e_ = (call);                                                                      \
+    if (e_ != cudaSuccess) return smb::SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
+  } while (0)
 
 // Every kernel launch of the library goes through a LaunchScope: it counts the launch
 // (sm_kernel_launch_count) and, while sm_profile_kernels(1) is active, brackets it with CUDA

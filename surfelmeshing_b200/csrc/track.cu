@@ -29,12 +29,6 @@ namespace smb {
 
 namespace {
 
-#define SM_CUDA(call)                                                                                   \
-  do {                                                                                                  \
-    const cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-  } while (0)
-
 constexpr int kLinearizeBlock = 256;
 constexpr int kLinearizeWarps = kLinearizeBlock / 32;
 constexpr int kSolveBlock = 256;
@@ -63,6 +57,38 @@ struct TrackState {
   double system[kTermsRGBD];   // sums of the last linearisation (the first kTerms for a depth-only one)
   u32 photometric_inliers;     // RGB-D, level 0, last linearisation
   float rms_intensity;         // RGB-D, level 0, last linearisation: sqrt(sum r_c^2 / photometric_inliers)
+};
+
+// The scratch of sm_track_frame_rgbd / sm_track_linearize_rgbd beyond TrackScratch's, created whole by the first
+// RGB-D call: the model colour the render writes, the live and model intensity pyramids, the partial rows of the
+// RGB-D linearisation's resident grid and the level-0 live intensity kept for the next SM_TRACK_PREVIOUS_FRAME call.
+struct TrackRGBDScratch {
+  u8* model_color = nullptr; size_t model_color_pitch = 0;
+  float* live_intensity[kMaxLevels] = {}; size_t live_intensity_pitch[kMaxLevels] = {};
+  float* model_intensity[kMaxLevels] = {}; size_t model_intensity_pitch[kMaxLevels] = {};
+  double* partials = nullptr;
+  int blocks = 0;
+  float* kept_intensity = nullptr; size_t kept_intensity_pitch = 0;
+};
+
+// The scratch of sm_track_frame / sm_track_linearize, created whole by the first call: the filtered live pyramid,
+// the rendered model view, two level-0 views of tracked frames (depth, normals) of which `previous` is the newest,
+// the partial rows, the device / pinned tracker state, the RGB-D half and what the newest sm_track_frame* left.
+struct TrackScratch {
+  u16* level[kMaxLevels] = {}; size_t level_pitch[kMaxLevels] = {};
+  float* model_depth = nullptr; size_t model_depth_pitch = 0;
+  float* model_normal = nullptr; size_t model_normal_pitch = 0;
+  float* view_depth[2] = {}; size_t view_depth_pitch[2] = {};
+  float* view_normal[2] = {}; size_t view_normal_pitch[2] = {};
+  double* partials = nullptr;
+  int blocks = 0;
+  TrackState* state = nullptr;
+  TrackState* host_state = nullptr;
+  TrackRGBDScratch* rgbd = nullptr;   // allocated by the first RGB-D call
+  int previous = 0;
+  bool has_previous = false;
+  float previous_pose[12] = {};       // the pose that call returned
+  bool previous_rgbd = false;         // that call was an RGB-D call
 };
 
 namespace {
@@ -591,70 +617,68 @@ void ComposeRigid(const double* a, const double* b, double* out) {
   }
 }
 
-// All scratch, the device state last: a non-null track_state means every buffer exists. A failed allocation frees
-// what was allocated, so the next call starts over.
-int AllocateTrackBuffers(sm_reconstruction* r) {
-  const int status = ResidentBlocks(k_track_linearize, kLinearizeBlock, r->sm_count, &r->track_blocks);
+int AllocateTrackBuffers(const sm_reconstruction* r, TrackScratch& t) {
+  const int status = ResidentBlocks(k_track_linearize, kLinearizeBlock, r->sm_count, &t.blocks);
   if (status != SM_OK) return status;
-  SM_CUDA(cudaMalloc(&r->track_partials, sizeof(double) * kTerms * r->track_blocks));
-  SM_CUDA(cudaMallocHost(&r->track_host_state, sizeof(TrackState)));
+  SM_CUDA(cudaMalloc(&t.partials, sizeof(double) * kTerms * t.blocks));
+  SM_CUDA(cudaMallocHost(&t.host_state, sizeof(TrackState)));
   const size_t W = static_cast<size_t>(r->d.width), H = static_cast<size_t>(r->d.height);
   for (int l = 0; l < kMaxLevels; ++l) {
     if (!LevelUsable(r, l)) break;
     const LevelCamera c = ScaledCamera(r, l);
-    SM_CUDA(cudaMallocPitch(&r->track_level[l], &r->track_level_pitch[l], sizeof(u16) * c.width, c.height));
+    SM_CUDA(cudaMallocPitch(&t.level[l], &t.level_pitch[l], sizeof(u16) * c.width, c.height));
   }
-  SM_CUDA(cudaMallocPitch(&r->track_model_depth, &r->track_model_depth_pitch, sizeof(float) * W, H));
-  SM_CUDA(cudaMallocPitch(&r->track_model_normal, &r->track_model_normal_pitch, 3 * sizeof(float) * W, H));
+  SM_CUDA(cudaMallocPitch(&t.model_depth, &t.model_depth_pitch, sizeof(float) * W, H));
+  SM_CUDA(cudaMallocPitch(&t.model_normal, &t.model_normal_pitch, 3 * sizeof(float) * W, H));
   for (int k = 0; k < 2; ++k) {
-    SM_CUDA(cudaMallocPitch(&r->track_view_depth[k], &r->track_view_depth_pitch[k], sizeof(float) * W, H));
-    SM_CUDA(cudaMallocPitch(&r->track_view_normal[k], &r->track_view_normal_pitch[k], 3 * sizeof(float) * W, H));
+    SM_CUDA(cudaMallocPitch(&t.view_depth[k], &t.view_depth_pitch[k], sizeof(float) * W, H));
+    SM_CUDA(cudaMallocPitch(&t.view_normal[k], &t.view_normal_pitch[k], 3 * sizeof(float) * W, H));
   }
-  SM_CUDA(cudaMalloc(&r->track_state, sizeof(TrackState)));
+  SM_CUDA(cudaMalloc(&t.state, sizeof(TrackState)));
   return SM_OK;
 }
 
+// A non-null r->track means every buffer exists: a failed allocation frees the scratch, so the next call starts over.
 int EnsureTrackBuffers(sm_reconstruction* r) {
-  if (r->track_state != nullptr) return SM_OK;
-  const int status = AllocateTrackBuffers(r);
+  if (r->track) return SM_OK;
+  r->track = new TrackScratch();
+  const int status = AllocateTrackBuffers(r, *r->track);
   if (status != SM_OK) FreeTrackBuffers(r);
   return status;
 }
 
-// The RGB-D scratch, the kept intensity last: a non-null track_kept_intensity means every buffer exists.
-int AllocateTrackRGBDBuffers(sm_reconstruction* r) {
-  const int status = ResidentBlocks(k_track_linearize_rgbd, kLinearizeBlock, r->sm_count, &r->track_rgbd_blocks);
+int AllocateTrackRGBDBuffers(const sm_reconstruction* r, TrackRGBDScratch& g) {
+  const int status = ResidentBlocks(k_track_linearize_rgbd, kLinearizeBlock, r->sm_count, &g.blocks);
   if (status != SM_OK) return status;
-  SM_CUDA(cudaMalloc(&r->track_rgbd_partials, sizeof(double) * kTermsRGBD * r->track_rgbd_blocks));
+  SM_CUDA(cudaMalloc(&g.partials, sizeof(double) * kTermsRGBD * g.blocks));
   const size_t W = static_cast<size_t>(r->d.width), H = static_cast<size_t>(r->d.height);
-  SM_CUDA(cudaMallocPitch(&r->track_model_color, &r->track_model_color_pitch, 3 * W, H));
+  SM_CUDA(cudaMallocPitch(&g.model_color, &g.model_color_pitch, 3 * W, H));
   for (int l = 0; l < kMaxLevels; ++l) {
     if (!LevelUsable(r, l)) break;
     const LevelCamera c = ScaledCamera(r, l);
-    SM_CUDA(cudaMallocPitch(&r->track_live_intensity[l], &r->track_live_intensity_pitch[l], sizeof(float) * c.width,
-                            c.height));
-    SM_CUDA(cudaMallocPitch(&r->track_model_intensity[l], &r->track_model_intensity_pitch[l], sizeof(float) * c.width,
-                            c.height));
+    SM_CUDA(cudaMallocPitch(&g.live_intensity[l], &g.live_intensity_pitch[l], sizeof(float) * c.width, c.height));
+    SM_CUDA(cudaMallocPitch(&g.model_intensity[l], &g.model_intensity_pitch[l], sizeof(float) * c.width, c.height));
   }
-  SM_CUDA(cudaMallocPitch(&r->track_kept_intensity, &r->track_kept_intensity_pitch, sizeof(float) * W, H));
+  SM_CUDA(cudaMallocPitch(&g.kept_intensity, &g.kept_intensity_pitch, sizeof(float) * W, H));
   return SM_OK;
 }
 
-void FreeTrackRGBDBuffers(sm_reconstruction* r) {
-  for (int l = 0; l < kMaxLevels; ++l) {
-    cudaFree(r->track_live_intensity[l]); cudaFree(r->track_model_intensity[l]);
-    r->track_live_intensity[l] = nullptr; r->track_model_intensity[l] = nullptr;
-  }
-  cudaFree(r->track_model_color); cudaFree(r->track_rgbd_partials); cudaFree(r->track_kept_intensity);
-  r->track_model_color = nullptr; r->track_rgbd_partials = nullptr; r->track_kept_intensity = nullptr;
-  r->track_previous_rgbd = false;
+void FreeTrackRGBDBuffers(TrackScratch& t) {
+  TrackRGBDScratch* g = t.rgbd;
+  if (!g) return;
+  for (int l = 0; l < kMaxLevels; ++l) { cudaFree(g->live_intensity[l]); cudaFree(g->model_intensity[l]); }
+  cudaFree(g->model_color); cudaFree(g->partials); cudaFree(g->kept_intensity);
+  delete g;
+  t.rgbd = nullptr;
 }
 
+// A non-null rgbd means every RGB-D buffer exists: a failed allocation frees that half, so the next call starts over.
 int EnsureTrackRGBDBuffers(sm_reconstruction* r) {
   int status = EnsureTrackBuffers(r);
-  if (status != SM_OK || r->track_kept_intensity != nullptr) return status;
-  status = AllocateTrackRGBDBuffers(r);
-  if (status != SM_OK) FreeTrackRGBDBuffers(r);
+  if (status != SM_OK || r->track->rgbd) return status;
+  r->track->rgbd = new TrackRGBDScratch();
+  status = AllocateTrackRGBDBuffers(r, *r->track->rgbd);
+  if (status != SM_OK) FreeTrackRGBDBuffers(*r->track);
   return status;
 }
 
@@ -673,16 +697,17 @@ void LaunchIntensityPyramids(sm_reconstruction* r, cudaStream_t stream, int leve
                              size_t live_color_pitch, const u8* model_color, size_t model_color_pitch,
                              const float* model_depth, size_t model_depth_pitch, float* kept) {
   const int W = r->d.width, H = r->d.height;
+  const TrackRGBDScratch& g = *r->track->rgbd;
   {
     IntensityBaseArgs a;
     a.width = W; a.height = H;
     a.live_color = live_color; a.live_color_pitch = live_color_pitch;
     a.model_color = model_color; a.model_color_pitch = model_color_pitch;
-    a.model_kept = r->track_kept_intensity; a.model_kept_pitch = r->track_kept_intensity_pitch;
+    a.model_kept = g.kept_intensity; a.model_kept_pitch = g.kept_intensity_pitch;
     a.model_depth = model_depth; a.model_depth_pitch = model_depth_pitch;
-    a.live = r->track_live_intensity[0]; a.live_pitch = r->track_live_intensity_pitch[0];
-    a.model = r->track_model_intensity[0]; a.model_pitch = r->track_model_intensity_pitch[0];
-    a.kept = kept; a.kept_pitch = r->track_kept_intensity_pitch;
+    a.live = g.live_intensity[0]; a.live_pitch = g.live_intensity_pitch[0];
+    a.model = g.model_intensity[0]; a.model_pitch = g.model_intensity_pitch[0];
+    a.kept = kept; a.kept_pitch = g.kept_intensity_pitch;
     LaunchScope scope(stream, KID_TRACK_INTENSITY_BASE);
     LaunchKernel(k_track_intensity_base, dim3((W + 255) / 256, H), dim3(256), 0, stream, a);
   }
@@ -690,10 +715,10 @@ void LaunchIntensityPyramids(sm_reconstruction* r, cudaStream_t stream, int leve
     const LevelCamera s = ScaledCamera(r, l - 1), c = ScaledCamera(r, l);
     IntensityDownArgs a;
     a.src_width = s.width; a.src_height = s.height; a.width = c.width; a.height = c.height;
-    a.src[0] = r->track_live_intensity[l - 1]; a.src_pitch[0] = r->track_live_intensity_pitch[l - 1];
-    a.src[1] = r->track_model_intensity[l - 1]; a.src_pitch[1] = r->track_model_intensity_pitch[l - 1];
-    a.dst[0] = r->track_live_intensity[l]; a.dst_pitch[0] = r->track_live_intensity_pitch[l];
-    a.dst[1] = r->track_model_intensity[l]; a.dst_pitch[1] = r->track_model_intensity_pitch[l];
+    a.src[0] = g.live_intensity[l - 1]; a.src_pitch[0] = g.live_intensity_pitch[l - 1];
+    a.src[1] = g.model_intensity[l - 1]; a.src_pitch[1] = g.model_intensity_pitch[l - 1];
+    a.dst[0] = g.live_intensity[l]; a.dst_pitch[0] = g.live_intensity_pitch[l];
+    a.dst[1] = g.model_intensity[l]; a.dst_pitch[1] = g.model_intensity_pitch[l];
     LaunchScope scope(stream, KID_TRACK_INTENSITY_DOWN);
     LaunchKernel(k_track_intensity_down, dim3((c.width + 255) / 256, c.height, 2), dim3(256), 0, stream, a);
   }
@@ -715,8 +740,8 @@ LinearizeArgs MakeLinearizeArgs(const sm_reconstruction* r, const sm_track_param
   a.model_normal = model_normal; a.model_normal_pitch = model_normal_pitch;
   a.max_distance_squared = tp.max_point_distance * tp.max_point_distance;
   a.cos_max_angle = static_cast<float>(std::cos(static_cast<double>(tp.max_normal_angle_deg) * M_PI / 180.0));
-  a.state = r->track_state;
-  a.partials = r->track_partials;
+  a.state = r->track->state;
+  a.partials = r->track->partials;
   return a;
 }
 
@@ -724,9 +749,9 @@ SolveArgs MakeSolveArgs(const sm_reconstruction* r, const sm_track_params& tp, i
   SolveArgs s;
   s.level = level;
   s.solve = solve ? 1 : 0;
-  s.blocks = r->track_blocks;
-  s.partials = r->track_partials;
-  s.state = r->track_state;
+  s.blocks = r->track->blocks;
+  s.partials = r->track->partials;
+  s.state = r->track->state;
   s.min_inlier_fraction = tp.min_inlier_fraction;
   s.convergence_rotation = tp.convergence_rotation;
   s.convergence_translation = tp.convergence_translation;
@@ -734,40 +759,41 @@ SolveArgs MakeSolveArgs(const sm_reconstruction* r, const sm_track_params& tp, i
 }
 
 void LaunchIteration(sm_reconstruction* r, cudaStream_t stream, const LinearizeArgs& la, const SolveArgs& sa) {
-  { LaunchScope scope(stream, KID_TRACK_LINEARIZE); LaunchKernel(k_track_linearize, dim3(r->track_blocks), dim3(kLinearizeBlock), 0, stream, la); }
+  { LaunchScope scope(stream, KID_TRACK_LINEARIZE); LaunchKernel(k_track_linearize, dim3(r->track->blocks), dim3(kLinearizeBlock), 0, stream, la); }
   { LaunchScope scope(stream, KID_TRACK_SOLVE); LaunchKernel(k_track_solve, dim3(1), dim3(kSolveBlock), 0, stream, sa); }
 }
 
 // One RGB-D iteration at la.level, over the pyramids LaunchIntensityPyramids built.
 void LaunchIterationRGBD(sm_reconstruction* r, cudaStream_t stream, const sm_track_rgbd_params& rp,
                          const LinearizeArgs& la, SolveArgs sa) {
+  const TrackRGBDScratch& rgbd = *r->track->rgbd;
   LinearizeRGBDArgs g;
   g.icp = la;
-  g.icp.partials = r->track_rgbd_partials;
-  g.live_intensity = r->track_live_intensity[la.level]; g.live_intensity_pitch = r->track_live_intensity_pitch[la.level];
-  g.model_intensity = r->track_model_intensity[la.level];
-  g.model_intensity_pitch = r->track_model_intensity_pitch[la.level];
+  g.icp.partials = rgbd.partials;
+  g.live_intensity = rgbd.live_intensity[la.level]; g.live_intensity_pitch = rgbd.live_intensity_pitch[la.level];
+  g.model_intensity = rgbd.model_intensity[la.level];
+  g.model_intensity_pitch = rgbd.model_intensity_pitch[la.level];
   g.lambda2 = static_cast<double>(rp.photometric_weight) * static_cast<double>(rp.photometric_weight);
   g.max_residual = rp.max_intensity_residual;
   g.min_gradient2 = rp.min_gradient * rp.min_gradient;
-  sa.blocks = r->track_rgbd_blocks;
-  sa.partials = r->track_rgbd_partials;
-  { LaunchScope scope(stream, KID_TRACK_LINEARIZE_RGBD); LaunchKernel(k_track_linearize_rgbd, dim3(r->track_rgbd_blocks), dim3(kLinearizeBlock), 0, stream, g); }
+  sa.blocks = rgbd.blocks;
+  sa.partials = rgbd.partials;
+  { LaunchScope scope(stream, KID_TRACK_LINEARIZE_RGBD); LaunchKernel(k_track_linearize_rgbd, dim3(rgbd.blocks), dim3(kLinearizeBlock), 0, stream, g); }
   { LaunchScope scope(stream, KID_TRACK_SOLVE_RGBD); LaunchKernel(k_track_solve_rgbd, dim3(1), dim3(kSolveBlock), 0, stream, sa); }
 }
 
 // Uploads a fresh state with `pose` as model_T_live.
 int UploadState(sm_reconstruction* r, cudaStream_t stream, const float* pose) {
-  TrackState* h = r->track_host_state;
+  TrackState* h = r->track->host_state;
   memset(h, 0, sizeof(TrackState));
   for (int k = 0; k < 12; ++k) h->pose[k] = pose[k];
   h->done_level = -1;
-  SM_CUDA(cudaMemcpyAsync(r->track_state, h, sizeof(TrackState), cudaMemcpyHostToDevice, stream));
+  SM_CUDA(cudaMemcpyAsync(r->track->state, h, sizeof(TrackState), cudaMemcpyHostToDevice, stream));
   return SM_OK;
 }
 
 int DownloadState(sm_reconstruction* r, cudaStream_t stream) {
-  SM_CUDA(cudaMemcpyAsync(r->track_host_state, r->track_state, sizeof(TrackState), cudaMemcpyDeviceToHost, stream));
+  SM_CUDA(cudaMemcpyAsync(r->track->host_state, r->track->state, sizeof(TrackState), cudaMemcpyDeviceToHost, stream));
   SM_CUDA(cudaStreamSynchronize(stream));
   return SM_OK;
 }
@@ -792,9 +818,9 @@ int TrackFrameImpl(sm_reconstruction* r, cudaStream_t stream, const sm_track_par
   if (!LevelUsable(r, tp.levels - 1)) return bad("the coarsest level is smaller than 3 x 3 pixels");
   if (const char* why = CheckTrackParams(tp)) return bad(why);
   if (tp.model_source != SM_TRACK_CLOUD && tp.model_source != SM_TRACK_PREVIOUS_FRAME) return bad("unknown model_source");
-  if (tp.model_source == SM_TRACK_PREVIOUS_FRAME && !r->track_has_previous)
+  if (tp.model_source == SM_TRACK_PREVIOUS_FRAME && !(r->track && r->track->has_previous))
     return bad("SM_TRACK_PREVIOUS_FRAME needs an earlier sm_track_frame call on this handle");
-  if (color && tp.model_source == SM_TRACK_PREVIOUS_FRAME && !r->track_previous_rgbd)
+  if (color && tp.model_source == SM_TRACK_PREVIOUS_FRAME && !r->track->previous_rgbd)
     return bad("SM_TRACK_PREVIOUS_FRAME needs the handle's previous tracking call to be an RGB-D call");
   for (int k = 0; k < 12; ++k) if (!Finite(guess[k])) return bad("global_T_guess must be finite");
   if (!(Finite(pp.depth_scaling) && pp.depth_scaling > 0.f)) return bad("depth_scaling must be finite and > 0");
@@ -806,7 +832,7 @@ int TrackFrameImpl(sm_reconstruction* r, cudaStream_t stream, const sm_track_par
   double guess_d[12], model_T_global[12], global_T_model[12], init[12];
   for (int k = 0; k < 12; ++k) {
     guess_d[k] = guess[k];
-    global_T_model[k] = tp.model_source == SM_TRACK_CLOUD ? guess_d[k] : r->track_previous_pose[k];
+    global_T_model[k] = tp.model_source == SM_TRACK_CLOUD ? guess_d[k] : r->track->previous_pose[k];
   }
   if (!ProjectToRigid(guess_d)) return bad("the rotation of global_T_guess must have a positive determinant");
   if (tp.model_source == SM_TRACK_CLOUD) {
@@ -826,64 +852,65 @@ int TrackFrameImpl(sm_reconstruction* r, cudaStream_t stream, const sm_track_par
   if (status != SM_OK) return status;
   r->last_stream = stream;
   const int W = r->d.width, H = r->d.height;
+  TrackScratch& t = *r->track;
 
   // 1. live pyramid
   status = StageBilateral(stream, pp.bilateral_filter_sigma_xy, pp.bilateral_filter_sigma_depth_factor, 0,
                           pp.bilateral_filter_radius_factor, static_cast<u16>(pp.depth_scaling * pp.max_depth),
-                          pp.depth_valid_region_radius, W, H, depth, depth_pitch, r->track_level[0], r->track_level_pitch[0]);
+                          pp.depth_valid_region_radius, W, H, depth, depth_pitch, t.level[0], t.level_pitch[0]);
   if (status != SM_OK) return status;
   for (int l = 1; l < tp.levels; ++l) {
     const LevelCamera c = ScaledCamera(r, l);
-    status = StageDownscaleMedian(stream, 0, W, H, r->track_level[0], r->track_level_pitch[0], c.width, c.height,
-                                  r->track_level[l], r->track_level_pitch[l]);
+    status = StageDownscaleMedian(stream, 0, W, H, t.level[0], t.level_pitch[0], c.width, c.height, t.level[l],
+                                  t.level_pitch[l]);
     if (status != SM_OK) return status;
   }
 
   // 2. model view and the initial model_T_live
-  const float* model_depth = r->track_model_depth;
-  const float* model_normal = r->track_model_normal;
-  size_t model_depth_pitch = r->track_model_depth_pitch, model_normal_pitch = r->track_model_normal_pitch;
+  const float* model_depth = t.model_depth;
+  const float* model_normal = t.model_normal;
+  size_t model_depth_pitch = t.model_depth_pitch, model_normal_pitch = t.model_normal_pitch;
   if (tp.model_source == SM_TRACK_CLOUD) {
     sm_render_params rp;
     rp.width = W; rp.height = H; rp.fx = r->fx; rp.fy = r->fy; rp.cx = r->cx; rp.cy = r->cy;
     rp.near_depth = kModelNear; rp.far_depth = kModelFar;
-    status = RenderSurfels(r, stream, rp, view_f, r->track_model_depth, r->track_model_depth_pitch,
-                           color ? r->track_model_color : nullptr, color ? r->track_model_color_pitch : 0,
-                           r->track_model_normal, r->track_model_normal_pitch, nullptr, 0);
+    status = RenderSurfels(r, stream, rp, view_f, t.model_depth, t.model_depth_pitch,
+                           color ? t.rgbd->model_color : nullptr, color ? t.rgbd->model_color_pitch : 0,
+                           t.model_normal, t.model_normal_pitch, nullptr, 0);
     if (status != SM_OK) return status;
   } else {
-    model_depth = r->track_view_depth[r->track_previous];
-    model_normal = r->track_view_normal[r->track_previous];
-    model_depth_pitch = r->track_view_depth_pitch[r->track_previous];
-    model_normal_pitch = r->track_view_normal_pitch[r->track_previous];
+    model_depth = t.view_depth[t.previous];
+    model_normal = t.view_normal[t.previous];
+    model_depth_pitch = t.view_depth_pitch[t.previous];
+    model_normal_pitch = t.view_normal_pitch[t.previous];
   }
   // the intensity pyramids (P1-P3); this frame's level-0 intensity replaces the kept one after it is read
   if (color)
     LaunchIntensityPyramids(r, stream, tp.levels, color->live, color->live_pitch,
-                            tp.model_source == SM_TRACK_CLOUD ? r->track_model_color : nullptr, r->track_model_color_pitch,
-                            model_depth, model_depth_pitch, r->track_kept_intensity);
+                            tp.model_source == SM_TRACK_CLOUD ? t.rgbd->model_color : nullptr, t.rgbd->model_color_pitch,
+                            model_depth, model_depth_pitch, t.rgbd->kept_intensity);
   status = UploadState(r, stream, init_f);
   if (status != SM_OK) return status;
 
   // 3. this frame's level-0 view, the model of the next SM_TRACK_PREVIOUS_FRAME call
-  const int view = r->track_has_previous ? 1 - r->track_previous : 0;
+  const int view = t.has_previous ? 1 - t.previous : 0;
   {
     LiveViewArgs v;
     const LevelCamera c = ScaledCamera(r, 0);
     v.width = c.width; v.height = c.height;
     v.fx = c.fx; v.fy = c.fy; v.cx = c.cx; v.cy = c.cy;
     v.inv_depth_scaling = 1.0f / pp.depth_scaling;
-    v.live = r->track_level[0]; v.live_pitch = r->track_level_pitch[0];
-    v.depth = r->track_view_depth[view]; v.depth_pitch = r->track_view_depth_pitch[view];
-    v.normal = r->track_view_normal[view]; v.normal_pitch = r->track_view_normal_pitch[view];
+    v.live = t.level[0]; v.live_pitch = t.level_pitch[0];
+    v.depth = t.view_depth[view]; v.depth_pitch = t.view_depth_pitch[view];
+    v.normal = t.view_normal[view]; v.normal_pitch = t.view_normal_pitch[view];
     LaunchScope scope(stream, KID_TRACK_LIVE_VIEW);
     LaunchKernel(k_track_live_view, dim3((W + 255) / 256, H), dim3(256), 0, stream, v);
   }
 
   // 4. Gauss-Newton, coarse to fine
   for (int l = tp.levels - 1; l >= 0; --l) {
-    const LinearizeArgs la = MakeLinearizeArgs(r, tp, pp.depth_scaling, l, r->track_level[l], r->track_level_pitch[l],
-                                               model_depth, model_depth_pitch, model_normal, model_normal_pitch);
+    const LinearizeArgs la = MakeLinearizeArgs(r, tp, pp.depth_scaling, l, t.level[l], t.level_pitch[l], model_depth,
+                                               model_depth_pitch, model_normal, model_normal_pitch);
     const SolveArgs sa = MakeSolveArgs(r, tp, l, true);
     for (int it = 0; it < tp.iterations[l]; ++it) {
       if (color && color->params->photometric_weight > 0.f) LaunchIterationRGBD(r, stream, *color->params, la, sa);
@@ -896,7 +923,7 @@ int TrackFrameImpl(sm_reconstruction* r, cudaStream_t stream, const sm_track_par
   // 5. one synchronisation, then the result
   status = DownloadState(r, stream);
   if (status != SM_OK) return status;
-  const TrackState& h = *r->track_host_state;
+  const TrackState& h = *t.host_state;
   double out[12];
   if (h.lost) {
     for (int k = 0; k < 12; ++k) out[k] = guess[k];   // the caller's guess, unchanged
@@ -908,11 +935,11 @@ int TrackFrameImpl(sm_reconstruction* r, cudaStream_t stream, const sm_track_par
   }
   for (int k = 0; k < 12; ++k) {
     pose_out[k] = static_cast<float>(out[k]);
-    r->track_previous_pose[k] = pose_out[k];
+    t.previous_pose[k] = pose_out[k];
   }
-  r->track_previous = view;
-  r->track_has_previous = true;
-  r->track_previous_rgbd = color != nullptr;
+  t.previous = view;
+  t.has_previous = true;
+  t.previous_rgbd = color != nullptr;
   if (result) {
     result->tracked = h.lost ? 0 : 1;
     result->iterations = h.iterations;
@@ -966,7 +993,7 @@ int TrackLinearizeImpl(sm_reconstruction* r, cudaStream_t stream, const sm_track
   if (status != SM_OK) return status;
   status = DownloadState(r, stream);
   if (status != SM_OK) return status;
-  const TrackState& h = *r->track_host_state;
+  const TrackState& h = *r->track->host_state;
   for (int k = 0; k < kSystemTerms; ++k) out_system[k] = h.system[k];
   *out_inliers = static_cast<uint32_t>(h.system[kTermInliers]);
   if (color) {
@@ -1009,19 +1036,16 @@ int TrackLinearizeRGBD(sm_reconstruction* r, cudaStream_t stream, const sm_track
 }
 
 void FreeTrackBuffers(sm_reconstruction* r) {
-  FreeTrackRGBDBuffers(r);
-  for (int l = 0; l < kMaxLevels; ++l) { cudaFree(r->track_level[l]); r->track_level[l] = nullptr; }
-  cudaFree(r->track_model_depth); cudaFree(r->track_model_normal);
-  r->track_model_depth = nullptr; r->track_model_normal = nullptr;
-  for (int k = 0; k < 2; ++k) {
-    cudaFree(r->track_view_depth[k]); cudaFree(r->track_view_normal[k]);
-    r->track_view_depth[k] = nullptr; r->track_view_normal[k] = nullptr;
-  }
-  cudaFree(r->track_partials); cudaFree(r->track_state);
-  if (r->track_host_state) cudaFreeHost(r->track_host_state);
-  r->track_partials = nullptr;
-  r->track_state = nullptr;
-  r->track_host_state = nullptr;
+  TrackScratch* t = r->track;
+  if (!t) return;
+  FreeTrackRGBDBuffers(*t);
+  for (int l = 0; l < kMaxLevels; ++l) cudaFree(t->level[l]);
+  cudaFree(t->model_depth); cudaFree(t->model_normal);
+  for (int k = 0; k < 2; ++k) { cudaFree(t->view_depth[k]); cudaFree(t->view_normal[k]); }
+  cudaFree(t->partials); cudaFree(t->state);
+  if (t->host_state) cudaFreeHost(t->host_state);
+  delete t;
+  r->track = nullptr;
 }
 
 }  // namespace smb

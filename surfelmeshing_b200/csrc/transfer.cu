@@ -30,13 +30,15 @@
 
 namespace smb {
 
-namespace {
+// The staging of sm_transfer_delta_to_cpu, created by the first delta transfer: the device record list (grown to
+// surfels_size() in large steps) and its cursor, and the pinned host copy of the records.
+struct TransferScratch {
+  u32* index = nullptr; float* values = nullptr; u32* cursor = nullptr;
+  u32 capacity = 0;
+  u32* host = nullptr; size_t host_capacity = 0;   // in 32-bit words
+};
 
-#define SM_CUDA(call)                                                                                   \
-  do {                                                                                                  \
-    const cudaError_t e_ = (call);                                                                      \
-    if (e_ != cudaSuccess) return SetError(SM_ERR_CUDA, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-  } while (0)
+namespace {
 
 #define SM_S(row, i) d.surfels[static_cast<size_t>(row) * d.stride + (i)]
 #define SM_SU(row, i) reinterpret_cast<u32*>(d.surfels)[static_cast<size_t>(row) * d.stride + (i)]
@@ -221,10 +223,12 @@ void RecordOperation(sm_reconstruction* r, int stamp_threshold) {
 }
 
 void FreeTransferBuffers(sm_reconstruction* r) {
-  cudaFree(r->delta_index); cudaFree(r->delta_values); cudaFree(r->delta_cursor);
-  if (r->delta_host) cudaFreeHost(r->delta_host);
-  r->delta_index = nullptr; r->delta_values = nullptr; r->delta_cursor = nullptr; r->delta_host = nullptr;
-  r->delta_capacity = 0; r->delta_host_capacity = 0;
+  TransferScratch* s = r->transfer;
+  if (!s) return;
+  cudaFree(s->index); cudaFree(s->values); cudaFree(s->cursor);
+  if (s->host) cudaFreeHost(s->host);
+  delete s;
+  r->transfer = nullptr;
 }
 
 int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_index, sm_transfer_token* token, float* x,
@@ -250,49 +254,51 @@ int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_inde
   }
   if (!full && threshold <= 0) full = true;  // every stamp is inside a window: everything may have moved
   if (!full && n > 0) {
+    if (!r->transfer) r->transfer = new TransferScratch();
+    TransferScratch& s = *r->transfer;
     // staging list sized for the worst case (every slot changed), grown in large steps
-    if (r->delta_capacity < n) {
+    if (s.capacity < n) {
       SM_CUDA(cudaStreamSynchronize(stream));
-      cudaFree(r->delta_index); cudaFree(r->delta_values);
-      r->delta_index = nullptr; r->delta_values = nullptr;
+      cudaFree(s.index); cudaFree(s.values);
+      s.index = nullptr; s.values = nullptr;
       const size_t cap = std::min<size_t>(r->d.stride, std::max<size_t>(2 * static_cast<size_t>(n), 1u << 20));
-      SM_CUDA(cudaMalloc(&r->delta_index, sizeof(u32) * cap));
-      SM_CUDA(cudaMalloc(&r->delta_values, sizeof(float) * 8 * cap));
-      r->delta_capacity = static_cast<u32>(cap);
+      SM_CUDA(cudaMalloc(&s.index, sizeof(u32) * cap));
+      SM_CUDA(cudaMalloc(&s.values, sizeof(float) * 8 * cap));
+      s.capacity = static_cast<u32>(cap);
     }
-    if (!r->delta_cursor) SM_CUDA(cudaMalloc(&r->delta_cursor, sizeof(u32)));
-    SM_CUDA(cudaMemsetAsync(r->delta_cursor, 0, sizeof(u32), stream));
+    if (!s.cursor) SM_CUDA(cudaMalloc(&s.cursor, sizeof(u32)));
+    SM_CUDA(cudaMemsetAsync(s.cursor, 0, sizeof(u32), stream));
     DeltaArgs a;
     a.count_slot = r->count_slot;
     a.count_at_token = static_cast<u32>(token->surfel_count);
     a.stamp_threshold = threshold;
     a.epoch_at_token = static_cast<u32>(token->epoch);
-    a.capacity = r->delta_capacity;
-    a.cursor = r->delta_cursor;
-    a.index = r->delta_index;
-    a.values = r->delta_values;
+    a.capacity = s.capacity;
+    a.cursor = s.cursor;
+    a.index = s.index;
+    a.values = s.values;
     { LaunchScope scope(stream, KID_DELTA_SELECT); LaunchKernel(k_delta_select, dim3(r->sm_count * 8), dim3(kBlock), 0, stream, r->d, a); }
     status = CheckLaunch("delta select");
     if (status != SM_OK) return status;
     u32 changed = 0;
-    SM_CUDA(cudaMemcpyAsync(&changed, r->delta_cursor, sizeof(u32), cudaMemcpyDeviceToHost, stream));
+    SM_CUDA(cudaMemcpyAsync(&changed, s.cursor, sizeof(u32), cudaMemcpyDeviceToHost, stream));
     SM_CUDA(cudaStreamSynchronize(stream));
     st.d2h_bytes += sizeof(u32);
     if (static_cast<size_t>(changed) * 9 > static_cast<size_t>(n) * 8) {
       full = true;  // the records (9 words each) would be more bytes than the eight rows
     } else if (changed > 0) {
       const size_t words = static_cast<size_t>(changed) * 9;
-      if (r->delta_host_capacity < words) {
-        if (r->delta_host) cudaFreeHost(r->delta_host);
-        r->delta_host = nullptr;
+      if (s.host_capacity < words) {
+        if (s.host) cudaFreeHost(s.host);
+        s.host = nullptr;
         const size_t cap = std::max<size_t>(2 * words, 1u << 20);
-        SM_CUDA(cudaMallocHost(&r->delta_host, sizeof(u32) * cap));
-        r->delta_host_capacity = cap;
+        SM_CUDA(cudaMallocHost(&s.host, sizeof(u32) * cap));
+        s.host_capacity = cap;
       }
-      u32* host_index = r->delta_host;
-      float* host_values = reinterpret_cast<float*>(r->delta_host + changed);
-      SM_CUDA(cudaMemcpyAsync(host_index, r->delta_index, sizeof(u32) * changed, cudaMemcpyDeviceToHost, stream));
-      SM_CUDA(cudaMemcpy2DAsync(host_values, sizeof(float) * changed, r->delta_values, sizeof(float) * r->delta_capacity,
+      u32* host_index = s.host;
+      float* host_values = reinterpret_cast<float*>(s.host + changed);
+      SM_CUDA(cudaMemcpyAsync(host_index, s.index, sizeof(u32) * changed, cudaMemcpyDeviceToHost, stream));
+      SM_CUDA(cudaMemcpy2DAsync(host_values, sizeof(float) * changed, s.values, sizeof(float) * s.capacity,
                                 sizeof(float) * changed, 8, cudaMemcpyDeviceToHost, stream));
       SM_CUDA(cudaStreamSynchronize(stream));
       st.d2h_bytes += sizeof(u32) * words;

@@ -80,6 +80,14 @@ def test_library_reads_no_environment():
     assert not readers, readers
 
 
+def test_library_defines_sm_cuda_once():
+    """Every translation unit reports a failed CUDA call the same way, through the one SM_CUDA of sm_kernels.cuh."""
+    csrc = ROOT / "surfelmeshing_b200" / "csrc"
+    definitions = [f"{p.name}:{i}" for p in sorted(csrc.iterdir()) if p.is_file()
+                   for i, line in enumerate(p.read_text().splitlines(), 1) if re.match(r"\s*#\s*define\s+SM_CUDA\b", line)]
+    assert [d.split(":")[0] for d in definitions] == ["sm_kernels.cuh"], definitions
+
+
 def test_library_selects_no_compile_time_variant():
     """The committed sources build one product: a preprocessor conditional may only tell device from host
     compilation (__CUDA_ARCH__). A variant is a patched tree or extra nvcc flags in a separate build."""

@@ -137,6 +137,45 @@ def test_whole_stream_knobs(product, vga, knob):
     assert near(got.surfels_size, want.surfels_size) and near(got.surfel_count, want.surfel_count)
 
 
+def test_every_feature_allocates_and_frees_its_scratch(product, vga):
+    """One handle creates the scratch of every feature on first use, then closes: the frame loop with host frames at a
+    pyramid level, a session, both renders, both trackers, triangulation, the persistent mesh, hole filling and the
+    delta transfer's staging. A second handle does the same after the first one's frees, with sm_mesh_update first,
+    which creates the meshing scratch without sm_triangulate."""
+    st, others = vga
+    cam = CAM.scaled(1)
+    pp, ip = params(cam)
+    n = 20
+    depth, color = st.depth[:n].cpu().pin_memory(), st.color[:n].cpu().pin_memory()
+    f = n - 1
+    live_depth, live_color = st.depth[f, ::2, ::2].contiguous(), st.color[f, ::2, ::2].contiguous()
+    view = (st.frame_T_global[f], cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy)
+    for update_first in (False, True):
+        rec = make(cam)
+        rec.configure("pyramid_level", 1)
+        stats = rec.stream_run(None, depth, color, st.global_T_frame[:n], st.frame_T_global[:n], others[:n], pp, ip,
+                               K // 2, n - K // 2)
+        assert stats.frames_integrated == n - K
+        assert run_session(rec, st, 12, pp, ip, "pinned").frames_integrated == 12 - K
+        rec.track(live_depth, st.global_T_frame[f], pp=pp)
+        rec.track_rgbd(live_depth, live_color, st.global_T_frame[f], pp=pp)
+        assert int((rec.render(*view)["index"] >= 0).sum()) > 0
+        if update_first:
+            rec.mesh_update()
+        triangles, _ = rec.triangulate()
+        if not update_first:
+            rec.mesh_update()
+        assert len(triangles) > 0
+        rec.fill_holes(triangles)
+        rec.render_mesh(triangles, *view)
+        buffers, token = R.make_cpu_buffers(rec.surfels_size()), TransferToken()
+        assert rec.TransferDeltaToCPU(None, f, buffers, token).full_transfer == 1
+        rec.Regularize(None, f, ip.regularizer_weight, ip.radius_factor_for_regularization_neighbors, 1)
+        assert rec.TransferDeltaToCPU(None, f, buffers, token).full_transfer == 0   # through the staging list
+        rec.close()
+    torch.cuda.synchronize()
+
+
 def test_hand_off_between_pushes(product, vga):
     st, others = vga
     pp, ip = params()
