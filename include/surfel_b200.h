@@ -259,7 +259,9 @@ int sm_transfer_all_to_cpu(sm_reconstruction* r, void* stream, uint32_t frame_in
  * that were never filled: the call then does a full transfer) and is updated; with the
  * reference's write/read double buffer (cuda_surfels_cpu.h:83-124) keep one token per buffer.
  * After sm_reset / sm_load_state, or when most of the cloud changed, the call falls back to the
- * full transfer. Synchronises `stream`. */
+ * full transfer. Every sm_create, sm_reset and sm_load_state takes a fresh generation from one
+ * process-wide counter, so a token filled from another handle, or from a destroyed one, also
+ * gets the full transfer. Synchronises `stream`. */
 typedef struct sm_transfer_token {
   uint64_t generation;    /* 0 = never */
   uint64_t epoch;

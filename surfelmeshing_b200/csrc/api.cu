@@ -431,6 +431,7 @@ int sm_create(sm_reconstruction** out, uint64_t max_surfel_count, int32_t width,
     return SetError(SM_ERR_INVALID_ARGUMENT, "sm_create: bad argument");
   }
   sm_reconstruction* r = new sm_reconstruction();
+  r->state_generation = NextStateGeneration();
   const int status = CreateImpl(r, max_surfel_count, width, height, fx, fy, cx, cy);
   if (status != SM_OK) {
     const std::string message = g_last_error;  // sm_destroy must not overwrite the cause
@@ -476,7 +477,7 @@ int sm_reset(sm_reconstruction* r, void* stream) {
   r->count_slot = 0;
   r->rasters_cleared = false;
   r->last_stream = static_cast<cudaStream_t>(stream);
-  ++r->state_generation;  // tokens of earlier transfers no longer apply
+  r->state_generation = NextStateGeneration();  // tokens of earlier transfers no longer apply
   r->op_history.clear();
   return SM_OK;
 }
@@ -824,7 +825,7 @@ int sm_load_state(sm_reconstruction* r, void* stream_v, const float* host_rows, 
   SM_CUDA(cudaStreamSynchronize(stream));
   r->count_slot = 0;
   r->last_stream = stream;
-  ++r->state_generation;  // tokens of earlier transfers no longer apply
+  r->state_generation = NextStateGeneration();  // tokens of earlier transfers no longer apply
   r->op_history.clear();
   return SM_OK;
 }

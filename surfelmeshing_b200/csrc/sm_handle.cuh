@@ -107,7 +107,9 @@ struct sm_reconstruction {
   int pyramid_level = 0;
   // delta transfer (transfer.cu): operation counter, per-operation regularisation thresholds
   smb::u32 op_epoch = 0;
-  uint64_t state_generation = 1;   // bumped by sm_reset / sm_load_state
+  // Which cloud the handle holds: a fresh value of one process-wide counter at sm_create, sm_reset and
+  // sm_load_state (NextStateGeneration), so a token can only match the cloud it was filled from.
+  uint64_t state_generation = 0;
   struct Operation { smb::u32 epoch; int stamp_threshold; };
   std::vector<Operation> op_history;
   // incremental session (sm_session_begin .. sm_session_end); nullptr = none open
@@ -140,6 +142,7 @@ void CountLaunches(unsigned long long n);
 unsigned long long LaunchCount();
 // transfer.cu
 void RecordOperation(sm_reconstruction* r, int stamp_threshold);   // one Integrate() / Regularize(): ++op_epoch
+uint64_t NextStateGeneration();   // 1, 2, 3, ... across every handle of the process
 void FreeTransferBuffers(sm_reconstruction* r);
 int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_index, sm_transfer_token* token, float* x,
                   float* y, float* z, float* radius_squared, float* nx, float* ny, float* nz,

@@ -21,6 +21,7 @@
 // This is a superset of the changed slots, so the arrays end up identical to a full transfer.
 
 #include <algorithm>
+#include <atomic>
 #include <cstring>
 #include <exception>
 #include <string>
@@ -214,6 +215,13 @@ int UpdateVisualizationBuffers(sm_reconstruction* r, cudaStream_t stream, const 
   r->last_stream = stream;
   { LaunchScope scope(stream, KID_VIZ_BUFFERS); LaunchKernel(k_viz_buffers, dim3(r->sm_count * 8), dim3(kBlock), 0, stream, r->d, a); }
   return CheckLaunch("visualization buffers");
+}
+
+uint64_t NextStateGeneration() {
+  // One counter for the whole process: a per-handle count would let a token filled from one handle (or from a
+  // destroyed one) pass for another handle's cloud. 0 stays "never filled".
+  static std::atomic<uint64_t> next{1};
+  return next.fetch_add(1, std::memory_order_relaxed);
 }
 
 void RecordOperation(sm_reconstruction* r, int stamp_threshold) {
