@@ -976,12 +976,64 @@ int sm_load_state(sm_reconstruction* r, void* stream, const float* host_rows,
 
 /* Scratch rasters of the last Integrate, de-interleaved into the reference's
  * per-pixel buffers (cuda_surfel_reconstruction.h:133-144), tightly packed
- * W*H host arrays; any pointer may be NULL. */
+ * W*H host arrays; any pointer may be NULL. After sm_compact the rasters name
+ * old slots: the call returns SM_ERR_INVALID_ARGUMENT until the next Integrate. */
 int sm_download_rasters(sm_reconstruction* r, void* stream,
                         uint32_t* supporting_surfels, uint32_t* supporting_surfel_counts,
                         float* supporting_surfel_depth_sums, uint32_t* conflicting_surfels,
                         float* first_surfel_depth, uint8_t* new_surfel_flag_vector,
                         uint32_t* new_surfel_indices);
+
+/* ---- reclaiming the slots of merged surfels (DESIGN.md section 1 row f15, section 5.13) ----------------------
+ * A merge never frees its slot (like the reference, kernels.cu:1987: radius^2 = -1), so surfels_size() only grows
+ * and a long session reaches the surfel cap with far fewer live surfels. sm_compact removes the merged slots in
+ * place. It is never called by the library itself.
+ *  1. Which slots go: slot i in [0, surfels_size()) is removed iff its radius^2 (row 7) < 0, the merge mark of
+ *     Integrate(); every other slot is kept.
+ *  2. Stable order: a kept slot moves from i to the number of kept slots below i. old_to_new[i] is that index, or
+ *     SM_INVALID_SURFEL_INDEX for a removed slot.
+ *  3. State after the call: every row sm_dump_state defines is the gather of the old rows through the map (rows
+ *     11-16 and 23 are scratch), except that a neighbour link (rows 19-22) is replaced by the new index of the slot
+ *     it names; a link that names a removed slot (or one >= surfels_size()) becomes SM_INVALID_SURFEL_INDEX and is
+ *     counted in links_dropped. surfels_size() = surfel_count() = slots_after, the merge count is 0, both
+ *     regularisation record buffers hold the gathered current records (as after sm_load_state), and the sticky
+ *     cap-overflow flag stays as it is (the call itself does not report it).
+ *  4. Nothing to remove: when the merge count (sm_dump_state's merge_count) is 0, or no slot carries the mark,
+ *     the call launches no kernel and changes nothing; old_to_new, if given, is the identity. The delta-transfer
+ *     token stays valid.
+ *  5. Otherwise the handle takes a fresh state generation: the next sm_transfer_delta_to_cpu with an older token
+ *     does a full transfer.
+ *  6. Memory: allocated by the first call that removes something, freed by sm_destroy: the map and one row of
+ *     scratch (8 bytes per slot of the cap), and CUB's scan storage. The SoA and the records are compacted in
+ *     place.
+ *  7. SM_ERR_INVALID_ARGUMENT, with no launch, for a NULL handle, or old_to_new non-NULL with map_capacity <
+ *     surfels_size(). stats and old_to_new (DEVICE, surfels_size() entries) may be NULL.
+ * What else names a slot:
+ *  - The persistent mesh of sm_mesh_update is carried over when no slot it uses was removed, that is, when no
+ *    surfel merged since the last update (compact right after sm_mesh_update): its snapshot, umbrellas, per-slot
+ *    stats and the triangle lists are remapped (mesh_remapped = 1). sm_mesh_read(SM_MESH_ALL) then returns the
+ *    remapped mesh and an update with no change in between reports slots_changed == 0 and empty deltas; a corner of
+ *    the last update's removed list whose slot was removed reads SM_INVALID_SURFEL_INDEX. Otherwise the mesh is
+ *    dropped (mesh_remapped = 0): sm_mesh_read fails and the next update rebuilds everything.
+ *  - sm_download_rasters refuses until the next Integrate.
+ *  - An open session: the call is allowed between pushes, on the session's stream. In frame-graph mode the front
+ *    half of the frame in flight (projection, association, merge decisions, blending) runs again on the new slots,
+ *    and the merge count the session reports becomes 0.
+ *  - Outside the handle the caller must rebuild or remap (with old_to_new): sm_knn_index objects built from the
+ *    reconstruction, triangle lists from sm_triangulate or sm_mesh_fill_holes, visualisation buffers and their
+ *    latest_mesh_surfel_count, and CPU copies keyed by slot. The keyframe database holds poses and codes only.
+ * The call synchronises `stream` (the counters; the map; the end), plus once more when a mesh is carried over. */
+typedef struct sm_compact_stats {
+  uint64_t slots_before;      /* surfels_size() before */
+  uint64_t slots_after;       /* surfels_size() after == surfel_count() */
+  uint64_t merged_removed;
+  uint64_t links_dropped;     /* neighbour links (rows 19-22) of kept slots that named a removed slot */
+  int32_t  mesh_remapped;     /* 1 if a persistent sm_mesh_update mesh existed and was carried over */
+  int32_t  reserved;
+} sm_compact_stats;
+int sm_compact(sm_reconstruction* r, void* stream,
+               uint32_t* old_to_new /* device, slots_before entries; may be NULL */, uint64_t map_capacity,
+               sm_compact_stats* stats /* may be NULL */);
 
 /* ---- RGB-D stream runner (the frame loop of APP/main.cc:885-1223) ---------
  * Runs preprocess + Integrate over frames [first_frame, last_frame) of a
@@ -1065,8 +1117,8 @@ int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32
  * sm_update_visualization_buffers, sm_export_vertices, sm_dump_state, sm_download_rasters,
  * sm_frame_counters, sm_knn_build_from_reconstruction, sm_render_surfels, sm_render_mesh, sm_track_frame,
  * sm_track_linearize, sm_track_frame_rgbd, sm_track_linearize_rgbd, sm_relocalise,
- * sm_mesh_update, sm_mesh_read, sm_triangulate, sm_surfel_count / sm_surfels_size) and
- * sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
+ * sm_mesh_update, sm_mesh_read, sm_triangulate, sm_surfel_count / sm_surfels_size),
+ * sm_compact, and sm_regularize, which main.cc calls between frames (:1573-1579). In frame-graph mode the step a push
  * launches has also decided the merges of the next frame (k_merge runs in the step's front half), which
  * that frame's Integrate() applies in the next step. The device merge counter then already includes them, so
  * the push snapshots it first, and while the session is open the count queries report the snapshot:

@@ -166,6 +166,15 @@ class CUDASurfelReconstruction {
   inline u32 surfel_count() const { u32 v = 0; Check(sm_surfel_count(handle_, &v)); return v; }
   inline u32 surfels_size() const { u32 v = 0; Check(sm_surfels_size(handle_, &v)); return v; }
 
+  // Extension (no counterpart in the reference): reclaims the slots of merged surfels (sm_compact). old_to_new
+  // (device, surfels_size() entries, may be null) receives the new slot of every old one; a CPU meshing consumer
+  // keyed by slot (SurfelMeshing::IntegrateCUDABuffers) must apply it or restart from a full transfer.
+  sm_compact_stats Compact(cudaStream_t stream, u32* old_to_new = nullptr, uint64_t map_capacity = 0) {
+    sm_compact_stats stats;
+    Check(sm_compact(handle_, stream, old_to_new, map_capacity, &stats));
+    return stats;
+  }
+
  private:
   static void ToRowMajor(const SE3f& t, float* out) {
     const auto m = t.matrix3x4();

@@ -237,6 +237,14 @@ class HoleStats(C.Structure):
                 ("loops_rejected", C.c_uint64), ("loops_conflicting", C.c_uint64), ("triangles_added", C.c_uint64),
                 ("boundary_edges_after", C.c_uint64)]
 
+
+class CompactStats(C.Structure):
+    """sm_compact_stats: surfels_size() before and after, the merged slots removed, the neighbour links of kept slots
+    that named a removed slot, and whether the persistent sm_mesh_update mesh was carried over."""
+    _fields_ = [("slots_before", C.c_uint64), ("slots_after", C.c_uint64), ("merged_removed", C.c_uint64),
+                ("links_dropped", C.c_uint64), ("mesh_remapped", C.c_int32), ("reserved", C.c_int32)]
+
+
 _P = C.c_void_p
 _SZ = C.c_size_t
 _F = C.c_float
@@ -334,6 +342,7 @@ _PRODUCT_ONLY = {
     "keyframe_db_read": (C.c_int, [_P, _U32, _P, _P]),
     "relocalise": (C.c_int, [_P, _P, _P, C.POINTER(RelocParams), C.POINTER(PreprocessParams),
                              C.POINTER(TrackRGBDParams), _P, _SZ, _P, _SZ, _P, C.POINTER(RelocResult)]),
+    "compact": (C.c_int, [_P, _P, _P, C.c_uint64, C.POINTER(CompactStats)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

@@ -133,7 +133,8 @@ const char* KernelName(int id) {
       "k_mesh_render_splat", "k_mesh_render_splat_large", "k_mesh_render_resolve",
       "k_track_intensity_base", "k_track_intensity_down", "k_track_linearize_rgbd", "k_track_solve_rgbd",
       "k_reloc_encode", "k_reloc_distance", "k_reloc_select", "k_hole_edges", "k_hole_boundary", "k_hole_sort",
-      "k_hole_walk", "k_hole_conflict", "k_hole_scan", "k_hole_write"};
+      "k_hole_walk", "k_hole_conflict", "k_hole_scan", "k_hole_write", "k_compact_map", "k_compact_scatter",
+      "k_compact_store", "k_compact_mesh"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -244,6 +245,7 @@ int IntegrateImpl(sm_reconstruction* r, cudaStream_t stream, u32 frame_index, co
   int status = IntegrateFrame(stream, r->d, f, p.do_blending != 0, r->rasters_cleared, r->plan, &r->events);
   r->rasters_cleared = false;
   if (status != SM_OK) return status;
+  r->rasters_stale = false;
   NoteIntegratedFrame(r->d, frame_index);
   const int old_slot = r->count_slot;
   r->count_slot = (r->count_slot + 1) % kCountSlots;  // k_new_surfel_scan wrote the next slot
@@ -466,6 +468,7 @@ int sm_destroy(sm_reconstruction* r) {
   FreeTrackBuffers(r);
   FreeMeshBuffers(r);
   FreeHoleBuffers(r);
+  FreeCompactBuffers(r);
   delete r;
   cudaGetLastError();
   return SM_OK;
@@ -835,6 +838,9 @@ int sm_download_rasters(sm_reconstruction* r, void* stream_v, uint32_t* supporti
                         uint32_t* conflicting_surfels, float* first_surfel_depth, uint8_t* new_surfel_flag_vector,
                         uint32_t* new_surfel_indices) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (r->rasters_stale) {
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_download_rasters: sm_compact ran after the last Integrate (its rasters name old slots)");
+  }
   const size_t P = static_cast<size_t>(r->d.width) * r->d.height;
   std::vector<PixelAssoc> assoc(P);
   SM_CUDA(cudaMemcpyAsync(assoc.data(), r->d.assoc, sizeof(PixelAssoc) * P, cudaMemcpyDeviceToHost, stream));

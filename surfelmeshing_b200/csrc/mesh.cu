@@ -1143,6 +1143,72 @@ int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& 
   return SM_OK;
 }
 
+namespace {
+
+// words[0] = 1 if a slot removed by sm_compact was present at the last update, words[1] = removed slots below n_prev.
+__global__ void k_mesh_compact_check(const u32* map, const u32* snapshot, u32 n_prev, u32* words) {
+  for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n_prev; i += gridDim.x * blockDim.x) {
+    if (map[i] != kNone) continue;
+    atomicAdd(words + 1, 1u);
+    if (__uint_as_float(snapshot[static_cast<size_t>(i) * kSnapshotWords + 3]) > 0.f) words[0] = 1u;
+  }
+}
+
+// Every corner of `count` triangles through the map (a removed slot, or one >= n, becomes kNone).
+__global__ void k_mesh_compact_remap(u32* corners, u64 count, const u32* map, u32 n) {
+  for (u64 i = blockIdx.x * static_cast<u64>(blockDim.x) + threadIdx.x; i < 3 * count;
+       i += static_cast<u64>(gridDim.x) * blockDim.x) {
+    const u32 v = corners[i];
+    corners[i] = v < n ? map[v] : kNone;
+  }
+}
+
+}  // namespace
+
+int MeshCompact(sm_reconstruction* r, cudaStream_t stream, const u32* map, u32 n, u32* scratch, u32* words,
+                u32* host_words, int* remapped) {
+  *remapped = 0;
+  MeshLive* L = r->mesh ? r->mesh->live : nullptr;
+  if (!L || !L->valid) return SM_OK;
+  const u32 n_prev = L->n_prev;
+  const int blocks = 4 * r->sm_count;
+  if (n_prev > n) { L->valid = false; return SM_OK; }   // (an sm_reset / sm_load_state since: a full rebuild anyway)
+  if (n_prev > 0) {
+    SM_CUDA(cudaMemsetAsync(words, 0, 2 * sizeof(u32), stream));
+    { LaunchScope scope(stream, KID_COMPACT_MESH); LaunchKernel(k_mesh_compact_check, dim3(blocks), dim3(256), 0, stream, map, static_cast<const u32*>(L->snapshot), n_prev, words); }
+    SM_CUDA(cudaMemcpyAsync(host_words, words, 2 * sizeof(u32), cudaMemcpyDeviceToHost, stream));
+    SM_CUDA(cudaStreamSynchronize(stream));
+    // A slot merged after the update is still a corner of the mesh, which names it: the next update rebuilds all.
+    if (host_words[0]) { L->valid = false; return SM_OK; }
+  } else {
+    host_words[1] = 0;
+  }
+  const u32 kept = n_prev - host_words[1];
+  const int sms = r->sm_count;
+  int status = CompactWords(stream, sms, map, n_prev, kept, L->snapshot, kSnapshotWords, scratch, false);
+  if (status == SM_OK) status = CompactWords(stream, sms, map, n_prev, kept, reinterpret_cast<u32*>(L->umbrella), 2 * kUmbrella, scratch, true);
+  if (status == SM_OK) status = CompactWords(stream, sms, map, n_prev, kept, L->umbrella_count, 1, scratch, false);
+  if (status == SM_OK) status = CompactWords(stream, sms, map, n_prev, kept, L->word, 1, scratch, false);
+  if (status == SM_OK) status = CompactBytes(stream, sms, map, n_prev, kept, L->overflow, scratch);
+  // offsets: the removed slots own no triangle, so the kept ones keep theirs, and the end moves down to `kept`
+  u32* offsets = L->offsets[L->current];
+  if (status == SM_OK) status = CompactWords(stream, sms, map, n_prev, kept, offsets, 1, scratch, false);
+  if (status != SM_OK) return status;
+  if (kept < n_prev) SM_CUDA(cudaMemcpyAsync(offsets + kept, offsets + n_prev, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  const struct { uint3* list; u64 count; } lists[3] = {
+      {L->triangles[L->current], L->triangle_count}, {L->added, L->added_count}, {L->removed, L->removed_count}};
+  for (const auto& t : lists) {
+    if (t.count == 0) continue;
+    LaunchScope scope(stream, KID_COMPACT_MESH);
+    LaunchKernel(k_mesh_compact_remap, dim3(blocks), dim3(256), 0, stream, reinterpret_cast<u32*>(t.list), t.count, map, n);
+  }
+  status = CheckLaunch("compact: mesh");
+  if (status != SM_OK) return status;
+  L->n_prev = kept;
+  *remapped = 1;
+  return SM_OK;
+}
+
 int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t* triangles, uint64_t capacity,
              uint64_t* count) {
   auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_mesh_read: ") + why).c_str()); };

@@ -475,6 +475,7 @@ int GraphStep(RunContext& c, FrameLoop& g, int it, uint32_t* integrated) {
       // sm_frame_counters, sm_surfel_count, the hand-off calls between the pushes of a session)
       UseSet(r->d, r->sets[set]);
       r->count_slot = new_slot;
+      r->rasters_stale = false;
     }
   }
   {  // front: frame `front`
@@ -923,6 +924,30 @@ int SessionEnd(sm_reconstruction* r, sm_stream_stats* stats) {
   FreeSession(ss);
   r->session = nullptr;
   return status;
+}
+
+int SessionRefront(sm_reconstruction* r, cudaStream_t stream) {
+  StreamSession* ss = r->session;
+  if (!ss || !ss->loop.graph || ss->next_step <= ss->loop.it0) return SM_OK;   // serial mode: nothing in flight
+  SM_CUDA(cudaMemsetAsync(ss->merge_count, 0, sizeof(u32), stream));   // merges up to the newest integrated frame
+  RunContext& c = ss->c;
+  const int frame = ss->next_step;   // the last push ran this frame's front half (GraphStep: front = it + 1)
+  if (!c.Active(frame)) return SM_OK;
+  const int set = frame % kSets;
+  DeviceState d = r->d;
+  UseSet(d, r->sets[set]);
+  int status = ClearAssociationRasters(stream, d);
+  if (status != SM_OK) return status;
+  // k_blend reads the pre-blend copy and rewrites the frame's depth from it, so it can run again
+  const FrameParams f = c.Params(frame, set);
+  const FrameKernel kernels[4] = {FK_PROJECT, FK_ASSOCIATE, FK_MERGE, FK_BLEND};
+  for (int i = 0; i < (ss->loop.blending ? 4 : 3); ++i) {
+    KernelLaunch k;
+    status = DescribeFrameKernel(kernels[i], r->plan, d, f, &k);
+    if (status != SM_OK) return status;
+    LaunchOnStream(stream, k, false);
+  }
+  return CheckLaunch("sm_compact: front half of the frame in flight");
 }
 
 void FreeRunBuffers(sm_reconstruction* r) {

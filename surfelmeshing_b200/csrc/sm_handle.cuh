@@ -70,6 +70,7 @@ struct RenderScratch;    // render.cu: sm_render_surfels / sm_render_mesh
 struct TrackScratch;     // track.cu: sm_track_frame* / sm_track_linearize*
 struct MeshScratch;      // mesh.cu: sm_triangulate, and the persistent mesh of sm_mesh_update
 struct HoleScratch;      // holes.cu: the buffers of sm_mesh_fill_holes
+struct CompactScratch;   // compact.cu: the map and the row scratch of sm_compact
 
 }  // namespace smb
 
@@ -81,6 +82,7 @@ struct sm_reconstruction {
   float fx = 0, fy = 0, cx = 0, cy = 0;
   int count_slot = 0;             // Counters::surfel_count slot holding the current count
   bool rasters_cleared = false;   // the fused pre-processing tail already reset the rasters
+  bool rasters_stale = false;     // sm_compact ran after the last Integrate: its rasters name old slots
   smb::IntegrateEvents events{};
   smb::TieBreakConfig tiebreak{};
   smb::TieBreak last_tiebreak{};  // of the most recent frame (decodes the supporting raster, sm_download_rasters)
@@ -124,6 +126,7 @@ struct sm_reconstruction {
   smb::TrackScratch* track = nullptr;
   smb::MeshScratch* mesh = nullptr;
   smb::HoleScratch* holes = nullptr;
+  smb::CompactScratch* compact = nullptr;
 };
 
 namespace smb {
@@ -192,6 +195,21 @@ int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t*
 int FillHoles(sm_reconstruction* r, cudaStream_t stream, const sm_hole_params& p, const uint32_t* triangles,
               uint64_t count, uint32_t* fill, uint64_t capacity, sm_hole_stats* stats);
 void FreeHoleBuffers(sm_reconstruction* r);
+// compact.cu
+int Compact(sm_reconstruction* r, cudaStream_t stream, uint32_t* old_to_new, uint64_t map_capacity,
+            sm_compact_stats* stats);
+void FreeCompactBuffers(sm_reconstruction* r);
+// In place: word w of record k' = word w of record i, old_to_new[i] = k' < kept, for every word of records of
+// `record_words` 32-bit words (bytes) over slots [0, n), one word at a time through `scratch` (>= kept words).
+// `remap`: the words name slots and are replaced by their new index (SM_INVALID_SURFEL_INDEX for a removed one).
+int CompactWords(cudaStream_t stream, int sm_count, const u32* old_to_new, u32 n, u32 kept, u32* base,
+                 u32 record_words, u32* scratch, bool remap);
+int CompactBytes(cudaStream_t stream, int sm_count, const u32* old_to_new, u32 n, u32 kept, u8* base, u32* scratch);
+// mesh.cu: carries the persistent mesh of sm_mesh_update over a compaction of slots [0, n) (`words`: 2 device
+// words, `host_words` their pinned mirror); *remapped = 1 if it was carried over, 0 if there was none or it was
+// dropped (the next update then rebuilds everything).
+int MeshCompact(sm_reconstruction* r, cudaStream_t stream, const u32* old_to_new, u32 n, u32* scratch, u32* words,
+                u32* host_words, int* remapped);
 // pipeline.cu
 int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
               const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats);
@@ -201,6 +219,9 @@ int SessionPush(sm_reconstruction* r, const u16* depth, size_t depth_pitch, cons
                 bool on_host, const float* global_T_frame, const float* frame_T_global, sm_session_status* status);
 int SessionEnd(sm_reconstruction* r, sm_stream_stats* stats);
 void FreeRunBuffers(sm_reconstruction* r);
+// After sm_compact in an open frame-graph session: runs the front half of the frame in flight again on `stream`
+// (its association, merge decisions and blending named the old slots) and resets the reported merge count.
+int SessionRefront(sm_reconstruction* r, cudaStream_t stream);
 // out (3x4) = scale(other_T_global) . scale(global_T_ref) (sm_outlier_filter_transforms)
 void OutlierFilterTransform(float depth_scaling, const float* global_T_ref, const float* other_T_global, float* out);
 }  // namespace smb

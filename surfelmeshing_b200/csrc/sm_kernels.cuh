@@ -47,6 +47,7 @@ enum KernelId {
   KID_TRACK_INTENSITY_BASE, KID_TRACK_INTENSITY_DOWN, KID_TRACK_LINEARIZE_RGBD, KID_TRACK_SOLVE_RGBD,
   KID_RELOC_ENCODE, KID_RELOC_DISTANCE, KID_RELOC_SELECT,
   KID_HOLE_EDGES, KID_HOLE_BOUNDARY, KID_HOLE_SORT, KID_HOLE_WALK, KID_HOLE_CONFLICT, KID_HOLE_SCAN, KID_HOLE_WRITE,
+  KID_COMPACT_MAP, KID_COMPACT_SCATTER, KID_COMPACT_STORE, KID_COMPACT_MESH,
   KID_COUNT
 };
 const char* KernelName(int id);

@@ -20,7 +20,7 @@ import torch
 
 from . import _lib
 from . import mesh_io
-from ._lib import (HoleParams, HoleStats, IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats,
+from ._lib import (CompactStats, HoleParams, HoleStats, IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats,
                    PreprocessParams, RelocParams, RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult,
                    TrackRGBDParams, TrackRGBDResult,
                    TransferStats, TransferToken, VisualizationParams)
@@ -761,8 +761,24 @@ class CUDASurfelReconstruction:
                       int(first_frame), int(last_frame), C.byref(stats))
         return stats
 
+    def compact(self, stream=None, return_map: bool = False):
+        """sm_compact: removes the slots of merged surfels in place, keeping the order of the others. Returns
+        CompactStats, or (CompactStats, old_to_new) with `return_map`: an int64 CUDA tensor of surfels_size()
+        entries before the call, the new slot of each old one or -1 for a removed slot (remap_triangles applies it).
+        Between the pushes of a session, call it through the session (StreamSession.compact), on its stream."""
+        stats = CompactStats()
+        if not return_map:
+            self.lib.call("compact", self._h, _stream_handle(stream), None, 0, C.byref(stats))
+            return stats
+        n = self.surfels_size()
+        out = torch.empty(max(n, 1), dtype=torch.int32, device="cuda")
+        self.lib.call("compact", self._h, _stream_handle(stream), C.c_void_p(out.data_ptr()), n, C.byref(stats))
+        old_to_new = out[:n].to(torch.int64) & 0xFFFFFFFF
+        old_to_new[old_to_new == _lib.INVALID_SURFEL_INDEX] = -1
+        return stats, old_to_new
+
     def session(self, pp: PreprocessParams, ip: IntegrateParams, frame_size, first_frame_index: int = 0,
-                stream=None) -> "StreamSession":
+                stream=None, compact_when_free_below: Optional[float] = None) -> "StreamSession":
         """An incremental session (sm_session_begin): the frame loop of APP/main.cc:885-1293 with frames pushed
         one at a time. `frame_size` = (width, height) of the sensor frames. Use as a context manager::
 
@@ -770,8 +786,10 @@ class CUDASurfelReconstruction:
                 for depth, color, g, l in frames:
                     s.push(depth, color, g, l)
             s.stats   # StreamStats of sm_session_end
+
+        `compact_when_free_below` (a fraction of the surfel cap, default None = never): see StreamSession.
         """
-        return StreamSession(self, pp, ip, frame_size, first_frame_index, stream)
+        return StreamSession(self, pp, ip, frame_size, first_frame_index, stream, compact_when_free_below)
 
 
 class KeyframeDatabase:
@@ -880,15 +898,33 @@ def _frame_arg(a, channels: int):
     return C.c_void_p(a.ctypes.data), a.strides[0], 1, a
 
 
+def remap_triangles(triangles: torch.Tensor, old_to_new: torch.Tensor) -> torch.Tensor:
+    """A triangle list [T, 3] over the slots before sm_compact, over the slots after it (CUDASurfelReconstruction.
+    compact(return_map=True)). A triangle with a removed corner is dropped; the others keep their order and
+    corners. Lists from sm_triangulate or sm_mesh_fill_holes name present slots only, which sm_compact keeps."""
+    tri = triangles.reshape(-1, 3).to(device=old_to_new.device, dtype=torch.int64)
+    mapped = old_to_new[tri]
+    return mapped[(mapped >= 0).all(dim=1)].to(triangles.dtype)
+
+
 class StreamSession:
-    """An open sm_session_begin on a CUDASurfelReconstruction (see CUDASurfelReconstruction.session)."""
+    """An open sm_session_begin on a CUDASurfelReconstruction (see CUDASurfelReconstruction.session).
+
+    With `compact_when_free_below` = f (0 < f < 1), every push is followed by sm_compact when fewer than f x the
+    surfel cap slots are free (surfels_size() > (1 - f) x cap): a long session is then bounded by the surfels it
+    holds rather than by every surfel it created. The check costs a synchronisation per push. `compactions` holds
+    the CompactStats of every compaction of the session, by policy or by compact()."""
 
     def __init__(self, rec: CUDASurfelReconstruction, pp: PreprocessParams, ip: IntegrateParams, frame_size,
-                 first_frame_index: int = 0, stream=None):
+                 first_frame_index: int = 0, stream=None, compact_when_free_below: Optional[float] = None):
+        if compact_when_free_below is not None and not 0.0 < compact_when_free_below < 1.0:
+            raise ValueError("compact_when_free_below must be a fraction of the surfel cap in (0, 1)")
         self.rec, self.pp, self.ip = rec, pp, ip
         self.width, self.height = (int(v) for v in frame_size)
         self.stream = _stream_handle(stream)
         self.stats: Optional[StreamStats] = None
+        self.compact_when_free_below = compact_when_free_below
+        self.compactions: list = []
         rec.lib.call("session_begin", rec._h, self.stream, C.byref(pp), C.byref(ip), self.width, self.height,
                      int(first_frame_index))
         self.open = True
@@ -909,7 +945,16 @@ class StreamSession:
         status = SessionStatus()
         self.rec.lib.call("session_push", self.rec._h, dp, dpitch, cp, cpitch, d_host, g.ctypes.data_as(C.c_void_p),
                           l.ctypes.data_as(C.c_void_p), C.byref(status))
+        f = self.compact_when_free_below
+        if f is not None and self.rec.surfels_size() > (1.0 - f) * self.rec.max_surfel_count:
+            self.compact()
         return status
+
+    def compact(self, return_map: bool = False):
+        """sm_compact between two pushes, on the session's stream (CUDASurfelReconstruction.compact)."""
+        result = self.rec.compact(self.stream, return_map)
+        self.compactions.append(result[0] if return_map else result)
+        return result
 
     def end(self) -> StreamStats:
         """sm_session_end: integrates what is left and returns the session's StreamStats."""
@@ -958,18 +1003,22 @@ class TrackedSession:
     restarts from that pose; if not, the frame is held out of the session (not pushed, push() returns None) and the
     next frame tries again. `trajectory` stays indexed by frame, with NaN poses for held-out frames. `states` holds
     "tracked", "relocalised" or "lost" per frame (without `reloc` a "lost" frame is pushed with its guess, as
-    above) and `reloc_results` the RelocResult of each relocalisation (None where none was tried)."""
+    above) and `reloc_results` the RelocResult of each relocalisation (None where none was tried).
+
+    `compact_when_free_below` and compact() are StreamSession's: the merged slots are reclaimed between pushes."""
 
     def __init__(self, rec: CUDASurfelReconstruction, pp: PreprocessParams, ip: IntegrateParams, first_pose,
                  params: Optional[TrackParams] = None, first_frame_index: int = 0, stream=None,
-                 rgbd: Optional[TrackRGBDParams] = None, reloc: Optional[RelocParams] = None):
+                 rgbd: Optional[TrackRGBDParams] = None, reloc: Optional[RelocParams] = None,
+                 compact_when_free_below: Optional[float] = None):
         self.rec, self.pp = rec, pp
         self.params = TrackParams.defaults() if params is None else params
         self.rgbd = rgbd
         self.reloc = reloc
         self.first_pose = np.asarray(first_pose, np.float32).reshape(3, 4)
         self.database = KeyframeDatabase(rec, reloc) if reloc is not None else None
-        self.session = StreamSession(rec, pp, ip, (rec.width, rec.height), first_frame_index, stream)
+        self.session = StreamSession(rec, pp, ip, (rec.width, rec.height), first_frame_index, stream,
+                                     compact_when_free_below)
         self.trajectory: list = []
         self.results: list = []
         self.states: list = []
@@ -1023,6 +1072,10 @@ class TrackedSession:
         status = self.session.push(depth, color, pose, invert_rigid(pose))
         self.integrated = status.last_integrated_frame >= 0
         return status
+
+    def compact(self, return_map: bool = False):
+        """sm_compact between two pushes (StreamSession.compact)."""
+        return self.session.compact(return_map)
 
     def end(self) -> StreamStats:
         return self.session.end()
