@@ -916,6 +916,115 @@ int sm_mesh_fill_holes(sm_reconstruction* r, void* stream, const sm_hole_params*
                        uint32_t* fill /* device, 3 x capacity; may be NULL with capacity 0 */, uint64_t capacity,
                        sm_hole_stats* stats);
 
+/* ---- simplifying a triangle mesh (DESIGN.md section 1 row f16, section 5.14) ----------------------------------
+ * The mesh of sm_triangulate has one vertex per meshed surfel, so flat walls and table tops are described by
+ * thousands of triangles. sm_mesh_simplify removes vertices by half-edge collapses ranked by Garland-Heckbert plane
+ * quadrics: a slot u is removed and its triangles are given to a neighbour v; no vertex moves, so every corner of the
+ * output is still a slot of the handle (sm_render_mesh, sm_mesh_fill_holes, sm_compact's remap and the OBJ export
+ * take it as they take the full mesh). It takes an edge-manifold, consistently oriented triangle list over the
+ * handle's slots (as sm_mesh_fill_holes does) and returns a list over a subset of its slots. The collapses run in
+ * rounds of collapses with disjoint closed neighbourhoods, so the result does not depend on thread order.
+ * Positions are read from the rows 3-5 mirror of the smooth positions, which the call refreshes as sm_triangulate
+ * does; nothing else of the surfel state, and not the persistent mesh of sm_mesh_update, is written.
+ *
+ * p_i, n_i (rows 8-10 normalised, "unit normal"), the fp32 conventions and rule 4 are those of sm_triangulate; cos_n
+ * and cos_t come from the two angles of sm_simplify_params the same way. P_i = p_i converted to double. Quadric
+ * arithmetic is IEEE double with every product, sum, quotient and square root rounded on its own, in the order
+ * written: (a + b) + c means a + b first. Input triangle t = (a, b, c) keeps its input position t throughout.
+ *  S1. Quadrics. e1 = P_b - P_a, e2 = P_c - P_a, g = (e1.y*e2.z - e1.z*e2.y, e1.z*e2.x - e1.x*e2.z,
+ *      e1.x*e2.y - e1.y*e2.x), gg = (g.x*g.x + g.y*g.y) + g.z*g.z. If gg > 0: s = sqrt(gg), m = (g.x/s, g.y/s,
+ *      g.z/s), d = -((m.x*P_a.x + m.y*P_a.y) + m.z*P_a.z), and K_t has the ten entries (k0..k9) = (m.x*m.x,
+ *      m.x*m.y, m.x*m.z, m.x*d, m.y*m.y, m.y*m.z, m.y*d, m.z*m.z, m.z*d, d*d); otherwise K_t = 0. Q_i = ((0 + K_t1)
+ *      + K_t2) + ..., entry by entry, over the input triangles t1 < t2 < ... that have corner i. The cost of
+ *      quadric q at x = (x, y, z): r0 = ((q0*x + q1*y) + q2*z) + q3, r1 = ((q1*x + q4*y) + q5*z) + q6,
+ *      r2 = ((q2*x + q5*y) + q7*z) + q8, r3 = ((q3*x + q6*y) + q8*z) + q9, E = ((r0*x + r1*y) + r2*z) + r3: the sum
+ *      of squared distances (m^2) to the planes of the triangles q gathers.
+ *  S2. Round state: the current list (each triangle with its input position). N(i) = the distinct slots that share
+ *      a current triangle with i, deg(i) = |N(i)|. An edge of i is present in only one direction: i is a boundary
+ *      vertex. No boundary vertex is ever removed, and no boundary edge changes.
+ *  S3. Candidates. u is a candidate iff it is not a boundary vertex, its current triangles form one closed fan
+ *      (following (u, a, b) -> the triangle (u, b, c) visits all of them before it comes back), and 3 <= deg(u) <=
+ *      SM_MESH_MAX_VALENCE. Its ring r_0..r_{d-1} (d = deg(u)) is the fan order from the triangle of smallest input
+ *      position, (u, r_j, r_{j+1 mod d}) being its triangles. A collapse u -> v = r_k, with o1 = r_{k-1 mod d} and
+ *      o2 = r_{k+1 mod d} (the opposite corners of the two triangles on {u, v}), is valid iff:
+ *      (a) link condition: N(u) and N(v) share exactly o1 and o2;
+ *      (b) deg(u) + deg(v) - 4 <= SM_MESH_MAX_VALENCE;
+ *      (c) every triangle (u, r_j, r_{j+1}) without v, with u replaced by v and the winding kept, passes H4's
+ *          geometric tests (unit normals at its three corners, n_a.n_b >= cos_n for each pair, g.n_c > 0 at each
+ *          corner for rule 4's g in the rotation that starts at its smallest slot, and rule 4's angle test with
+ *          cos_t at each corner), and does not have the three slots of a current triangle (which stops a
+ *          tetrahedron from collapsing further);
+ *      (d) E = the cost of (Q_u + Q_v) (entry by entry) at P_v is finite and cost = (E > 0 ? E : +0) <= max_cost.
+ *      best(u) = the valid v with the smallest (cost, v); key(u) = bits(f) << 32 | u, where f = float(cost)
+ *      (round to nearest), taken as +0 when it is below the smallest normal float.
+ *  S4. Independent selection. Every candidate with a best(u) takes the minimum of its key into mark[y] for each y of
+ *      N[u] = {u} + N(u); u is selected iff mark[y] == key(u) for every y of N[u]. Two selected slots have
+ *      disjoint closed neighbourhoods, so no selected collapse changes the validity, the cost or the result of
+ *      another, and a round equals its collapses applied one after the other in any order.
+ *  S5. Budget. With target_triangles > 0 and T - 2 s < target_triangles (T current triangles, s selected), only
+ *      the ceil((T - target_triangles) / 2) selected slots of smallest key are collapsed, and the call stops. Every
+ *      collapse removes exactly two triangles ({u, v} is an interior edge).
+ *  S6. Apply u -> v: the two triangles on {u, v} are deleted, u is replaced by v in every other triangle of u, and
+ *      Q_v = Q_v + Q_u entry by entry.
+ *  S7. Rounds. Before each round: stop (SM_SIMPLIFY_STOP_TARGET) if target_triangles > 0 and T <= target_triangles;
+ *      else stop (SM_SIMPLIFY_STOP_MAX_ROUNDS) if max_rounds rounds have been applied; else select (S3, S4), and
+ *      stop (SM_SIMPLIFY_STOP_CONVERGED) if nothing is selected, else apply (S5, S6): one more round.
+ *  S8. Output. Every current triangle rotated to start at its smallest slot, the winding kept; ordered by that slot,
+ *      then by input position. The output is edge-manifold and consistently oriented, V - E + F, the boundary edges
+ *      and the boundary loops are those of the input, and a triangle that changed is counter-clockwise about the
+ *      normals of its three corners.
+ * stats: triangles_in = count; triangles_out (set also when the capacity is too small); vertices_in / vertices_out
+ * = the slots that are corners of the input / output; collapses; rounds (rounds applied); boundary_edges = directed
+ * edges of the input whose reverse is not one (those of the output too); max_cost_applied = the largest cost of an
+ * applied collapse (0 without one); stop_reason. All zero when the call fails for any other reason.
+ *
+ * out is a DEVICE buffer of 3 x capacity uint32 (may be NULL with capacity 0: a count query); triangles_out <=
+ * count, so capacity = count always suffices; if capacity < triangles_out the call returns SM_ERR_CAPACITY with the
+ * stats set and writes nothing. SM_ERR_INVALID_ARGUMENT, with no launch, for NULL params or stats, triangles NULL
+ * with count > 0, out NULL with capacity > 0, out overlapping triangles (both as 3 x uint32 arrays of count and
+ * capacity triangles), count >= 2^28, max_cost negative or NaN, an angle outside (0, 180] or max_rounds outside
+ * [0, SM_SIMPLIFY_MAX_ROUNDS]; and, found on the device and reported after the call's second synchronisation with
+ * nothing written, for the inputs sm_mesh_fill_holes refuses (a corner that is not a present slot below
+ * surfels_size(), a repeated corner, a directed edge that occurs twice). The call synchronises `stream` on
+ * surfels_size(), after the input checks, once per round (selected and triangle counts), and at the end, plus once,
+ * with cudaFree's device synchronisation, in a call whose buffers grow (by x 1.5); on return the output is written
+ * by work enqueued on `stream`. Memory (allocated by the first call, grown with the input and surfels_size(), freed
+ * by sm_destroy; sm_create allocates nothing for it): 120 to 168 bytes per triangle of capacity (a directed-edge
+ * hash table of which a call uses and clears the power of two >= 6 x count: 48 to 96; the working list: 12; the
+ * corner keys unsorted and sorted: 48; the scan counts: 12), the radix sort's scratch (about 24 more per triangle)
+ * and 136 bytes per slot (the quadric: 80; the fan range, the mark, the key, the best neighbour and its cost, the
+ * slot list and the selected keys sorted and unsorted: 56). */
+#define SM_MESH_MAX_VALENCE 32
+#define SM_SIMPLIFY_MAX_ROUNDS 1024
+#define SM_SIMPLIFY_STOP_TARGET 1      /* the triangle count reached target_triangles */
+#define SM_SIMPLIFY_STOP_CONVERGED 2   /* no collapse was selected */
+#define SM_SIMPLIFY_STOP_MAX_ROUNDS 3  /* max_rounds rounds were applied */
+typedef struct sm_simplify_params {
+  uint64_t target_triangles;             /* 0 = no count bound */
+  double max_cost;                       /* 1e-6 m^2; >= 0 (+inf: no cost bound) */
+  float max_angle_between_normals_deg;   /* 90, as sm_mesh_params */
+  float max_triangle_angle_deg;          /* 170, as sm_mesh_params */
+  int32_t max_rounds;                    /* 64; in [0, SM_SIMPLIFY_MAX_ROUNDS]; 0 = check and reorder only */
+  int32_t reserved;                      /* 0 */
+} sm_simplify_params;
+typedef struct sm_simplify_stats {
+  uint64_t triangles_in;
+  uint64_t triangles_out;          /* always set, also when the capacity was too small */
+  uint64_t vertices_in, vertices_out;
+  uint64_t collapses;
+  uint64_t rounds;
+  uint64_t boundary_edges;         /* of the input, and of the output */
+  double max_cost_applied;         /* m^2 */
+  int32_t stop_reason;             /* SM_SIMPLIFY_STOP_* */
+  int32_t reserved;
+} sm_simplify_stats;
+/* Host only, no device needed. */
+void sm_default_simplify_params(sm_simplify_params* p);
+int sm_mesh_simplify(sm_reconstruction* r, void* stream, const sm_simplify_params* p,
+                     const uint32_t* triangles /* device, 3 x count */, uint64_t count,
+                     uint32_t* out /* device, 3 x capacity; may be NULL with capacity 0 */, uint64_t capacity,
+                     sm_simplify_stats* stats);
+
 /* ---- radius-limited k-nearest-neighbour queries for the meshing thread (SURVEY section 8 f4) ----
  * Replaces CompressedOctree::FindNearestSurfelsWithinRadius<include_completed_surfels, include_free_surfels>
  * (octree.h:471, octree.cc:313-470; callers surfel_meshing.cc:421 <false, true> and :821 <true, false>) for a BATCH of

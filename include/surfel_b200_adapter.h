@@ -175,6 +175,17 @@ class CUDASurfelReconstruction {
     return stats;
   }
 
+  // Extension (no counterpart in the reference): a triangle list over the slots (device, 3 x count) simplified by
+  // half-edge collapses (sm_mesh_simplify) into `out` (device, 3 x count suffices); every corner stays a slot.
+  sm_simplify_stats SimplifyMesh(cudaStream_t stream, const u32* triangles, uint64_t count, u32* out,
+                                 const sm_simplify_params* params = nullptr) {
+    sm_simplify_params defaults;
+    sm_default_simplify_params(&defaults);
+    sm_simplify_stats stats;
+    Check(sm_mesh_simplify(handle_, stream, params ? params : &defaults, triangles, count, out, count, &stats));
+    return stats;
+  }
+
  private:
   static void ToRowMajor(const SE3f& t, float* out) {
     const auto m = t.matrix3x4();

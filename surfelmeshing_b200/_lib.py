@@ -238,6 +238,35 @@ class HoleStats(C.Structure):
                 ("boundary_edges_after", C.c_uint64)]
 
 
+MESH_MAX_VALENCE = 32
+SIMPLIFY_MAX_ROUNDS = 1024
+SIMPLIFY_STOP_TARGET, SIMPLIFY_STOP_CONVERGED, SIMPLIFY_STOP_MAX_ROUNDS = 1, 2, 3
+
+
+class SimplifyParams(C.Structure):
+    """sm_simplify_params: the triangle budget (0: none), the largest collapse cost (m^2), the normal gate, the
+    largest triangle angle and the most rounds."""
+    _fields_ = [("target_triangles", C.c_uint64), ("max_cost", C.c_double),
+                ("max_angle_between_normals_deg", C.c_float), ("max_triangle_angle_deg", C.c_float),
+                ("max_rounds", C.c_int32), ("reserved", C.c_int32)]
+
+    @classmethod
+    def defaults(cls, **overrides) -> "SimplifyParams":
+        p = cls(0, 1e-6, 90.0, 170.0, 64, 0)
+        for k, v in overrides.items():
+            setattr(p, k, v)
+        return p
+
+
+class SimplifyStats(C.Structure):
+    """sm_simplify_stats: triangles and corner slots in and out, collapses and rounds applied, the boundary edges
+    (unchanged), the largest cost applied (m^2) and why the call stopped (SIMPLIFY_STOP_*)."""
+    _fields_ = [("triangles_in", C.c_uint64), ("triangles_out", C.c_uint64), ("vertices_in", C.c_uint64),
+                ("vertices_out", C.c_uint64), ("collapses", C.c_uint64), ("rounds", C.c_uint64),
+                ("boundary_edges", C.c_uint64), ("max_cost_applied", C.c_double), ("stop_reason", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 class CompactStats(C.Structure):
     """sm_compact_stats: surfels_size() before and after, the merged slots removed, the neighbour links of kept slots
     that named a removed slot, and whether the persistent sm_mesh_update mesh was carried over."""
@@ -343,6 +372,9 @@ _PRODUCT_ONLY = {
     "relocalise": (C.c_int, [_P, _P, _P, C.POINTER(RelocParams), C.POINTER(PreprocessParams),
                              C.POINTER(TrackRGBDParams), _P, _SZ, _P, _SZ, _P, C.POINTER(RelocResult)]),
     "compact": (C.c_int, [_P, _P, _P, C.c_uint64, C.POINTER(CompactStats)]),
+    "default_simplify_params": (None, [C.POINTER(SimplifyParams)]),
+    "mesh_simplify": (C.c_int, [_P, _P, C.POINTER(SimplifyParams), _P, C.c_uint64, _P, C.c_uint64,
+                                C.POINTER(SimplifyStats)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

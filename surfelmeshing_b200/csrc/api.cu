@@ -134,7 +134,9 @@ const char* KernelName(int id) {
       "k_track_intensity_base", "k_track_intensity_down", "k_track_linearize_rgbd", "k_track_solve_rgbd",
       "k_reloc_encode", "k_reloc_distance", "k_reloc_select", "k_hole_edges", "k_hole_boundary", "k_hole_sort",
       "k_hole_walk", "k_hole_conflict", "k_hole_scan", "k_hole_write", "k_compact_map", "k_compact_scatter",
-      "k_compact_store", "k_compact_mesh"};
+      "k_compact_store", "k_compact_mesh", "k_simplify_edges", "k_simplify_fans", "k_simplify_sort",
+      "k_simplify_quadrics", "k_simplify_candidates", "k_simplify_select", "k_simplify_apply", "k_simplify_scan",
+      "k_simplify_write"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -469,6 +471,7 @@ int sm_destroy(sm_reconstruction* r) {
   FreeMeshBuffers(r);
   FreeHoleBuffers(r);
   FreeCompactBuffers(r);
+  FreeSimplifyBuffers(r);
   delete r;
   cudaGetLastError();
   return SM_OK;

@@ -25,6 +25,7 @@
 
 #include "sm_handle.cuh"
 #include "sm_knn.cuh"
+#include "sm_mesh_edges.cuh"
 
 namespace smb {
 
@@ -33,13 +34,6 @@ namespace {
 constexpr int kBlock = 256;
 constexpr int kMaxHole = SM_MESH_MAX_HOLE;
 constexpr u32 kNone = 0xFFFFFFFFu;
-// Below this, the 3 x count hole edges index as u32 and x 1.5 of them still counts as the int of CUB's sort.
-constexpr u64 kMaxTriangles = 1ull << 28;
-
-// Input errors found on the device (HoleCounters::errors).
-constexpr u32 kBadCorner = 1;      // index >= surfels_size(), or a slot that is not present
-constexpr u32 kRepeatedCorner = 2;
-constexpr u32 kDuplicateEdge = 4;
 
 }  // namespace
 
@@ -88,53 +82,13 @@ struct HoleArgs {
   HoleCounters* counters;
 };
 
-#define SM_S(row, i) a.rows[static_cast<size_t>(row) * a.stride + (i)]
-
-__device__ __forceinline__ float dot3p(float3 a, float3 b) { return fadd(fadd(fmul(a.x, b.x), fmul(a.y, b.y)), fmul(a.z, b.z)); }
-__device__ __forceinline__ float3 sub3(float3 a, float3 b) { return make_float3(fsub(a.x, b.x), fsub(a.y, b.y), fsub(a.z, b.z)); }
 __device__ __forceinline__ float cross2(float2 a, float2 b) { return fsub(fmul(a.x, b.y), fmul(a.y, b.x)); }
 __device__ __forceinline__ float dot2(float2 a, float2 b) { return fadd(fmul(a.x, b.x), fmul(a.y, b.y)); }
 
-__device__ __forceinline__ float3 position(const HoleArgs& a, u32 i) {
-  return make_float3(SM_S(SM_ROW_SMOOTH_X, i), SM_S(SM_ROW_SMOOTH_Y, i), SM_S(SM_ROW_SMOOTH_Z, i));
-}
+__device__ __forceinline__ float3 position(const HoleArgs& a, u32 i) { return slot_position(a.rows, a.stride, i); }
 
-// Rows 8-10 times 1 / sqrt(n . n) (IEEE); false unless n . n is finite and > 0 (sm_triangulate's unit normal).
 __device__ __forceinline__ bool unit_normal(const HoleArgs& a, u32 i, float3* out) {
-  const float3 n = make_float3(SM_S(SM_ROW_NORMAL_X, i), SM_S(SM_ROW_NORMAL_Y, i), SM_S(SM_ROW_NORMAL_Z, i));
-  const float s = dot3p(n, n);
-  if (!(s > 0.f) || !isfinite(s)) return false;
-  const float inv = __fdiv_rn(1.f, __fsqrt_rn(s));
-  *out = make_float3(fmul(n.x, inv), fmul(n.y, inv), fmul(n.z, inv));
-  return true;
-}
-
-__device__ __forceinline__ u64 edge_key(u32 tail, u32 head) { return (static_cast<u64>(tail) << 32) | head; }
-__device__ __forceinline__ u32 tail_of(u64 key) { return static_cast<u32>(key >> 32); }
-__device__ __forceinline__ u32 head_of(u64 key) { return static_cast<u32>(key); }
-
-// splitmix64's finaliser: the probe start of a key.
-__device__ __forceinline__ u64 mix(u64 x) {
-  x ^= x >> 30; x *= 0xBF58476D1CE4E5B9ull;
-  x ^= x >> 27; x *= 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
-
-// Inserts key; false if it was there already.
-__device__ __forceinline__ bool table_insert(u64* table, u64 mask, u64 key, u64* slot_out) {
-  for (u64 slot = mix(key) & mask;; slot = (slot + 1) & mask) {
-    const u64 old = atomicCAS(reinterpret_cast<unsigned long long*>(table + slot), kEmptyKey, key);
-    if (old == kEmptyKey || old == key) { *slot_out = slot; return old == kEmptyKey; }
-  }
-}
-
-// The slot of key, or ~0 when it is absent.
-__device__ __forceinline__ u64 table_find(const u64* table, u64 mask, u64 key) {
-  for (u64 slot = mix(key) & mask;; slot = (slot + 1) & mask) {
-    const u64 k = table[slot];
-    if (k == key) return slot;
-    if (k == kEmptyKey) return ~0ull;
-  }
+  return slot_unit_normal(a.rows, a.stride, i, out);
 }
 
 __device__ __forceinline__ bool is_edge(const HoleArgs& a, u32 tail, u32 head) {
@@ -143,19 +97,8 @@ __device__ __forceinline__ bool is_edge(const HoleArgs& a, u32 tail, u32 head) {
 
 __global__ void __launch_bounds__(kBlock) k_hole_edges(HoleArgs a) {
   for (u32 t = blockIdx.x * blockDim.x + threadIdx.x; t < a.count; t += gridDim.x * blockDim.x) {
-    const uint3 c = a.triangles[t];
-    u32 error = 0;
-    for (int s = 0; s < 3; ++s) {
-      const u32 i = s == 0 ? c.x : (s == 1 ? c.y : c.z);
-      if (i >= a.n || !(SM_S(SM_ROW_RADIUS_SQUARED, i) > 0.f)) error |= kBadCorner;
-    }
-    if (c.x == c.y || c.y == c.z || c.z == c.x) error |= kRepeatedCorner;
-    if (!error) {
-      u64 slot;
-      if (!table_insert(a.edge_table, a.edge_mask, edge_key(c.x, c.y), &slot)) error |= kDuplicateEdge;
-      if (!table_insert(a.edge_table, a.edge_mask, edge_key(c.y, c.z), &slot)) error |= kDuplicateEdge;
-      if (!table_insert(a.edge_table, a.edge_mask, edge_key(c.z, c.x), &slot)) error |= kDuplicateEdge;
-    }
+    const u32 error = check_and_insert_triangle(a.rows + static_cast<size_t>(SM_ROW_RADIUS_SQUARED) * a.stride, a.n,
+                                                a.triangles[t], a.edge_table, a.edge_mask);
     if (error) atomicOr(&a.counters->errors, error);
   }
 }
@@ -228,13 +171,6 @@ __device__ u32 successor(const HoleArgs& a, u32 u, u32 v) {
     if (!(hb < h || (hb == h && cross2(qb, q) < 0.f))) return kNone;
   }
   return best;
-}
-
-// Rule 4's angle test at one corner with edges (g, h).
-__device__ __forceinline__ bool angle_too_large(float cos_triangle, float3 g, float3 h) {
-  const float d = dot3p(g, h);
-  const float l = __fsqrt_rn(fmul(dot3p(g, g), dot3p(h, h)));
-  return d < fmul(cos_triangle, l);
 }
 
 // H4's geometric part for the triangle (x0, x1, x2) (loop order): its weight w, or +inf when it is invalid.
@@ -389,12 +325,6 @@ __global__ void __launch_bounds__(kBlock) k_hole_write(HoleArgs a) {
   }
 }
 
-u64 PowerOfTwoAtLeast(u64 v) {
-  u64 p = 1;
-  while (p < v) p <<= 1;
-  return p;
-}
-
 // Per-triangle scratch for `count` triangles (x 1.5 when it grows).
 int EnsureTriangleScratch(HoleScratch& s, u64 count) {
   if (count <= s.triangle_capacity) return SM_OK;
@@ -472,7 +402,7 @@ int FillHoles(sm_reconstruction* r, cudaStream_t stream, const sm_hole_params& p
     return bad("angles must be in (0, 180] degrees");
   if (!triangles && count > 0) return bad("triangles is NULL with a count > 0");
   if (!fill && capacity > 0) return bad("fill is NULL with a capacity > 0");
-  if (count >= kMaxTriangles) return bad("2^28 triangles or more");
+  if (count >= kMaxMeshTriangles) return bad("2^28 triangles or more");
   r->last_stream = stream;
   int status = FetchCounters(r, stream);
   if (status == SM_ERR_CUDA) return status;   // (a surfel-cap overflow of an earlier frame does not matter here)
@@ -514,10 +444,7 @@ int FillHoles(sm_reconstruction* r, cudaStream_t stream, const sm_hole_params& p
   { LaunchScope scope(stream, KID_HOLE_BOUNDARY); LaunchKernel(k_hole_boundary, dim3(Grid(3 * count, r->sm_count)), dim3(kBlock), 0, stream, a); }
   SM_CUDA(cudaMemcpyAsync(s.host_counters, s.counters, sizeof(HoleCounters), cudaMemcpyDeviceToHost, stream));
   SM_CUDA(cudaStreamSynchronize(stream));
-  const u32 errors = s.host_counters->errors;
-  if (errors & kBadCorner) return bad("a corner is not a present slot below surfels_size()");
-  if (errors & kRepeatedCorner) return bad("a triangle has a repeated corner");
-  if (errors & kDuplicateEdge) return bad("a directed edge occurs twice (the input must be edge-manifold and consistently oriented)");
+  if (const char* why = MeshInputError(s.host_counters->errors)) return bad(why);
   const u32 H = s.host_counters->hole_edges;
   stats->boundary_edges = H;
   stats->boundary_edges_after = H;

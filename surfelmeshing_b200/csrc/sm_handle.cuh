@@ -71,6 +71,7 @@ struct TrackScratch;     // track.cu: sm_track_frame* / sm_track_linearize*
 struct MeshScratch;      // mesh.cu: sm_triangulate, and the persistent mesh of sm_mesh_update
 struct HoleScratch;      // holes.cu: the buffers of sm_mesh_fill_holes
 struct CompactScratch;   // compact.cu: the map and the row scratch of sm_compact
+struct SimplifyScratch;  // simplify.cu: the buffers of sm_mesh_simplify
 
 }  // namespace smb
 
@@ -127,6 +128,7 @@ struct sm_reconstruction {
   smb::MeshScratch* mesh = nullptr;
   smb::HoleScratch* holes = nullptr;
   smb::CompactScratch* compact = nullptr;
+  smb::SimplifyScratch* simplify = nullptr;
 };
 
 namespace smb {
@@ -199,6 +201,10 @@ void FreeHoleBuffers(sm_reconstruction* r);
 int Compact(sm_reconstruction* r, cudaStream_t stream, uint32_t* old_to_new, uint64_t map_capacity,
             sm_compact_stats* stats);
 void FreeCompactBuffers(sm_reconstruction* r);
+// simplify.cu
+int Simplify(sm_reconstruction* r, cudaStream_t stream, const sm_simplify_params& p, const uint32_t* triangles,
+             uint64_t count, uint32_t* out, uint64_t capacity, sm_simplify_stats* stats);
+void FreeSimplifyBuffers(sm_reconstruction* r);
 // In place: word w of record k' = word w of record i, old_to_new[i] = k' < kept, for every word of records of
 // `record_words` 32-bit words (bytes) over slots [0, n), one word at a time through `scratch` (>= kept words).
 // `remap`: the words name slots and are replaced by their new index (SM_INVALID_SURFEL_INDEX for a removed one).

@@ -48,6 +48,8 @@ enum KernelId {
   KID_RELOC_ENCODE, KID_RELOC_DISTANCE, KID_RELOC_SELECT,
   KID_HOLE_EDGES, KID_HOLE_BOUNDARY, KID_HOLE_SORT, KID_HOLE_WALK, KID_HOLE_CONFLICT, KID_HOLE_SCAN, KID_HOLE_WRITE,
   KID_COMPACT_MAP, KID_COMPACT_SCATTER, KID_COMPACT_STORE, KID_COMPACT_MESH,
+  KID_SIMPLIFY_EDGES, KID_SIMPLIFY_FANS, KID_SIMPLIFY_SORT, KID_SIMPLIFY_QUADRICS, KID_SIMPLIFY_CANDIDATES,
+  KID_SIMPLIFY_SELECT, KID_SIMPLIFY_APPLY, KID_SIMPLIFY_SCAN, KID_SIMPLIFY_WRITE,
   KID_COUNT
 };
 const char* KernelName(int id);

@@ -21,14 +21,21 @@ def _g(a: np.ndarray) -> list[str]:
     return [f"{float(v):g}" for v in a]
 
 
-def write_obj(path, positions, colors, triangles) -> tuple[int, int]:
+def write_obj(path, positions, colors, triangles, referenced_only: bool = False) -> tuple[int, int]:
     """OBJ as Mesh3fCu8::WriteAsOBJ writes it: one "v x y z r g b" line per kept slot (colour / 255), then one
     "f a b c" line per triangle with 1-based vertex numbers. triangles hold slot indices; every corner must be a
-    kept slot. Returns (vertices, faces) written."""
+    kept slot. With referenced_only, the kept slots are only those that are a corner of a triangle (still in slot
+    order), as a simplified mesh wants. Returns (vertices, faces) written."""
     positions = np.asarray(positions, np.float32).reshape(-1, 3)
     colors = np.asarray(colors, np.uint8).reshape(-1, 3)
     triangles = np.asarray(triangles, np.int64).reshape(-1, 3)
     kept, remap = present_vertices(positions)
+    if referenced_only:
+        used = np.zeros(len(positions), bool)
+        used[triangles.ravel()] = True
+        kept = kept[used[kept]]
+        remap = np.full(len(positions), -1, np.int64)
+        remap[kept] = np.arange(len(kept))
     faces = remap[triangles] if len(triangles) else np.zeros((0, 3), np.int64)
     if (faces < 0).any():
         raise ValueError("a triangle uses a merged slot")

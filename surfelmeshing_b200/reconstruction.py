@@ -20,7 +20,7 @@ import torch
 
 from . import _lib
 from . import mesh_io
-from ._lib import (CompactStats, HoleParams, HoleStats, IntegrateParams, Library, MeshParams, MeshStats, MeshUpdateStats,
+from ._lib import (CompactStats, HoleParams, HoleStats, IntegrateParams, SimplifyParams, SimplifyStats, Library, MeshParams, MeshStats, MeshUpdateStats,
                    PreprocessParams, RelocParams, RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult,
                    TrackRGBDParams, TrackRGBDResult,
                    TransferStats, TransferToken, VisualizationParams)
@@ -628,6 +628,25 @@ class CUDASurfelReconstruction:
                       C.c_void_p(out.data_ptr()), capacity, C.byref(stats))
         return out[:int(stats.triangles_added)], stats
 
+    def simplify_mesh(self, triangles, params: Optional[SimplifyParams] = None, stream=None):
+        """sm_mesh_simplify: `triangles` (an int32 CUDA tensor [T, 3] of slot indices, edge-manifold and consistently
+        oriented, as triangulate() and fill_holes() give it) with slots removed by half-edge collapses, down to
+        params.target_triangles or params.max_cost (include/surfel_b200.h gives the rules). Synchronous. Returns
+        (int32 CUDA tensor [T', 3] over a subset of the slots, in the mesh's convention; SimplifyStats). The output
+        is never longer than the input, so one call with capacity T suffices."""
+        p = SimplifyParams.defaults() if params is None else params
+        if not (isinstance(triangles, torch.Tensor) and triangles.is_cuda and triangles.dtype == torch.int32
+                and triangles.dim() == 2 and triangles.shape[1] == 3):
+            raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+        tri = triangles.contiguous()
+        out = torch.empty((max(len(tri), 1), 3), dtype=torch.int32, device="cuda")
+        if isinstance(stream, torch.cuda.Stream):
+            out.record_stream(stream)
+        stats = SimplifyStats()
+        self.lib.call("mesh_simplify", self._h, _stream_handle(stream), C.byref(p), C.c_void_p(tri.data_ptr()),
+                      len(tri), C.c_void_p(out.data_ptr()), len(tri), C.byref(stats))
+        return out[:int(stats.triangles_out)], stats
+
     def export_vertices_host(self, stream=None):
         """sm_export_vertices into host arrays: positions [n, 3] float32 (NaN rows for merged slots), colours
         [n, 3] uint8, n = surfels_size()."""
@@ -640,16 +659,19 @@ class CUDASurfelReconstruction:
         return pos[:3 * n].cpu().numpy().reshape(n, 3), col[:3 * n].cpu().numpy().reshape(n, 3)
 
     def save_mesh_obj(self, path, params: Optional[MeshParams] = None, stream=None,
-                      holes: Optional[HoleParams] = None) -> MeshStats:
+                      holes: Optional[HoleParams] = None, simplify: Optional[SimplifyParams] = None) -> MeshStats:
         """The reference's SaveMeshAsOBJ (main.cc:128-175): the non-merged slots in slot order with their colour,
         and the triangles of triangulate() over them (1-based, remapped to that order). With `holes`, the
-        triangles of fill_holes(holes) follow the mesh's."""
+        triangles of fill_holes(holes) follow the mesh's. With `simplify`, the mesh (with its fill) goes through
+        simplify_mesh(simplify), and only the slots that are corners of its triangles are written, in slot order."""
         tri, stats = self.triangulate(params, stream)
         if holes is not None:
             fill, _ = self.fill_holes(tri, holes, stream)
             tri = torch.cat([tri, fill])
+        if simplify is not None:
+            tri, _ = self.simplify_mesh(tri, simplify, stream)
         positions, colors = self.export_vertices_host(stream)
-        mesh_io.write_obj(path, positions, colors, tri.cpu().numpy())
+        mesh_io.write_obj(path, positions, colors, tri.cpu().numpy(), referenced_only=simplify is not None)
         return stats
 
     def save_point_cloud_ply(self, path, stream=None) -> int:
