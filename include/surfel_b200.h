@@ -1025,6 +1025,117 @@ int sm_mesh_simplify(sm_reconstruction* r, void* stream, const sm_simplify_param
                      uint32_t* out /* device, 3 x capacity; may be NULL with capacity 0 */, uint64_t capacity,
                      sm_simplify_stats* stats);
 
+/* ---- texturing a triangle mesh from posed colour images (DESIGN.md section 1 row f17, section 5.15) ------------
+ * The mesh calls carry one colour per vertex (row 24 of the corner's slot), so a simplified mesh loses the colour
+ * detail between its vertices. sm_mesh_texture gives every triangle of a caller's list a patch of a texture atlas
+ * and fills each texel from the colour images of caller-chosen views that see it: the visibility-weighted mean of
+ * their bilinear samples, the corner colours where no view sees the texel. Any list of triangles over present slots
+ * is accepted (manifoldness is not required), e.g. the output of sm_triangulate, sm_mesh_fill_holes or
+ * sm_mesh_simplify. Positions are the current SMOOTH positions (what sm_render_mesh draws); the call only reads the
+ * surfel state.
+ *
+ * fp32 with denormals flushed to zero and no contraction, every product, sum, quotient and square root rounded on
+ * its own (IEEE), in the order written: (a + b) + c means a + b first; |d|^2 = (d.x*d.x + d.y*d.y) + d.z*d.z. p_i is
+ * the smooth position of slot i; t is a triangle's position in the list; its corners k = 0, 1, 2 in list order.
+ *  X1. Input. Every corner must be a present slot (radius^2 > 0) below surfels_size() and no triangle may repeat a
+ *      corner. 0 triangles are legal.
+ *  X2. Tile class. e_k = |p_(k+2) - p_(k+1)|^2 (indices mod 3) is the squared length of the edge opposite corner k;
+ *      a = the first k with the largest e_k (in the order 0, 1, 2; a NaN is never larger), b = a + 1, c = a + 2
+ *      (mod 3): the rotation of t that starts at a, winding kept. L = sqrt(max(e_c, e_b)) (the legs ab and ac). The
+ *      tile side s is the smallest of 8, 16, ..., SM_TEXTURE_MAX_TILE with L <= float(s - 4) * texel_size; if none
+ *      is, s = SM_TEXTURE_MAX_TILE and the triangle counts in tiles_clamped.
+ *  X3. Layout. The triangles sorted by (s descending, t ascending); within one s, the 2j-th and (2j+1)-th share the
+ *      j-th s x s square of that s, as its half 0 and half 1. The squares in that order (larger s first, then j) get
+ *      running area offsets o (the sum of s^2 of the squares before); a square's origin (x0, y0) in texels is the
+ *      Morton (Z-order) decode of o (x from the even bits, y from the odd ones). Every earlier square is at least as
+ *      large, so o is a multiple of s^2 and the square is the aligned block of codes [o, o + s^2): squares never
+ *      overlap. The atlas width W is the smallest power of two with W * W >= the total area, its height H the
+ *      largest y0 + s (0 x 0 for an empty list).
+ *  X4. UV. Texel (i, j) of a square is the atlas texel (x0 + i, y0 + j), its centre at (i + 0.5, j + 0.5) in square
+ *      coordinates. Half 0 is the texels with i + j <= s - 1 and its triangle's (a, b, c) sit at (1, 1), (s - 3, 1),
+ *      (1, s - 3); half 1 is those with i + j >= s, its (a, b, c) at (s - 1, s - 1), (3, s - 1), (s - 1, 3). A bilinear
+ *      lookup (texel centres at integer + 0.5) at any point of a UV triangle reads only texels of its own half. The
+ *      uv output holds, per triangle in list order and per corner in list order, (float(x0 + X) / float(W),
+ *      float(y0 + Y) / float(H)) for the corner's (X, Y) above.
+ *  X5. Texel point. For texel (i, j) of a half: x = float(i) + 0.5, y = float(j) + 0.5, q = float(s - 4); half 0:
+ *      alpha = (x - 1) / q, beta = (y - 1) / q; half 1: alpha = (float(s - 1) - x) / q, beta = (float(s - 1) - y) / q.
+ *      Clamp to the triangle: alpha = max(alpha, 0), beta = max(beta, 0), and if alpha + beta > 1: alpha =
+ *      alpha / (alpha + beta), beta = 1 - alpha. X = (p_a + alpha * (p_b - p_a)) + beta * (p_c - p_a), per
+ *      component. The geometric normal: e1 = p_b - p_a, e2 = p_c - p_a, g = (e1.y*e2.z - e1.z*e2.y,
+ *      e1.z*e2.x - e1.x*e2.z, e1.x*e2.y - e1.y*e2.x), n = g * (1 / sqrt(|g|^2)); a triangle whose |g|^2 is not finite
+ *      and > 0 has no normal and no view contributes to it.
+ *  X6. One view's sample, views in array order. c = view_T_global * X and m = R(view_T_global) * n as in rule 1 of
+ *      sm_render_surfels. The view contributes nothing unless near_depth <= c.z <= far_depth; with (u, v) = (fx *
+ *      (c.x / c.z) + cx, fy * (c.y / c.z) + cy) (T3 of sm_render_mesh), px = u - 0.5, py = v - 0.5: unless 0 <= px <
+ *      float(width - 1) and 0 <= py < float(height - 1) (the 2 x 2 bilinear footprint lies in the image); unless
+ *      D > 0 and |D - c.z| <= depth_tolerance * c.z, D the depth that sm_render_mesh draws for the same triangle list
+ *      and camera, without disks, at pixel (int(u), int(v)); unless cos_theta = -((m.x*c.x + m.y*c.y) + m.z*c.z) /
+ *      sqrt(|c|^2) >= float(cos(max_view_angle_deg)) (computed in double). Then w = cos_theta / (c.z * c.z) and, with
+ *      x0 = floor(px), fx = px - x0, y0 = floor(py), fy = py - y0 and V_xy the channel at pixel (x0 + x, y0 + y) as a
+ *      float, the sample of a channel is top + fy * (bot - top), top = V_00 + fx * (V_10 - V_00), bot = V_01 + fx *
+ *      (V_11 - V_01). Per texel S_ch = S_ch + w * sample_ch and S_w = S_w + w, from 0.
+ *  X7. Resolve. If S_w > 0, channel ch = the u8 of S_ch / S_w + 0.5, truncated, 255 if it is >= 255. Otherwise
+ *      (texels_fallback) the corner blend: with C_k = float(channel ch of row 24 of slot k), ((1 - alpha) - beta) * C_a
+ *      + alpha * C_b, then + beta * C_c, + 0.5, truncated, 255 if >= 255. Atlas texels of no half (the empty half 1
+ *      of a square whose s has an odd count, and every texel at or past the total area's last code) are 0.
+ *  X8. Stats: triangles = count; atlas_width = W and atlas_height = H; texels = the texels of all halves used
+ *      (s (s + 1) / 2 for half 0, s (s - 1) / 2 for half 1); texels_seen (S_w > 0) and texels_fallback (the rest);
+ *      tiles_clamped; views_used = the views that contribute to at least one texel. The first five are set also on
+ *      a layout query and on SM_ERR_CAPACITY (the last three 0); all are zero when the call fails otherwise.
+ *
+ * atlas is a DEVICE buffer of packed u8x3 texels (r, g, b) with atlas_pitch bytes per row and room for
+ * atlas_capacity_width x atlas_capacity_height texels; only the W x H texels at its start are written (bytes past
+ * 3 W of a row and rows past H stay untouched). atlas NULL with a 0 x 0 capacity is a layout query. If W >
+ * max_atlas_side, or the capacity is smaller than W x H, the call returns SM_ERR_CAPACITY with the stats set and
+ * writes nothing; a caller that hits max_atlas_side raises texel_size. uv (DEVICE, 6 x count floats, may be NULL) is
+ * written together with the atlas. Each view's colour is a DEVICE u8x3 image of its camera's size, color_pitch bytes
+ * per row. SM_ERR_INVALID_ARGUMENT, with no launch, for NULL params or stats, triangles NULL with count > 0, count >=
+ * 2^28, views NULL with view_count > 0, view_count outside [0, SM_TEXTURE_MAX_VIEWS], a view camera or pose that
+ * sm_render_mesh refuses, a view colour that is NULL or whose pitch is below 3 x width, texel_size not finite and
+ * > 0, max_atlas_side outside [8, SM_TEXTURE_MAX_ATLAS_SIDE], max_view_angle_deg outside (0, 90], depth_tolerance
+ * negative, NaN or infinite, atlas NULL with a capacity that is not 0 x 0, a negative capacity, atlas_pitch below 3
+ * x atlas_capacity_width, or uv overlapping the triangles or the atlas; and, found on the device and reported after
+ * the call's second synchronisation with nothing written, for a list that breaks X1.
+ * The call synchronises `stream` three times (surfels_size(); the input checks and the layout; the end), plus once,
+ * with cudaFree's device synchronisation, in a call whose buffers grow (by x 1.5); the per-view work is ordered on
+ * `stream` without a host round trip. Memory (allocated by the first call, grown with the input, freed by
+ * sm_destroy; sm_create allocates nothing for it): 24 bytes per triangle of capacity (sort keys in and out, the
+ * tile records) plus the radix sort's scratch, 16 bytes per texel of the laid-out area (the float4 accumulators),
+ * 4 bytes per pixel of the largest view (its depth) and sm_render_mesh's own scratch. */
+#define SM_TEXTURE_MAX_TILE 512
+#define SM_TEXTURE_MAX_VIEWS 1024
+#define SM_TEXTURE_MAX_ATLAS_SIDE 32768
+typedef struct sm_texture_params {
+  float texel_size;            /* metres per texel; 0.004 (about one VGA pixel at 1.4 m) */
+  int32_t max_atlas_side;      /* 16384; in [8, SM_TEXTURE_MAX_ATLAS_SIDE] */
+  float max_view_angle_deg;    /* 75; in (0, 90]: views seeing a texel more obliquely do not contribute */
+  float depth_tolerance;       /* 0.01, relative to the texel's camera depth; >= 0 */
+} sm_texture_params;
+typedef struct sm_texture_stats {
+  uint64_t triangles;
+  int32_t atlas_width, atlas_height;
+  uint64_t texels;                 /* in the halves of all tiles */
+  uint64_t texels_seen;            /* at least one view contributed */
+  uint64_t texels_fallback;        /* no view contributed: the corner blend */
+  uint64_t tiles_clamped;          /* triangles whose tile was capped at SM_TEXTURE_MAX_TILE */
+  uint64_t views_used;             /* views that contributed to at least one texel */
+} sm_texture_stats;
+typedef struct sm_texture_view {
+  sm_render_params camera;     /* size, intrinsics (pixel-corner convention), near/far: as sm_render_mesh */
+  float view_T_global[12];     /* 3x4 row-major, global -> camera */
+  const uint8_t* color;        /* DEVICE, packed u8x3 rows (r, g, b), as the stream frames */
+  size_t color_pitch;
+} sm_texture_view;
+/* Host only, no device needed. */
+void sm_default_texture_params(sm_texture_params* p);
+int sm_mesh_texture(sm_reconstruction* r, void* stream, const sm_texture_params* p,
+                    const uint32_t* triangles /* device, 3 x count */, uint64_t count,
+                    const sm_texture_view* views /* host array */, int32_t view_count,
+                    uint8_t* atlas /* device u8x3, pitched; NULL with 0 x 0 capacity = layout query */,
+                    size_t atlas_pitch, int32_t atlas_capacity_width, int32_t atlas_capacity_height,
+                    float* uv /* device, 6 x count: (u, v) per corner in the listed order, in [0, 1]; may be NULL */,
+                    sm_texture_stats* stats);
+
 /* ---- radius-limited k-nearest-neighbour queries for the meshing thread (SURVEY section 8 f4) ----
  * Replaces CompressedOctree::FindNearestSurfelsWithinRadius<include_completed_surfels, include_free_surfels>
  * (octree.h:471, octree.cc:313-470; callers surfel_meshing.cc:421 <false, true> and :821 <true, false>) for a BATCH of

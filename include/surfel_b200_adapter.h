@@ -186,6 +186,22 @@ class CUDASurfelReconstruction {
     return stats;
   }
 
+  // Extension (no counterpart in the reference): a texture atlas for a triangle list over the slots (device, 3 x
+  // count) from posed colour views (sm_mesh_texture): `atlas` (device u8x3, atlas_pitch bytes per row, room for
+  // capacity_width x capacity_height texels) and `uv` (device, 6 x count, may be null). A call with a null atlas and
+  // a 0 x 0 capacity only lays the atlas out: the returned stats give its size.
+  sm_texture_stats TextureMesh(cudaStream_t stream, const u32* triangles, uint64_t count, const sm_texture_view* views,
+                               int view_count, u8* atlas, size_t atlas_pitch, int capacity_width, int capacity_height,
+                               float* uv, const sm_texture_params* params = nullptr) {
+    sm_texture_params defaults;
+    sm_default_texture_params(&defaults);
+    sm_texture_stats stats;
+    const int status = sm_mesh_texture(handle_, stream, params ? params : &defaults, triangles, count, views,
+                                       view_count, atlas, atlas_pitch, capacity_width, capacity_height, uv, &stats);
+    if (!(status == SM_ERR_CAPACITY && atlas == nullptr)) Check(status);
+    return stats;
+  }
+
  private:
   static void ToRowMajor(const SE3f& t, float* out) {
     const auto m = t.matrix3x4();

@@ -267,6 +267,40 @@ class SimplifyStats(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+TEXTURE_MAX_TILE = 512
+TEXTURE_MAX_VIEWS = 1024
+TEXTURE_MAX_ATLAS_SIDE = 32768
+
+
+class TextureParams(C.Structure):
+    """sm_texture_params: metres per texel, the largest atlas side, the most oblique view that contributes (degrees)
+    and the relative depth tolerance of the visibility test."""
+    _fields_ = [("texel_size", C.c_float), ("max_atlas_side", C.c_int32), ("max_view_angle_deg", C.c_float),
+                ("depth_tolerance", C.c_float)]
+
+    @classmethod
+    def defaults(cls, **overrides) -> "TextureParams":
+        p = cls(0.004, 16384, 75.0, 0.01)
+        for k, v in overrides.items():
+            setattr(p, k, v)
+        return p
+
+
+class TextureStats(C.Structure):
+    """sm_texture_stats: triangles, the atlas size, the texels of all half-tiles, those some view saw and those that
+    took the corner blend, the tiles capped at TEXTURE_MAX_TILE and the views that contributed."""
+    _fields_ = [("triangles", C.c_uint64), ("atlas_width", C.c_int32), ("atlas_height", C.c_int32),
+                ("texels", C.c_uint64), ("texels_seen", C.c_uint64), ("texels_fallback", C.c_uint64),
+                ("tiles_clamped", C.c_uint64), ("views_used", C.c_uint64)]
+
+
+class TextureViewDesc(C.Structure):
+    """sm_texture_view: the camera (as sm_render_mesh takes it), view_T_global (3x4 row-major) and the device colour
+    image (packed u8x3 rows) with its pitch in bytes."""
+    _fields_ = [("camera", RenderParams), ("view_T_global", C.c_float * 12), ("color", C.c_void_p),
+                ("color_pitch", C.c_size_t)]
+
+
 class CompactStats(C.Structure):
     """sm_compact_stats: surfels_size() before and after, the merged slots removed, the neighbour links of kept slots
     that named a removed slot, and whether the persistent sm_mesh_update mesh was carried over."""
@@ -375,6 +409,9 @@ _PRODUCT_ONLY = {
     "default_simplify_params": (None, [C.POINTER(SimplifyParams)]),
     "mesh_simplify": (C.c_int, [_P, _P, C.POINTER(SimplifyParams), _P, C.c_uint64, _P, C.c_uint64,
                                 C.POINTER(SimplifyStats)]),
+    "default_texture_params": (None, [C.POINTER(TextureParams)]),
+    "mesh_texture": (C.c_int, [_P, _P, C.POINTER(TextureParams), _P, C.c_uint64, C.POINTER(TextureViewDesc), _I, _P,
+                               _SZ, _I, _I, _P, C.POINTER(TextureStats)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

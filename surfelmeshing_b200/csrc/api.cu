@@ -136,7 +136,7 @@ const char* KernelName(int id) {
       "k_hole_walk", "k_hole_conflict", "k_hole_scan", "k_hole_write", "k_compact_map", "k_compact_scatter",
       "k_compact_store", "k_compact_mesh", "k_simplify_edges", "k_simplify_fans", "k_simplify_sort",
       "k_simplify_quadrics", "k_simplify_candidates", "k_simplify_select", "k_simplify_apply", "k_simplify_scan",
-      "k_simplify_write"};
+      "k_simplify_write", "k_tex_classes", "k_tex_sort", "k_tex_place", "k_tex_uv", "k_tex_accumulate", "k_tex_resolve"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }
 
@@ -472,6 +472,7 @@ int sm_destroy(sm_reconstruction* r) {
   FreeHoleBuffers(r);
   FreeCompactBuffers(r);
   FreeSimplifyBuffers(r);
+  FreeTextureBuffers(r);
   delete r;
   cudaGetLastError();
   return SM_OK;

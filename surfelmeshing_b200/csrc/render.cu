@@ -479,6 +479,19 @@ __global__ void __launch_bounds__(kResolveBlock) k_mesh_render_resolve(DeviceSta
 
 bool Finite(float v) { return std::isfinite(v); }
 
+}  // namespace
+
+const char* RenderCameraError(const sm_render_params& p, const float* view_T_global) {
+  if (p.width <= 0 || p.height <= 0) return "width and height must be > 0";
+  if (!Finite(p.fx) || !Finite(p.fy) || p.fx == 0.f || p.fy == 0.f) return "fx and fy must be finite and non-zero";
+  if (!Finite(p.cx) || !Finite(p.cy)) return "cx and cy must be finite";
+  if (!(p.near_depth > 0.f) || !(p.far_depth > p.near_depth)) return "need 0 < near_depth < far_depth";
+  for (int k = 0; k < 12; ++k) if (!Finite(view_T_global[k])) return "view_T_global must be finite";
+  return nullptr;
+}
+
+namespace {
+
 // The key raster grows to `pixels`; the list, its count and the grids are set up once.
 int EnsureRenderBuffers(sm_reconstruction* r, cudaStream_t stream, size_t pixels) {
   if (!r->render) r->render = new RenderScratch();
@@ -507,11 +520,7 @@ int MakeRenderArgs(sm_reconstruction* r, cudaStream_t stream, const char* name, 
                    const float* view_T_global, float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch,
                    float* normal, size_t normal_pitch, uint32_t* index, size_t index_pitch, RenderArgs* out) {
   auto bad = [name](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string(name) + ": " + why).c_str()); };
-  if (p.width <= 0 || p.height <= 0) return bad("width and height must be > 0");
-  if (!Finite(p.fx) || !Finite(p.fy) || p.fx == 0.f || p.fy == 0.f) return bad("fx and fy must be finite and non-zero");
-  if (!Finite(p.cx) || !Finite(p.cy)) return bad("cx and cy must be finite");
-  if (!(p.near_depth > 0.f) || !(p.far_depth > p.near_depth)) return bad("need 0 < near_depth < far_depth");
-  for (int k = 0; k < 12; ++k) if (!Finite(view_T_global[k])) return bad("view_T_global must be finite");
+  if (const char* why = RenderCameraError(p, view_T_global)) return bad(why);
   if (!depth && !color && !normal && !index) return bad("all outputs are NULL");
   const size_t w = static_cast<size_t>(p.width);
   if ((depth && depth_pitch < w * sizeof(float)) || (color && color_pitch < w * 3) ||

@@ -72,6 +72,7 @@ struct MeshScratch;      // mesh.cu: sm_triangulate, and the persistent mesh of 
 struct HoleScratch;      // holes.cu: the buffers of sm_mesh_fill_holes
 struct CompactScratch;   // compact.cu: the map and the row scratch of sm_compact
 struct SimplifyScratch;  // simplify.cu: the buffers of sm_mesh_simplify
+struct TextureScratch;   // texture.cu: the buffers of sm_mesh_texture
 
 }  // namespace smb
 
@@ -129,6 +130,7 @@ struct sm_reconstruction {
   smb::HoleScratch* holes = nullptr;
   smb::CompactScratch* compact = nullptr;
   smb::SimplifyScratch* simplify = nullptr;
+  smb::TextureScratch* texture = nullptr;
 };
 
 namespace smb {
@@ -163,6 +165,8 @@ int RenderMesh(sm_reconstruction* r, cudaStream_t stream, const sm_render_params
                uint8_t* color, size_t color_pitch, float* normal, size_t normal_pitch, uint32_t* index,
                size_t index_pitch);
 void FreeRenderBuffers(sm_reconstruction* r);
+// The camera and pose checks of sm_render_surfels and sm_render_mesh: the reason a camera is refused, or nullptr.
+const char* RenderCameraError(const sm_render_params& p, const float* view_T_global);
 // track.cu
 int TrackFrame(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const sm_preprocess_params& pp,
                const u16* depth, size_t depth_pitch, const float* guess, float* pose_out, sm_track_result* result);
@@ -205,6 +209,11 @@ void FreeCompactBuffers(sm_reconstruction* r);
 int Simplify(sm_reconstruction* r, cudaStream_t stream, const sm_simplify_params& p, const uint32_t* triangles,
              uint64_t count, uint32_t* out, uint64_t capacity, sm_simplify_stats* stats);
 void FreeSimplifyBuffers(sm_reconstruction* r);
+// texture.cu
+int Texture(sm_reconstruction* r, cudaStream_t stream, const sm_texture_params& p, const uint32_t* triangles,
+            uint64_t count, const sm_texture_view* views, int32_t view_count, uint8_t* atlas, size_t atlas_pitch,
+            int32_t atlas_capacity_width, int32_t atlas_capacity_height, float* uv, sm_texture_stats* stats);
+void FreeTextureBuffers(sm_reconstruction* r);
 // In place: word w of record k' = word w of record i, old_to_new[i] = k' < kept, for every word of records of
 // `record_words` 32-bit words (bytes) over slots [0, n), one word at a time through `scratch` (>= kept words).
 // `remap`: the words name slots and are replaced by their new index (SM_INVALID_SURFEL_INDEX for a removed one).

@@ -50,6 +50,7 @@ enum KernelId {
   KID_COMPACT_MAP, KID_COMPACT_SCATTER, KID_COMPACT_STORE, KID_COMPACT_MESH,
   KID_SIMPLIFY_EDGES, KID_SIMPLIFY_FANS, KID_SIMPLIFY_SORT, KID_SIMPLIFY_QUADRICS, KID_SIMPLIFY_CANDIDATES,
   KID_SIMPLIFY_SELECT, KID_SIMPLIFY_APPLY, KID_SIMPLIFY_SCAN, KID_SIMPLIFY_WRITE,
+  KID_TEXTURE_CLASSES, KID_TEXTURE_SORT, KID_TEXTURE_PLACE, KID_TEXTURE_UV, KID_TEXTURE_ACCUMULATE, KID_TEXTURE_RESOLVE,
   KID_COUNT
 };
 const char* KernelName(int id);

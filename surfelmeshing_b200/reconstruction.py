@@ -21,7 +21,8 @@ import torch
 from . import _lib
 from . import mesh_io
 from ._lib import (CompactStats, HoleParams, HoleStats, IntegrateParams, SimplifyParams, SimplifyStats, Library, MeshParams, MeshStats, MeshUpdateStats,
-                   PreprocessParams, RelocParams, RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats, TrackParams, TrackResult,
+                   PreprocessParams, RelocParams, RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats,
+                   TextureParams, TextureStats, TextureViewDesc, TrackParams, TrackResult,
                    TrackRGBDParams, TrackRGBDResult,
                    TransferStats, TransferToken, VisualizationParams)
 
@@ -98,6 +99,35 @@ def shade_normals(normal: torch.Tensor) -> torch.Tensor:
     intensity = (0.8 * (-n[..., 2]) + 0.2).clamp(0.0, 1.0)
     value = torch.round(intensity * 255.0).to(torch.uint8)
     return torch.where((n != 0).any(dim=2), value, torch.zeros_like(value))
+
+
+class TextureView:
+    """One posed colour image for CUDASurfelReconstruction.texture_mesh(): a uint8 CUDA tensor [H, W, 3] (r, g, b,
+    row-pitched), the synthetic.Camera it was taken with (pixel-corner intrinsics, size H x W), and its pose as
+    view_T_global (global -> camera) or global_T_view (camera -> global; inverted in float64). Only surfaces with
+    near <= camera depth <= far take colour from it."""
+
+    def __init__(self, color: torch.Tensor, camera, view_T_global=None, global_T_view=None, near: float = 0.1,
+                 far: float = 100.0):
+        if (view_T_global is None) == (global_T_view is None):
+            raise ValueError("give exactly one of view_T_global and global_T_view")
+        if not (isinstance(color, torch.Tensor) and color.is_cuda and color.dtype == torch.uint8
+                and tuple(color.shape) == (camera.height, camera.width, 3)):
+            raise ValueError(f"color must be a uint8 CUDA tensor of shape {(camera.height, camera.width, 3)}")
+        self.color = color if color.stride(2) == 1 and color.stride(1) == 3 else color.contiguous()
+        self.camera = camera
+        self.view_T_global = _mat12(view_T_global if view_T_global is not None else invert_rigid(global_T_view))
+        self.near, self.far = float(near), float(far)
+
+    def desc(self) -> TextureViewDesc:
+        c = self.camera
+        d = TextureViewDesc()
+        d.camera = RenderParams(c.width, c.height, float(c.fx), float(c.fy), float(c.cx), float(c.cy), self.near,
+                                self.far)
+        d.view_T_global = (C.c_float * 12)(*self.view_T_global.tolist())
+        d.color = self.color.data_ptr()
+        d.color_pitch = self.color.stride(0)
+        return d
 
 
 # ---------------------------------------------------------------------------------------
@@ -647,6 +677,43 @@ class CUDASurfelReconstruction:
                       len(tri), C.c_void_p(out.data_ptr()), len(tri), C.byref(stats))
         return out[:int(stats.triangles_out)], stats
 
+    def texture_mesh(self, triangles, views: Sequence[TextureView], params: Optional[TextureParams] = None,
+                     stream=None):
+        """sm_mesh_texture: a texture atlas for `triangles` (an int32 CUDA tensor [T, 3] of present slots, any list
+        without repeated corners) from the colour images of `views` (TextureView, in the order their samples are
+        summed; include/surfel_b200.h gives the rules). Synchronous. Lays the atlas out first (a query that writes
+        nothing), then fills it. Returns (atlas uint8 CUDA tensor [H, W, 3], row 0 first; uv float32 CUDA tensor
+        [T, 3, 2], (u, v) in [0, 1] per corner of each triangle in its listed order, v = 0 at row 0; TextureStats).
+        Raises SurfelError (SM_ERR_CAPACITY) when the atlas would be wider than params.max_atlas_side: raise
+        params.texel_size then."""
+        p = TextureParams.defaults() if params is None else params
+        if not (isinstance(triangles, torch.Tensor) and triangles.is_cuda and triangles.dtype == torch.int32
+                and triangles.dim() == 2 and triangles.shape[1] == 3):
+            raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+        tri = triangles.contiguous()
+        views = list(views)
+        descs = (TextureViewDesc * max(len(views), 1))(*[v.desc() for v in views])
+        handle = _stream_handle(stream)
+        stats = TextureStats()
+        fn = self.lib.fn["mesh_texture"]
+        tri_ptr = C.c_void_p(tri.data_ptr()) if len(tri) else None
+        status = fn(self._h, handle, C.byref(p), tri_ptr, len(tri), descs, len(views), None, 0, 0, 0, None,
+                    C.byref(stats))
+        if status == _lib.SM_OK:   # an empty list: an empty atlas
+            return (torch.zeros((0, 0, 3), dtype=torch.uint8, device="cuda"),
+                    torch.zeros((0, 3, 2), dtype=torch.float32, device="cuda"), stats)
+        if status != _lib.SM_ERR_CAPACITY or stats.atlas_width > p.max_atlas_side:
+            raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+        W, H = int(stats.atlas_width), int(stats.atlas_height)
+        atlas = torch.empty((H, W, 3), dtype=torch.uint8, device="cuda")
+        uv = torch.empty((len(tri), 3, 2), dtype=torch.float32, device="cuda")
+        if isinstance(stream, torch.cuda.Stream):
+            atlas.record_stream(stream)
+            uv.record_stream(stream)
+        self.lib.call("mesh_texture", self._h, handle, C.byref(p), tri_ptr, len(tri), descs, len(views),
+                      C.c_void_p(atlas.data_ptr()), 3 * W, W, H, C.c_void_p(uv.data_ptr()), C.byref(stats))
+        return atlas, uv, stats
+
     def export_vertices_host(self, stream=None):
         """sm_export_vertices into host arrays: positions [n, 3] float32 (NaN rows for merged slots), colours
         [n, 3] uint8, n = surfels_size()."""
@@ -659,19 +726,34 @@ class CUDASurfelReconstruction:
         return pos[:3 * n].cpu().numpy().reshape(n, 3), col[:3 * n].cpu().numpy().reshape(n, 3)
 
     def save_mesh_obj(self, path, params: Optional[MeshParams] = None, stream=None,
-                      holes: Optional[HoleParams] = None, simplify: Optional[SimplifyParams] = None) -> MeshStats:
+                      holes: Optional[HoleParams] = None, simplify: Optional[SimplifyParams] = None,
+                      texture: Optional[TextureParams] = None,
+                      views: Optional[Sequence[TextureView]] = None) -> MeshStats:
         """The reference's SaveMeshAsOBJ (main.cc:128-175): the non-merged slots in slot order with their colour,
         and the triangles of triangulate() over them (1-based, remapped to that order). With `holes`, the
         triangles of fill_holes(holes) follow the mesh's. With `simplify`, the mesh (with its fill) goes through
-        simplify_mesh(simplify), and only the slots that are corners of its triangles are written, in slot order."""
+        simplify_mesh(simplify), and only the slots that are corners of its triangles are written, in slot order.
+        With `texture`, the final triangles are textured from `views` by texture_mesh(texture): the OBJ gets one
+        texture coordinate per triangle corner and names the material of `path` with the suffix .mtl, whose
+        diffuse map is the atlas written to `path` with the suffix .png."""
         tri, stats = self.triangulate(params, stream)
         if holes is not None:
             fill, _ = self.fill_holes(tri, holes, stream)
             tri = torch.cat([tri, fill])
         if simplify is not None:
             tri, _ = self.simplify_mesh(tri, simplify, stream)
+        uvs, material = None, None
+        if texture is not None:
+            from pathlib import Path
+            atlas, uv, _ = self.texture_mesh(tri, views or [], texture, stream)
+            png, mtl = Path(path).with_suffix(".png"), Path(path).with_suffix(".mtl")
+            image = atlas.cpu().numpy() if atlas.numel() else np.zeros((1, 1, 3), np.uint8)
+            mesh_io.write_png(png, image)
+            mesh_io.write_mtl(mtl, png.name)
+            uvs, material = uv.cpu().numpy(), mtl.name
         positions, colors = self.export_vertices_host(stream)
-        mesh_io.write_obj(path, positions, colors, tri.cpu().numpy(), referenced_only=simplify is not None)
+        mesh_io.write_obj(path, positions, colors, tri.cpu().numpy(), referenced_only=simplify is not None, uvs=uvs,
+                          material=material)
         return stats
 
     def save_point_cloud_ply(self, path, stream=None) -> int:
