@@ -448,8 +448,12 @@ class Library:
         """Calls a status-returning entry point and raises SurfelError on failure."""
         status = self.fn[name](*args)
         if status != SM_OK:
-            raise SurfelError(status, self.fn["last_error"]().decode(errors="replace"))
+            raise self.error(status)
         return status
+
+    def error(self, status: int) -> SurfelError:
+        """The SurfelError of a failed status an entry point returned, with the library's last error message."""
+        return SurfelError(status, self.fn["last_error"]().decode(errors="replace"))
 
     def version(self) -> str:
         return self.fn["version"]().decode()

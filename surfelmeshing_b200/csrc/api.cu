@@ -1,7 +1,8 @@
-// api.cu — C ABI of libsurfel_b200.so (include/surfel_b200.h): the handle that replaces
-// class vis::CUDASurfelReconstruction (APP/cuda_surfel_reconstruction.{h,cc}), the host
-// wrappers that replace APP/cuda_surfel_reconstruction_kernels.cc and the RGB-D stream
-// runner that replaces the frame loop of APP/main.cc:885-1223.
+// api.cu — the handle of libsurfel_b200.so's C ABI (include/surfel_b200.h), which replaces class
+// vis::CUDASurfelReconstruction (APP/cuda_surfel_reconstruction.{h,cc}) and the host wrappers of
+// APP/cuda_surfel_reconstruction_kernels.cc: create / destroy / reset, pre-processing, Integrate() and
+// regularisation, the count queries, state transfer, timings and profiling, and sm_configure. Every other
+// entry point is defined in the file of the feature it runs.
 
 #include <algorithm>
 #include <atomic>
@@ -158,22 +159,13 @@ LaunchScope::~LaunchScope() {
   }
 }
 
-}  // namespace smb
-
-using namespace smb;
-
-namespace {
-// Calls that would change what an open session builds on (sm_session_begin, include/surfel_b200.h).
 int RejectInSession(const char* call) {
   return SetError(SM_ERR_INVALID_ARGUMENT, (std::string(call) + ": a stream session is open on this handle (sm_session_end first)").c_str());
 }
-}  // namespace
-
-namespace smb {
 
 int FetchCounters(sm_reconstruction* r, cudaStream_t stream) {
   SM_CUDA(cudaMemcpyAsync(r->host_counters, r->d.counters, sizeof(Counters), cudaMemcpyDeviceToHost, stream));
-  if (r->reported_merge_count) {   // an open frame-graph session (pipeline.cu: SessionPush)
+  if (r->reported_merge_count) {   // an open frame-graph session (pipeline.cu: sm_session_push)
     SM_CUDA(cudaMemcpyAsync(&r->host_counters->merge_count, r->reported_merge_count, sizeof(u32), cudaMemcpyDeviceToHost,
                             stream));
   }
@@ -271,6 +263,8 @@ int IntegrateImpl(sm_reconstruction* r, cudaStream_t stream, u32 frame_index, co
 }
 
 }  // namespace smb
+
+using namespace smb;
 
 namespace {
 
@@ -505,70 +499,6 @@ int sm_preprocess(sm_reconstruction* r, void* stream, const sm_preprocess_params
   return status;
 }
 
-int sm_bilateral_filter_and_depth_cutoff(void* stream, float sigma_xy, float sigma_value_factor,
-                                         uint16_t value_to_ignore, float radius_factor, uint16_t max_depth,
-                                         float depth_valid_region_radius, int32_t width, int32_t height,
-                                         const uint16_t* in_depth, size_t in_pitch, uint16_t* out_depth,
-                                         size_t out_pitch) {
-  return StageBilateral(static_cast<cudaStream_t>(stream), sigma_xy, sigma_value_factor, value_to_ignore,
-                        radius_factor, max_depth, depth_valid_region_radius, width, height, in_depth, in_pitch,
-                        out_depth, out_pitch);
-}
-
-int sm_outlier_depth_map_fusion(void* stream, int32_t other_count, int32_t required_count, float tolerance, float fx,
-                                float fy, float cx, float cy, int32_t width, int32_t height, const uint16_t* in_depth,
-                                size_t in_pitch, const uint16_t* const* other_depths, const size_t* other_pitches,
-                                const float* others_TR_reference, uint16_t* out_depth, size_t out_pitch) {
-  return StageOutlier(static_cast<cudaStream_t>(stream), other_count, required_count, tolerance, fx, fy, cx, cy,
-                      width, height, in_depth, in_pitch, other_depths, other_pitches, others_TR_reference, out_depth,
-                      out_pitch);
-}
-
-int sm_median_filter_and_densify_depth_map(void* stream, int32_t iterations, int32_t width, int32_t height,
-                                           const uint16_t* in_depth, size_t in_pitch, uint16_t* out_depth,
-                                           size_t out_pitch, uint16_t* scratch, size_t scratch_pitch) {
-  return StageMedianDensify(static_cast<cudaStream_t>(stream), iterations, width, height, in_depth, in_pitch, out_depth,
-                            out_pitch, scratch, scratch_pitch);
-}
-
-int sm_downscale_using_median_while_excluding(void* stream, uint16_t value_to_ignore, int32_t in_width,
-                                              int32_t in_height, const uint16_t* in, size_t in_pitch,
-                                              int32_t out_width, int32_t out_height, uint16_t* out,
-                                              size_t out_pitch) {
-  return StageDownscaleMedian(static_cast<cudaStream_t>(stream), value_to_ignore, in_width, in_height, in, in_pitch,
-                              out_width, out_height, out, out_pitch);
-}
-
-int sm_color_image_pyramid(void* stream, int32_t levels, int32_t width, int32_t height, const uint8_t* in,
-                           size_t in_pitch, uint8_t* out, size_t out_pitch) {
-  return StageColorPyramid(static_cast<cudaStream_t>(stream), levels, width, height, in, in_pitch, out, out_pitch);
-}
-
-int sm_erode_depth_map(void* stream, int32_t radius, int32_t width, int32_t height, const uint16_t* in_depth,
-                       size_t in_pitch, uint16_t* out_depth, size_t out_pitch) {
-  return StageErode(static_cast<cudaStream_t>(stream), radius, width, height, in_depth, in_pitch, out_depth,
-                    out_pitch);
-}
-
-int sm_compute_normals_and_drop_bad_pixels(void* stream, float observation_angle_threshold_deg, float depth_scaling,
-                                           float fx, float fy, float cx, float cy, int32_t width, int32_t height,
-                                           const uint16_t* in_depth, size_t in_pitch, uint16_t* out_depth,
-                                           size_t out_pitch, float* out_normals, size_t normals_pitch) {
-  return StageNormals(static_cast<cudaStream_t>(stream), observation_angle_threshold_deg, depth_scaling, fx, fy, cx,
-                      cy, width, height, in_depth, in_pitch, out_depth, out_pitch,
-                      reinterpret_cast<float2*>(out_normals), normals_pitch);
-}
-
-int sm_compute_point_radii_and_remove_isolated_pixels(void* stream, float point_radius_extension_factor,
-                                                      float point_radius_clamp_factor, float depth_scaling, float fx,
-                                                      float fy, float cx, float cy, int32_t width, int32_t height,
-                                                      const uint16_t* in_depth, size_t in_pitch, float* out_radius,
-                                                      size_t radius_pitch, uint16_t* out_depth, size_t out_pitch) {
-  return StageRadii(static_cast<cudaStream_t>(stream), point_radius_extension_factor, point_radius_clamp_factor,
-                    depth_scaling, fx, fy, cx, cy, width, height, in_depth, in_pitch, out_radius, radius_pitch,
-                    out_depth, out_pitch);
-}
-
 int sm_integrate(sm_reconstruction* r, void* stream, uint32_t frame_index, const sm_integrate_params* p,
                  uint16_t* depth, size_t depth_pitch, const float* normals, size_t normals_pitch, const float* radius,
                  size_t radius_pitch, const uint8_t* color, size_t color_pitch, const float global_T_local[12],
@@ -625,137 +555,6 @@ int sm_transfer_all_to_cpu(sm_reconstruction* r, void* stream_v, uint32_t /*fram
   SM_CUDA(cudaMemcpyAsync(nz, s + SM_ROW_NORMAL_Z * st, bytes, cudaMemcpyDeviceToHost, stream));
   SM_CUDA(cudaMemcpyAsync(last_update_stamp, s + SM_ROW_LAST_UPDATE_STAMP * st, bytes, cudaMemcpyDeviceToHost, stream));
   return status;
-}
-
-int sm_transfer_delta_to_cpu(sm_reconstruction* r, void* stream, uint32_t frame_index, sm_transfer_token* token,
-                             float* x, float* y, float* z, float* radius_squared, float* nx, float* ny, float* nz,
-                             uint32_t* last_update_stamp, sm_transfer_stats* stats) {
-  if (!r || !token) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_transfer_delta_to_cpu: null argument");
-  return TransferDelta(r, static_cast<cudaStream_t>(stream), frame_index, token, x, y, z, radius_squared, nx, ny, nz,
-                       last_update_stamp, stats);
-}
-
-int sm_update_visualization_buffers(sm_reconstruction* r, void* stream, const sm_visualization_params* p,
-                                    float* vertex_buffer, uint32_t* neighbor_index_buffer, float* normal_vertex_buffer) {
-  if (!r || !p) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_update_visualization_buffers: null argument");
-  return UpdateVisualizationBuffers(r, static_cast<cudaStream_t>(stream), *p, vertex_buffer, neighbor_index_buffer,
-                                    normal_vertex_buffer);
-}
-
-int sm_render_surfels(sm_reconstruction* r, void* stream, const sm_render_params* p, const float view_T_global[12],
-                      float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch, float* normal,
-                      size_t normal_pitch, uint32_t* index, size_t index_pitch) {
-  if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_surfels: null argument");
-  return RenderSurfels(r, static_cast<cudaStream_t>(stream), *p, view_T_global, depth, depth_pitch, color, color_pitch,
-                       normal, normal_pitch, index, index_pitch);
-}
-
-int sm_render_mesh(sm_reconstruction* r, void* stream, const sm_render_params* p, const float view_T_global[12],
-                   const uint32_t* triangles, uint64_t triangle_count, int32_t flags, float* depth, size_t depth_pitch,
-                   uint8_t* color, size_t color_pitch, float* normal, size_t normal_pitch, uint32_t* index,
-                   size_t index_pitch) {
-  if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_mesh: null argument");
-  return RenderMesh(r, static_cast<cudaStream_t>(stream), *p, view_T_global, triangles, triangle_count, flags, depth,
-                    depth_pitch, color, color_pitch, normal, normal_pitch, index, index_pitch);
-}
-
-void sm_default_track_params(sm_track_params* p) {
-  p->levels = 3;
-  p->iterations[0] = 4; p->iterations[1] = 5; p->iterations[2] = 10; p->iterations[3] = 0;
-  p->max_point_distance = 0.05f;
-  p->max_normal_angle_deg = 20.0f;
-  p->min_inlier_fraction = 0.1f;
-  p->convergence_rotation = 1e-5f;
-  p->convergence_translation = 1e-5f;
-  p->model_source = SM_TRACK_CLOUD;
-}
-
-int sm_track_frame(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_preprocess_params* pp,
-                   const uint16_t* depth, size_t depth_pitch, const float global_T_guess[12], float global_T_out[12],
-                   sm_track_result* result) {
-  if (!r || !tp || !pp || !depth || !global_T_guess || !global_T_out || !result)
-    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_frame: null argument");
-  return TrackFrame(r, static_cast<cudaStream_t>(stream), *tp, *pp, depth, depth_pitch, global_T_guess, global_T_out,
-                    result);
-}
-
-int sm_track_linearize(sm_reconstruction* r, void* stream, const sm_track_params* tp, int32_t level,
-                       float depth_scaling, const uint16_t* live_depth, size_t live_pitch, const float* model_depth,
-                       size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
-                       const float model_T_live[12], double out_system[27], uint32_t* out_inliers) {
-  if (!r || !tp || !live_depth || !model_depth || !model_normal || !model_T_live || !out_system || !out_inliers)
-    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_linearize: null argument");
-  return TrackLinearize(r, static_cast<cudaStream_t>(stream), *tp, level, depth_scaling, live_depth, live_pitch,
-                        model_depth, model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system,
-                        out_inliers);
-}
-
-void sm_default_track_rgbd_params(sm_track_rgbd_params* p) {
-  p->photometric_weight = 1e-4f;
-  p->max_intensity_residual = 40.0f;
-  p->min_gradient = 2.0f;
-}
-
-int sm_track_frame_rgbd(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_preprocess_params* pp,
-                        const sm_track_rgbd_params* rp, const uint16_t* depth, size_t depth_pitch, const uint8_t* color,
-                        size_t color_pitch, const float global_T_guess[12], float global_T_out[12],
-                        sm_track_rgbd_result* result) {
-  if (!r || !tp || !pp || !rp || !depth || !color || !global_T_guess || !global_T_out || !result)
-    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_frame_rgbd: null argument");
-  const TrackColor c{rp, color, color_pitch, nullptr, 0};
-  return TrackFrameRGBD(r, static_cast<cudaStream_t>(stream), *tp, *pp, c, depth, depth_pitch, global_T_guess,
-                        global_T_out, result);
-}
-
-int sm_track_linearize_rgbd(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_track_rgbd_params* rp,
-                            int32_t level, float depth_scaling, const uint16_t* live_depth, size_t live_pitch,
-                            const uint8_t* live_color, size_t live_color_pitch, const float* model_depth,
-                            size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
-                            const uint8_t* model_color, size_t model_color_pitch, const float model_T_live[12],
-                            double out_system[27], double* out_sum_rc2, uint32_t* out_inliers,
-                            uint32_t* out_photometric_inliers) {
-  if (!r || !tp || !rp || !live_depth || !live_color || !model_depth || !model_normal || !model_color || !model_T_live ||
-      !out_system || !out_sum_rc2 || !out_inliers || !out_photometric_inliers)
-    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_linearize_rgbd: null argument");
-  const TrackColor c{rp, live_color, live_color_pitch, model_color, model_color_pitch};
-  return TrackLinearizeRGBD(r, static_cast<cudaStream_t>(stream), *tp, c, level, depth_scaling, live_depth, live_pitch,
-                            model_depth, model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system,
-                            out_sum_rc2, out_inliers, out_photometric_inliers);
-}
-
-void sm_default_mesh_params(sm_mesh_params* p) {
-  p->neighbor_radius_factor = 2.0f;
-  p->max_angle_between_normals_deg = 90.0f;
-  p->max_triangle_angle_deg = 170.0f;
-}
-
-int sm_triangulate(sm_reconstruction* r, void* stream, const sm_mesh_params* p, uint32_t* triangles, uint64_t capacity,
-                   sm_mesh_stats* stats) {
-  if (!r || !p || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_triangulate: null argument");
-  return Triangulate(r, static_cast<cudaStream_t>(stream), *p, triangles, capacity, stats);
-}
-
-int sm_mesh_update(sm_reconstruction* r, void* stream, const sm_mesh_params* p, sm_mesh_update_stats* stats) {
-  if (!r || !p || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_update: null argument");
-  return MeshUpdate(r, static_cast<cudaStream_t>(stream), *p, stats);
-}
-
-int sm_mesh_read(sm_reconstruction* r, void* stream, int32_t which, uint32_t* triangles, uint64_t capacity,
-                 uint64_t* count) {
-  if (!r || !count) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_read: null argument");
-  return MeshRead(r, static_cast<cudaStream_t>(stream), which, triangles, capacity, count);
-}
-
-void sm_default_hole_params(sm_hole_params* p) {
-  p->max_hole_edges = 8;
-  p->max_angle_between_normals_deg = 90.0f;
-  p->max_triangle_angle_deg = 180.0f;
-}
-
-int sm_mesh_fill_holes(sm_reconstruction* r, void* stream, const sm_hole_params* p, const uint32_t* triangles,
-                       uint64_t count, uint32_t* fill, uint64_t capacity, sm_hole_stats* stats) {
-  if (!r || !p || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_fill_holes: null argument");
-  return FillHoles(r, static_cast<cudaStream_t>(stream), *p, triangles, count, fill, capacity, stats);
 }
 
 int sm_export_vertices(sm_reconstruction* r, void* stream, float* position_buffer, uint8_t* color_buffer) {
@@ -918,50 +717,6 @@ int sm_timeline_read(sm_reconstruction* r, uint64_t* out, int32_t frames) {
   }
   SM_CUDA(cudaMemcpy2D(out, row, r->d.timeline, device_row, device_row, frames, cudaMemcpyDeviceToHost));
   return SM_OK;
-}
-
-// The frame loop of APP/main.cc:885-1223 on a synthetic stream (pipeline.cu).
-int sm_stream_run(sm_reconstruction* r, void* stream_v, const sm_stream_desc* s, const sm_preprocess_params* pp,
-                  const sm_integrate_params* ip, int32_t first_frame, int32_t last_frame, sm_stream_stats* stats) {
-  if (!r || !s || !pp || !ip) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_stream_run: null argument");
-  if (r->session) return RejectInSession("sm_stream_run");
-  return StreamRun(r, static_cast<cudaStream_t>(stream_v), s, pp, ip, first_frame, last_frame, stats);
-}
-
-int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32_t frame_count,
-                                 const float* global_T_frame, const float* frame_T_global, int32_t frame, float* out) {
-  if (!global_T_frame || !frame_T_global || !out) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: null argument");
-  if (other_count < 2 || other_count > 8 || other_count % 2 != 0)
-    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: other_count must be 2, 4, 6 or 8");
-  const int half = other_count / 2;
-  if (frame < half || frame >= frame_count - half)
-    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: the frame needs other_count/2 frames on both sides (main.cc:987-992)");
-  const float* ref = global_T_frame + 12 * static_cast<size_t>(frame);
-  for (int i = 0; i < half; ++i) {
-    OutlierFilterTransform(depth_scaling, ref, frame_T_global + 12 * static_cast<size_t>(frame - (i + 1)), out + 12 * i);
-    OutlierFilterTransform(depth_scaling, ref, frame_T_global + 12 * static_cast<size_t>(frame + (i + 1)), out + 12 * (half + i));
-  }
-  return SM_OK;
-}
-
-// An incremental session on the handle (pipeline.cu).
-int sm_session_begin(sm_reconstruction* r, void* stream, const sm_preprocess_params* pp, const sm_integrate_params* ip,
-                     int32_t frame_width, int32_t frame_height, uint32_t first_frame_index) {
-  if (!r || !pp || !ip) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_begin: null argument");
-  return SessionBegin(r, static_cast<cudaStream_t>(stream), pp, ip, frame_width, frame_height, first_frame_index);
-}
-
-int sm_session_push(sm_reconstruction* r, const uint16_t* depth, size_t depth_pitch, const uint8_t* color,
-                    size_t color_pitch, int32_t frame_on_host, const float global_T_frame[12],
-                    const float frame_T_global[12], sm_session_status* status) {
-  if (!r) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_push: null argument");
-  return SessionPush(r, depth, depth_pitch, color, color_pitch, frame_on_host != 0, global_T_frame, frame_T_global,
-                     status);
-}
-
-int sm_session_end(sm_reconstruction* r, sm_stream_stats* stats) {
-  if (!r) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_end: null argument");
-  return SessionEnd(r, stats);
 }
 
 // Named tuning / experiment knobs of a handle (no counterpart in the reference):

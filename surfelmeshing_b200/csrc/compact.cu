@@ -145,8 +145,14 @@ void FreeCompactBuffers(sm_reconstruction* r) {
   r->compact = nullptr;
 }
 
-int Compact(sm_reconstruction* r, cudaStream_t stream, uint32_t* old_to_new, uint64_t map_capacity,
-            sm_compact_stats* stats) {
+}  // namespace smb
+
+using namespace smb;
+
+extern "C" int sm_compact(sm_reconstruction* r, void* stream_v, uint32_t* old_to_new, uint64_t map_capacity,
+                          sm_compact_stats* stats) {
+  if (!r) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_compact: null handle");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   r->last_stream = stream;
   int status = FetchCounters(r, stream);
   if (status == SM_ERR_CUDA) return status;   // (the sticky cap-overflow flag is no reason not to compact)
@@ -250,12 +256,4 @@ int Compact(sm_reconstruction* r, cudaStream_t stream, uint32_t* old_to_new, uin
   out.mesh_remapped = mesh_remapped;
   if (stats) *stats = out;
   return SM_OK;
-}
-
-}  // namespace smb
-
-extern "C" int sm_compact(sm_reconstruction* r, void* stream, uint32_t* old_to_new, uint64_t map_capacity,
-                          sm_compact_stats* stats) {
-  if (!r) return smb::SetError(SM_ERR_INVALID_ARGUMENT, "sm_compact: null handle");
-  return smb::Compact(r, static_cast<cudaStream_t>(stream), old_to_new, map_capacity, stats);
 }

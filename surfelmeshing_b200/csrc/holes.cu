@@ -31,7 +31,6 @@ namespace smb {
 
 namespace {
 
-constexpr int kBlock = 256;
 constexpr int kMaxHole = SM_MESH_MAX_HOLE;
 constexpr u32 kNone = 0xFFFFFFFFu;
 
@@ -371,12 +370,6 @@ int EnsureHoleScratch(HoleScratch& s, u32 edges) {
   return SM_OK;
 }
 
-float CosDegrees(float deg) { return static_cast<float>(std::cos(static_cast<double>(deg) * (M_PI / 180.0))); }
-
-int Grid(u64 items, int sm_count) {
-  return static_cast<int>(std::max<u64>(1, std::min<u64>((items + kBlock - 1) / kBlock, 8ull * sm_count)));
-}
-
 }  // namespace
 
 void FreeHoleBuffers(sm_reconstruction* r) {
@@ -392,17 +385,30 @@ void FreeHoleBuffers(sm_reconstruction* r) {
   r->holes = nullptr;
 }
 
-int FillHoles(sm_reconstruction* r, cudaStream_t stream, const sm_hole_params& p, const uint32_t* triangles,
-              uint64_t count, uint32_t* fill, uint64_t capacity, sm_hole_stats* stats) {
+}  // namespace smb
+
+using namespace smb;
+
+extern "C" {
+
+void sm_default_hole_params(sm_hole_params* p) {
+  p->max_hole_edges = 8;
+  p->max_angle_between_normals_deg = 90.0f;
+  p->max_triangle_angle_deg = 180.0f;
+}
+
+int sm_mesh_fill_holes(sm_reconstruction* r, void* stream_v, const sm_hole_params* params, const uint32_t* triangles,
+                       uint64_t count, uint32_t* fill, uint64_t capacity, sm_hole_stats* stats) {
+  if (!r || !params || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_fill_holes: null argument");
   auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_mesh_fill_holes: ") + why).c_str()); };
-  auto angle_ok = [](float deg) { return std::isfinite(deg) && deg > 0.f && deg <= 180.f; };
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const sm_hole_params& p = *params;
   *stats = sm_hole_stats{};
   if (p.max_hole_edges < 3 || p.max_hole_edges > kMaxHole) return bad("max_hole_edges must be in [3, SM_MESH_MAX_HOLE]");
-  if (!angle_ok(p.max_angle_between_normals_deg) || !angle_ok(p.max_triangle_angle_deg))
+  if (!AngleInRange(p.max_angle_between_normals_deg) || !AngleInRange(p.max_triangle_angle_deg))
     return bad("angles must be in (0, 180] degrees");
-  if (!triangles && count > 0) return bad("triangles is NULL with a count > 0");
-  if (!fill && capacity > 0) return bad("fill is NULL with a capacity > 0");
-  if (count >= kMaxMeshTriangles) return bad("2^28 triangles or more");
+  if (const char* why = TriangleListError(triangles, count, !fill && capacity > 0 ? "fill is NULL with a capacity > 0" : nullptr))
+    return bad(why);
   r->last_stream = stream;
   int status = FetchCounters(r, stream);
   if (status == SM_ERR_CUDA) return status;   // (a surfel-cap overflow of an earlier frame does not matter here)
@@ -502,4 +508,4 @@ int FillHoles(sm_reconstruction* r, cudaStream_t stream, const sm_hole_params& p
   return CheckLaunch("fill holes");
 }
 
-}  // namespace smb
+}  // extern "C"

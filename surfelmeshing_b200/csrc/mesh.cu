@@ -23,6 +23,7 @@
 
 #include "sm_handle.cuh"
 #include "sm_knn.cuh"
+#include "sm_mesh_edges.cuh"
 
 namespace smb {
 
@@ -80,8 +81,6 @@ struct MeshArgs {
 
 __device__ __forceinline__ float dot2(float ax, float ay, float bx, float by) { return fadd(fmul(ax, bx), fmul(ay, by)); }
 __device__ __forceinline__ float cross2(float ax, float ay, float bx, float by) { return fsub(fmul(ax, by), fmul(ay, bx)); }
-__device__ __forceinline__ float dot3p(float3 a, float3 b) { return fadd(fadd(fmul(a.x, b.x), fmul(a.y, b.y)), fmul(a.z, b.z)); }
-__device__ __forceinline__ float3 sub3(float3 a, float3 b) { return make_float3(fsub(a.x, b.x), fsub(a.y, b.y), fsub(a.z, b.z)); }
 
 __device__ __forceinline__ float3 position(const MeshArgs& a, u32 i) {
   return make_float3(SM_S(SM_ROW_SMOOTH_X, i), SM_S(SM_ROW_SMOOTH_Y, i), SM_S(SM_ROW_SMOOTH_Z, i));
@@ -702,18 +701,28 @@ int CheckMeshParams(const sm_mesh_params& p, const char* who) {
   const float f = p.neighbor_radius_factor;
   const float f2 = f * f;
   if (!std::isfinite(f) || !(f > 0.f) || !std::isfinite(f2)) return bad("neighbor_radius_factor must be finite and > 0");
-  auto angle_ok = [](float deg) { return std::isfinite(deg) && deg > 0.f && deg <= 180.f; };
-  if (!angle_ok(p.max_angle_between_normals_deg) || !angle_ok(p.max_triangle_angle_deg))
+  if (!AngleInRange(p.max_angle_between_normals_deg) || !AngleInRange(p.max_triangle_angle_deg))
     return bad("angles must be in (0, 180] degrees");
   return SM_OK;
 }
 
-float CosDegrees(float deg) { return static_cast<float>(std::cos(static_cast<double>(deg) * (M_PI / 180.0))); }
-
 }  // namespace
 
-int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, uint32_t* triangles,
-                uint64_t capacity, sm_mesh_stats* stats) {
+}  // namespace smb
+
+using namespace smb;
+
+extern "C" void sm_default_mesh_params(sm_mesh_params* p) {
+  p->neighbor_radius_factor = 2.0f;
+  p->max_angle_between_normals_deg = 90.0f;
+  p->max_triangle_angle_deg = 170.0f;
+}
+
+extern "C" int sm_triangulate(sm_reconstruction* r, void* stream_v, const sm_mesh_params* params, uint32_t* triangles,
+                              uint64_t capacity, sm_mesh_stats* stats) {
+  if (!r || !params || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_triangulate: null argument");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const sm_mesh_params& p = *params;
   const int checked = CheckMeshParams(p, "sm_triangulate");
   if (checked != SM_OK) return checked;
   if (!triangles && capacity > 0)
@@ -797,6 +806,8 @@ int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params&
   }
   return CheckLaunch("triangulate");
 }
+
+namespace smb {
 
 // The persistent mesh of sm_mesh_update. Per-slot arrays hold `slots` entries and grow (keeping what the previous
 // update left) with surfels_size(); the triangle arrays grow with the mesh and its deltas.
@@ -972,7 +983,13 @@ void FreeMeshBuffers(sm_reconstruction* r) {
   r->mesh = nullptr;
 }
 
-int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, sm_mesh_update_stats* stats) {
+}  // namespace smb
+
+extern "C" int sm_mesh_update(sm_reconstruction* r, void* stream_v, const sm_mesh_params* params,
+                              sm_mesh_update_stats* stats) {
+  if (!r || !params || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_update: null argument");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const sm_mesh_params& p = *params;
   int status = CheckMeshParams(p, "sm_mesh_update");
   if (status != SM_OK) return status;
   *stats = sm_mesh_update_stats{};
@@ -1143,6 +1160,8 @@ int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& 
   return SM_OK;
 }
 
+namespace smb {
+
 namespace {
 
 // words[0] = 1 if a slot removed by sm_compact was present at the last update, words[1] = removed slots below n_prev.
@@ -1209,8 +1228,12 @@ int MeshCompact(sm_reconstruction* r, cudaStream_t stream, const u32* map, u32 n
   return SM_OK;
 }
 
-int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t* triangles, uint64_t capacity,
-             uint64_t* count) {
+}  // namespace smb
+
+extern "C" int sm_mesh_read(sm_reconstruction* r, void* stream_v, int32_t which, uint32_t* triangles,
+                            uint64_t capacity, uint64_t* count) {
+  if (!r || !count) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_read: null argument");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_mesh_read: ") + why).c_str()); };
   if (which != SM_MESH_ALL && which != SM_MESH_ADDED && which != SM_MESH_REMOVED) return bad("unknown `which`");
   if (!triangles && capacity > 0) return bad("triangles is NULL with a capacity > 0");
@@ -1227,5 +1250,3 @@ int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t*
   if (size > 0) SM_CUDA(cudaMemcpyAsync(triangles, src, sizeof(uint3) * size, cudaMemcpyDeviceToDevice, stream));
   return SM_OK;
 }
-
-}  // namespace smb

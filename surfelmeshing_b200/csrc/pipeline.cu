@@ -653,8 +653,17 @@ double MillisecondsSince(std::chrono::steady_clock::time_point t0) {
 
 }  // namespace
 
-int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
-              const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats) {
+}  // namespace smb
+
+using namespace smb;
+
+// The frame loop of APP/main.cc:885-1223 on a synthetic stream.
+extern "C" int sm_stream_run(sm_reconstruction* r, void* stream_v, const sm_stream_desc* s,
+                             const sm_preprocess_params* pp, const sm_integrate_params* ip, int32_t first_frame,
+                             int32_t last_frame, sm_stream_stats* stats) {
+  if (!r || !s || !pp || !ip) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_stream_run: null argument");
+  if (r->session) return RejectInSession("sm_stream_run");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   RunContext c;
   c.s = s;
   int status = SetupContext(c, r, pp, ip, s->width, s->height);
@@ -689,6 +698,10 @@ int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s
 // incremental sessions (sm_session_begin / push / end)
 // ---------------------------------------------------------------------------------------------
 
+namespace smb {
+
+namespace {
+
 void OutlierFilterTransform(float depth_scaling, const float* global_T_ref, const float* other_T_global, float* out) {
   // scale(other_T_global) . scale(global_T_ref), both 3x4 with an implicit last row (0 0 0 1); the
   // translations are multiplied by depth_scaling. Every product and sum in double, in the order the header gives.
@@ -707,6 +720,8 @@ void OutlierFilterTransform(float depth_scaling, const float* global_T_ref, cons
     }
   }
 }
+
+}  // namespace
 
 struct StreamSession {
   RunContext c;
@@ -741,7 +756,7 @@ void FreeSession(StreamSession* ss) {
   delete ss;
 }
 
-// A CUDA error inside a session: leave no work in flight and close it, as StreamRun's failure path does.
+// A CUDA error inside a session: leave no work in flight and close it, as sm_stream_run's failure path does.
 int AbortSession(sm_reconstruction* r, int status) {
   cudaDeviceSynchronize();
   r->reported_merge_count = nullptr;
@@ -754,8 +769,14 @@ constexpr int kMaxSessionFrameIndex = 1 << 30;   // frame indices stay far from 
 
 }  // namespace
 
-int SessionBegin(sm_reconstruction* r, cudaStream_t stream, const sm_preprocess_params* pp,
-                 const sm_integrate_params* ip, int width, int height, uint32_t first_frame_index) {
+}  // namespace smb
+
+// An incremental session on the handle.
+extern "C" int sm_session_begin(sm_reconstruction* r, void* stream_v, const sm_preprocess_params* pp,
+                                const sm_integrate_params* ip, int32_t width, int32_t height,
+                                uint32_t first_frame_index) {
+  if (!r || !pp || !ip) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_begin: null argument");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   if (r->session) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_begin: a stream session is already open on this handle");
   const int K = pp->outlier_filtering_frame_count;
   if (K < 2 || K > 8 || K % 2 != 0) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_begin: outlier_filtering_frame_count must be 2, 4, 6 or 8");
@@ -800,8 +821,11 @@ int SessionBegin(sm_reconstruction* r, cudaStream_t stream, const sm_preprocess_
   return SM_OK;
 }
 
-int SessionPush(sm_reconstruction* r, const u16* depth, size_t depth_pitch, const uint8_t* color, size_t color_pitch,
-                bool on_host, const float* global_T_frame, const float* frame_T_global, sm_session_status* out) {
+extern "C" int sm_session_push(sm_reconstruction* r, const uint16_t* depth, size_t depth_pitch, const uint8_t* color,
+                               size_t color_pitch, int32_t frame_on_host, const float global_T_frame[12],
+                               const float frame_T_global[12], sm_session_status* out) {
+  if (!r) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_push: null argument");
+  const bool on_host = frame_on_host != 0;
   StreamSession* ss = r->session;
   if (!ss) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_push: no stream session is open on this handle (sm_session_begin)");
   RunContext& c = ss->c;
@@ -895,6 +919,8 @@ int SessionPush(sm_reconstruction* r, const u16* depth, size_t depth_pitch, cons
   return SM_OK;
 }
 
+namespace smb {
+
 int SessionEnd(sm_reconstruction* r, sm_stream_stats* stats) {
   StreamSession* ss = r->session;
   if (!ss) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_end: no stream session is open on this handle (sm_session_begin)");
@@ -969,3 +995,28 @@ void FreeRunBuffers(sm_reconstruction* r) {
 }
 
 }  // namespace smb
+
+extern "C" {
+
+int sm_session_end(sm_reconstruction* r, sm_stream_stats* stats) {
+  if (!r) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_session_end: null argument");
+  return SessionEnd(r, stats);
+}
+
+int sm_outlier_filter_transforms(int32_t other_count, float depth_scaling, int32_t frame_count,
+                                 const float* global_T_frame, const float* frame_T_global, int32_t frame, float* out) {
+  if (!global_T_frame || !frame_T_global || !out) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: null argument");
+  if (other_count < 2 || other_count > 8 || other_count % 2 != 0)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: other_count must be 2, 4, 6 or 8");
+  const int half = other_count / 2;
+  if (frame < half || frame >= frame_count - half)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_outlier_filter_transforms: the frame needs other_count/2 frames on both sides (main.cc:987-992)");
+  const float* ref = global_T_frame + 12 * static_cast<size_t>(frame);
+  for (int i = 0; i < half; ++i) {
+    OutlierFilterTransform(depth_scaling, ref, frame_T_global + 12 * static_cast<size_t>(frame - (i + 1)), out + 12 * i);
+    OutlierFilterTransform(depth_scaling, ref, frame_T_global + 12 * static_cast<size_t>(frame + (i + 1)), out + 12 * (half + i));
+  }
+  return SM_OK;
+}
+
+}  // extern "C"

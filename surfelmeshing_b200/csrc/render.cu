@@ -645,3 +645,26 @@ void FreeRenderBuffers(sm_reconstruction* r) {
 }
 
 }  // namespace smb
+
+using namespace smb;
+
+extern "C" {
+
+int sm_render_surfels(sm_reconstruction* r, void* stream, const sm_render_params* p, const float view_T_global[12],
+                      float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch, float* normal,
+                      size_t normal_pitch, uint32_t* index, size_t index_pitch) {
+  if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_surfels: null argument");
+  return RenderSurfels(r, static_cast<cudaStream_t>(stream), *p, view_T_global, depth, depth_pitch, color, color_pitch,
+                       normal, normal_pitch, index, index_pitch);
+}
+
+int sm_render_mesh(sm_reconstruction* r, void* stream, const sm_render_params* p, const float view_T_global[12],
+                   const uint32_t* triangles, uint64_t triangle_count, int32_t flags, float* depth, size_t depth_pitch,
+                   uint8_t* color, size_t color_pitch, float* normal, size_t normal_pitch, uint32_t* index,
+                   size_t index_pitch) {
+  if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_mesh: null argument");
+  return RenderMesh(r, static_cast<cudaStream_t>(stream), *p, view_T_global, triangles, triangle_count, flags, depth,
+                    depth_pitch, color, color_pitch, normal, normal_pitch, index, index_pitch);
+}
+
+}  // extern "C"

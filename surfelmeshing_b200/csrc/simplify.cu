@@ -38,7 +38,6 @@ namespace smb {
 
 namespace {
 
-constexpr int kBlock = 256;
 constexpr int kMaxValence = SM_MESH_MAX_VALENCE;
 constexpr u32 kNone = 0xFFFFFFFFu;   // no slot; also every corner of a deleted triangle
 constexpr u64 kNoKey = ~0ull;
@@ -432,12 +431,6 @@ int EnsureSortScratch(SimplifyScratch& s) {
   return SM_OK;
 }
 
-float CosDegrees(float deg) { return static_cast<float>(std::cos(static_cast<double>(deg) * (M_PI / 180.0))); }
-
-int Grid(u64 items, int sm_count) {
-  return static_cast<int>(std::max<u64>(1, std::min<u64>((items + kBlock - 1) / kBlock, 8ull * sm_count)));
-}
-
 int BitsFor(u32 n) {
   int b = 0;
   while (b < 32 && (n >> b) != 0) ++b;
@@ -466,24 +459,37 @@ void FreeSimplifyBuffers(sm_reconstruction* r) {
   r->simplify = nullptr;
 }
 
-int Simplify(sm_reconstruction* r, cudaStream_t stream, const sm_simplify_params& p, const uint32_t* triangles,
-             uint64_t count, uint32_t* out, uint64_t capacity, sm_simplify_stats* stats) {
+}  // namespace smb
+
+using namespace smb;
+
+extern "C" {
+
+void sm_default_simplify_params(sm_simplify_params* p) {
+  p->target_triangles = 0;
+  p->max_cost = 1e-6;
+  p->max_angle_between_normals_deg = 90.0f;
+  p->max_triangle_angle_deg = 170.0f;
+  p->max_rounds = 64;
+  p->reserved = 0;
+}
+
+int sm_mesh_simplify(sm_reconstruction* r, void* stream_v, const sm_simplify_params* params, const uint32_t* triangles,
+                     uint64_t count, uint32_t* out, uint64_t capacity, sm_simplify_stats* stats) {
+  if (!r || !params || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_simplify: null argument");
   auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_mesh_simplify: ") + why).c_str()); };
-  auto angle_ok = [](float deg) { return std::isfinite(deg) && deg > 0.f && deg <= 180.f; };
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const sm_simplify_params& p = *params;
   *stats = sm_simplify_stats{};
   if (!(p.max_cost >= 0.0)) return bad("max_cost must be >= 0");
-  if (!angle_ok(p.max_angle_between_normals_deg) || !angle_ok(p.max_triangle_angle_deg))
+  if (!AngleInRange(p.max_angle_between_normals_deg) || !AngleInRange(p.max_triangle_angle_deg))
     return bad("angles must be in (0, 180] degrees");
   if (p.max_rounds < 0 || p.max_rounds > SM_SIMPLIFY_MAX_ROUNDS) return bad("max_rounds must be in [0, SM_SIMPLIFY_MAX_ROUNDS]");
-  if (!triangles && count > 0) return bad("triangles is NULL with a count > 0");
-  if (!out && capacity > 0) return bad("out is NULL with a capacity > 0");
-  if (count >= kMaxMeshTriangles) return bad("2^28 triangles or more");
-  if (count > 0 && capacity > 0) {
-    const uintptr_t t0 = reinterpret_cast<uintptr_t>(triangles), t1 = t0 + 12 * count;
-    const uintptr_t o0 = reinterpret_cast<uintptr_t>(out);
-    const uintptr_t o1 = capacity > (UINTPTR_MAX - o0) / 12 ? UINTPTR_MAX : o0 + 12 * capacity;
-    if (t0 < o1 && o0 < t1) return bad("out overlaps triangles");
-  }
+  if (const char* why = TriangleListError(triangles, count, !out && capacity > 0 ? "out is NULL with a capacity > 0" : nullptr))
+    return bad(why);
+  // (12 x capacity can pass 2^64: saturated, like the end of the range)
+  if (count > 0 && capacity > 0 && Overlap(triangles, 12 * count, out, capacity > UINT64_MAX / 12 ? UINT64_MAX : 12 * capacity))
+    return bad("out overlaps triangles");
   r->last_stream = stream;
   int status = FetchCounters(r, stream);
   if (status == SM_ERR_CUDA) return status;   // (a surfel-cap overflow of an earlier frame does not matter here)
@@ -632,19 +638,4 @@ int Simplify(sm_reconstruction* r, cudaStream_t stream, const sm_simplify_params
   return CheckLaunch("simplify");
 }
 
-}  // namespace smb
-
-void sm_default_simplify_params(sm_simplify_params* p) {
-  p->target_triangles = 0;
-  p->max_cost = 1e-6;
-  p->max_angle_between_normals_deg = 90.0f;
-  p->max_triangle_angle_deg = 170.0f;
-  p->max_rounds = 64;
-  p->reserved = 0;
-}
-
-int sm_mesh_simplify(sm_reconstruction* r, void* stream, const sm_simplify_params* p, const uint32_t* triangles,
-                     uint64_t count, uint32_t* out, uint64_t capacity, sm_simplify_stats* stats) {
-  if (!r || !p || !stats) return smb::SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_simplify: null argument");
-  return smb::Simplify(r, static_cast<cudaStream_t>(stream), *p, triangles, count, out, capacity, stats);
-}
+}  // extern "C"

@@ -1,5 +1,5 @@
-// sm_handle.cuh — the handle behind the C ABI (struct sm_reconstruction), shared by api.cu
-// (entry points) and pipeline.cu (the RGB-D stream runner and its frame graph).
+// sm_handle.cuh — the handle behind the C ABI (struct sm_reconstruction), shared by api.cu, which
+// creates it, and the files whose entry points work on it.
 #pragma once
 
 #include <vector>
@@ -135,6 +135,8 @@ struct sm_reconstruction {
 
 namespace smb {
 // api.cu
+// Calls that would change what an open session builds on (sm_session_begin, include/surfel_b200.h).
+int RejectInSession(const char* call);
 int FetchCounters(sm_reconstruction* r, cudaStream_t stream);
 FrameParams MakeFrameParams(const sm_reconstruction* r, u32 frame_index, int count_slot, const sm_integrate_params& p,
                             u16* depth, size_t depth_pitch, const u16* depth_pre, size_t depth_pre_pitch,
@@ -151,11 +153,6 @@ unsigned long long LaunchCount();
 void RecordOperation(sm_reconstruction* r, int stamp_threshold);   // one Integrate() / Regularize(): ++op_epoch
 uint64_t NextStateGeneration();   // 1, 2, 3, ... across every handle of the process
 void FreeTransferBuffers(sm_reconstruction* r);
-int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_index, sm_transfer_token* token, float* x,
-                  float* y, float* z, float* radius_squared, float* nx, float* ny, float* nz,
-                  uint32_t* last_update_stamp, sm_transfer_stats* stats);
-int UpdateVisualizationBuffers(sm_reconstruction* r, cudaStream_t stream, const sm_visualization_params& p, float* vertex,
-                               uint32_t* neighbor_index, float* normal_vertex);
 // render.cu
 int RenderSurfels(sm_reconstruction* r, cudaStream_t stream, const sm_render_params& p, const float* view_T_global,
                   float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch, float* normal,
@@ -170,10 +167,6 @@ const char* RenderCameraError(const sm_render_params& p, const float* view_T_glo
 // track.cu
 int TrackFrame(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const sm_preprocess_params& pp,
                const u16* depth, size_t depth_pitch, const float* guess, float* pose_out, sm_track_result* result);
-int TrackLinearize(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, int level, float depth_scaling,
-                   const u16* live, size_t live_pitch, const float* model_depth, size_t model_depth_pitch,
-                   const float* model_normal, size_t model_normal_pitch, const float* model_T_live, double* out_system,
-                   uint32_t* out_inliers);
 // The photometric part of an RGB-D call (sm_track_frame_rgbd / sm_track_linearize_rgbd): the parameters, the raw
 // live colour and, for the linearisation alone, the caller's model colour.
 struct TrackColor {
@@ -184,35 +177,16 @@ struct TrackColor {
 int TrackFrameRGBD(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const sm_preprocess_params& pp,
                    const TrackColor& color, const u16* depth, size_t depth_pitch, const float* guess, float* pose_out,
                    sm_track_rgbd_result* result);
-int TrackLinearizeRGBD(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const TrackColor& color,
-                       int level, float depth_scaling, const u16* live, size_t live_pitch, const float* model_depth,
-                       size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
-                       const float* model_T_live, double* out_system, double* out_sum_rc2, uint32_t* out_inliers,
-                       uint32_t* out_photometric_inliers);
 void FreeTrackBuffers(sm_reconstruction* r);
 // mesh.cu
-int Triangulate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, uint32_t* triangles,
-                uint64_t capacity, sm_mesh_stats* stats);
 void FreeMeshBuffers(sm_reconstruction* r);
-int MeshUpdate(sm_reconstruction* r, cudaStream_t stream, const sm_mesh_params& p, sm_mesh_update_stats* stats);
-int MeshRead(sm_reconstruction* r, cudaStream_t stream, int32_t which, uint32_t* triangles, uint64_t capacity,
-             uint64_t* count);
 // holes.cu
-int FillHoles(sm_reconstruction* r, cudaStream_t stream, const sm_hole_params& p, const uint32_t* triangles,
-              uint64_t count, uint32_t* fill, uint64_t capacity, sm_hole_stats* stats);
 void FreeHoleBuffers(sm_reconstruction* r);
 // compact.cu
-int Compact(sm_reconstruction* r, cudaStream_t stream, uint32_t* old_to_new, uint64_t map_capacity,
-            sm_compact_stats* stats);
 void FreeCompactBuffers(sm_reconstruction* r);
 // simplify.cu
-int Simplify(sm_reconstruction* r, cudaStream_t stream, const sm_simplify_params& p, const uint32_t* triangles,
-             uint64_t count, uint32_t* out, uint64_t capacity, sm_simplify_stats* stats);
 void FreeSimplifyBuffers(sm_reconstruction* r);
 // texture.cu
-int Texture(sm_reconstruction* r, cudaStream_t stream, const sm_texture_params& p, const uint32_t* triangles,
-            uint64_t count, const sm_texture_view* views, int32_t view_count, uint8_t* atlas, size_t atlas_pitch,
-            int32_t atlas_capacity_width, int32_t atlas_capacity_height, float* uv, sm_texture_stats* stats);
 void FreeTextureBuffers(sm_reconstruction* r);
 // In place: word w of record k' = word w of record i, old_to_new[i] = k' < kept, for every word of records of
 // `record_words` 32-bit words (bytes) over slots [0, n), one word at a time through `scratch` (>= kept words).
@@ -226,17 +200,9 @@ int CompactBytes(cudaStream_t stream, int sm_count, const u32* old_to_new, u32 n
 int MeshCompact(sm_reconstruction* r, cudaStream_t stream, const u32* old_to_new, u32 n, u32* scratch, u32* words,
                 u32* host_words, int* remapped);
 // pipeline.cu
-int StreamRun(sm_reconstruction* r, cudaStream_t stream, const sm_stream_desc* s, const sm_preprocess_params* pp,
-              const sm_integrate_params* ip, int first_frame, int last_frame, sm_stream_stats* stats);
-int SessionBegin(sm_reconstruction* r, cudaStream_t stream, const sm_preprocess_params* pp,
-                 const sm_integrate_params* ip, int width, int height, uint32_t first_frame_index);
-int SessionPush(sm_reconstruction* r, const u16* depth, size_t depth_pitch, const uint8_t* color, size_t color_pitch,
-                bool on_host, const float* global_T_frame, const float* frame_T_global, sm_session_status* status);
 int SessionEnd(sm_reconstruction* r, sm_stream_stats* stats);
 void FreeRunBuffers(sm_reconstruction* r);
 // After sm_compact in an open frame-graph session: runs the front half of the frame in flight again on `stream`
 // (its association, merge decisions and blending named the old slots) and resets the reported merge count.
 int SessionRefront(sm_reconstruction* r, cudaStream_t stream);
-// out (3x4) = scale(other_T_global) . scale(global_T_ref) (sm_outlier_filter_transforms)
-void OutlierFilterTransform(float depth_scaling, const float* global_T_ref, const float* other_T_global, float* out);
 }  // namespace smb

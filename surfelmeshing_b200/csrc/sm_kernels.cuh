@@ -459,12 +459,6 @@ int DescribePreprocess(KernelLaunch* bilateral, KernelLaunch* outlier, KernelLau
 int StageBilateral(cudaStream_t stream, float sigma_xy, float sigma_value_factor, u16 value_to_ignore,
                    float radius_factor, u16 max_depth, float depth_valid_region_radius, int width, int height,
                    const u16* in, size_t in_pitch, u16* out, size_t out_pitch);
-int StageOutlier(cudaStream_t stream, int other_count, int required_count, float tolerance, float fx, float fy,
-                 float cx, float cy, int width, int height, const u16* in, size_t in_pitch,
-                 const u16* const* other_depths, const size_t* other_pitches, const float* others_TR_reference,
-                 u16* out, size_t out_pitch);
-int StageErode(cudaStream_t stream, int radius, int width, int height, const u16* in, size_t in_pitch, u16* out,
-               size_t out_pitch);
 int StageMedianDensify(cudaStream_t stream, int iterations, int width, int height, const u16* in, size_t in_pitch,
                        u16* out, size_t out_pitch, u16* scratch, size_t scratch_pitch);
 // The input downscaling of --pyramid_level: median depth blocks of up to 16 x 16 pixels, and `levels`
@@ -473,12 +467,6 @@ int StageDownscaleMedian(cudaStream_t stream, u16 value_to_ignore, int in_width,
                          size_t in_pitch, int out_width, int out_height, u16* out, size_t out_pitch);
 int StageColorPyramid(cudaStream_t stream, int levels, int width, int height, const u8* in, size_t in_pitch, u8* out,
                       size_t out_pitch);
-int StageNormals(cudaStream_t stream, float observation_angle_threshold_deg, float depth_scaling, float fx, float fy,
-                 float cx, float cy, int width, int height, const u16* in, size_t in_pitch, u16* out, size_t out_pitch,
-                 float2* normals, size_t normals_pitch);
-int StageRadii(cudaStream_t stream, float point_radius_extension_factor, float point_radius_clamp_factor,
-               float depth_scaling, float fx, float fy, float cx, float cy, int width, int height, const u16* in,
-               size_t in_pitch, float* radius, size_t radius_pitch, u16* out, size_t out_pitch);
 
 // ---- integrate.cu ---------------------------------------------------------------------------
 struct IntegrateEvents {

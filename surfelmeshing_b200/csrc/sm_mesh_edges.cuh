@@ -1,8 +1,13 @@
 // sm_mesh_edges.cuh — the directed-edge hash table, the input checks and the fp32 corner geometry of a triangle list
-// over the handle's slots, shared by holes.cu (sm_mesh_fill_holes) and simplify.cu (sm_mesh_simplify). Both take an
-// edge-manifold, consistently oriented list, refuse the same inputs and test new triangles by rule 4. The library is
-// built without relocatable device code, so each translation unit compiles its own copy.
+// over the handle's slots, shared by holes.cu (sm_mesh_fill_holes), simplify.cu (sm_mesh_simplify) and texture.cu
+// (sm_mesh_texture), and the host checks of those three calls and of mesh.cu (sm_triangulate, sm_mesh_update). The
+// first two take an edge-manifold, consistently oriented list, refuse the same inputs and test new triangles by rule 4.
+// The library is built without relocatable device code, so each translation unit compiles its own copy.
 #pragma once
+
+#include <algorithm>
+#include <cmath>
+#include <cstdint>
 
 #include "sm_handle.cuh"
 #include "sm_knn.cuh"
@@ -10,6 +15,8 @@
 namespace smb {
 
 namespace {
+
+constexpr int kBlock = 256;   // the one-thread-per-item mesh kernels of holes.cu, simplify.cu and texture.cu
 
 // Below this, the 3 x count corners and edges index as u32 and x 1.5 of them still counts as the int of CUB's sort.
 constexpr u64 kMaxMeshTriangles = 1ull << 28;
@@ -106,6 +113,35 @@ inline const char* MeshInputError(u32 errors) {
   if (errors & kRepeatedCorner) return "a triangle has a repeated corner";
   if (errors & kDuplicateEdge) return "a directed edge occurs twice (the input must be edge-manifold and consistently oriented)";
   return nullptr;
+}
+
+// An angle parameter of a mesh call in degrees: finite and in (0, 180].
+inline bool AngleInRange(float deg) { return std::isfinite(deg) && deg > 0.f && deg <= 180.f; }
+
+// The cosine the kernels compare against, through double.
+inline float CosDegrees(float deg) { return static_cast<float>(std::cos(static_cast<double>(deg) * (M_PI / 180.0))); }
+
+// Blocks of kBlock threads for one thread per item: at least one, at most 8 per SM (the kernels stride).
+inline int Grid(u64 items, int sm_count) {
+  return static_cast<int>(std::max<u64>(1, std::min<u64>((items + kBlock - 1) / kBlock, 8ull * sm_count)));
+}
+
+// The reason the input list of `count` triangles is refused, or nullptr. `output_error`, the caller's check of its
+// output list (nullptr: it passed), is reported between the two checks.
+inline const char* TriangleListError(const uint32_t* triangles, u64 count, const char* output_error = nullptr) {
+  if (!triangles && count > 0) return "triangles is NULL with a count > 0";
+  if (output_error) return output_error;
+  if (count >= kMaxMeshTriangles) return "2^28 triangles or more";
+  return nullptr;
+}
+
+// Whether the bytes [a, a + a_bytes) and [b, b + b_bytes) overlap. An end past the top of the address space is taken
+// as the top, so a range of any length from the caller compares correctly.
+inline bool Overlap(const void* a, u64 a_bytes, const void* b, u64 b_bytes) {
+  const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+  const uintptr_t a1 = a_bytes > UINTPTR_MAX - a0 ? UINTPTR_MAX : a0 + a_bytes;
+  const uintptr_t b1 = b_bytes > UINTPTR_MAX - b0 ? UINTPTR_MAX : b0 + b_bytes;
+  return a0 < b1 && b0 < a1;
 }
 
 }  // namespace

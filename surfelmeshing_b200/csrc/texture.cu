@@ -34,7 +34,6 @@ namespace smb {
 
 namespace {
 
-constexpr int kBlock = 256;
 constexpr int kClasses = 7;            // q = 0 .. 6: s = SM_TEXTURE_MAX_TILE >> q = 512 .. 8
 constexpr int kMaxTileLog2 = 9;
 constexpr u32 kTriangleBits = 28;      // count < 2^28 (kMaxMeshTriangles)
@@ -421,15 +420,6 @@ int EnsurePixelScratch(TextureScratch& s, size_t pixels) {
   return SM_OK;
 }
 
-int Grid(u64 items, int sm_count) {
-  return static_cast<int>(std::max<u64>(1, std::min<u64>((items + kBlock - 1) / kBlock, 8ull * sm_count)));
-}
-
-bool Overlap(const void* a, u64 a_bytes, const void* b, u64 b_bytes) {
-  const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
-  return a0 < b0 + b_bytes && b0 < a0 + a_bytes;
-}
-
 }  // namespace
 
 void FreeTextureBuffers(sm_reconstruction* r) {
@@ -443,18 +433,34 @@ void FreeTextureBuffers(sm_reconstruction* r) {
   r->texture = nullptr;
 }
 
-int Texture(sm_reconstruction* r, cudaStream_t stream, const sm_texture_params& p, const uint32_t* triangles,
-            uint64_t count, const sm_texture_view* views, int32_t view_count, uint8_t* atlas, size_t atlas_pitch,
-            int32_t atlas_capacity_width, int32_t atlas_capacity_height, float* uv, sm_texture_stats* stats) {
+}  // namespace smb
+
+using namespace smb;
+
+extern "C" {
+
+void sm_default_texture_params(sm_texture_params* p) {
+  p->texel_size = 0.004f;
+  p->max_atlas_side = 16384;
+  p->max_view_angle_deg = 75.0f;
+  p->depth_tolerance = 0.01f;
+}
+
+int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_params* params, const uint32_t* triangles,
+                    uint64_t count, const sm_texture_view* views, int32_t view_count, uint8_t* atlas,
+                    size_t atlas_pitch, int32_t atlas_capacity_width, int32_t atlas_capacity_height, float* uv,
+                    sm_texture_stats* stats) {
+  if (!r || !params || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_texture: null argument");
   auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_mesh_texture: ") + why).c_str()); };
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const sm_texture_params& p = *params;
   *stats = sm_texture_stats{};
   if (!std::isfinite(p.texel_size) || !(p.texel_size > 0.f)) return bad("texel_size must be finite and > 0");
   if (p.max_atlas_side < 8 || p.max_atlas_side > SM_TEXTURE_MAX_ATLAS_SIDE)
     return bad("max_atlas_side must be in [8, SM_TEXTURE_MAX_ATLAS_SIDE]");
   if (!(p.max_view_angle_deg > 0.f && p.max_view_angle_deg <= 90.f)) return bad("max_view_angle_deg must be in (0, 90]");
   if (!(p.depth_tolerance >= 0.f) || !std::isfinite(p.depth_tolerance)) return bad("depth_tolerance must be finite and >= 0");
-  if (!triangles && count > 0) return bad("triangles is NULL with a count > 0");
-  if (count >= kMaxMeshTriangles) return bad("2^28 triangles or more");
+  if (const char* why = TriangleListError(triangles, count)) return bad(why);
   if (view_count < 0 || view_count > SM_TEXTURE_MAX_VIEWS) return bad("view_count must be in [0, SM_TEXTURE_MAX_VIEWS]");
   if (!views && view_count > 0) return bad("views is NULL with a view_count > 0");
   size_t max_pixels = 1;
@@ -565,7 +571,7 @@ int Texture(sm_reconstruction* r, cudaStream_t stream, const sm_texture_params& 
   SM_CUDA(cudaMemsetAsync(s.accum, 0, sizeof(float4) * area, stream));
   if (uv) { LaunchScope scope(stream, KID_TEXTURE_UV); LaunchKernel(k_tex_uv, dim3(grid), dim3(kBlock), 0, stream, a); }
   const int texel_grid = Grid(area, r->sm_count);
-  const float cos_max = static_cast<float>(std::cos(static_cast<double>(p.max_view_angle_deg) * (M_PI / 180.0)));
+  const float cos_max = CosDegrees(p.max_view_angle_deg);
   for (int32_t k = 0; k < view_count; ++k) {
     const sm_texture_view& view = views[k];
     const sm_render_params& cam = view.camera;
@@ -596,20 +602,4 @@ int Texture(sm_reconstruction* r, cudaStream_t stream, const sm_texture_params& 
   return CheckLaunch("texture");
 }
 
-}  // namespace smb
-
-void sm_default_texture_params(sm_texture_params* p) {
-  p->texel_size = 0.004f;
-  p->max_atlas_side = 16384;
-  p->max_view_angle_deg = 75.0f;
-  p->depth_tolerance = 0.01f;
-}
-
-int sm_mesh_texture(sm_reconstruction* r, void* stream, const sm_texture_params* p, const uint32_t* triangles,
-                    uint64_t count, const sm_texture_view* views, int32_t view_count, uint8_t* atlas,
-                    size_t atlas_pitch, int32_t atlas_capacity_width, int32_t atlas_capacity_height, float* uv,
-                    sm_texture_stats* stats) {
-  if (!r || !p || !stats) return smb::SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_texture: null argument");
-  return smb::Texture(r, static_cast<cudaStream_t>(stream), *p, triangles, count, views, view_count, atlas,
-                      atlas_pitch, atlas_capacity_width, atlas_capacity_height, uv, stats);
-}
+}  // extern "C"

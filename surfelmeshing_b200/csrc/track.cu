@@ -1016,25 +1016,6 @@ int TrackFrameRGBD(sm_reconstruction* r, cudaStream_t stream, const sm_track_par
   return TrackFrameImpl(r, stream, tp, pp, &color, depth, depth_pitch, guess, pose_out, &result->depth, result);
 }
 
-int TrackLinearize(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, int level, float depth_scaling,
-                   const u16* live, size_t live_pitch, const float* model_depth, size_t model_depth_pitch,
-                   const float* model_normal, size_t model_normal_pitch, const float* model_T_live, double* out_system,
-                   uint32_t* out_inliers) {
-  return TrackLinearizeImpl(r, stream, tp, nullptr, level, depth_scaling, live, live_pitch, model_depth,
-                            model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system, out_inliers,
-                            nullptr, nullptr);
-}
-
-int TrackLinearizeRGBD(sm_reconstruction* r, cudaStream_t stream, const sm_track_params& tp, const TrackColor& color,
-                       int level, float depth_scaling, const u16* live, size_t live_pitch, const float* model_depth,
-                       size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
-                       const float* model_T_live, double* out_system, double* out_sum_rc2, uint32_t* out_inliers,
-                       uint32_t* out_photometric_inliers) {
-  return TrackLinearizeImpl(r, stream, tp, &color, level, depth_scaling, live, live_pitch, model_depth,
-                            model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system, out_inliers,
-                            out_sum_rc2, out_photometric_inliers);
-}
-
 void FreeTrackBuffers(sm_reconstruction* r) {
   TrackScratch* t = r->track;
   if (!t) return;
@@ -1049,3 +1030,73 @@ void FreeTrackBuffers(sm_reconstruction* r) {
 }
 
 }  // namespace smb
+
+using namespace smb;
+
+extern "C" {
+
+void sm_default_track_params(sm_track_params* p) {
+  p->levels = 3;
+  p->iterations[0] = 4; p->iterations[1] = 5; p->iterations[2] = 10; p->iterations[3] = 0;
+  p->max_point_distance = 0.05f;
+  p->max_normal_angle_deg = 20.0f;
+  p->min_inlier_fraction = 0.1f;
+  p->convergence_rotation = 1e-5f;
+  p->convergence_translation = 1e-5f;
+  p->model_source = SM_TRACK_CLOUD;
+}
+
+void sm_default_track_rgbd_params(sm_track_rgbd_params* p) {
+  p->photometric_weight = 1e-4f;
+  p->max_intensity_residual = 40.0f;
+  p->min_gradient = 2.0f;
+}
+
+int sm_track_frame(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_preprocess_params* pp,
+                   const uint16_t* depth, size_t depth_pitch, const float global_T_guess[12], float global_T_out[12],
+                   sm_track_result* result) {
+  if (!r || !tp || !pp || !depth || !global_T_guess || !global_T_out || !result)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_frame: null argument");
+  return TrackFrame(r, static_cast<cudaStream_t>(stream), *tp, *pp, depth, depth_pitch, global_T_guess, global_T_out,
+                    result);
+}
+
+int sm_track_linearize(sm_reconstruction* r, void* stream, const sm_track_params* tp, int32_t level,
+                       float depth_scaling, const uint16_t* live_depth, size_t live_pitch, const float* model_depth,
+                       size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
+                       const float model_T_live[12], double out_system[27], uint32_t* out_inliers) {
+  if (!r || !tp || !live_depth || !model_depth || !model_normal || !model_T_live || !out_system || !out_inliers)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_linearize: null argument");
+  return TrackLinearizeImpl(r, static_cast<cudaStream_t>(stream), *tp, nullptr, level, depth_scaling, live_depth,
+                            live_pitch, model_depth, model_depth_pitch, model_normal, model_normal_pitch, model_T_live,
+                            out_system, out_inliers, nullptr, nullptr);
+}
+
+int sm_track_frame_rgbd(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_preprocess_params* pp,
+                        const sm_track_rgbd_params* rp, const uint16_t* depth, size_t depth_pitch, const uint8_t* color,
+                        size_t color_pitch, const float global_T_guess[12], float global_T_out[12],
+                        sm_track_rgbd_result* result) {
+  if (!r || !tp || !pp || !rp || !depth || !color || !global_T_guess || !global_T_out || !result)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_frame_rgbd: null argument");
+  const TrackColor c{rp, color, color_pitch, nullptr, 0};
+  return TrackFrameRGBD(r, static_cast<cudaStream_t>(stream), *tp, *pp, c, depth, depth_pitch, global_T_guess,
+                        global_T_out, result);
+}
+
+int sm_track_linearize_rgbd(sm_reconstruction* r, void* stream, const sm_track_params* tp, const sm_track_rgbd_params* rp,
+                            int32_t level, float depth_scaling, const uint16_t* live_depth, size_t live_pitch,
+                            const uint8_t* live_color, size_t live_color_pitch, const float* model_depth,
+                            size_t model_depth_pitch, const float* model_normal, size_t model_normal_pitch,
+                            const uint8_t* model_color, size_t model_color_pitch, const float model_T_live[12],
+                            double out_system[27], double* out_sum_rc2, uint32_t* out_inliers,
+                            uint32_t* out_photometric_inliers) {
+  if (!r || !tp || !rp || !live_depth || !live_color || !model_depth || !model_normal || !model_color || !model_T_live ||
+      !out_system || !out_sum_rc2 || !out_inliers || !out_photometric_inliers)
+    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_track_linearize_rgbd: null argument");
+  const TrackColor c{rp, live_color, live_color_pitch, model_color, model_color_pitch};
+  return TrackLinearizeImpl(r, static_cast<cudaStream_t>(stream), *tp, &c, level, depth_scaling, live_depth, live_pitch,
+                            model_depth, model_depth_pitch, model_normal, model_normal_pitch, model_T_live, out_system,
+                            out_inliers, out_sum_rc2, out_photometric_inliers);
+}
+
+}  // extern "C"

@@ -198,25 +198,6 @@ int FullTransfer(sm_reconstruction* r, cudaStream_t stream, u32 n, float* const 
 
 }  // namespace
 
-int UpdateVisualizationBuffers(sm_reconstruction* r, cudaStream_t stream, const sm_visualization_params& p, float* vertex,
-                               uint32_t* neighbor_index, float* normal_vertex) {
-  if (p.point_size_in_floats < 4 && vertex) return SetError(SM_ERR_INVALID_ARGUMENT, "point_size_in_floats < 4");
-  if (neighbor_index && (reinterpret_cast<uintptr_t>(neighbor_index) & 15)) return SetError(SM_ERR_INVALID_ARGUMENT, "neighbor index buffer must be 16-byte aligned");
-  VizArgs a;
-  a.count_slot = r->count_slot;
-  a.frame_index = p.frame_index;
-  a.active_window = p.surfel_integration_active_window_size;
-  a.latest_triangulated_frame_index = p.latest_triangulated_frame_index;
-  a.latest_mesh_surfel_count = p.latest_mesh_surfel_count;
-  a.point_size_in_floats = p.point_size_in_floats;
-  // the reference's if / else-if chain (kernels.cu:404-414)
-  a.mode = p.visualize_last_update_timestamp ? 1 : p.visualize_creation_timestamp ? 2 : p.visualize_radii ? 3 : p.visualize_normals ? 4 : 0;
-  a.vertex = vertex; a.neighbor_index = neighbor_index; a.normal_vertex = normal_vertex;
-  r->last_stream = stream;
-  { LaunchScope scope(stream, KID_VIZ_BUFFERS); LaunchKernel(k_viz_buffers, dim3(r->sm_count * 8), dim3(kBlock), 0, stream, r->d, a); }
-  return CheckLaunch("visualization buffers");
-}
-
 uint64_t NextStateGeneration() {
   // One counter for the whole process: a per-handle count would let a token filled from one handle (or from a
   // destroyed one) pass for another handle's cloud. 0 stays "never filled".
@@ -239,10 +220,17 @@ void FreeTransferBuffers(sm_reconstruction* r) {
   r->transfer = nullptr;
 }
 
-int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_index, sm_transfer_token* token, float* x,
-                  float* y, float* z, float* radius_squared, float* nx, float* ny, float* nz,
-                  uint32_t* last_update_stamp, sm_transfer_stats* stats) {
-  (void)frame_index;
+}  // namespace smb
+
+using namespace smb;
+
+extern "C" {
+
+int sm_transfer_delta_to_cpu(sm_reconstruction* r, void* stream_v, uint32_t /*frame_index*/, sm_transfer_token* token,
+                             float* x, float* y, float* z, float* radius_squared, float* nx, float* ny, float* nz,
+                             uint32_t* last_update_stamp, sm_transfer_stats* stats) {
+  if (!r || !token) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_transfer_delta_to_cpu: null argument");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   r->last_stream = stream;
   int status = FetchCounters(r, stream);
   if (status != SM_OK) return status;
@@ -358,4 +346,26 @@ int TransferDelta(sm_reconstruction* r, cudaStream_t stream, uint32_t frame_inde
   return SM_OK;
 }
 
-}  // namespace smb
+int sm_update_visualization_buffers(sm_reconstruction* r, void* stream_v, const sm_visualization_params* params,
+                                    float* vertex, uint32_t* neighbor_index, float* normal_vertex) {
+  if (!r || !params) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_update_visualization_buffers: null argument");
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const sm_visualization_params& p = *params;
+  if (p.point_size_in_floats < 4 && vertex) return SetError(SM_ERR_INVALID_ARGUMENT, "point_size_in_floats < 4");
+  if (neighbor_index && (reinterpret_cast<uintptr_t>(neighbor_index) & 15)) return SetError(SM_ERR_INVALID_ARGUMENT, "neighbor index buffer must be 16-byte aligned");
+  VizArgs a;
+  a.count_slot = r->count_slot;
+  a.frame_index = p.frame_index;
+  a.active_window = p.surfel_integration_active_window_size;
+  a.latest_triangulated_frame_index = p.latest_triangulated_frame_index;
+  a.latest_mesh_surfel_count = p.latest_mesh_surfel_count;
+  a.point_size_in_floats = p.point_size_in_floats;
+  // the reference's if / else-if chain (kernels.cu:404-414)
+  a.mode = p.visualize_last_update_timestamp ? 1 : p.visualize_creation_timestamp ? 2 : p.visualize_radii ? 3 : p.visualize_normals ? 4 : 0;
+  a.vertex = vertex; a.neighbor_index = neighbor_index; a.normal_vertex = normal_vertex;
+  r->last_stream = stream;
+  { LaunchScope scope(stream, KID_VIZ_BUFFERS); LaunchKernel(k_viz_buffers, dim3(r->sm_count * 8), dim3(kBlock), 0, stream, r->d, a); }
+  return CheckLaunch("visualization buffers");
+}
+
+}  // extern "C"

@@ -76,6 +76,13 @@ def _raster(t: torch.Tensor, channels: int = 1):
     return C.c_void_p(t.data_ptr()), t.stride(0) * t.element_size()
 
 
+def _check_triangles(triangles) -> None:
+    """The triangle list of the mesh calls: an int32 CUDA tensor [T, 3] of slot indices."""
+    if not (isinstance(triangles, torch.Tensor) and triangles.is_cuda and triangles.dtype == torch.int32
+            and triangles.dim() == 2 and triangles.shape[1] == 3):
+        raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+
+
 def _mat12(m) -> np.ndarray:
     a = np.ascontiguousarray(np.asarray(m, dtype=np.float32).reshape(-1)[:12])
     assert a.size == 12
@@ -414,9 +421,7 @@ class CUDASurfelReconstruction:
         unknown = [o for o in outputs if o not in RENDER_OUTPUTS]
         if unknown or not outputs:
             raise ValueError(f"outputs must be a non-empty subset of {RENDER_OUTPUTS}, got {outputs}")
-        if not isinstance(triangles, torch.Tensor) or triangles.dim() != 2 or triangles.shape[1] != 3 or \
-                triangles.dtype != torch.int32 or not triangles.is_cuda:
-            raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+        _check_triangles(triangles)
         triangles = triangles.contiguous()
         H, W = int(height), int(width)
         shapes = {"depth": ((H, W), torch.float32), "color": ((H, W, 3), torch.uint8),
@@ -592,7 +597,7 @@ class CUDASurfelReconstruction:
                 capacity = max(int(stats.triangle_count), 1)
                 continue
             if status != _lib.SM_OK:
-                raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+                raise self.lib.error(status)
             return out[:int(stats.triangle_count)], stats
         raise AssertionError("unreachable")
 
@@ -617,7 +622,7 @@ class CUDASurfelReconstruction:
         count = C.c_uint64()
         status = self.lib.fn["mesh_read"](self._h, handle, code, None, 0, C.byref(count))
         if status not in (_lib.SM_OK, _lib.SM_ERR_CAPACITY):
-            raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+            raise self.lib.error(status)
         capacity = max(int(count.value), 1)
         for attempt in range(2):
             out = torch.empty((capacity, 3), dtype=torch.int32, device="cuda")
@@ -629,7 +634,7 @@ class CUDASurfelReconstruction:
                 capacity = max(int(count.value), 1)
                 continue
             if status != _lib.SM_OK:
-                raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+                raise self.lib.error(status)
             return out[:int(count.value)]
         raise AssertionError("unreachable")
 
@@ -640,16 +645,14 @@ class CUDASurfelReconstruction:
         tensor [F, 3], in the mesh's convention, to be appended to `triangles`; HoleStats). Asks for the count first
         (capacity 0), then writes."""
         p = HoleParams.defaults() if params is None else params
-        if not (isinstance(triangles, torch.Tensor) and triangles.is_cuda and triangles.dtype == torch.int32
-                and triangles.dim() == 2 and triangles.shape[1] == 3):
-            raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+        _check_triangles(triangles)
         tri = triangles.contiguous()
         handle = _stream_handle(stream)
         stats = HoleStats()
         fn = self.lib.fn["mesh_fill_holes"]
         status = fn(self._h, handle, C.byref(p), C.c_void_p(tri.data_ptr()), len(tri), None, 0, C.byref(stats))
         if status not in (_lib.SM_OK, _lib.SM_ERR_CAPACITY):
-            raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+            raise self.lib.error(status)
         capacity = max(int(stats.triangles_added), 1)
         out = torch.empty((capacity, 3), dtype=torch.int32, device="cuda")
         if isinstance(stream, torch.cuda.Stream):
@@ -665,9 +668,7 @@ class CUDASurfelReconstruction:
         (int32 CUDA tensor [T', 3] over a subset of the slots, in the mesh's convention; SimplifyStats). The output
         is never longer than the input, so one call with capacity T suffices."""
         p = SimplifyParams.defaults() if params is None else params
-        if not (isinstance(triangles, torch.Tensor) and triangles.is_cuda and triangles.dtype == torch.int32
-                and triangles.dim() == 2 and triangles.shape[1] == 3):
-            raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+        _check_triangles(triangles)
         tri = triangles.contiguous()
         out = torch.empty((max(len(tri), 1), 3), dtype=torch.int32, device="cuda")
         if isinstance(stream, torch.cuda.Stream):
@@ -687,9 +688,7 @@ class CUDASurfelReconstruction:
         Raises SurfelError (SM_ERR_CAPACITY) when the atlas would be wider than params.max_atlas_side: raise
         params.texel_size then."""
         p = TextureParams.defaults() if params is None else params
-        if not (isinstance(triangles, torch.Tensor) and triangles.is_cuda and triangles.dtype == torch.int32
-                and triangles.dim() == 2 and triangles.shape[1] == 3):
-            raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
+        _check_triangles(triangles)
         tri = triangles.contiguous()
         views = list(views)
         descs = (TextureViewDesc * max(len(views), 1))(*[v.desc() for v in views])
@@ -703,7 +702,7 @@ class CUDASurfelReconstruction:
             return (torch.zeros((0, 0, 3), dtype=torch.uint8, device="cuda"),
                     torch.zeros((0, 3, 2), dtype=torch.float32, device="cuda"), stats)
         if status != _lib.SM_ERR_CAPACITY or stats.atlas_width > p.max_atlas_side:
-            raise _lib.SurfelError(status, self.lib.fn["last_error"]().decode(errors="replace"))
+            raise self.lib.error(status)
         W, H = int(stats.atlas_width), int(stats.atlas_height)
         atlas = torch.empty((H, W, 3), dtype=torch.uint8, device="cuda")
         uv = torch.empty((len(tri), 3, 2), dtype=torch.float32, device="cuda")
