@@ -1136,6 +1136,79 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream, const sm_texture_params*
                     float* uv /* device, 6 x count: (u, v) per corner in the listed order, in [0, 1]; may be NULL */,
                     sm_texture_stats* stats);
 
+/* ---- connected pieces of a triangle mesh (DESIGN.md section 1 row f18, section 5.16) ----------------------------
+ * The surfel mesher leaves small floating pieces behind: a pair of surfels at a depth edge, or a few surfels the
+ * normal gate cut off from their neighbours. sm_mesh_components splits a caller's triangle list into its connected
+ * pieces, gives every triangle the number of its piece and every piece its size, area and bounds, and returns the
+ * triangles of the pieces that pass the thresholds of sm_component_params (e.g. before sm_mesh_simplify and
+ * sm_mesh_texture, so floaters take no part of the budget or the atlas). Positions are the current SMOOTH positions
+ * (what sm_render_mesh draws); the call only reads the surfel state.
+ *
+ * t is a triangle's position in the list.
+ *  C1. Input. Every corner must be a present slot (radius^2 > 0) below surfels_size() and no triangle may repeat a
+ *      corner (X1 of sm_mesh_texture). Manifoldness is not required. 0 triangles are legal.
+ *  C2. Adjacency. Triangles s and t are adjacent when they share an undirected edge {a, b}, in either winding and
+ *      with any number of triangles on that edge. A piece is a class of the transitive closure of this relation: a
+ *      triangle with no adjacent triangle is a piece of its own, and two pieces that touch only at a slot stay two.
+ *  C3. Numbering. Pieces are numbered 0, 1, ... in the order of their smallest triangle position; labels[t] is the
+ *      number of t's piece. Partition and numbering do not depend on thread order.
+ *  C4. Area. P_i = the smooth position of slot i converted to double; e1, e2, g and gg as in S1 of sm_mesh_simplify
+ *      (each double operation rounded on its own); a_t = 0.5 * sqrt(gg). q_t = rint(a_t * 2^30) (ties to even),
+ *      capped at 2^36; q_t = 0 when a_t is not finite. A piece's area units Q = the integer sum of its q_t (below
+ *      2^64 for count < 2^28), so any summation order gives the same bits. Its area is double(Q) * 2^-30 (m^2).
+ *  C5. Bounds. A piece's lo / hi are the per-axis min / max of the fp32 smooth positions of its triangles' corners,
+ *      compared in IEEE totalOrder (-0 < +0).
+ *  C6. Keep. A piece is kept iff its triangle count >= min_triangles, Q >= rint(min_area * 2^30) (computed on the
+ *      host in double), and keep_largest is 0 or its rank is below keep_largest; the rank orders all pieces by
+ *      (Q descending, number ascending).
+ *  C7. Output. The triangles of kept pieces, in input order, corners and winding unchanged. Stats: triangles_in =
+ *      count, triangles_out, components, components_kept, and the triangle count and area of the rank-0 piece. All
+ *      zero when the call fails for any reason other than capacity.
+ *
+ * out is a DEVICE buffer of 3 x out_capacity uint32 (may be NULL with out_capacity 0: a count query); labels (DEVICE,
+ * count int32) and table (DEVICE, table_capacity entries, piece p at entry p) may be NULL. If out_capacity <
+ * triangles_out, or table is not NULL and table_capacity < components, the call returns SM_ERR_CAPACITY with the
+ * stats set and writes nothing; both counts are at most count, so capacities of count always suffice.
+ * SM_ERR_INVALID_ARGUMENT, with no launch, for NULL params or stats, triangles NULL with count > 0, out NULL with
+ * out_capacity > 0, table NULL with table_capacity > 0, count >= 2^28, min_area negative, NaN or infinite, or out,
+ * labels or table overlapping the triangles or each other; and, found on the device and reported after the call's
+ * second synchronisation with nothing written, for a list that breaks C1.
+ * The call synchronises `stream` three times (surfels_size(); the input checks and the numbering; the end), plus
+ * once, with cudaFree's device synchronisation, in a call whose buffers grow (by x 1.5); on return the output is
+ * written by work enqueued on `stream`. Memory (allocated by the first call, grown with the input, freed by
+ * sm_destroy; sm_create allocates nothing for it): 60 to 108 bytes per triangle of capacity (an undirected-edge hash
+ * table of which a call uses and clears the power of two >= 4 x count slots, a u64 key and a u32 owner each: 48 to
+ * 96; the union-find parents: 4; the root flags and the keep flags, each scanned: 8) and 68 bytes per piece (the
+ * triangle count, the first triangle and the keep flag: 12; Q: 8; the ordered-int bounds: 24; the rank sort's keys
+ * and values in and out: 24), plus the radix sort's scratch. */
+typedef struct sm_component_params {
+  uint64_t min_triangles;   /* 10; pieces with fewer triangles are dropped (0 and 1 keep every piece) */
+  double min_area;          /* 0 m^2; finite, >= 0; pieces with less area are dropped */
+  uint64_t keep_largest;    /* 0 = no limit; else only the keep_largest pieces of largest area can be kept */
+} sm_component_params;
+typedef struct sm_component_stats {
+  uint64_t triangles_in, triangles_out;
+  uint64_t components, components_kept;
+  uint64_t largest_triangles;   /* of the rank-0 piece (0 for an empty list) */
+  double largest_area;          /* m^2, of the rank-0 piece */
+} sm_component_stats;
+typedef struct sm_mesh_component {
+  uint64_t triangles;
+  double area;                  /* m^2: double(Q) * 2^-30 */
+  float lo[3], hi[3];           /* smooth-position bounds of its corners */
+  uint32_t first_triangle;      /* its smallest triangle position */
+  int32_t kept;                 /* 1 if its triangles are in out */
+} sm_mesh_component;
+/* Host only, no device needed. */
+void sm_default_component_params(sm_component_params* p);
+int sm_mesh_components(sm_reconstruction* r, void* stream, const sm_component_params* p,
+                       const uint32_t* triangles /* device, 3 x count */, uint64_t count,
+                       uint32_t* out /* device, 3 x out_capacity; may be NULL with out_capacity 0 */,
+                       uint64_t out_capacity,
+                       int32_t* labels /* device, count; may be NULL */,
+                       sm_mesh_component* table /* device, table_capacity; may be NULL with table_capacity 0 */,
+                       uint64_t table_capacity, sm_component_stats* stats);
+
 /* ---- radius-limited k-nearest-neighbour queries for the meshing thread (SURVEY section 8 f4) ----
  * Replaces CompressedOctree::FindNearestSurfelsWithinRadius<include_completed_surfels, include_free_surfels>
  * (octree.h:471, octree.cc:313-470; callers surfel_meshing.cc:421 <false, true> and :821 <true, false>) for a BATCH of

@@ -186,6 +186,21 @@ class CUDASurfelReconstruction {
     return stats;
   }
 
+  // Extension (no counterpart in the reference): the connected pieces of a triangle list over the slots (device, 3 x
+  // count) (sm_mesh_components): the triangles of the kept pieces into `out` (device, 3 x count), each triangle's
+  // piece number into `labels` (device, count, may be null) and the pieces into `table` (device, table_capacity
+  // entries, may be null with 0).
+  sm_component_stats MeshComponents(cudaStream_t stream, const u32* triangles, uint64_t count, u32* out,
+                                    int32_t* labels = nullptr, sm_mesh_component* table = nullptr,
+                                    uint64_t table_capacity = 0, const sm_component_params* params = nullptr) {
+    sm_component_params defaults;
+    sm_default_component_params(&defaults);
+    sm_component_stats stats;
+    Check(sm_mesh_components(handle_, stream, params ? params : &defaults, triangles, count, out, count, labels, table,
+                             table_capacity, &stats));
+    return stats;
+  }
+
   // Extension (no counterpart in the reference): a texture atlas for a triangle list over the slots (device, 3 x
   // count) from posed colour views (sm_mesh_texture): `atlas` (device u8x3, atlas_pitch bytes per row, room for
   // capacity_width x capacity_height texels) and `uv` (device, 6 x count, may be null). A call with a null atlas and

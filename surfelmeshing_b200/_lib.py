@@ -301,6 +301,33 @@ class TextureViewDesc(C.Structure):
                 ("color_pitch", C.c_size_t)]
 
 
+class ComponentParams(C.Structure):
+    """sm_component_params: the fewest triangles and the least area (m^2) of a kept piece, and how many of the
+    largest pieces may be kept (0: no limit)."""
+    _fields_ = [("min_triangles", C.c_uint64), ("min_area", C.c_double), ("keep_largest", C.c_uint64)]
+
+    @classmethod
+    def defaults(cls, **overrides) -> "ComponentParams":
+        p = cls(10, 0.0, 0)
+        for k, v in overrides.items():
+            setattr(p, k, v)
+        return p
+
+
+class ComponentStats(C.Structure):
+    """sm_component_stats: triangles in and out, pieces and pieces kept, and the triangle count and area (m^2) of the
+    largest piece."""
+    _fields_ = [("triangles_in", C.c_uint64), ("triangles_out", C.c_uint64), ("components", C.c_uint64),
+                ("components_kept", C.c_uint64), ("largest_triangles", C.c_uint64), ("largest_area", C.c_double)]
+
+
+class MeshComponent(C.Structure):
+    """sm_mesh_component: one piece's triangle count, area (m^2), smooth-position bounds, smallest triangle position
+    and whether it is kept."""
+    _fields_ = [("triangles", C.c_uint64), ("area", C.c_double), ("lo", C.c_float * 3), ("hi", C.c_float * 3),
+                ("first_triangle", C.c_uint32), ("kept", C.c_int32)]
+
+
 class CompactStats(C.Structure):
     """sm_compact_stats: surfels_size() before and after, the merged slots removed, the neighbour links of kept slots
     that named a removed slot, and whether the persistent sm_mesh_update mesh was carried over."""
@@ -412,6 +439,9 @@ _PRODUCT_ONLY = {
     "default_texture_params": (None, [C.POINTER(TextureParams)]),
     "mesh_texture": (C.c_int, [_P, _P, C.POINTER(TextureParams), _P, C.c_uint64, C.POINTER(TextureViewDesc), _I, _P,
                                _SZ, _I, _I, _P, C.POINTER(TextureStats)]),
+    "default_component_params": (None, [C.POINTER(ComponentParams)]),
+    "mesh_components": (C.c_int, [_P, _P, C.POINTER(ComponentParams), _P, C.c_uint64, _P, C.c_uint64, _P, _P,
+                                  C.c_uint64, C.POINTER(ComponentStats)]),
 }
 
 EXPORTED_SYMBOLS = sorted(["sm_" + n for n in list(_SIGNATURES) + list(_PRODUCT_ONLY)])

@@ -28,7 +28,7 @@ CSRC = PKG_DIR / "csrc"
 LIB_PATH = PKG_DIR / "libsurfel_b200.so"
 SOURCES = ["api.cu", "pipeline.cu", "transfer.cu", "preprocess.cu", "integrate.cu", "regularize.cu", "knn.cu",
            "render.cu", "track.cu", "mesh.cu", "reloc.cu", "holes.cu", "compact.cu",
-           "simplify.cu", "texture.cu"]
+           "simplify.cu", "texture.cu", "components.cu"]
 HEADERS = ["sm_math.cuh", "sm_kernels.cuh", "sm_handle.cuh", "sm_knn.cuh", "sm_mesh_edges.cuh",
            "../../include/surfel_b200.h"]
 

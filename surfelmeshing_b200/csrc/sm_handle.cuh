@@ -73,6 +73,7 @@ struct HoleScratch;      // holes.cu: the buffers of sm_mesh_fill_holes
 struct CompactScratch;   // compact.cu: the map and the row scratch of sm_compact
 struct SimplifyScratch;  // simplify.cu: the buffers of sm_mesh_simplify
 struct TextureScratch;   // texture.cu: the buffers of sm_mesh_texture
+struct ComponentScratch;  // components.cu: the buffers of sm_mesh_components
 
 }  // namespace smb
 
@@ -131,6 +132,7 @@ struct sm_reconstruction {
   smb::CompactScratch* compact = nullptr;
   smb::SimplifyScratch* simplify = nullptr;
   smb::TextureScratch* texture = nullptr;
+  smb::ComponentScratch* components = nullptr;
 };
 
 namespace smb {
@@ -188,6 +190,8 @@ void FreeCompactBuffers(sm_reconstruction* r);
 void FreeSimplifyBuffers(sm_reconstruction* r);
 // texture.cu
 void FreeTextureBuffers(sm_reconstruction* r);
+// components.cu
+void FreeComponentBuffers(sm_reconstruction* r);
 // In place: word w of record k' = word w of record i, old_to_new[i] = k' < kept, for every word of records of
 // `record_words` 32-bit words (bytes) over slots [0, n), one word at a time through `scratch` (>= kept words).
 // `remap`: the words name slots and are replaced by their new index (SM_INVALID_SURFEL_INDEX for a removed one).

@@ -1,7 +1,8 @@
-// sm_mesh_edges.cuh — the directed-edge hash table, the input checks and the fp32 corner geometry of a triangle list
-// over the handle's slots, shared by holes.cu (sm_mesh_fill_holes), simplify.cu (sm_mesh_simplify) and texture.cu
-// (sm_mesh_texture), and the host checks of those three calls and of mesh.cu (sm_triangulate, sm_mesh_update). The
-// first two take an edge-manifold, consistently oriented list, refuse the same inputs and test new triangles by rule 4.
+// sm_mesh_edges.cuh — the edge hash table, the input checks and the fp32 corner geometry of a triangle list over the
+// handle's slots, shared by holes.cu (sm_mesh_fill_holes), simplify.cu (sm_mesh_simplify), texture.cu
+// (sm_mesh_texture) and components.cu (sm_mesh_components), and the host checks of those four calls and of mesh.cu
+// (sm_triangulate, sm_mesh_update). The first two take an edge-manifold, consistently oriented list, refuse the same
+// inputs and test new triangles by rule 4.
 // The library is built without relocatable device code, so each translation unit compiles its own copy.
 #pragma once
 
@@ -16,7 +17,7 @@ namespace smb {
 
 namespace {
 
-constexpr int kBlock = 256;   // the one-thread-per-item mesh kernels of holes.cu, simplify.cu and texture.cu
+constexpr int kBlock = 256;   // the one-thread-per-item mesh kernels of holes.cu, simplify.cu, texture.cu, components.cu
 
 // Below this, the 3 x count corners and edges index as u32 and x 1.5 of them still counts as the int of CUB's sort.
 constexpr u64 kMaxMeshTriangles = 1ull << 28;
@@ -29,6 +30,9 @@ constexpr u32 kDuplicateEdge = 4;
 __device__ __forceinline__ u64 edge_key(u32 tail, u32 head) { return (static_cast<u64>(tail) << 32) | head; }
 __device__ __forceinline__ u32 tail_of(u64 key) { return static_cast<u32>(key >> 32); }
 __device__ __forceinline__ u32 head_of(u64 key) { return static_cast<u32>(key); }
+
+// The key of the undirected edge {a, b}: the directed key from the smaller slot.
+__device__ __forceinline__ u64 undirected_edge_key(u32 a, u32 b) { return a < b ? edge_key(a, b) : edge_key(b, a); }
 
 // splitmix64's finaliser: the probe start of a key.
 __device__ __forceinline__ u64 mix(u64 x) {
@@ -57,14 +61,20 @@ __device__ __forceinline__ u64 table_find(const u64* table, u64 mask, u64 key) {
 // Checks triangle c of a list over slots [0, n) (row 7 = radius^2 of a slot, with `stride`) and inserts its three
 // directed edges into the table. Returns the error bits it found; a triangle with a bad or repeated corner inserts
 // nothing.
-__device__ __forceinline__ u32 check_and_insert_triangle(const float* radius_squared, u32 n, uint3 c, u64* table,
-                                                         u64 mask) {
+// The error bits of triangle c over slots [0, n) (row 7 = radius^2 of a slot): kBadCorner, kRepeatedCorner.
+__device__ __forceinline__ u32 triangle_corner_errors(const float* radius_squared, u32 n, uint3 c) {
   u32 error = 0;
   for (int s = 0; s < 3; ++s) {
     const u32 i = s == 0 ? c.x : (s == 1 ? c.y : c.z);
     if (i >= n || !(radius_squared[i] > 0.f)) error |= kBadCorner;
   }
   if (c.x == c.y || c.y == c.z || c.z == c.x) error |= kRepeatedCorner;
+  return error;
+}
+
+__device__ __forceinline__ u32 check_and_insert_triangle(const float* radius_squared, u32 n, uint3 c, u64* table,
+                                                         u64 mask) {
+  u32 error = triangle_corner_errors(radius_squared, n, c);
   if (!error) {
     u64 slot;
     if (!table_insert(table, mask, edge_key(c.x, c.y), &slot)) error |= kDuplicateEdge;

@@ -20,7 +20,7 @@ import torch
 
 from . import _lib
 from . import mesh_io
-from ._lib import (CompactStats, HoleParams, HoleStats, IntegrateParams, SimplifyParams, SimplifyStats, Library, MeshParams, MeshStats, MeshUpdateStats,
+from ._lib import (CompactStats, ComponentParams, ComponentStats, HoleParams, HoleStats, IntegrateParams, SimplifyParams, SimplifyStats, Library, MeshComponent, MeshParams, MeshStats, MeshUpdateStats,
                    PreprocessParams, RelocParams, RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats,
                    TextureParams, TextureStats, TextureViewDesc, TrackParams, TrackResult,
                    TrackRGBDParams, TrackRGBDResult,
@@ -678,6 +678,41 @@ class CUDASurfelReconstruction:
                       len(tri), C.c_void_p(out.data_ptr()), len(tri), C.byref(stats))
         return out[:int(stats.triangles_out)], stats
 
+    def mesh_components(self, triangles, params: Optional[ComponentParams] = None, stream=None):
+        """sm_mesh_components: the connected pieces of `triangles` (an int32 CUDA tensor [T, 3] of present slots, any
+        list without repeated corners; two triangles are connected when they share an edge; include/surfel_b200.h
+        gives the rules), and the triangles of the pieces that pass params (by default, pieces of at least 10
+        triangles). Synchronous. Returns (kept int32 CUDA tensor [T', 3], the input's triangles in input order;
+        labels int32 CUDA tensor [T], the number of each triangle's piece, pieces numbered by their first triangle;
+        the piece table, a dict of CUDA tensors over the P pieces: "triangles" int64 [P], "area" float64 [P] (m^2),
+        "lo" and "hi" float32 [P, 3] (smooth-position bounds), "first_triangle" int64 [P], "kept" bool [P];
+        ComponentStats)."""
+        p = ComponentParams.defaults() if params is None else params
+        _check_triangles(triangles)
+        tri = triangles.contiguous()
+        T = len(tri)
+        size = C.sizeof(MeshComponent)
+        out = torch.empty((max(T, 1), 3), dtype=torch.int32, device="cuda")
+        labels = torch.empty(max(T, 1), dtype=torch.int32, device="cuda")
+        raw = torch.empty((max(T, 1), size), dtype=torch.uint8, device="cuda")
+        if isinstance(stream, torch.cuda.Stream):
+            for t in (out, labels, raw):
+                t.record_stream(stream)
+        stats = ComponentStats()
+        self.lib.call("mesh_components", self._h, _stream_handle(stream), C.byref(p),
+                      C.c_void_p(tri.data_ptr()) if T else None, T, C.c_void_p(out.data_ptr()), T,
+                      C.c_void_p(labels.data_ptr()), C.c_void_p(raw.data_ptr()), T, C.byref(stats))
+        raw = raw[:int(stats.components)]
+        offset = {name: getattr(MeshComponent, name).offset for name, _ in MeshComponent._fields_}
+        table = {"triangles": raw[:, offset["triangles"]:offset["triangles"] + 8].contiguous().view(torch.int64)[:, 0],
+                 "area": raw[:, offset["area"]:offset["area"] + 8].contiguous().view(torch.float64)[:, 0],
+                 "lo": raw[:, offset["lo"]:offset["lo"] + 12].contiguous().view(torch.float32),
+                 "hi": raw[:, offset["hi"]:offset["hi"] + 12].contiguous().view(torch.float32),
+                 "first_triangle": raw[:, offset["first_triangle"]:offset["first_triangle"] + 4].contiguous()
+                 .view(torch.int32)[:, 0].to(torch.int64),
+                 "kept": raw[:, offset["kept"]:offset["kept"] + 4].contiguous().view(torch.int32)[:, 0] != 0}
+        return out[:int(stats.triangles_out)], labels[:T], table, stats
+
     def texture_mesh(self, triangles, views: Sequence[TextureView], params: Optional[TextureParams] = None,
                      stream=None):
         """sm_mesh_texture: a texture atlas for `triangles` (an int32 CUDA tensor [T, 3] of present slots, any list
@@ -727,11 +762,14 @@ class CUDASurfelReconstruction:
     def save_mesh_obj(self, path, params: Optional[MeshParams] = None, stream=None,
                       holes: Optional[HoleParams] = None, simplify: Optional[SimplifyParams] = None,
                       texture: Optional[TextureParams] = None,
-                      views: Optional[Sequence[TextureView]] = None) -> MeshStats:
+                      views: Optional[Sequence[TextureView]] = None,
+                      components: Optional[ComponentParams] = None) -> MeshStats:
         """The reference's SaveMeshAsOBJ (main.cc:128-175): the non-merged slots in slot order with their colour,
         and the triangles of triangulate() over them (1-based, remapped to that order). With `holes`, the
-        triangles of fill_holes(holes) follow the mesh's. With `simplify`, the mesh (with its fill) goes through
-        simplify_mesh(simplify), and only the slots that are corners of its triangles are written, in slot order.
+        triangles of fill_holes(holes) follow the mesh's. With `components`, only the triangles of the pieces that
+        mesh_components(components) keeps go on (after the fill, so floaters take no part of a simplification budget
+        or of the atlas). With `simplify`, the mesh goes through simplify_mesh(simplify). With `components` or
+        `simplify`, only the slots that are corners of the final triangles are written, in slot order.
         With `texture`, the final triangles are textured from `views` by texture_mesh(texture): the OBJ gets one
         texture coordinate per triangle corner and names the material of `path` with the suffix .mtl, whose
         diffuse map is the atlas written to `path` with the suffix .png."""
@@ -739,6 +777,8 @@ class CUDASurfelReconstruction:
         if holes is not None:
             fill, _ = self.fill_holes(tri, holes, stream)
             tri = torch.cat([tri, fill])
+        if components is not None:
+            tri = self.mesh_components(tri, components, stream)[0]
         if simplify is not None:
             tri, _ = self.simplify_mesh(tri, simplify, stream)
         uvs, material = None, None
@@ -751,8 +791,8 @@ class CUDASurfelReconstruction:
             mesh_io.write_mtl(mtl, png.name)
             uvs, material = uv.cpu().numpy(), mtl.name
         positions, colors = self.export_vertices_host(stream)
-        mesh_io.write_obj(path, positions, colors, tri.cpu().numpy(), referenced_only=simplify is not None, uvs=uvs,
-                          material=material)
+        mesh_io.write_obj(path, positions, colors, tri.cpu().numpy(),
+                          referenced_only=simplify is not None or components is not None, uvs=uvs, material=material)
         return stats
 
     def save_point_cloud_ply(self, path, stream=None) -> int:

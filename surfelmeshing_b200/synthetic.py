@@ -216,8 +216,9 @@ class SyntheticStream:
 
 
 def make_stream(camera: Camera, frame_count: int, stream_id: int = 0, sigma_depth=None, depth_scaling: float = 5000.0,
-                other_count: int = 8, device="cpu", dropout: float = 0.002) -> SyntheticStream:
-    """Generates a stream on `device` (CPU or CUDA; the GPU only does the ray casting)."""
+                other_count: int = 8, device="cpu", dropout: float = 0.002, noise_scale: float = 1.0) -> SyntheticStream:
+    """Generates a stream on `device` (CPU or CUDA; the GPU only does the ray casting). `noise_scale` multiplies the
+    depth-dependent noise model (used when sigma_depth is None)."""
     device = torch.device(device)
     poses64 = trajectory(frame_count, stream_id)
     gen = torch.Generator(device="cpu")
@@ -229,7 +230,7 @@ def make_stream(camera: Camera, frame_count: int, stream_id: int = 0, sigma_dept
         z, rgb = _raycast(camera, torch.from_numpy(poses64[i]).to(device), device)
         noise = torch.randn((H, W), generator=gen, dtype=torch.float64).to(device)
         if sigma_depth is None:
-            sigma = 0.0012 + 0.0019 * (z.clamp(max=10.0) - 0.4) ** 2
+            sigma = noise_scale * (0.0012 + 0.0019 * (z.clamp(max=10.0) - 0.4) ** 2)
         else:
             sigma = torch.full_like(z, float(sigma_depth))
         zn = z + sigma * noise
