@@ -57,8 +57,7 @@ struct ComponentCounters {
 
 // The scratch of sm_mesh_components: per triangle and per piece.
 struct ComponentScratch {
-  ComponentCounters* counters = nullptr;
-  ComponentCounters* host_counters = nullptr;
+  CounterMirror<ComponentCounters> counters;
   u64 triangle_capacity = 0;
   u64* edge_keys = nullptr;       // a power of two >= 4 x triangle_capacity
   u32* edge_owner = nullptr;      // the smallest triangle position on the edge
@@ -307,36 +306,39 @@ __global__ void __launch_bounds__(kBlock) k_cc_table(ComponentArgs a) {
   }
 }
 
+void FreeTriangleScratch(ComponentScratch& s) {
+  FreeAndClear(s.edge_keys, s.edge_owner, s.parent, s.roots, s.keep, s.scan_sums);
+  s.triangle_capacity = 0;
+}
+
 // Per-triangle scratch for `count` triangles (x 1.5 when it grows).
 int EnsureTriangleScratch(ComponentScratch& s, u64 count) {
   if (count <= s.triangle_capacity) return SM_OK;
-  const u64 cap = std::max<u64>(count + count / 2, 1024);
-  cudaFree(s.edge_keys); cudaFree(s.edge_owner); cudaFree(s.parent); cudaFree(s.roots); cudaFree(s.keep);
-  cudaFree(s.scan_sums);   // cudaFree synchronises the device: an earlier call may still use the buffers
-  s.edge_keys = nullptr; s.edge_owner = nullptr; s.parent = nullptr; s.roots = nullptr; s.keep = nullptr;
-  s.scan_sums = nullptr; s.triangle_capacity = 0;
+  const u64 cap = GrownCapacity(count);
+  FreeTriangleScratch(s);
   const u64 slots = PowerOfTwoAtLeast(4 * cap);
-  const u64 tiles = (cap + 1 + kScanTile - 1) / kScanTile;
   SM_CUDA(cudaMalloc(&s.edge_keys, sizeof(u64) * slots));
   SM_CUDA(cudaMalloc(&s.edge_owner, sizeof(u32) * slots));
   SM_CUDA(cudaMalloc(&s.parent, sizeof(u32) * cap));
   SM_CUDA(cudaMalloc(&s.roots, sizeof(u32) * (cap + 1)));
   SM_CUDA(cudaMalloc(&s.keep, sizeof(u32) * (cap + 1)));
-  SM_CUDA(cudaMalloc(&s.scan_sums, sizeof(u32) * tiles));
+  SM_CUDA(cudaMalloc(&s.scan_sums, sizeof(u32) * ScanTiles(cap + 1)));
   s.triangle_capacity = cap;
   return SM_OK;
+}
+
+void FreePieceScratch(ComponentScratch& s) {
+  FreeAndClear(s.count, s.q, s.lo, s.hi, s.first, s.kept, s.sort_keys, s.sorted_keys, s.sort_values, s.sorted_values,
+               s.sort_temp);
+  s.sort_temp_bytes = 0;
+  s.piece_capacity = 0;
 }
 
 // Per-piece scratch for `pieces` pieces (x 1.5 when it grows), with the rank sort's scratch.
 int EnsurePieceScratch(ComponentScratch& s, u64 pieces) {
   if (pieces <= s.piece_capacity) return SM_OK;
-  const u64 cap = std::max<u64>(pieces + pieces / 2, 1024);
-  cudaFree(s.count); cudaFree(s.q); cudaFree(s.lo); cudaFree(s.hi); cudaFree(s.first); cudaFree(s.kept);
-  cudaFree(s.sort_keys); cudaFree(s.sorted_keys); cudaFree(s.sort_values); cudaFree(s.sorted_values);
-  cudaFree(s.sort_temp);
-  s.count = nullptr; s.q = nullptr; s.lo = nullptr; s.hi = nullptr; s.first = nullptr; s.kept = nullptr;
-  s.sort_keys = nullptr; s.sorted_keys = nullptr; s.sort_values = nullptr; s.sorted_values = nullptr;
-  s.sort_temp = nullptr; s.sort_temp_bytes = 0; s.piece_capacity = 0;
+  const u64 cap = GrownCapacity(pieces);
+  FreePieceScratch(s);
   size_t temp = 0;
   SM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, temp, static_cast<const u64*>(nullptr), static_cast<u64*>(nullptr),
                                           static_cast<const u32*>(nullptr), static_cast<u32*>(nullptr),
@@ -357,32 +359,14 @@ int EnsurePieceScratch(ComponentScratch& s, u64 pieces) {
   return SM_OK;
 }
 
-// The exclusive scan of knn.cu over values[0, n].
-int Scan(cudaStream_t stream, u32* values, u32 n, u32* sums) {
-  const u32 scan_n = n + 1;
-  const u32 tiles = (scan_n + kScanTile - 1) / kScanTile;
-  SM_CUDA(cudaMemsetAsync(values + n, 0, sizeof(u32), stream));
-  { LaunchScope scope(stream, KID_COMPONENTS_SCAN); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(values, scan_n, sums); }
-  { LaunchScope scope(stream, KID_COMPONENTS_SCAN); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(sums, tiles); }
-  { LaunchScope scope(stream, KID_COMPONENTS_SCAN); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(values, scan_n, sums); }
-  return SM_OK;
-}
-
-// Bytes of `count` items of `size` bytes, saturated like the end of an address range.
-u64 Bytes(u64 count, u64 size) { return count > UINT64_MAX / size ? UINT64_MAX : count * size; }
-
 }  // namespace
 
 void FreeComponentBuffers(sm_reconstruction* r) {
   ComponentScratch* s = r->components;
   if (!s) return;
-  cudaFree(s->counters);
-  if (s->host_counters) cudaFreeHost(s->host_counters);
-  cudaFree(s->edge_keys); cudaFree(s->edge_owner); cudaFree(s->parent); cudaFree(s->roots); cudaFree(s->keep);
-  cudaFree(s->scan_sums);
-  cudaFree(s->count); cudaFree(s->q); cudaFree(s->lo); cudaFree(s->hi); cudaFree(s->first); cudaFree(s->kept);
-  cudaFree(s->sort_keys); cudaFree(s->sorted_keys); cudaFree(s->sort_values); cudaFree(s->sorted_values);
-  cudaFree(s->sort_temp);
+  FreeTriangleScratch(*s);
+  FreePieceScratch(*s);
+  FreeCounters(s->counters);
   delete s;
   r->components = nullptr;
 }
@@ -433,17 +417,12 @@ int sm_mesh_components(sm_reconstruction* r, void* stream_v, const sm_component_
   const double min_units = std::nearbyint(p.min_area * 0x1p30);
   const unsigned long long min_q = min_units >= 0x1p64 ? UINT64_MAX : static_cast<unsigned long long>(min_units);
 
-  if (!r->components) {   // published only with both counter buffers, so a failed first call is retried whole
-    ComponentCounters* counters = nullptr;
-    ComponentCounters* host_counters = nullptr;
-    SM_CUDA(cudaMalloc(&counters, sizeof(ComponentCounters)));
-    if (const cudaError_t e = cudaMallocHost(&host_counters, sizeof(ComponentCounters)); e != cudaSuccess) {
-      cudaFree(counters);
-      return SetError(SM_ERR_CUDA, (std::string("cudaMallocHost: ") + cudaGetErrorString(e)).c_str());
-    }
+  if (!r->components) {   // published only with its counters, so a failed first call is retried whole
+    CounterMirror<ComponentCounters> counters;
+    status = CreateCounters(counters);
+    if (status != SM_OK) return status;
     r->components = new ComponentScratch();
     r->components->counters = counters;
-    r->components->host_counters = host_counters;
   }
   ComponentScratch& s = *r->components;
   status = EnsureTriangleScratch(s, count);
@@ -464,9 +443,9 @@ int sm_mesh_components(sm_reconstruction* r, void* stream_v, const sm_component_
   a.keep = s.keep;
   a.min_triangles = p.min_triangles;
   a.min_q = min_q;
-  a.counters = s.counters;
-  ComponentCounters* c = s.counters;
-  const ComponentCounters& h = *s.host_counters;
+  a.counters = s.counters.device;
+  ComponentCounters* c = s.counters.device;
+  const ComponentCounters& h = *s.counters.host;
   const int grid = Grid(count, r->sm_count);
   SM_CUDA(cudaMemsetAsync(c, 0, sizeof(ComponentCounters), stream));
   SM_CUDA(cudaMemsetAsync(&c->largest, 0xFF, sizeof(u32), stream));
@@ -475,11 +454,11 @@ int sm_mesh_components(sm_reconstruction* r, void* stream_v, const sm_component_
   { LaunchScope scope(stream, KID_COMPONENTS_EDGES); LaunchKernel(k_cc_edges, dim3(grid), dim3(kBlock), 0, stream, a); }
   { LaunchScope scope(stream, KID_COMPONENTS_HOOK); LaunchKernel(k_cc_hook, dim3(grid), dim3(kBlock), 0, stream, a); }
   { LaunchScope scope(stream, KID_COMPONENTS_NUMBER); LaunchKernel(k_cc_number, dim3(grid), dim3(kBlock), 0, stream, a); }
-  status = Scan(stream, s.roots, a.count, s.scan_sums);
-  if (status != SM_OK) return status;
+  SM_CUDA(cudaMemsetAsync(s.roots + count, 0, sizeof(u32), stream));
+  ScanInPlace(stream, s.roots, a.count + 1, s.scan_sums, KID_COMPONENTS_SCAN);
   SM_CUDA(cudaMemcpyAsync(&c->components, s.roots + count, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
-  SM_CUDA(cudaMemcpyAsync(s.host_counters, c, sizeof(ComponentCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
+  status = ReadCounters(s.counters, stream);
+  if (status != SM_OK) return status;
   if (const char* why = MeshInputError(h.errors)) return bad(why);
   const u32 pieces = h.components;
 
@@ -514,21 +493,18 @@ int sm_mesh_components(sm_reconstruction* r, void* stream_v, const sm_component_
   }
   { LaunchScope scope(stream, KID_COMPONENTS_RANK); LaunchKernel(k_cc_keep, dim3(piece_grid), dim3(kBlock), 0, stream, a); }
   { LaunchScope scope(stream, KID_COMPONENTS_WRITE); LaunchKernel(k_cc_flags, dim3(grid), dim3(kBlock), 0, stream, a); }
-  status = Scan(stream, s.keep, a.count, s.scan_sums);
-  if (status != SM_OK) return status;
+  SM_CUDA(cudaMemsetAsync(s.keep + count, 0, sizeof(u32), stream));
+  ScanInPlace(stream, s.keep, a.count + 1, s.scan_sums, KID_COMPONENTS_SCAN);
   SM_CUDA(cudaMemcpyAsync(&c->triangles_out, s.keep + count, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
-  SM_CUDA(cudaMemcpyAsync(s.host_counters, c, sizeof(ComponentCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
+  status = ReadCounters(s.counters, stream);
+  if (status != SM_OK) return status;
   stats->triangles_in = count;
   stats->triangles_out = h.triangles_out;
   stats->components = pieces;
   stats->components_kept = h.kept;
   stats->largest_triangles = h.largest_triangles;
   stats->largest_area = std::ldexp(static_cast<double>(h.largest_q), -30);
-  if (out_capacity < h.triangles_out) {
-    return SetError(SM_ERR_CAPACITY, ("sm_mesh_components: " + std::to_string(h.triangles_out) +
-                                      " triangles do not fit the capacity of " + std::to_string(out_capacity)).c_str());
-  }
+  if (out_capacity < h.triangles_out) return TriangleCapacityError("sm_mesh_components", h.triangles_out, out_capacity);
   if (table && table_capacity < pieces) {
     return SetError(SM_ERR_CAPACITY, ("sm_mesh_components: " + std::to_string(pieces) +
                                       " pieces do not fit the table capacity of " + std::to_string(table_capacity)).c_str());

@@ -45,8 +45,7 @@ struct HoleCounters {
 
 // The scratch of sm_mesh_fill_holes: per input triangle (the edge table, the unsorted hole edges) and per hole edge.
 struct HoleScratch {
-  HoleCounters* counters = nullptr;
-  HoleCounters* host_counters = nullptr;
+  CounterMirror<HoleCounters> counters;
   u64* edge_table = nullptr; u64 edge_table_size = 0;   // a power of two >= 6 x triangle_capacity
   u64* unsorted = nullptr; u64 unsorted_capacity = 0;   // 3 x triangles
   u64 triangle_capacity = 0;
@@ -324,13 +323,16 @@ __global__ void __launch_bounds__(kBlock) k_hole_write(HoleArgs a) {
   }
 }
 
+void FreeTriangleScratch(HoleScratch& s) {
+  FreeAndClear(s.edge_table, s.unsorted);
+  s.triangle_capacity = 0;
+}
+
 // Per-triangle scratch for `count` triangles (x 1.5 when it grows).
 int EnsureTriangleScratch(HoleScratch& s, u64 count) {
   if (count <= s.triangle_capacity) return SM_OK;
-  const u64 cap = std::max<u64>(count + count / 2, 1024);
-  cudaFree(s.edge_table);   // cudaFree synchronises the device: an earlier call may still use the buffers
-  cudaFree(s.unsorted);
-  s.edge_table = nullptr; s.unsorted = nullptr; s.triangle_capacity = 0;
+  const u64 cap = GrownCapacity(count);
+  FreeTriangleScratch(s);
   const u64 table = PowerOfTwoAtLeast(6 * cap);
   SM_CUDA(cudaMalloc(&s.edge_table, sizeof(u64) * table));
   SM_CUDA(cudaMalloc(&s.unsorted, sizeof(u64) * 3 * cap));
@@ -339,28 +341,28 @@ int EnsureTriangleScratch(HoleScratch& s, u64 count) {
   return SM_OK;
 }
 
+void FreeHoleScratch(HoleScratch& s) {
+  FreeAndClear(s.sorted, s.sort_temp, s.loop_vertices, s.loop_triangles, s.loop_length, s.counts, s.scan_sums,
+               s.diag_keys, s.diag_lo, s.diag_hi);
+  s.hole_capacity = 0;
+}
+
 // Per-hole-edge scratch for `edges` hole edges (x 1.5 when it grows).
 int EnsureHoleScratch(HoleScratch& s, u32 edges) {
   if (edges <= s.hole_capacity) return SM_OK;
-  const u64 cap = std::max<u64>(edges + static_cast<u64>(edges) / 2, 1024);
-  cudaFree(s.sorted); cudaFree(s.sort_temp); cudaFree(s.loop_vertices); cudaFree(s.loop_triangles);
-  cudaFree(s.loop_length); cudaFree(s.counts); cudaFree(s.scan_sums); cudaFree(s.diag_keys); cudaFree(s.diag_lo);
-  cudaFree(s.diag_hi);
-  s.sorted = nullptr; s.sort_temp = nullptr; s.loop_vertices = nullptr; s.loop_triangles = nullptr;
-  s.loop_length = nullptr; s.counts = nullptr; s.scan_sums = nullptr; s.diag_keys = nullptr; s.diag_lo = nullptr;
-  s.diag_hi = nullptr; s.hole_capacity = 0;
+  const u64 cap = GrownCapacity(edges);
+  FreeHoleScratch(s);
   size_t temp = 0;
   SM_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, temp, static_cast<const u64*>(nullptr), static_cast<u64*>(nullptr),
                                          static_cast<int>(cap)));
   const u64 diag = PowerOfTwoAtLeast(2 * cap);
-  const u64 tiles = (cap + 1 + kScanTile - 1) / kScanTile;
   SM_CUDA(cudaMalloc(&s.sorted, sizeof(u64) * cap));
   SM_CUDA(cudaMalloc(&s.sort_temp, temp));
   SM_CUDA(cudaMalloc(&s.loop_vertices, sizeof(u32) * kMaxHole * cap));
   SM_CUDA(cudaMalloc(&s.loop_triangles, sizeof(u16) * (kMaxHole - 2) * cap));
   SM_CUDA(cudaMalloc(&s.loop_length, cap));
   SM_CUDA(cudaMalloc(&s.counts, sizeof(u32) * (cap + 1)));
-  SM_CUDA(cudaMalloc(&s.scan_sums, sizeof(u32) * tiles));
+  SM_CUDA(cudaMalloc(&s.scan_sums, sizeof(u32) * ScanTiles(cap + 1)));
   SM_CUDA(cudaMalloc(&s.diag_keys, sizeof(u64) * diag));
   SM_CUDA(cudaMalloc(&s.diag_lo, sizeof(u32) * diag));
   SM_CUDA(cudaMalloc(&s.diag_hi, sizeof(u32) * diag));
@@ -375,12 +377,9 @@ int EnsureHoleScratch(HoleScratch& s, u32 edges) {
 void FreeHoleBuffers(sm_reconstruction* r) {
   HoleScratch* s = r->holes;
   if (!s) return;
-  cudaFree(s->counters);
-  if (s->host_counters) cudaFreeHost(s->host_counters);
-  cudaFree(s->edge_table); cudaFree(s->unsorted);
-  cudaFree(s->sorted); cudaFree(s->sort_temp); cudaFree(s->loop_vertices); cudaFree(s->loop_triangles);
-  cudaFree(s->loop_length); cudaFree(s->counts); cudaFree(s->scan_sums); cudaFree(s->diag_keys);
-  cudaFree(s->diag_lo); cudaFree(s->diag_hi);
+  FreeTriangleScratch(*s);
+  FreeHoleScratch(*s);
+  FreeCounters(s->counters);
   delete s;
   r->holes = nullptr;
 }
@@ -415,10 +414,12 @@ int sm_mesh_fill_holes(sm_reconstruction* r, void* stream_v, const sm_hole_param
   if (count == 0) return SM_OK;
   const u32 n = r->host_counters->surfel_count[r->count_slot];
 
-  if (!r->holes) {
+  if (!r->holes) {   // published only with its counters, so a failed first call is retried whole
+    CounterMirror<HoleCounters> counters;
+    status = CreateCounters(counters);
+    if (status != SM_OK) return status;
     r->holes = new HoleScratch();
-    SM_CUDA(cudaMalloc(&r->holes->counters, sizeof(HoleCounters)));
-    SM_CUDA(cudaMallocHost(&r->holes->host_counters, sizeof(HoleCounters)));
+    r->holes->counters = counters;
   }
   HoleScratch& s = *r->holes;
   status = EnsureTriangleScratch(s, count);
@@ -439,19 +440,20 @@ int sm_mesh_fill_holes(sm_reconstruction* r, void* stream_v, const sm_hole_param
   a.edge_mask = edge_slots - 1;
   a.unsorted = s.unsorted;
   a.fill = reinterpret_cast<uint3*>(fill);
-  a.counters = s.counters;
+  a.counters = s.counters.device;
   if (n > 0) {
     status = MirrorRegRecords(stream, r->d, n, r->sm_count);   // rows 3-5 <- the current smooth positions
     if (status != SM_OK) return status;
   }
-  SM_CUDA(cudaMemsetAsync(s.counters, 0, sizeof(HoleCounters), stream));
+  SM_CUDA(cudaMemsetAsync(s.counters.device, 0, sizeof(HoleCounters), stream));
   SM_CUDA(cudaMemsetAsync(s.edge_table, 0xFF, sizeof(u64) * edge_slots, stream));
   { LaunchScope scope(stream, KID_HOLE_EDGES); LaunchKernel(k_hole_edges, dim3(Grid(count, r->sm_count)), dim3(kBlock), 0, stream, a); }
   { LaunchScope scope(stream, KID_HOLE_BOUNDARY); LaunchKernel(k_hole_boundary, dim3(Grid(3 * count, r->sm_count)), dim3(kBlock), 0, stream, a); }
-  SM_CUDA(cudaMemcpyAsync(s.host_counters, s.counters, sizeof(HoleCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
-  if (const char* why = MeshInputError(s.host_counters->errors)) return bad(why);
-  const u32 H = s.host_counters->hole_edges;
+  status = ReadCounters(s.counters, stream);
+  if (status != SM_OK) return status;
+  const HoleCounters& c = *s.counters.host;
+  if (const char* why = MeshInputError(c.errors)) return bad(why);
+  const u32 H = c.hole_edges;
   stats->boundary_edges = H;
   stats->boundary_edges_after = H;
   if (H == 0) return CheckLaunch("fill holes");
@@ -482,25 +484,17 @@ int sm_mesh_fill_holes(sm_reconstruction* r, void* stream_v, const sm_hole_param
   const int grid = Grid(H, r->sm_count);
   { LaunchScope scope(stream, KID_HOLE_WALK); LaunchKernel(k_hole_walk, dim3(grid), dim3(kBlock), 0, stream, a); }
   { LaunchScope scope(stream, KID_HOLE_CONFLICT); LaunchKernel(k_hole_conflict, dim3(grid), dim3(kBlock), 0, stream, a); }
-  const u32 scan_n = H + 1;
-  const u32 tiles = (scan_n + kScanTile - 1) / kScanTile;
-  { LaunchScope scope(stream, KID_HOLE_SCAN); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(s.counts, scan_n, s.scan_sums); }
-  { LaunchScope scope(stream, KID_HOLE_SCAN); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(s.scan_sums, tiles); }
-  { LaunchScope scope(stream, KID_HOLE_SCAN); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(s.counts, scan_n, s.scan_sums); }
-  SM_CUDA(cudaMemcpyAsync(&s.counters->triangles, s.counts + H, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
-  SM_CUDA(cudaMemcpyAsync(s.host_counters, s.counters, sizeof(HoleCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
-  const HoleCounters& c = *s.host_counters;
+  ScanInPlace(stream, s.counts, H + 1, s.scan_sums, KID_HOLE_SCAN);
+  SM_CUDA(cudaMemcpyAsync(&s.counters.device->triangles, s.counts + H, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  status = ReadCounters(s.counters, stream);
+  if (status != SM_OK) return status;
   stats->loops_found = c.loops_found;
   stats->loops_filled = c.loops_filled;
   stats->loops_rejected = c.loops_rejected;
   stats->loops_conflicting = c.loops_conflicting;
   stats->triangles_added = c.triangles;
   stats->boundary_edges_after = H - c.filled_edges;
-  if (capacity < stats->triangles_added) {
-    return SetError(SM_ERR_CAPACITY, ("sm_mesh_fill_holes: " + std::to_string(stats->triangles_added) +
-                                      " triangles do not fit the capacity of " + std::to_string(capacity)).c_str());
-  }
+  if (capacity < stats->triangles_added) return TriangleCapacityError("sm_mesh_fill_holes", stats->triangles_added, capacity);
   if (stats->triangles_added > 0) {
     LaunchScope scope(stream, KID_HOLE_WRITE);
     LaunchKernel(k_hole_write, dim3(grid), dim3(kBlock), 0, stream, a);

@@ -128,7 +128,7 @@ int CreateIndex(sm_knn_index* k, u32 max_points) {
   SM_CUDA(cudaDeviceGetAttribute(&k->sm_count, cudaDevAttrMultiProcessorCount, k->device));
   k->capacity = max_points;
   k->table_size = NextPowerOfTwo(std::max<u32>(1024u, 2u * max_points));
-  const u32 tiles = (k->table_size + 1 + kScanTile - 1) / kScanTile;
+  const u32 tiles = ScanTiles(k->table_size + 1);
   SM_CUDA(cudaMalloc(&k->bucket_start, sizeof(u32) * (static_cast<size_t>(k->table_size) + 1)));
   SM_CUDA(cudaMalloc(&k->bucket_cursor, sizeof(u32) * static_cast<size_t>(k->table_size)));
   SM_CUDA(cudaMalloc(&k->scan_sums, sizeof(u32) * tiles));
@@ -167,7 +167,7 @@ int KnnBuild(sm_knn_index* k, cudaStream_t stream, u32 n, const float* x, const 
   BuildArgs a{n, x, y, z, radius_squared, state, k->inverse_cell_size, k->table_size - 1, k->bucket_start,
               k->bucket_cursor, k->point_bucket, k->records};
   const u32 scan_n = k->table_size + 1;
-  const u32 tiles = (scan_n + kScanTile - 1) / kScanTile;
+  const u32 tiles = ScanTiles(scan_n);
   if (n > 0) {
     const int blocks = static_cast<int>(std::min<u32>((n + kBuildBlock - 1) / kBuildBlock, 8u * k->sm_count));
     k_knn_count<<<blocks, kBuildBlock, 0, stream>>>(a);

@@ -48,8 +48,7 @@ struct MeshScratch {
   u32* counts = nullptr;
   u32* scan_sums = nullptr;
   u32 slots = 0;
-  MeshCounters* counters = nullptr;
-  MeshCounters* host_counters = nullptr;
+  CounterMirror<MeshCounters> counters;
   int umbrella_blocks = 0, emit_blocks = 0;
   MeshLive* live = nullptr;   // created by the first sm_mesh_update
 };
@@ -658,40 +657,45 @@ __global__ void __launch_bounds__(kEmitBlock) k_mesh_recheck(MeshArgs a, UpdateA
 
 void FreeSlotScratch(MeshScratch& m) {
   KnnDestroy(m.index);
-  cudaFree(m.umbrella);
-  cudaFree(m.umbrella_count);
-  cudaFree(m.counts);
-  cudaFree(m.scan_sums);
   m.index = nullptr;
-  m.umbrella = nullptr;
-  m.umbrella_count = nullptr;
-  m.counts = nullptr;
-  m.scan_sums = nullptr;
+  FreeAndClear(m.umbrella, m.umbrella_count, m.counts, m.scan_sums);
   m.slots = 0;
 }
 
-// Scratch for n slots (grown, never shrunk); the counters and the grids are set up once.
+// Scratch for n slots (grown, never shrunk); the grids and the counters are set up once. The counters come last: a
+// first call that fails leaves them empty, and the next call sets everything up again.
 int EnsureMeshScratch(sm_reconstruction* r, u32 n) {
   if (!r->mesh) r->mesh = new MeshScratch();
   MeshScratch& m = *r->mesh;
-  if (!m.counters) {
-    SM_CUDA(cudaMalloc(&m.counters, sizeof(MeshCounters)));
-    SM_CUDA(cudaMallocHost(&m.host_counters, sizeof(MeshCounters)));
+  if (!m.counters.device) {
     int status = ResidentBlocks(k_mesh_umbrella, kUmbrellaBlock, r->sm_count, &m.umbrella_blocks);
     if (status == SM_OK) status = ResidentBlocks(k_mesh_count, kEmitBlock, r->sm_count, &m.emit_blocks);
+    if (status == SM_OK) status = CreateCounters(m.counters);
     if (status != SM_OK) return status;
   }
   if (n <= m.slots) return SM_OK;
-  FreeSlotScratch(m);   // cudaFree synchronises the device: an earlier call may still use the buffers
+  FreeSlotScratch(m);
   const int status = KnnCreate(&m.index, n);
   if (status != SM_OK) return status;
-  const u32 tiles = (n + 1 + kScanTile - 1) / kScanTile;
   SM_CUDA(cudaMalloc(&m.umbrella, sizeof(uint2) * kUmbrella * static_cast<size_t>(n)));
   SM_CUDA(cudaMalloc(&m.umbrella_count, sizeof(u32) * static_cast<size_t>(n)));
   SM_CUDA(cudaMalloc(&m.counts, sizeof(u32) * (static_cast<size_t>(n) + 1)));
-  SM_CUDA(cudaMalloc(&m.scan_sums, sizeof(u32) * tiles));
+  SM_CUDA(cudaMalloc(&m.scan_sums, sizeof(u32) * ScanTiles(n + 1)));
   m.slots = n;
   return SM_OK;
+}
+
+QueryArgs IndexQuery(const sm_knn_index* k) {
+  QueryArgs q{};
+  q.max_result_count = kMaxResults;
+  q.radius_scale = 1.f;
+  q.include_completed = 1;
+  q.include_free = 1;
+  q.inverse_cell_size = k->inverse_cell_size;
+  q.mask = k->table_size - 1;
+  q.bucket_start = k->bucket_start;
+  q.records = k->records;
+  return q;
 }
 
 
@@ -749,16 +753,17 @@ extern "C" int sm_triangulate(sm_reconstruction* r, void* stream_v, const sm_mes
   a.umbrella_count = m.umbrella_count;
   a.counts = m.counts;
   a.triangles = reinterpret_cast<uint3*>(triangles);
-  a.counters = m.counters;
+  a.counters = m.counters.device;
   status = MirrorRegRecords(stream, r->d, n, r->sm_count);   // rows 3-5 <- the current smooth positions
   if (status != SM_OK) return status;
-  SM_CUDA(cudaMemsetAsync(m.counters, 0, sizeof(MeshCounters), stream));
+  SM_CUDA(cudaMemsetAsync(m.counters.device, 0, sizeof(MeshCounters), stream));
   const int bound_blocks = static_cast<int>(std::min<u32>((n + kBoundBlock - 1) / kBoundBlock, 4u * r->sm_count));
   { LaunchScope scope(stream, KID_MESH_BOUND); LaunchKernel(k_mesh_bound, dim3(bound_blocks), dim3(kBoundBlock), 0, stream, a); }
-  SM_CUDA(cudaMemcpyAsync(m.host_counters, m.counters, sizeof(MeshCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
+  status = ReadCounters(m.counters, stream);
+  if (status != SM_OK) return status;
+  const MeshCounters& h = *m.counters.host;
   float max_r2;
-  std::memcpy(&max_r2, &m.host_counters->max_radius_squared_bits, sizeof(float));
+  std::memcpy(&max_r2, &h.max_radius_squared_bits, sizeof(float));
   if (!(max_r2 > 0.f)) return SM_OK;   // no present slot
   // Cell size: twice the largest query radius, so that a query touches at most 3 cells per axis.
   const float cell_size = 2.f * std::sqrt(max_r2 * f2);
@@ -767,39 +772,22 @@ extern "C" int sm_triangulate(sm_reconstruction* r, void* stream_v, const sm_mes
   status = KnnBuild(m.index, stream, n, s + SM_ROW_SMOOTH_X * st, s + SM_ROW_SMOOTH_Y * st,
                     s + SM_ROW_SMOOTH_Z * st, s + SM_ROW_RADIUS_SQUARED * st, nullptr, cell_size);
   if (status != SM_OK) return status;
-  sm_knn_index* k = m.index;
-  a.q = QueryArgs{};
-  a.q.max_result_count = kMaxResults;
-  a.q.radius_scale = 1.f;
-  a.q.include_completed = 1;
-  a.q.include_free = 1;
-  a.q.inverse_cell_size = k->inverse_cell_size;
-  a.q.mask = k->table_size - 1;
-  a.q.bucket_start = k->bucket_start;
-  a.q.records = k->records;
+  a.q = IndexQuery(m.index);
   const int umbrella_blocks =
       static_cast<int>(std::min<u32>((n + kUmbrellaBlock / 32 - 1) / (kUmbrellaBlock / 32), m.umbrella_blocks));
   const int emit_blocks = static_cast<int>(std::min<u32>((n + kEmitBlock - 1) / kEmitBlock, m.emit_blocks));
   { LaunchScope scope(stream, KID_MESH_UMBRELLA); LaunchKernel(k_mesh_umbrella, dim3(umbrella_blocks), dim3(kUmbrellaBlock), 0, stream, a); }
   SM_CUDA(cudaMemsetAsync(m.counts + n, 0, sizeof(u32), stream));
   { LaunchScope scope(stream, KID_MESH_COUNT); LaunchKernel(k_mesh_count, dim3(emit_blocks), dim3(kEmitBlock), 0, stream, a); }
-  const u32 scan_n = n + 1;
-  const u32 tiles = (scan_n + kScanTile - 1) / kScanTile;
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(m.counts, scan_n, m.scan_sums); }
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(m.scan_sums, tiles); }
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(m.counts, scan_n, m.scan_sums); }
-  SM_CUDA(cudaMemcpyAsync(&m.counters->triangle_count, m.counts + n, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
-  SM_CUDA(cudaMemcpyAsync(m.host_counters, m.counters, sizeof(MeshCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
-  const MeshCounters& h = *m.host_counters;
+  ScanInPlace(stream, m.counts, n + 1, m.scan_sums, KID_MESH_SCAN);
+  SM_CUDA(cudaMemcpyAsync(&m.counters.device->triangle_count, m.counts + n, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  status = ReadCounters(m.counters, stream);
+  if (status != SM_OK) return status;
   stats->triangle_count = h.triangle_count;
   stats->vertices_meshed = h.vertices_meshed;
   stats->boundary_edges = h.boundary_edges;
   stats->umbrella_overflows = h.umbrella_overflows;
-  if (capacity < stats->triangle_count) {
-    return SetError(SM_ERR_CAPACITY, ("sm_triangulate: " + std::to_string(stats->triangle_count) +
-                                      " triangles do not fit the capacity of " + std::to_string(capacity)).c_str());
-  }
+  if (capacity < stats->triangle_count) return TriangleCapacityError("sm_triangulate", stats->triangle_count, capacity);
   if (stats->triangle_count > 0) {
     LaunchScope scope(stream, KID_MESH_WRITE);
     LaunchKernel(k_mesh_write, dim3(emit_blocks), dim3(kEmitBlock), 0, stream, a);
@@ -829,8 +817,7 @@ struct MeshLive {
   u64 triangle_capacity[2] = {0, 0};
   uint3* added = nullptr; u64 added_capacity = 0;
   uint3* removed = nullptr; u64 removed_capacity = 0;
-  UpdateCounters* counters = nullptr;
-  UpdateCounters* host_counters = nullptr;  // pinned
+  CounterMirror<UpdateCounters> counters;
   // scratch of one update
   u8* in_a = nullptr;
   u8* in_r = nullptr;
@@ -851,11 +838,11 @@ void FreeLive(MeshLive* L) {
                   static_cast<void*>(L->overflow), static_cast<void*>(L->word), static_cast<void*>(L->offsets[0]),
                   static_cast<void*>(L->offsets[1]), static_cast<void*>(L->triangles[0]),
                   static_cast<void*>(L->triangles[1]), static_cast<void*>(L->added), static_cast<void*>(L->removed),
-                  static_cast<void*>(L->counters), static_cast<void*>(L->in_a), static_cast<void*>(L->in_r),
-                  static_cast<void*>(L->rebuild_list), static_cast<void*>(L->added_offsets),
-                  static_cast<void*>(L->removed_offsets), static_cast<void*>(L->scan_sums), static_cast<void*>(L->points)})
+                  static_cast<void*>(L->in_a), static_cast<void*>(L->in_r), static_cast<void*>(L->rebuild_list),
+                  static_cast<void*>(L->added_offsets), static_cast<void*>(L->removed_offsets),
+                  static_cast<void*>(L->scan_sums), static_cast<void*>(L->points)})
     cudaFree(q);
-  if (L->host_counters) cudaFreeHost(L->host_counters);
+  FreeCounters(L->counters);
   KnnDestroy(L->changed_index);
   delete L;
 }
@@ -898,21 +885,19 @@ class Growth {
   bool done_ = false;
 };
 
-// The counters and grids on the first call; per-slot arrays for `slots` slots (x 1.5 when they grow, behind one
-// synchronisation).
+// The grids and the counters on the first call (the counters last, as in EnsureMeshScratch); per-slot arrays for
+// `slots` slots (x 1.5 when they grow, behind one synchronisation).
 int EnsureLive(MeshLive& L, cudaStream_t stream, u32 slots, int sm_count) {
-  if (!L.counters) {
-    SM_CUDA(cudaMalloc(&L.counters, sizeof(UpdateCounters)));
-    SM_CUDA(cudaMemset(L.counters, 0, sizeof(UpdateCounters)));
-    SM_CUDA(cudaMallocHost(&L.host_counters, sizeof(UpdateCounters)));
+  if (!L.counters.device) {
     int status = ResidentBlocks(k_mesh_umbrella_update, kUmbrellaBlock, sm_count, &L.umbrella_blocks);
     if (status == SM_OK) status = ResidentBlocks(k_mesh_recheck<false>, kEmitBlock, sm_count, &L.emit_blocks);
+    if (status == SM_OK) status = CreateCounters(L.counters);
     if (status != SM_OK) return status;
+    SM_CUDA(cudaMemset(L.counters.device, 0, sizeof(UpdateCounters)));
   }
   if (slots <= L.slots) return SM_OK;
   const size_t cap = std::max<size_t>(slots, static_cast<size_t>(L.slots) * 3 / 2);
   const size_t keep = L.n_prev;   // (0 unless the previous update completed)
-  const size_t tiles = (cap + 1 + kScanTile - 1) / kScanTile;
   Growth g(stream);
   g.grow(&L.snapshot, cap * kSnapshotWords, keep * kSnapshotWords);
   g.grow(&L.umbrella, cap * kUmbrella, keep * kUmbrella);
@@ -926,7 +911,7 @@ int EnsureLive(MeshLive& L, cudaStream_t stream, u32 slots, int sm_count) {
   g.grow(&L.rebuild_list, cap, 0);
   g.grow(&L.added_offsets, cap + 1, 0);
   g.grow(&L.removed_offsets, cap + 1, 0);
-  g.grow(&L.scan_sums, tiles, 0);
+  g.grow(&L.scan_sums, ScanTiles(cap + 1), 0);
   g.grow(&L.points, 4 * 2 * cap, 0);
   const int status = g.finish();
   if (status != SM_OK) return status;
@@ -937,33 +922,12 @@ int EnsureLive(MeshLive& L, cudaStream_t stream, u32 slots, int sm_count) {
 // A triangle buffer of at least `count` (x 1.5 when it grows); its content is not kept.
 int EnsureTriangles(uint3** p, u64* capacity, u64 count) {
   if (count <= *capacity) return SM_OK;
-  const u64 grown = std::max<u64>(count + count / 2, 1024);
-  cudaFree(*p);
-  *p = nullptr;
+  const u64 grown = GrownCapacity(count);
+  FreeAndClear(*p);
   *capacity = 0;
   SM_CUDA(cudaMalloc(p, sizeof(uint3) * grown));
   *capacity = grown;
   return SM_OK;
-}
-
-void ScanCounts(cudaStream_t stream, u32* values, u32 count, u32* sums) {
-  const u32 tiles = (count + kScanTile - 1) / kScanTile;
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(values, count, sums); }
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(sums, tiles); }
-  { LaunchScope scope(stream, KID_MESH_SCAN); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(values, count, sums); }
-}
-
-QueryArgs IndexQuery(const sm_knn_index* k) {
-  QueryArgs q{};
-  q.max_result_count = kMaxResults;
-  q.radius_scale = 1.f;
-  q.include_completed = 1;
-  q.include_free = 1;
-  q.inverse_cell_size = k->inverse_cell_size;
-  q.mask = k->table_size - 1;
-  q.bucket_start = k->bucket_start;
-  q.records = k->records;
-  return q;
 }
 
 int Grid(u32 items, int block, int resident) {
@@ -976,8 +940,7 @@ void FreeMeshBuffers(sm_reconstruction* r) {
   MeshScratch* m = r->mesh;
   if (!m) return;
   FreeSlotScratch(*m);
-  cudaFree(m->counters);
-  if (m->host_counters) cudaFreeHost(m->host_counters);
+  FreeCounters(m->counters);
   FreeLive(m->live);
   delete m;
   r->mesh = nullptr;
@@ -1007,7 +970,7 @@ extern "C" int sm_mesh_update(sm_reconstruction* r, void* stream_v, const sm_mes
   const u32 n_prev = L.n_prev, n_max = std::max(n, n_prev);
   status = EnsureLive(L, stream, std::max(n_max, 1u), r->sm_count);
   if (status != SM_OK) return status;
-  if (!was_valid) SM_CUDA(cudaMemsetAsync(L.counters, 0, sizeof(UpdateCounters), stream));
+  if (!was_valid) SM_CUDA(cudaMemsetAsync(L.counters.device, 0, sizeof(UpdateCounters), stream));
   bool everything = !was_valid || n < n_prev || std::memcmp(&p, &L.params, sizeof(p)) != 0;
   const int previous = L.current, next = previous ^ 1;
 
@@ -1021,7 +984,7 @@ extern "C" int sm_mesh_update(sm_reconstruction* r, void* stream_v, const sm_mes
   a.cos_triangle = CosDegrees(p.max_triangle_angle_deg);
   a.umbrella = L.umbrella;
   a.umbrella_count = L.umbrella_count;
-  a.counters = &L.counters->bound;
+  a.counters = &L.counters.device->bound;
   UpdateArgs u{};
   u.n_prev = n_prev;
   u.n_max = n_max;
@@ -1039,10 +1002,10 @@ extern "C" int sm_mesh_update(sm_reconstruction* r, void* stream_v, const sm_mes
   u.new_offsets = L.offsets[next];
   u.added_offsets = L.added_offsets;
   u.removed_offsets = L.removed_offsets;
-  u.counters = L.counters;
+  u.counters = L.counters.device;
 
   const size_t per_call = offsetof(UpdateCounters, bound);
-  SM_CUDA(cudaMemsetAsync(reinterpret_cast<char*>(L.counters) + per_call, 0, sizeof(UpdateCounters) - per_call, stream));
+  SM_CUDA(cudaMemsetAsync(reinterpret_cast<char*>(L.counters.device) + per_call, 0, sizeof(UpdateCounters) - per_call, stream));
   if (n > 0) {
     status = MirrorRegRecords(stream, r->d, n, r->sm_count);   // rows 3-5 <- the current smooth positions
     if (status != SM_OK) return status;
@@ -1054,11 +1017,11 @@ extern "C" int sm_mesh_update(sm_reconstruction* r, void* stream_v, const sm_mes
     LaunchScope scope(stream, KID_MESH_CHANGES);
     LaunchKernel(k_mesh_changes, dim3(Grid(n_max, kEmitBlock, L.emit_blocks)), dim3(kEmitBlock), 0, stream, a, u);
   }
-  SM_CUDA(cudaMemcpyAsync(L.host_counters, L.counters, sizeof(UpdateCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
-  const u32 changed = L.host_counters->changed;
+  status = ReadCounters(L.counters, stream);
+  if (status != SM_OK) return status;
+  const u32 changed = L.counters.host->changed;
   float max_r2;
-  std::memcpy(&max_r2, &L.host_counters->bound.max_radius_squared_bits, sizeof(float));
+  std::memcpy(&max_r2, &L.counters.host->bound.max_radius_squared_bits, sizeof(float));
   if (!(max_r2 > 0.f)) everything = true;   // no present slot: every umbrella is empty, no query runs
   // Past this share of changed slots, marking A (an index over 2 |C| points and a query per slot) costs more than
   // the list can save: every slot is rebuilt, as sm_triangulate does.
@@ -1117,15 +1080,15 @@ extern "C" int sm_mesh_update(sm_reconstruction* r, void* stream_v, const sm_mes
     LaunchScope scope(stream, KID_MESH_RECHECK);
     LaunchKernel(k_mesh_recheck<false>, dim3(emit_blocks), dim3(kEmitBlock), 0, stream, a, u);
   }
-  ScanCounts(stream, u.new_offsets, n_max + 1, L.scan_sums);
-  ScanCounts(stream, u.added_offsets, n_max + 1, L.scan_sums);
-  ScanCounts(stream, u.removed_offsets, n_max + 1, L.scan_sums);
-  SM_CUDA(cudaMemcpyAsync(&L.counters->triangle_count, u.new_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
-  SM_CUDA(cudaMemcpyAsync(&L.counters->added, u.added_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
-  SM_CUDA(cudaMemcpyAsync(&L.counters->removed, u.removed_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
-  SM_CUDA(cudaMemcpyAsync(L.host_counters, L.counters, sizeof(UpdateCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
-  const UpdateCounters h = *L.host_counters;
+  ScanInPlace(stream, u.new_offsets, n_max + 1, L.scan_sums, KID_MESH_SCAN);
+  ScanInPlace(stream, u.added_offsets, n_max + 1, L.scan_sums, KID_MESH_SCAN);
+  ScanInPlace(stream, u.removed_offsets, n_max + 1, L.scan_sums, KID_MESH_SCAN);
+  SM_CUDA(cudaMemcpyAsync(&L.counters.device->triangle_count, u.new_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  SM_CUDA(cudaMemcpyAsync(&L.counters.device->added, u.added_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  SM_CUDA(cudaMemcpyAsync(&L.counters.device->removed, u.removed_offsets + n_max, sizeof(u32), cudaMemcpyDeviceToDevice, stream));
+  status = ReadCounters(L.counters, stream);
+  if (status != SM_OK) return status;
+  const UpdateCounters h = *L.counters.host;
   status = EnsureTriangles(&L.triangles[next], &L.triangle_capacity[next], h.triangle_count);
   if (status == SM_OK) status = EnsureTriangles(&L.added, &L.added_capacity, h.added);
   if (status == SM_OK) status = EnsureTriangles(&L.removed, &L.removed_capacity, h.removed);
@@ -1242,10 +1205,7 @@ extern "C" int sm_mesh_read(sm_reconstruction* r, void* stream_v, int32_t which,
   const uint3* src = which == SM_MESH_ALL ? L->triangles[L->current] : (which == SM_MESH_ADDED ? L->added : L->removed);
   const u64 size = which == SM_MESH_ALL ? L->triangle_count : (which == SM_MESH_ADDED ? L->added_count : L->removed_count);
   *count = size;
-  if (capacity < size) {
-    return SetError(SM_ERR_CAPACITY, ("sm_mesh_read: " + std::to_string(size) + " triangles do not fit the capacity of " +
-                                      std::to_string(capacity)).c_str());
-  }
+  if (capacity < size) return TriangleCapacityError("sm_mesh_read", size, capacity);
   r->last_stream = stream;
   if (size > 0) SM_CUDA(cudaMemcpyAsync(triangles, src, sizeof(uint3) * size, cudaMemcpyDeviceToDevice, stream));
   return SM_OK;

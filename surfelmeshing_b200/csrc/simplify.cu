@@ -58,8 +58,7 @@ struct SimplifyCounters {
 
 // The scratch of sm_mesh_simplify: per input triangle and per slot.
 struct SimplifyScratch {
-  SimplifyCounters* counters = nullptr;
-  SimplifyCounters* host_counters = nullptr;
+  CounterMirror<SimplifyCounters> counters;
   u64 triangle_capacity = 0;
   u64* edge_table = nullptr;      // a power of two >= 6 x triangle_capacity
   uint3* tri = nullptr;           // the working list by input position
@@ -374,33 +373,36 @@ __global__ void __launch_bounds__(kBlock) k_simplify_write(SimplifyArgs a) {
   }
 }
 
+void FreeTriangleScratch(SimplifyScratch& s) {
+  FreeAndClear(s.edge_table, s.tri, s.corners, s.sorted, s.counts, s.scan_sums);
+  s.triangle_capacity = 0;
+}
+
 // Per-triangle scratch for `count` triangles (x 1.5 when it grows).
 int EnsureTriangleScratch(SimplifyScratch& s, u64 count) {
   if (count <= s.triangle_capacity) return SM_OK;
-  const u64 cap = std::max<u64>(count + count / 2, 1024);
-  cudaFree(s.edge_table); cudaFree(s.tri); cudaFree(s.corners); cudaFree(s.sorted); cudaFree(s.counts);
-  cudaFree(s.scan_sums);   // cudaFree synchronises the device: an earlier call may still use the buffers
-  s.edge_table = nullptr; s.tri = nullptr; s.corners = nullptr; s.sorted = nullptr; s.counts = nullptr;
-  s.scan_sums = nullptr; s.triangle_capacity = 0;
-  const u64 tiles = (3 * cap + 1 + kScanTile - 1) / kScanTile;
+  const u64 cap = GrownCapacity(count);
+  FreeTriangleScratch(s);
   SM_CUDA(cudaMalloc(&s.edge_table, sizeof(u64) * PowerOfTwoAtLeast(6 * cap)));
   SM_CUDA(cudaMalloc(&s.tri, sizeof(uint3) * cap));
   SM_CUDA(cudaMalloc(&s.corners, sizeof(u64) * 3 * cap));
   SM_CUDA(cudaMalloc(&s.sorted, sizeof(u64) * 3 * cap));
   SM_CUDA(cudaMalloc(&s.counts, sizeof(u32) * (3 * cap + 1)));
-  SM_CUDA(cudaMalloc(&s.scan_sums, sizeof(u32) * tiles));
+  SM_CUDA(cudaMalloc(&s.scan_sums, sizeof(u32) * ScanTiles(3 * cap + 1)));
   s.triangle_capacity = cap;
   return SM_OK;
+}
+
+void FreeSlotScratch(SimplifyScratch& s) {
+  FreeAndClear(s.quadric, s.begin, s.end, s.mark, s.key, s.best, s.cost, s.vertices, s.selected, s.selected_sorted);
+  s.slot_capacity = 0;
 }
 
 // Per-slot scratch for `n` slots (x 1.5 when it grows).
 int EnsureSlotScratch(SimplifyScratch& s, u32 n) {
   if (n <= s.slot_capacity) return SM_OK;
-  const u64 cap = std::max<u64>(n + static_cast<u64>(n) / 2, 1024);
-  cudaFree(s.quadric); cudaFree(s.begin); cudaFree(s.end); cudaFree(s.mark); cudaFree(s.key); cudaFree(s.best);
-  cudaFree(s.cost); cudaFree(s.vertices); cudaFree(s.selected); cudaFree(s.selected_sorted);
-  s.quadric = nullptr; s.begin = nullptr; s.end = nullptr; s.mark = nullptr; s.key = nullptr; s.best = nullptr;
-  s.cost = nullptr; s.vertices = nullptr; s.selected = nullptr; s.selected_sorted = nullptr; s.slot_capacity = 0;
+  const u64 cap = GrownCapacity(n);
+  FreeSlotScratch(s);
   SM_CUDA(cudaMalloc(&s.quadric, sizeof(Quadric) * cap));
   SM_CUDA(cudaMalloc(&s.begin, sizeof(u32) * cap));
   SM_CUDA(cudaMalloc(&s.end, sizeof(u32) * cap));
@@ -415,6 +417,11 @@ int EnsureSlotScratch(SimplifyScratch& s, u32 n) {
   return SM_OK;
 }
 
+void FreeSortScratch(SimplifyScratch& s) {
+  FreeAndClear(s.sort_temp);
+  s.sort_temp_bytes = 0;
+}
+
 // The sort's scratch for the corners of triangle_capacity triangles and the keys of slot_capacity slots.
 int EnsureSortScratch(SimplifyScratch& s) {
   size_t corners = 0, keys = 0;
@@ -424,8 +431,7 @@ int EnsureSortScratch(SimplifyScratch& s) {
                                          static_cast<int>(s.slot_capacity)));
   const size_t bytes = std::max(corners, keys);
   if (bytes <= s.sort_temp_bytes) return SM_OK;
-  cudaFree(s.sort_temp);
-  s.sort_temp = nullptr; s.sort_temp_bytes = 0;
+  FreeSortScratch(s);
   SM_CUDA(cudaMalloc(&s.sort_temp, bytes));
   s.sort_temp_bytes = bytes;
   return SM_OK;
@@ -448,13 +454,10 @@ int Stop(const sm_simplify_params& p, u64 triangles, u64 rounds) {
 void FreeSimplifyBuffers(sm_reconstruction* r) {
   SimplifyScratch* s = r->simplify;
   if (!s) return;
-  cudaFree(s->counters);
-  if (s->host_counters) cudaFreeHost(s->host_counters);
-  cudaFree(s->edge_table); cudaFree(s->tri); cudaFree(s->corners); cudaFree(s->sorted); cudaFree(s->counts);
-  cudaFree(s->scan_sums);
-  cudaFree(s->quadric); cudaFree(s->begin); cudaFree(s->end); cudaFree(s->mark); cudaFree(s->key); cudaFree(s->best);
-  cudaFree(s->cost); cudaFree(s->vertices); cudaFree(s->selected); cudaFree(s->selected_sorted);
-  cudaFree(s->sort_temp);
+  FreeTriangleScratch(*s);
+  FreeSlotScratch(*s);
+  FreeSortScratch(*s);
+  FreeCounters(s->counters);
   delete s;
   r->simplify = nullptr;
 }
@@ -487,8 +490,7 @@ int sm_mesh_simplify(sm_reconstruction* r, void* stream_v, const sm_simplify_par
   if (p.max_rounds < 0 || p.max_rounds > SM_SIMPLIFY_MAX_ROUNDS) return bad("max_rounds must be in [0, SM_SIMPLIFY_MAX_ROUNDS]");
   if (const char* why = TriangleListError(triangles, count, !out && capacity > 0 ? "out is NULL with a capacity > 0" : nullptr))
     return bad(why);
-  // (12 x capacity can pass 2^64: saturated, like the end of the range)
-  if (count > 0 && capacity > 0 && Overlap(triangles, 12 * count, out, capacity > UINT64_MAX / 12 ? UINT64_MAX : 12 * capacity))
+  if (count > 0 && capacity > 0 && Overlap(triangles, 12 * count, out, Bytes(capacity, 12)))
     return bad("out overlaps triangles");
   r->last_stream = stream;
   int status = FetchCounters(r, stream);
@@ -499,17 +501,12 @@ int sm_mesh_simplify(sm_reconstruction* r, void* stream_v, const sm_simplify_par
   }
   const u32 n = r->host_counters->surfel_count[r->count_slot];
 
-  if (!r->simplify) {   // published only with both counter buffers, so a failed first call is retried whole
-    SimplifyCounters* counters = nullptr;
-    SimplifyCounters* host_counters = nullptr;
-    SM_CUDA(cudaMalloc(&counters, sizeof(SimplifyCounters)));
-    if (const cudaError_t e = cudaMallocHost(&host_counters, sizeof(SimplifyCounters)); e != cudaSuccess) {
-      cudaFree(counters);
-      return SetError(SM_ERR_CUDA, (std::string("cudaMallocHost: ") + cudaGetErrorString(e)).c_str());
-    }
+  if (!r->simplify) {   // published only with its counters, so a failed first call is retried whole
+    CounterMirror<SimplifyCounters> counters;
+    status = CreateCounters(counters);
+    if (status != SM_OK) return status;
     r->simplify = new SimplifyScratch();
     r->simplify->counters = counters;
-    r->simplify->host_counters = host_counters;
   }
   SimplifyScratch& s = *r->simplify;
   status = EnsureTriangleScratch(s, count);
@@ -538,19 +535,19 @@ int sm_mesh_simplify(sm_reconstruction* r, void* stream_v, const sm_simplify_par
   a.cos_normal = CosDegrees(p.max_angle_between_normals_deg);
   a.cos_triangle = CosDegrees(p.max_triangle_angle_deg);
   a.max_cost = p.max_cost;
-  a.counters = s.counters;
+  a.counters = s.counters.device;
   if (n > 0) {
     status = MirrorRegRecords(stream, r->d, n, r->sm_count);   // rows 3-5 <- the current smooth positions
     if (status != SM_OK) return status;
   }
-  SimplifyCounters* c = s.counters;
-  const SimplifyCounters& h = *s.host_counters;
+  SimplifyCounters* c = s.counters.device;
+  const SimplifyCounters& h = *s.counters.host;
   SM_CUDA(cudaMemsetAsync(c, 0, sizeof(SimplifyCounters), stream));
   SM_CUDA(cudaMemsetAsync(s.edge_table, 0xFF, sizeof(u64) * edge_slots, stream));
   { LaunchScope scope(stream, KID_SIMPLIFY_EDGES); LaunchKernel(k_simplify_edges, dim3(Grid(count, r->sm_count)), dim3(kBlock), 0, stream, a); }
   { LaunchScope scope(stream, KID_SIMPLIFY_EDGES); LaunchKernel(k_simplify_boundary, dim3(Grid(3 * count, r->sm_count)), dim3(kBlock), 0, stream, a); }
-  SM_CUDA(cudaMemcpyAsync(s.host_counters, c, sizeof(SimplifyCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
+  status = ReadCounters(s.counters, stream);
+  if (status != SM_OK) return status;
   if (const char* why = MeshInputError(h.errors)) return bad(why);
   const u64 boundary_edges = h.boundary_edges;
 
@@ -582,8 +579,8 @@ int sm_mesh_simplify(sm_reconstruction* r, void* stream_v, const sm_simplify_par
     SM_CUDA(cudaMemsetAsync(&c->selected, 0, sizeof(u32), stream));
     { LaunchScope scope(stream, KID_SIMPLIFY_CANDIDATES); LaunchKernel(k_simplify_candidates, dim3(vertex_grid), dim3(kBlock), 0, stream, a); }
     { LaunchScope scope(stream, KID_SIMPLIFY_SELECT); LaunchKernel(k_simplify_select, dim3(vertex_grid), dim3(kBlock), 0, stream, a); }
-    SM_CUDA(cudaMemcpyAsync(s.host_counters, c, sizeof(SimplifyCounters), cudaMemcpyDeviceToHost, stream));
-    SM_CUDA(cudaStreamSynchronize(stream));
+    status = ReadCounters(s.counters, stream);
+    if (status != SM_OK) return status;
     if (!have_vertices_in) { vertices_in = h.vertices; have_vertices_in = true; }
     const u64 selected = h.selected;
     if (selected == 0) { reason = SM_SIMPLIFY_STOP_CONVERGED; break; }
@@ -610,14 +607,10 @@ int sm_mesh_simplify(sm_reconstruction* r, void* stream_v, const sm_simplify_par
 
   // S8: the owner corners in (slot, position) order give the output order.
   { LaunchScope scope(stream, KID_SIMPLIFY_WRITE); LaunchKernel(k_simplify_owners, dim3(Grid(3 * T, r->sm_count)), dim3(kBlock), 0, stream, a); }
-  const u32 scan_n = static_cast<u32>(3 * T + 1);
-  const u32 tiles = (scan_n + kScanTile - 1) / kScanTile;
   SM_CUDA(cudaMemsetAsync(s.counts + 3 * T, 0, sizeof(u32), stream));
-  { LaunchScope scope(stream, KID_SIMPLIFY_SCAN); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(s.counts, scan_n, s.scan_sums); }
-  { LaunchScope scope(stream, KID_SIMPLIFY_SCAN); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(s.scan_sums, tiles); }
-  { LaunchScope scope(stream, KID_SIMPLIFY_SCAN); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(s.counts, scan_n, s.scan_sums); }
-  SM_CUDA(cudaMemcpyAsync(s.host_counters, c, sizeof(SimplifyCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
+  ScanInPlace(stream, s.counts, static_cast<u32>(3 * T + 1), s.scan_sums, KID_SIMPLIFY_SCAN);
+  status = ReadCounters(s.counters, stream);
+  if (status != SM_OK) return status;
   stats->triangles_in = count;
   stats->triangles_out = T;
   stats->vertices_in = have_vertices_in ? vertices_in : h.vertices;
@@ -627,10 +620,7 @@ int sm_mesh_simplify(sm_reconstruction* r, void* stream_v, const sm_simplify_par
   stats->boundary_edges = boundary_edges;
   std::memcpy(&stats->max_cost_applied, &h.max_cost_bits, sizeof(double));
   stats->stop_reason = reason;
-  if (capacity < T) {
-    return SetError(SM_ERR_CAPACITY, ("sm_mesh_simplify: " + std::to_string(T) + " triangles do not fit the capacity of " +
-                                      std::to_string(capacity)).c_str());
-  }
+  if (capacity < T) return TriangleCapacityError("sm_mesh_simplify", T, capacity);
   if (T > 0) {
     LaunchScope scope(stream, KID_SIMPLIFY_WRITE);
     LaunchKernel(k_simplify_write, dim3(Grid(3 * T, r->sm_count)), dim3(kBlock), 0, stream, a);

@@ -1,6 +1,7 @@
 // sm_knn.cuh — the k-NN index, its three-launch exclusive scan and the warp query core, shared by knn.cu (the
-// sm_knn_* entry points) and mesh.cu (sm_triangulate). The library is built without relocatable device code, so
-// the kernels and device functions live here and each translation unit compiles its own copy.
+// sm_knn_* entry points) and mesh.cu (sm_triangulate); the mesh calls use the scan too. The library is built without
+// relocatable device code, so the kernels and device functions live here and each translation unit compiles its own
+// copy.
 #pragma once
 
 #include <climits>
@@ -150,6 +151,17 @@ __global__ void __launch_bounds__(kScanBlock) k_knn_scan_add(u32* values, u32 n,
   for (int k = 0; k < kScanPerThread; ++k) {
     if (base + k < n) values[base + k] += offset;
   }
+}
+
+// The tiles of a scan over n values: the entries its tile sums take.
+inline u32 ScanTiles(u64 n) { return static_cast<u32>((n + kScanTile - 1) / kScanTile); }
+
+// The exclusive scan of values[0, n) in place, each of its launches in a LaunchScope of `id`.
+inline void ScanInPlace(cudaStream_t stream, u32* values, u32 n, u32* sums, KernelId id) {
+  const u32 tiles = ScanTiles(n);
+  { LaunchScope scope(stream, id); k_knn_scan_tiles<<<tiles, kScanBlock, 0, stream>>>(values, n, sums); }
+  { LaunchScope scope(stream, id); k_knn_scan_sums<<<1, kScanBlock, 0, stream>>>(sums, tiles); }
+  { LaunchScope scope(stream, id); k_knn_scan_add<<<tiles, kScanBlock, 0, stream>>>(values, n, sums); }
 }
 
 struct QueryArgs {

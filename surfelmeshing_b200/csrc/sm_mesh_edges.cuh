@@ -1,14 +1,15 @@
 // sm_mesh_edges.cuh — the edge hash table, the input checks and the fp32 corner geometry of a triangle list over the
 // handle's slots, shared by holes.cu (sm_mesh_fill_holes), simplify.cu (sm_mesh_simplify), texture.cu
-// (sm_mesh_texture) and components.cu (sm_mesh_components), and the host checks of those four calls and of mesh.cu
-// (sm_triangulate, sm_mesh_update). The first two take an edge-manifold, consistently oriented list, refuse the same
-// inputs and test new triangles by rule 4.
+// (sm_mesh_texture) and components.cu (sm_mesh_components), and the host checks and scratch handling of those four
+// calls and of mesh.cu (sm_triangulate, sm_mesh_update). The first two take an edge-manifold, consistently oriented
+// list, refuse the same inputs and test new triangles by rule 4.
 // The library is built without relocatable device code, so each translation unit compiles its own copy.
 #pragma once
 
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <string>
 
 #include "sm_handle.cuh"
 #include "sm_knn.cuh"
@@ -152,6 +153,59 @@ inline bool Overlap(const void* a, u64 a_bytes, const void* b, u64 b_bytes) {
   const uintptr_t a1 = a_bytes > UINTPTR_MAX - a0 ? UINTPTR_MAX : a0 + a_bytes;
   const uintptr_t b1 = b_bytes > UINTPTR_MAX - b0 ? UINTPTR_MAX : b0 + b_bytes;
   return a0 < b1 && b0 < a1;
+}
+
+// Bytes of `count` items of `size` bytes, saturated like the end of an address range.
+inline u64 Bytes(u64 count, u64 size) { return count > UINT64_MAX / size ? UINT64_MAX : count * size; }
+
+// The SM_ERR_CAPACITY of `who` when an output list of `capacity` triangles cannot take `count`.
+inline int TriangleCapacityError(const char* who, u64 count, u64 capacity) {
+  return SetError(SM_ERR_CAPACITY, (std::string(who) + ": " + std::to_string(count) +
+                                    " triangles do not fit the capacity of " + std::to_string(capacity)).c_str());
+}
+
+// The capacity a group of scratch buffers grows to when `need` items do not fit: x 1.5, at least `floor`.
+inline u64 GrownCapacity(u64 need, u64 floor = 1024) { return std::max<u64>(need + need / 2, floor); }
+
+// Frees each buffer and sets it to NULL. cudaFree synchronises the device: an earlier call may still use them.
+template <class... T>
+void FreeAndClear(T*&... buffers) { ((cudaFree(buffers), buffers = nullptr), ...); }
+
+// A call's device counter struct and its pinned host mirror.
+template <class T>
+struct CounterMirror {
+  T* device = nullptr;
+  T* host = nullptr;
+};
+
+// Both buffers or neither: on a failure nothing stays allocated and `c` stays empty, so the next call tries again.
+template <class T>
+int CreateCounters(CounterMirror<T>& c) {
+  T* device = nullptr;
+  T* host = nullptr;
+  SM_CUDA(cudaMalloc(&device, sizeof(T)));
+  if (const cudaError_t e = cudaMallocHost(&host, sizeof(T)); e != cudaSuccess) {
+    cudaFree(device);
+    return SetError(SM_ERR_CUDA, (std::string("cudaMallocHost: ") + cudaGetErrorString(e)).c_str());
+  }
+  c.device = device;
+  c.host = host;
+  return SM_OK;
+}
+
+template <class T>
+void FreeCounters(CounterMirror<T>& c) {
+  cudaFree(c.device);
+  if (c.host) cudaFreeHost(c.host);
+  c = CounterMirror<T>{};
+}
+
+// The first `bytes` of the device counters into the host mirror, then a synchronisation of the stream.
+template <class T>
+int ReadCounters(const CounterMirror<T>& c, cudaStream_t stream, size_t bytes = sizeof(T)) {
+  SM_CUDA(cudaMemcpyAsync(c.host, c.device, bytes, cudaMemcpyDeviceToHost, stream));
+  SM_CUDA(cudaStreamSynchronize(stream));
+  return SM_OK;
 }
 
 }  // namespace

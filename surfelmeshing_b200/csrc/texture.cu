@@ -62,8 +62,7 @@ struct TextureCounters {
 
 // The scratch of sm_mesh_texture: per triangle, per texel code and per pixel of the largest view.
 struct TextureScratch {
-  TextureCounters* counters = nullptr;
-  TextureCounters* host_counters = nullptr;
+  CounterMirror<TextureCounters> counters;
   u64 triangle_capacity = 0;
   u32* keys = nullptr;            // class << 28 | t, unsorted and sorted
   u32* sorted = nullptr;
@@ -379,14 +378,17 @@ __global__ void __launch_bounds__(kBlock) k_tex_resolve(TextureArgs a) {
   }
 }
 
+void FreeTriangleScratch(TextureScratch& s) {
+  FreeAndClear(s.keys, s.sorted, s.records, s.sort_temp);
+  s.sort_temp_bytes = 0;
+  s.triangle_capacity = 0;
+}
+
 // Per-triangle scratch for `count` triangles (x 1.5 when it grows).
 int EnsureTriangleScratch(TextureScratch& s, u64 count) {
   if (count <= s.triangle_capacity) return SM_OK;
-  const u64 cap = std::max<u64>(count + count / 2, 1024);
-  cudaFree(s.keys); cudaFree(s.sorted); cudaFree(s.records);   // cudaFree synchronises the device
-  cudaFree(s.sort_temp);
-  s.keys = nullptr; s.sorted = nullptr; s.records = nullptr; s.sort_temp = nullptr; s.sort_temp_bytes = 0;
-  s.triangle_capacity = 0;
+  const u64 cap = GrownCapacity(count);
+  FreeTriangleScratch(s);
   size_t temp = 0;
   SM_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, temp, static_cast<const u32*>(nullptr), static_cast<u32*>(nullptr),
                                          static_cast<int>(cap)));
@@ -399,22 +401,28 @@ int EnsureTriangleScratch(TextureScratch& s, u64 count) {
   return SM_OK;
 }
 
+void FreeTexelScratch(TextureScratch& s) {
+  FreeAndClear(s.accum);
+  s.texel_capacity = 0;
+}
+
 int EnsureTexelScratch(TextureScratch& s, u64 texels) {
   if (texels <= s.texel_capacity) return SM_OK;
-  const u64 cap = std::max<u64>(texels + texels / 2, 1 << 16);
-  cudaFree(s.accum);
-  s.accum = nullptr;
-  s.texel_capacity = 0;
+  const u64 cap = GrownCapacity(texels, 1 << 16);
+  FreeTexelScratch(s);
   SM_CUDA(cudaMalloc(&s.accum, sizeof(float4) * cap));
   s.texel_capacity = cap;
   return SM_OK;
 }
 
+void FreePixelScratch(TextureScratch& s) {
+  FreeAndClear(s.depth);
+  s.pixel_capacity = 0;
+}
+
 int EnsurePixelScratch(TextureScratch& s, size_t pixels) {
   if (pixels <= s.pixel_capacity) return SM_OK;
-  cudaFree(s.depth);
-  s.depth = nullptr;
-  s.pixel_capacity = 0;
+  FreePixelScratch(s);
   SM_CUDA(cudaMalloc(&s.depth, sizeof(float) * pixels));
   s.pixel_capacity = pixels;
   return SM_OK;
@@ -425,10 +433,10 @@ int EnsurePixelScratch(TextureScratch& s, size_t pixels) {
 void FreeTextureBuffers(sm_reconstruction* r) {
   TextureScratch* s = r->texture;
   if (!s) return;
-  cudaFree(s->counters);
-  if (s->host_counters) cudaFreeHost(s->host_counters);
-  cudaFree(s->keys); cudaFree(s->sorted); cudaFree(s->records); cudaFree(s->sort_temp);
-  cudaFree(s->accum); cudaFree(s->depth);
+  FreeTriangleScratch(*s);
+  FreeTexelScratch(*s);
+  FreePixelScratch(*s);
+  FreeCounters(s->counters);
   delete s;
   r->texture = nullptr;
 }
@@ -489,17 +497,12 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_param
   if (count == 0) return SM_OK;               // a 0 x 0 atlas: nothing to write
   const u32 n = r->host_counters->surfel_count[r->count_slot];
 
-  if (!r->texture) {   // published only with both counter buffers, so a failed first call is retried whole
-    TextureCounters* counters = nullptr;
-    TextureCounters* host_counters = nullptr;
-    SM_CUDA(cudaMalloc(&counters, sizeof(TextureCounters)));
-    if (const cudaError_t e = cudaMallocHost(&host_counters, sizeof(TextureCounters)); e != cudaSuccess) {
-      cudaFree(counters);
-      return SetError(SM_ERR_CUDA, (std::string("cudaMallocHost: ") + cudaGetErrorString(e)).c_str());
-    }
+  if (!r->texture) {   // published only with its counters, so a failed first call is retried whole
+    CounterMirror<TextureCounters> counters;
+    status = CreateCounters(counters);
+    if (status != SM_OK) return status;
     r->texture = new TextureScratch();
     r->texture->counters = counters;
-    r->texture->host_counters = host_counters;
   }
   TextureScratch& s = *r->texture;
   status = EnsureTriangleScratch(s, count);
@@ -514,9 +517,9 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_param
   a.count = static_cast<u32>(count);
   a.texel_size = p.texel_size;
   a.keys = s.keys; a.sorted = s.sorted; a.records = s.records;
-  a.counters = s.counters;
-  TextureCounters* c = s.counters;
-  const TextureCounters& h = *s.host_counters;
+  a.counters = s.counters.device;
+  TextureCounters* c = s.counters.device;
+  const TextureCounters& h = *s.counters.host;
   const int grid = Grid(count, r->sm_count);
   SM_CUDA(cudaMemsetAsync(c, 0, sizeof(TextureCounters), stream));
   { LaunchScope scope(stream, KID_TEXTURE_CLASSES); LaunchKernel(k_tex_classes, dim3(grid), dim3(kBlock), 0, stream, a); }
@@ -528,8 +531,8 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_param
   }
   { LaunchScope scope(stream, KID_TEXTURE_PLACE); LaunchKernel(k_tex_bases, dim3(1), dim3(1), 0, stream, c); }
   { LaunchScope scope(stream, KID_TEXTURE_PLACE); LaunchKernel(k_tex_place, dim3(grid), dim3(kBlock), 0, stream, a); }
-  SM_CUDA(cudaMemcpyAsync(s.host_counters, c, offsetof(TextureCounters, seen), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
+  status = ReadCounters(s.counters, stream, offsetof(TextureCounters, seen));
+  if (status != SM_OK) return status;
   if (const char* why = MeshInputError(h.errors)) return bad(why);
 
   const u64 area = h.layout.base[kClasses];
@@ -593,8 +596,8 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_param
     LaunchKernel(k_tex_accumulate, dim3(texel_grid), dim3(kBlock), 0, stream, a, v);
   }
   { LaunchScope scope(stream, KID_TEXTURE_RESOLVE); LaunchKernel(k_tex_resolve, dim3(texel_grid), dim3(kBlock), 0, stream, a); }
-  SM_CUDA(cudaMemcpyAsync(s.host_counters, c, sizeof(TextureCounters), cudaMemcpyDeviceToHost, stream));
-  SM_CUDA(cudaStreamSynchronize(stream));
+  status = ReadCounters(s.counters, stream);
+  if (status != SM_OK) return status;
   *stats = layout;
   stats->texels_seen = h.seen;
   stats->texels_fallback = h.fallback;

@@ -194,10 +194,13 @@ def test_errors_write_nothing_and_capacity_protocol():
               np.concatenate([tri[:3], [[-1, 2, -1]], tri[3:]])):
         assert call(t) == INVALID
         assert CW.stats_dict(stats) == dict.fromkeys(CW.STATS, 0) and untouched()
+    assert rec.lib.fn["last_error"]() == b"sm_mesh_components: a corner is not a present slot below surfels_size()"
     # a count query, out and table one short, then enough
     assert call(o=None, lab=None, tab=None) == _lib.SM_ERR_CAPACITY and CW.stats_dict(stats) == want_stats
     assert call(oc=K - 1) == _lib.SM_ERR_CAPACITY and CW.stats_dict(stats) == want_stats
+    assert rec.lib.fn["last_error"]() == f"sm_mesh_components: {K} triangles do not fit the capacity of {K - 1}".encode()
     assert call(tc=P - 1) == _lib.SM_ERR_CAPACITY and CW.stats_dict(stats) == want_stats
+    assert rec.lib.fn["last_error"]() == f"sm_mesh_components: {P} pieces do not fit the table capacity of {P - 1}".encode()
     assert untouched()
     assert call(oc=K, tc=P) == _lib.SM_OK and CW.stats_dict(stats) == want_stats
     assert np.array_equal(out[:K].cpu().numpy().astype(np.uint32), want_out) and (out[K:] == -7).all()

@@ -100,8 +100,13 @@ def test_capacity_error_writes_nothing():
     status = rec.lib.fn["triangulate"](rec._h, None, C.byref(p), C.c_void_p(buf.data_ptr()), want - 1, C.byref(stats))
     torch.cuda.synchronize()
     assert status == _lib.SM_ERR_CAPACITY
+    assert rec.lib.fn["last_error"]() == f"sm_triangulate: {want} triangles do not fit the capacity of {want - 1}".encode()
     assert stats.triangle_count == want and stats.vertices_meshed > 0
     assert (buf == -7).all()
+    p = MeshParams(0.0, 90, 170)
+    status = rec.lib.fn["triangulate"](rec._h, None, C.byref(p), C.c_void_p(buf.data_ptr()), want - 1, C.byref(stats))
+    assert status == _lib.SM_ERR_INVALID_ARGUMENT
+    assert rec.lib.fn["last_error"]() == b"sm_triangulate: neighbor_radius_factor must be finite and > 0"
     rec.close()
 
 

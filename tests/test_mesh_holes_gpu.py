@@ -152,11 +152,14 @@ def test_errors_write_nothing_and_capacity_protocol():
     for t in ([[0, 1, n]], [[0, 1, 64]], [[0, 0, 1]], tri[:1]):
         assert call(np.concatenate([tri, t])) == _lib.SM_ERR_INVALID_ARGUMENT
         assert stats.triangles_added == 0
+    assert rec.lib.fn["last_error"]() == b"sm_mesh_fill_holes: a directed edge occurs twice (the input must be " \
+        b"edge-manifold and consistently oriented)"
     assert (buf == -7).all()
     # a count query, then a capacity one short, then enough
     assert call(tri, out=None, capacity=0) == _lib.SM_ERR_CAPACITY
     assert stats.triangles_added == 4 and stats.loops_filled == 1
     assert call(tri, capacity=3) == _lib.SM_ERR_CAPACITY and stats.triangles_added == 4
+    assert rec.lib.fn["last_error"]() == b"sm_mesh_fill_holes: 4 triangles do not fit the capacity of 3"
     assert (buf == -7).all()
     assert call(tri) == _lib.SM_OK
     want, _ = HW.fill_holes(rows, tri)

@@ -212,10 +212,14 @@ def test_errors_write_nothing_and_capacity_protocol():
     for t in ([[0, 1, n]], [[0, 1, 64]], [[0, 0, 1]], tri[:1]):
         assert call(np.concatenate([tri, t])) == _lib.SM_ERR_INVALID_ARGUMENT
         assert stats.triangles_out == 0 and stats.stop_reason == 0
+    assert rec.lib.fn["last_error"]() == b"sm_mesh_simplify: a directed edge occurs twice (the input must be " \
+        b"edge-manifold and consistently oriented)"
     assert (buf == -7).all()
     # a count query, then a capacity one short, then enough
     assert call(out=None, capacity=0) == _lib.SM_ERR_CAPACITY and SW.stats_dict(stats) == want_s
     assert call(capacity=len(want) - 1) == _lib.SM_ERR_CAPACITY and stats.triangles_out == len(want)
+    assert rec.lib.fn["last_error"]() == \
+        f"sm_mesh_simplify: {len(want)} triangles do not fit the capacity of {len(want) - 1}".encode()
     assert (buf == -7).all()
     assert call() == _lib.SM_OK and SW.stats_dict(stats) == want_s
     got = buf[:len(want)].cpu().numpy().astype(np.uint32)

@@ -216,13 +216,19 @@ def test_errors_write_nothing_and_capacity_protocol():
     for t in ([[0, 1, n]], [[0, 0, 1]]):
         assert call(np.concatenate([tris, t])) == _lib.SM_ERR_INVALID_ARGUMENT
         assert TW.stats_dict(stats) == dict.fromkeys(TW.STATS, 0)
+    assert call(np.concatenate([tris, [[0, 1, n]]])) == _lib.SM_ERR_INVALID_ARGUMENT
+    assert rec.lib.fn["last_error"]() == b"sm_mesh_texture: a corner is not a present slot below surfels_size()"
     assert (atlas == 7).all() and (uv == -7.0).all()
     # a layout query, a capacity one texel short each way, max_atlas_side, then enough
     layout = dict(want_stats, texels_seen=0, texels_fallback=0, views_used=0)
     assert call(a=None) == _lib.SM_ERR_CAPACITY and TW.stats_dict(stats) == layout
     assert call(cw=W - 1) == _lib.SM_ERR_CAPACITY and TW.stats_dict(stats) == layout
+    assert rec.lib.fn["last_error"]() == \
+        f"sm_mesh_texture: a {W} x {H} atlas does not fit the capacity of {W - 1} x {H + 2}".encode()
     assert call(ch=H - 1) == _lib.SM_ERR_CAPACITY and TW.stats_dict(stats) == layout
     assert call(params=TextureParams.defaults(texel_size=p.texel_size, max_atlas_side=W - 1)) == _lib.SM_ERR_CAPACITY
+    assert rec.lib.fn["last_error"]() == \
+        f"sm_mesh_texture: the atlas needs a side of {W} texels, above max_atlas_side {W - 1}; raise texel_size".encode()
     assert (atlas == 7).all() and (uv == -7.0).all()
     assert call() == _lib.SM_OK and TW.stats_dict(stats) == want_stats
     got = atlas.cpu().numpy()

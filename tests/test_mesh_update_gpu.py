@@ -156,6 +156,7 @@ def test_errors_launch_nothing_and_capacity_writes_nothing():
     for p in [MeshParams(0.0, 90, 170), MeshParams(math.nan, 90, 170), MeshParams(math.inf, 90, 170),
               MeshParams(2, 0.0, 170), MeshParams(2, 180.5, 170), MeshParams(2, 90, math.nan)]:
         assert fn(rec._h, None, C.byref(p), C.byref(stats)) == _lib.SM_ERR_INVALID_ARGUMENT
+    assert rec.lib.fn["last_error"]() == b"sm_mesh_update: angles must be in (0, 180] degrees"
     p = MeshParams.defaults()
     assert fn(rec._h, None, None, C.byref(stats)) == _lib.SM_ERR_INVALID_ARGUMENT
     assert fn(rec._h, None, C.byref(p), None) == _lib.SM_ERR_INVALID_ARGUMENT
@@ -165,6 +166,7 @@ def test_errors_launch_nothing_and_capacity_writes_nothing():
     count = C.c_uint64()
     buf = torch.full((want - 1, 3), -7, dtype=torch.int32, device="cuda")
     assert read(rec._h, None, 0, C.c_void_p(buf.data_ptr()), want - 1, C.byref(count)) == _lib.SM_ERR_CAPACITY
+    assert rec.lib.fn["last_error"]() == f"sm_mesh_read: {want} triangles do not fit the capacity of {want - 1}".encode()
     torch.cuda.synchronize()
     assert count.value == want and (buf == -7).all()
     assert read(rec._h, None, 0, None, 0, C.byref(count)) == _lib.SM_ERR_CAPACITY and count.value == want
