@@ -236,10 +236,10 @@ int IntegrateImpl(sm_reconstruction* r, cudaStream_t stream, u32 frame_index, co
   const FrameParams f = MakeFrameParams(r, frame_index, r->count_slot, p, depth, depth_pitch, depth_pre, depth_pre_pitch,
                                         normals, normals_pitch, radius, radius_pitch, color, color_pitch,
                                         global_T_local, local_T_global);
-  r->last_tiebreak = f.tb;
   int status = IntegrateFrame(stream, r->d, f, p.do_blending != 0, r->rasters_cleared, r->plan, &r->events);
   r->rasters_cleared = false;
   if (status != SM_OK) return status;
+  r->last_tiebreak = f.tb;   // the rasters are this frame's only now: a refused frame leaves the last ones readable
   r->rasters_stale = false;
   NoteIntegratedFrame(r->d, frame_index);
   const int old_slot = r->count_slot;

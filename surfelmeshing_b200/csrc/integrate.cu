@@ -1353,6 +1353,13 @@ int IntegrateFrame(cudaStream_t stream, const DeviceState& d, const FrameParams&
   auto launch = [&](FrameKernel which, bool dependent) {
     if (status == SM_OK) status = LaunchFrameKernel(stream, which, plan, d, f, dependent);
   };
+  // A blend radius whose tile region does not fit an SM is refused before anything runs, so that a refused frame
+  // leaves the rasters, the state and the depth as they were.
+  if (do_blending) {
+    KernelLaunch blend;
+    status = DescribeFrameKernel(FK_BLEND, plan, d, f, &blend);
+    if (status != SM_OK) return status;
+  }
   record(0);
   if (!rasters_already_cleared) {
     status = ClearAssociationRasters(stream, d);

@@ -10,6 +10,10 @@
 //   neighbour update         kernels.cu:1197-1380, detach pass :1420-1437 over the slots that existed before
 //   new-surfel flags         kernels.cu:90-111, creation :133-231
 //
+// The front half that builds those rasters and the blended depth has its own entry points at the end of the file:
+// iw_associate (clear, min depth, association, the merge stage's conflicting write) and iw_blend (the measurement
+// blending), one surfel or one pixel at a time.
+//
 // It has no visible list, no gather levels, no update list and no short cuts: every slot walks every gate in the
 // reference's order. Arithmetic: IEEE single operations in the order sm_math.cuh documents, built with
 // -ffp-contract=off, denormals flushed as the kernels flush them. The SFU steps (rcp, rsqrt, sqrt) are replaced by
@@ -61,6 +65,31 @@ enum Branch {
   B_NUM
 };
 
+// Named mutations of the front half (iw_associate, iw_blend).
+enum {
+  FM_PX_GT0 = 1 << 0,                 // `px > 0` for the secondary-pixel rule's `px > 1`
+  FM_MIN_DEPTH_PRIMARY_ONLY = 1 << 1, // min depth splatted at the primary pixel only
+  FM_INACTIVE_ASSOCIATE = 1 << 2,     // surfels outside the active window splat min depth and associate
+  FM_OCCLUSION_GE = 1 << 3,           // >= for > at the occlusion gate
+  FM_RADIUS_GE0 = 1 << 4,             // radius^2 >= 0 for > 0 at the association
+  FM_NORMAL_TEST_ALWAYS = 1 << 5,     // the normal-compatibility test also when measurement >= z
+  FM_NO_MERGE_CONFLICT = 1 << 6,      // the merge stage's conflicting-surfel write dropped
+  FM_CENTRE_TAP = 1 << 7,             // the centre pixel counted as a tap of the blend average
+  FM_IN_PLACE_LEVEL = 1 << 8,         // an iteration also reads taps of its own level (in-place update)
+  FM_ONE_ITERATION_FEWER = 1 << 9,    // the blend stops one iteration early
+  FM_BORDER_RING = 1 << 10,           // image-border pixels allowed as ring pixels
+  FM_RING1_START_DEPTH = 1 << 11,     // the surfel-border ring also writes the depth at the start step
+};
+
+// Branch counters of the front half; tests/integrate_walk.py reads the names from this list.
+enum FrontBranch {
+  F_PRIMARY_ONLY, F_SEC_LEFT, F_SEC_DOWN, F_SEC_UP, F_SEC_RIGHT, F_SEC_BORDER, F_SEC_PX1_QUIRK, F_MEAS_ZERO,
+  F_CONFLICT_FIRST_EQ, F_CONFLICT_FIRST_NE, F_OCCLUDED, F_BACKFACING, F_NORMAL_TEST_RUN, F_NORMAL_TEST_FAIL,
+  F_RADIUS_ZERO, F_RADIUS_NEG, F_INACTIVE_VISIBLE, F_TIED_MIN_DEPTH, F_MERGE_CONFLICT_INACTIVE_OR_R0, F_ASSOCIATED,
+  F_RING0_ONLY, F_RING1_ONLY, F_BOTH_RINGS, F_LAST_LEVEL, F_DIES_EARLY, F_RING_ON_BORDER, F_START_DEPTH_ZERO,
+  F_NUM
+};
+
 enum { ST_UNCLEAR = 1, ST_LINKS_UNCLEAR = 2, ST_TOUCHED = 4, ST_REPLACED = 8, ST_INTEGRATED = 16, ST_MERGE_UNCLEAR = 32,
        ST_MERGE_CHAIN = 64 };
 
@@ -90,6 +119,7 @@ typedef struct {
   float *pbound, *nbound, *cbound;
   u32 *color_lo, *color_hi;
   u64* branch;
+  u32 front_mutations;     // FM_ bits of the front half (iw_associate, iw_blend); 0 in iw_integrate
 } Walk;
 
 #define R(row, i) w->rows[(u64)(row) * w->stride + (i)]
@@ -163,7 +193,10 @@ static Proj project_k(const Walk* w, float x, float y, float z, int k) {
   if (!q.in_image) return q;
   const float xf = fsub(u, (float)q.px), yf = fsub(v, (float)q.py);
   if (xf < yf) {
-    if (xf < fadd(-yf, 1.0f)) { q.side = 0; if (q.px > 1) { q.has2 = 1; q.ox = q.px - 1; } }      // note: > 1, not > 0
+    if (xf < fadd(-yf, 1.0f)) {                                                                  // note: > 1, not > 0
+      q.side = 0;
+      if (q.px > ((w->front_mutations & FM_PX_GT0) ? 0 : 1)) { q.has2 = 1; q.ox = q.px - 1; }
+    }
     else { q.side = 1; if (q.py < p->height - 1) { q.has2 = 1; q.oy = q.py + 1; } }
   } else {
     if (xf < fadd(-yf, 1.0f)) { q.side = 2; if (q.py > 0) { q.has2 = 1; q.oy = q.py - 1; } }
@@ -676,4 +709,317 @@ u64 iw_integrate(const iw_params* p, u64 n, u64 stride, float* rows, const u16* 
   }
   out_counts[0] = n_after; out_counts[1] = merges; out_counts[2] = unclear_merges;
   return n_after;
+}
+
+// ---- the front half: clear, min depth, association, conflicting surfel -----------------------------------------
+// iw_associate restates k_clear, RenderMinDepthCUDAKernel (kernels.cu:1466-1557), AssociateSurfelsCUDAKernel
+// (:1586-1808) and the conflicting-surfel write of MergeSurfelsCUDAKernel (:1885-1889), one surfel at a time. Which
+// of several supporters or conflicting surfels a pixel keeps is a race in the reference, so the walk does not pick
+// one: it lists every association that reaches the atomicCAS of :1688 (pixel, slot | secondary bit) and every
+// conflicting write (pixel, slot, stage 0 = association, 1 = merge).
+#define FMUT(m) (w->front_mutations & (m))
+#define SECONDARY_BIT 0x80000000u
+
+// Every pixel the surfel could touch for a reciprocal within 2 ulp.
+static void mark_unclear(const Walk* w, float x, float y, float z, u8* unclear) {
+  for (int k = -2; k <= 2; ++k) {
+    const Proj t = project_k(w, x, y, z, k);
+    if (!t.in_image) continue;
+    unclear[t.py * w->p->width + t.px] = 1;
+    if (t.has2) unclear[t.oy * w->p->width + t.ox] = 1;
+  }
+}
+
+static inline void local_position(const Walk* w, const float* rows, u64 n, u64 i, float* x, float* y, float* z) {
+  const float gx = rows[(u64)ROW_X * n + i], gy = rows[(u64)(ROW_X + 1) * n + i], gz = rows[(u64)(ROW_X + 2) * n + i];
+  *z = trow(w->p->local_T_global, 2, gx, gy, gz);
+  *x = trow(w->p->local_T_global, 0, gx, gy, gz);
+  *y = trow(w->p->local_T_global, 1, gx, gy, gz);
+}
+
+// rows: [25, n]. Per pixel: first (min depth), counts, sum_float (the float sum in association order: exact for one
+// or two terms), sum and sum_abs (float64 sums of z and |z|), unclear; ties: scratch. Events: sup_* (capacity 2 n)
+// and conf_* (capacity 3 n); out_counts = {supporter events, conflicting events}.
+void iw_associate(const iw_params* p, u64 n, const float* rows, const u16* depth, const float* normals, float* first,
+                  u32* counts, float* sum_float, double* sum, double* sum_abs, u8* unclear, u32* ties, u32* sup_pixel,
+                  u32* sup_key, u32* conf_pixel, u32* conf_surfel, u8* conf_stage, u64* out_counts, u64* branch) {
+  Walk walk, *w = &walk;
+  memset(w, 0, sizeof *w);
+  w->p = p;
+  w->front_mutations = p->mutations;
+  w->branch = branch;
+  w->inv_depth_scaling = 1.0f / p->depth_scaling;
+  w->cos_threshold = cosf(M_PI / 180.0f * p->normal_threshold_deg);
+  const int W = p->width, P = p->width * p->height;
+  const float* L = p->local_T_global;
+  const u32* stamps = (const u32*)rows + (u64)ROW_STAMP * n;
+  const float snf = p->sensor_noise_factor;
+  // k_clear (CUDABuffer::Clear of the five rasters)
+  for (int i = 0; i < P; ++i) {
+    first[i] = INFINITY; counts[i] = 0; sum_float[i] = 0.f; sum[i] = sum_abs[i] = 0.0; unclear[i] = 0; ties[i] = 0;
+  }
+  // RenderMinDepthCUDAKernel: atomicMin on the int-punned z, which orders positive floats as floats
+  for (u64 i = 0; i < n; ++i) {
+    if (!is_active(stamps[i], p->frame_index, p->active_window) && !FMUT(FM_INACTIVE_ASSOCIATE)) continue;
+    float x, y, z;
+    local_position(w, rows, n, i, &x, &y, &z);
+    if (!(z > 0.f)) continue;
+    int clear = 1;
+    const Proj q = project(w, x, y, z, &clear);
+    if (!clear) mark_unclear(w, x, y, z, unclear);
+    if (!q.in_image) continue;
+    float* f0 = &first[q.py * W + q.px];
+    if (z < *f0) *f0 = z;
+    if (q.has2 && !FMUT(FM_MIN_DEPTH_PRIMARY_ONLY)) {
+      float* f1 = &first[q.oy * W + q.ox];
+      if (z < *f1) *f1 = z;
+    }
+  }
+  // AssociateSurfelsCUDAKernel: ConsiderSurfelAssociationToPixel at the primary, then the secondary pixel
+  u64 ns = 0, nc = 0;
+  for (u64 i = 0; i < n; ++i) {
+    float x, y, z;
+    local_position(w, rows, n, i, &x, &y, &z);
+    if (!(z > 0.f)) continue;
+    int clear = 1;
+    const Proj q = project(w, x, y, z, &clear);
+    if (!q.in_image) continue;
+    if (!is_active(stamps[i], p->frame_index, p->active_window) && !FMUT(FM_INACTIVE_ASSOCIATE)) { CNT(F_INACTIVE_VISIBLE); continue; }
+    if (q.has2) CNT(F_SEC_LEFT + q.side);
+    else { CNT(F_PRIMARY_ONLY); CNT(q.side == 0 && q.px == 1 ? F_SEC_PX1_QUIRK : F_SEC_BORDER); }
+    const float nx = rows[(u64)ROW_NX * n + i], ny = rows[(u64)(ROW_NX + 1) * n + i], nz = rows[(u64)(ROW_NX + 2) * n + i];
+    const float r2 = rows[(u64)ROW_R2 * n + i];
+    const float lnx = rrow(L, 0, nx, ny, nz), lny = rrow(L, 1, nx, ny, nz), lnz = rrow(L, 2, nx, ny, nz);
+    // (1 / |p|) dot(p, n) > 0: the sign is the dot's unless the product underflows (FTZ) for some rsqrt within 2 ulp
+    const float dotp = ffma(z, lnz, ffma(x, lnx, fmul(y, lny)));
+    const float rs = frsqrt(sqnorm(x, y, z));
+    const int back = fmul(rs, dotp) > 0.f;
+    int facing_clear = 1;
+    for (int k = -2; k <= 2; ++k) if ((fmul(nudge(rs, k), dotp) > 0.f) != back) facing_clear = 0;
+    const int xs[2] = {q.px, q.ox}, ys[2] = {q.py, q.oy};
+    for (int k = 0; k < 1 + q.has2; ++k) {
+      const int pix = ys[k] * W + xs[k];
+      if (first[pix] == z && (k == 0 || !FMUT(FM_MIN_DEPTH_PRIMARY_ONLY))) ties[pix]++;
+      const float md = fmul(u2f(depth[pix]), w->inv_depth_scaling);
+      if (!(md > 0.f)) { CNT(F_MEAS_ZERO); continue; }
+      const float fv = first[pix];
+      if (fv < fmul(md, fadd(-snf, 1.0f))) {
+        CNT(fv == z ? F_CONFLICT_FIRST_EQ : F_CONFLICT_FIRST_NE);
+        if (fv == z) { conf_pixel[nc] = (u32)pix; conf_surfel[nc] = (u32)i; conf_stage[nc] = 0; ++nc; }
+        continue;
+      }
+      const float occlusion = fmul(fadd(snf, 1.0f), md);   // kProtectSlightlyOccludedSurfels = false
+      if (FMUT(FM_OCCLUSION_GE) ? z >= occlusion : z > occlusion) { CNT(F_OCCLUDED); continue; }
+      if (!facing_clear) unclear[pix] = 1;
+      if (back) { CNT(F_BACKFACING); continue; }   // kSurfelNormalToViewingDirThreshold = 0
+      if (md < z || FMUT(FM_NORMAL_TEST_ALWAYS)) {
+        CNT(F_NORMAL_TEST_RUN);
+        const float mnx = normals[2 * pix], mny = normals[2 * pix + 1];
+        const float s = measurement_normal_z(mnx, mny);
+        const int fail = ffma(-lnz, s, ffma(lnx, mnx, fmul(lny, mny))) < w->cos_threshold;
+        for (int k2 = -2; k2 <= 2; k2 += 4)
+          if ((ffma(-lnz, nudge(s, k2), ffma(lnx, mnx, fmul(lny, mny))) < w->cos_threshold) != fail) unclear[pix] = 1;
+        if (fail) { CNT(F_NORMAL_TEST_FAIL); continue; }
+      }
+      if (r2 == 0.f) CNT(F_RADIUS_ZERO);
+      else if (r2 < 0.f) CNT(F_RADIUS_NEG);
+      if (!(FMUT(FM_RADIUS_GE0) ? r2 >= 0.f : r2 > 0.f)) continue;   // kCheckScaleCompatibilityForIntegration = false
+      CNT(F_ASSOCIATED);
+      sup_pixel[ns] = (u32)pix;
+      sup_key[ns] = (u32)i | (k ? SECONDARY_BIT : 0u);
+      ++ns;
+      counts[pix] += 1;
+      sum_float[pix] = fadd(sum_float[pix], z);   // atom.add.f32 flushes subnormals as well
+      sum[pix] += (double)z;
+      sum_abs[pix] += fabs((double)z);
+    }
+  }
+  for (int i = 0; i < P; ++i) if (ties[i] >= 2) CNT(F_TIED_MIN_DEPTH);
+  // MergeSurfelsCUDAKernel up to its conflict gate: every surfel with radius^2 >= 0 (no active-window test, :2016-2017)
+  // at its primary pixel. It runs after the association, so its writes are the final ones where there are any.
+  for (u64 i = 0; i < n; ++i) {
+    const float r2 = rows[(u64)ROW_R2 * n + i];
+    if (!(r2 >= 0.f)) continue;
+    float x, y, z;
+    local_position(w, rows, n, i, &x, &y, &z);
+    if (!(z > 0.f)) continue;
+    int clear = 1;
+    const Proj q = project(w, x, y, z, &clear);
+    if (!clear) mark_unclear(w, x, y, z, unclear);   // surfels outside the active window were not marked above
+    if (!q.in_image) continue;
+    const int pix = q.py * W + q.px;
+    const float md = fmul(u2f(depth[pix]), w->inv_depth_scaling);
+    if (!(md > 0.f)) continue;
+    if (first[pix] < fmul(md, fadd(-snf, 1.0f)) && first[pix] == z && !FMUT(FM_NO_MERGE_CONFLICT)) {
+      conf_pixel[nc] = (u32)pix; conf_surfel[nc] = (u32)i; conf_stage[nc] = 1; ++nc;
+      if (!is_active(stamps[i], p->frame_index, p->active_window) || r2 == 0.f) CNT(F_MERGE_CONFLICT_INACTIVE_OR_R0);
+    }
+  }
+  out_counts[0] = ns;
+  out_counts[1] = nc;
+}
+
+// ---- the front half: measurement blending ---------------------------------------------------------------------
+// iw_blend restates BlendMeasurementsCUDA (kernels.cc:148-205): the start kernel (kernels.cu:563-615), then the
+// iteration kernel (:647-708) for iteration = 2 .. radius - 1, each over the whole image, on two full-image distance
+// maps (dist0 = distance_map, the measurement-border ring; dist1 = new_distance_map, the surfel-border ring) and two
+// delta buffers. A pixel is supported where its count is not 0.
+//
+// The start kernel writes the depth of a measurement-border pixel while other threads read the depth buffer to
+// classify their neighbours (the TODO at :610). That can change a classification only if the written depth is 0;
+// the walk classifies on the depth before the start step and counts F_START_DEPTH_ZERO where a written start depth is
+// 0. It cannot be: a supporter passed the conflict gate, so every z at the pixel is >= 0.95 of a measurement of at
+// least one unit, and the average rounds to 1 or more.
+//
+// Non-exact steps: rcp of the count, of the tap count (3, 5, 6, 7, 9) and of the depth scaling. The walk takes the
+// correctly rounded value and carries a bound on every delta (bound0 / bound1, absolute): at the start step by
+// evaluating every reciprocal within 2 ulp, through the levels by adding the taps' bounds, 2^-22 of an inexact
+// reciprocal and one ulp per rounding of a perturbed value. lo / hi: the depths those bounds allow.
+static inline float below(double v) { const float f = (float)v; return (double)f > v ? nextafterf(f, -INFINITY) : f; }
+static inline float above(double v) { const float f = (float)v; return (double)f < v ? nextafterf(f, INFINITY) : f; }
+static inline u16 to_depth(float v) { return (u16)f2u(v); }   // F2I.U32.TRUNC, stored as u16
+
+// One pixel of the iteration kernel for one ring: the average delta of its 3x3 neighbours of level it - 1, summed
+// row by row. Returns the tap count (0: no neighbour of that level).
+static int ring_average(const Walk* w, int x, int y, int it, const u8* dist, const float* delta, const double* bound,
+                        float* avg, double* avg_bound) {
+  const int W = w->p->width, H = w->p->height;
+  float s = 0.f;
+  double b = 0.0;
+  int count = 0;
+  for (int wy = y - 1; wy <= y + 1; ++wy) {
+    for (int wx = x - 1; wx <= x + 1; ++wx) {
+      if (wx < 0 || wy < 0 || wx >= W || wy >= H) continue;   // only with FM_BORDER_RING
+      const int q = wy * W + wx;
+      if (!(dist[q] == it - 1 || (FMUT(FM_IN_PLACE_LEVEL) && dist[q] == it))) continue;
+      s = fadd(s, delta[q]);
+      b += bound[q];
+      if (b > 0.0) b += EPS * (fabs(s) + b);
+      ++count;
+    }
+  }
+  if (FMUT(FM_CENTRE_TAP)) ++count;
+  if (count == 0) return 0;
+  const float rc = frcp(u2f((u32)count));
+  *avg = fmul(rc, s);
+  const int exact = nudge(rc, 1) == rc;
+  double ba = 0.0;
+  if (b > 0.0 || !exact) {
+    ba = (double)rc * (1.0 + 2.0 * EPS) * b + (exact ? 0.0 : 2.0 * EPS * rc * fabs(s));
+    ba += EPS * (fabs(*avg) + ba);
+  }
+  *avg_bound = ba;
+  return count;
+}
+
+static inline int on_border_ring(const iw_params* p, int x, int y) {
+  return x <= 1 || y <= 1 || x >= p->width - 2 || y >= p->height - 2;
+}
+
+// level_counts: [2][radius + 1] pixels per ring and level.
+void iw_blend(const iw_params* p, int radius, const u16* depth_pre, const u32* counts, const float* sums, u16* out,
+              u16* lo, u16* hi, u8* dist0, u8* dist1, float* delta0, float* delta1, double* bound0, double* bound1,
+              u64* level_counts, u64* branch) {
+  Walk walk, *w = &walk;
+  memset(w, 0, sizeof *w);
+  w->p = p;
+  w->front_mutations = p->mutations;
+  w->branch = branch;
+  const int W = p->width, H = p->height, P = W * H;
+  const float inv = 1.0f / p->depth_scaling, scaling = 1.0f / inv;   // api.cu: the reference's 1 / depth_correction_factor
+  const float rs = frcp(scaling);
+  const int ks_max = nudge(rs, 1) == rs ? 0 : 2;
+  u64* lc0 = level_counts;
+  u64* lc1 = level_counts + radius + 1;
+  for (int i = 0; i < P; ++i) {
+    out[i] = lo[i] = hi[i] = depth_pre[i];
+    dist0[i] = dist1[i] = 0;   // distance_map->Clear(0), new_distance_map->Clear(0)
+    delta0[i] = delta1[i] = 0.f;
+    bound0[i] = bound1[i] = 0.0;
+  }
+  const int border = FMUT(FM_BORDER_RING) ? 0 : 1;   // kBorder
+  // start kernel
+  for (int y = border; y < H - border; ++y) {
+    for (int x = border; x < W - border; ++x) {
+      const int pix = y * W + x;
+      if (depth_pre[pix] == 0 || counts[pix] == 0) continue;
+      int measurement_border = 0, surfel_border = 0;
+      for (int wy = y - 1; wy <= y + 1; ++wy) {
+        for (int wx = x - 1; wx <= x + 1; ++wx) {
+          if (wx < 0 || wy < 0 || wx >= W || wy >= H) continue;
+          if (depth_pre[wy * W + wx] == 0) measurement_border = 1;
+          else if (counts[wy * W + wx] == 0) surfel_border = 1;
+        }
+      }
+      const float d = u2f(depth_pre[pix]), s = sums[pix], rc = frcp(u2f(counts[pix]));
+      const int kc_max = nudge(rc, 1) == rc ? 0 : 2;
+      if (surfel_border) {
+        dist1[pix] = 1;
+        delta1[pix] = ffma(s, rc, -fmul(d, rs));
+        for (int kc = -kc_max; kc <= kc_max; ++kc) for (int ks = -ks_max; ks <= ks_max; ++ks) {
+          const float t = ffma(s, nudge(rc, kc), -fmul(d, nudge(rs, ks)));
+          bound1[pix] = fmax(bound1[pix], fabs((double)t - delta1[pix]));
+        }
+      }
+      if (measurement_border || (surfel_border && FMUT(FM_RING1_START_DEPTH))) {
+        const float avg = fmul(s, rc);
+        out[pix] = lo[pix] = hi[pix] = to_depth(ffma(avg, scaling, 0.5f));
+        for (int kc = -kc_max; kc <= kc_max; ++kc) {
+          const u16 t = to_depth(ffma(fmul(s, nudge(rc, kc)), scaling, 0.5f));
+          if (t < lo[pix]) lo[pix] = t;
+          if (t > hi[pix]) hi[pix] = t;
+        }
+        if (lo[pix] == 0) CNT(F_START_DEPTH_ZERO);
+      }
+      if (measurement_border) {
+        dist0[pix] = 1;
+        const float avg = fmul(s, rc);
+        delta0[pix] = ffma(-d, rs, avg);
+        for (int kc = -kc_max; kc <= kc_max; ++kc) for (int ks = -ks_max; ks <= ks_max; ++ks) {
+          const float t = ffma(-d, nudge(rs, ks), fmul(s, nudge(rc, kc)));
+          bound0[pix] = fmax(bound0[pix], fabs((double)t - delta0[pix]));
+        }
+      } else {
+        dist0[pix] = 255;   // unknown distance
+      }
+      if (measurement_border || surfel_border) {
+        CNT(measurement_border && surfel_border ? F_BOTH_RINGS : measurement_border ? F_RING0_ONLY : F_RING1_ONLY);
+        if (on_border_ring(p, x, y)) CNT(F_RING_ON_BORDER);
+      }
+      lc0[1] += measurement_border;
+      lc1[1] += surfel_border;
+    }
+  }
+  // iteration kernels (kernels.cc:190-204)
+  const float interpolation_factor_term = 1.0f / (radius - 1.0f);
+  const int end = FMUT(FM_ONE_ITERATION_FEWER) ? radius - 1 : radius;
+  for (int it = 2; it < end; ++it) {
+    const float scaled = fmul(ffma(-(float)(it - 1), interpolation_factor_term, 1.0f), scaling);
+    for (int y = border; y < H - border; ++y) {
+      for (int x = border; x < W - border; ++x) {
+        const int pix = y * W + x;
+        for (int ring = 0; ring < 2; ++ring) {
+          u8* dist = ring ? dist1 : dist0;
+          float* delta = ring ? delta1 : delta0;
+          double* bound = ring ? bound1 : bound0;
+          if (ring == 0 ? dist0[pix] != 255 : !(out[pix] != 0 && counts[pix] == 0 && dist1[pix] == 0)) continue;
+          float avg;
+          double b;
+          if (!ring_average(w, x, y, it, dist, delta, bound, &avg, &b)) continue;
+          dist[pix] = (u8)it;   // in place: the iteration reads level it - 1 only
+          delta[pix] = avg;
+          bound[pix] = b;
+          const float d = u2f(out[pix]);
+          out[pix] = to_depth(fadd(ffma(avg, scaled, 0.5f), d));
+          lo[pix] = b > 0.0 ? to_depth(fadd(ffma(below((double)avg - b), scaled, 0.5f), d)) : out[pix];
+          hi[pix] = b > 0.0 ? to_depth(fadd(ffma(above((double)avg + b), scaled, 0.5f), d)) : out[pix];
+          (ring ? lc1 : lc0)[it] += 1;
+          if (it == radius - 1) CNT(F_LAST_LEVEL);
+          if (on_border_ring(p, x, y)) CNT(F_RING_ON_BORDER);
+        }
+      }
+    }
+    if (lc0[it] == 0 && lc0[it - 1] > 0) CNT(F_DIES_EARLY);
+    if (lc1[it] == 0 && lc1[it - 1] > 0) CNT(F_DIES_EARLY);
+  }
 }

@@ -64,15 +64,22 @@ ST_UNCLEAR, ST_LINKS_UNCLEAR, ST_TOUCHED, ST_REPLACED, ST_INTEGRATED, ST_MERGE_U
 LINK_ROWS = slice(19, 23)
 
 
-def _enum(name_prefix, text):
-    body = re.search(r"enum Branch \{(.*?)\}", text, re.S).group(1)
+def _enum(name_prefix, text, name="Branch"):
+    body = re.search(rf"enum {name} \{{(.*?)\}}", text, re.S).group(1)
     body = re.sub(r"//.*", "", body)
     return [t.strip() for t in body.split(",") if t.strip().startswith(name_prefix)]
 
 
 _TEXT = SOURCE.read_text()
 BRANCHES = [b[2:].lower() for b in _enum("B_", _TEXT) if b != "B_NUM"]
-MUTATIONS = {m.group(1).lower(): 1 << int(m.group(2)) for m in re.finditer(r"MUT_(\w+) = 1 << (\d+)", _TEXT)}
+MUTATIONS = {m.group(1).lower(): 1 << int(m.group(2)) for m in re.finditer(r"\bMUT_(\w+) = 1 << (\d+)", _TEXT)}
+# the front half (iw_associate, iw_blend): its own counters and mutations
+FRONT_BRANCHES = [b[2:].lower() for b in _enum("F_", _TEXT, "FrontBranch") if b != "F_NUM"]
+FRONT_MUTATIONS = {m.group(1).lower(): 1 << int(m.group(2)) for m in re.finditer(r"\bFM_(\w+) = 1 << (\d+)", _TEXT)}
+ASSOCIATION_MUTATIONS = ("px_gt0", "min_depth_primary_only", "inactive_associate", "occlusion_ge", "radius_ge0",
+                         "normal_test_always", "no_merge_conflict")
+BLEND_MUTATIONS = tuple(m for m in FRONT_MUTATIONS if m not in ASSOCIATION_MUTATIONS)
+SECONDARY_BIT = 0x80000000
 
 
 class Params(C.Structure):
@@ -104,6 +111,10 @@ def load():
         _lib = C.CDLL(str(path))
         _lib.iw_integrate.restype = C.c_uint64
         _lib.iw_integrate.argtypes = [C.POINTER(Params), C.c_uint64, C.c_uint64] + [C.c_void_p] * 22
+        _lib.iw_associate.restype = None
+        _lib.iw_associate.argtypes = [C.POINTER(Params), C.c_uint64] + [C.c_void_p] * 17
+        _lib.iw_blend.restype = None
+        _lib.iw_blend.argtypes = [C.POINTER(Params), C.c_int] + [C.c_void_p] * 14
     return _lib
 
 
@@ -243,4 +254,172 @@ def hold(res, rows_before, rows_after, new_flag=None, new_index=None, excused=No
             detail.append(f"{name}: slots {slots}; slot {i}: status {int(res.status[i])} walk {want[:, i].tolist()} run {got[:, i].tolist()}"
                           f" before {np.asarray(rows_before)[:, i].tolist() if i < n else 'new'}")
         raise AssertionError(f"{label}: differs from the walk ({stats})\n" + "\n".join(detail))
+    return stats
+
+
+# ---- the front half: projection, association and measurement blending -------------------------------------------
+
+def _front_params(camera, ip, frame_index, local_T_global, mutations):
+    W, H, fx, fy, cx, cy = camera
+    mut = 0
+    for name in mutations:
+        mut |= FRONT_MUTATIONS[name]
+    l = np.asarray(local_T_global, np.float32).reshape(-1)[:12]
+    zeros = (C.c_float * 12)()
+    return Params(W, H, fx, fy, cx, cy, ip.depth_scaling, ip.sensor_noise_factor, 0.0, 0.0,
+                  ip.normal_compatibility_threshold_deg, ip.surfel_integration_active_window_size, int(frame_index), zeros,
+                  (C.c_float * 12)(*l), mut)
+
+
+def associate(rows, depth_pre, normals, camera, ip, frame_index, local_T_global, mutations=()):
+    """The association rasters one Integrate() builds from the state before the frame (rows [25, n]) and the pre-blend
+    depth and normals: the min depth, the supporter count, the supporter set (events sup_pixel / sup_key, key = slot |
+    SECONDARY_BIT for a secondary-pixel association), the depth sum (exact `sum` and the bound any summation order
+    keeps to), the legal conflicting surfels (`conflict_legal`: pixel * 2^32 + slot, sorted; `conflict_any`: the
+    pixels that have one) and the pixels whose outcome an SFU result within 2 ulp could change (`unclear`)."""
+    W, H = camera[0], camera[1]
+    P = W * H
+    rows = np.ascontiguousarray(rows, np.float32)
+    n = rows.shape[1]
+    depth_pre = np.ascontiguousarray(np.asarray(depth_pre).reshape(-1), np.uint16)
+    normals = np.ascontiguousarray(np.asarray(normals).reshape(-1), np.float32)
+    assert depth_pre.size == P and normals.size == 2 * P
+    p = _front_params(camera, ip, frame_index, local_T_global, mutations)
+    r = SimpleNamespace(first=np.empty(P, np.float32), counts=np.empty(P, np.uint32), sum_float=np.empty(P, np.float32),
+                        sum=np.empty(P, np.float64), sum_abs=np.empty(P, np.float64), unclear=np.empty(P, np.uint8))
+    ties = np.empty(P, np.uint32)
+    sup_pixel, sup_key = np.empty(2 * n + 1, np.uint32), np.empty(2 * n + 1, np.uint32)
+    conf_pixel, conf_surfel, conf_stage = np.empty(3 * n + 1, np.uint32), np.empty(3 * n + 1, np.uint32), np.empty(3 * n + 1, np.uint8)
+    counts = np.zeros(2, np.uint64)
+    branch = np.zeros(len(FRONT_BRANCHES) + 1, np.uint64)
+    load().iw_associate(C.byref(p), n, _p(rows), _p(depth_pre), _p(normals), _p(r.first), _p(r.counts), _p(r.sum_float),
+                        _p(r.sum), _p(r.sum_abs), _p(r.unclear), _p(ties), _p(sup_pixel), _p(sup_key), _p(conf_pixel),
+                        _p(conf_surfel), _p(conf_stage), _p(counts), _p(branch))
+    ns, nc = int(counts[0]), int(counts[1])
+    r.sup_pixel, r.sup_key = sup_pixel[:ns], sup_key[:ns]
+    conf_pixel, conf_surfel, conf_stage = conf_pixel[:nc], conf_surfel[:nc], conf_stage[:nc]
+    # the merge kernel runs after the association: where it writes, its writes are the final ones
+    merge_writes = np.zeros(P, bool)
+    merge_writes[conf_pixel[conf_stage == 1]] = True
+    legal = (conf_stage == 1) | ~merge_writes[conf_pixel]
+    r.conflict_legal = np.unique(conf_pixel[legal].astype(np.uint64) << np.uint64(32) | conf_surfel[legal])
+    r.conflict_any = np.zeros(P, bool)
+    r.conflict_any[conf_pixel] = True
+    r.merge_writes = merge_writes
+    # any order of float additions of k terms lies within (k - 1) 2^-24 sum |z| of the exact sum; one or two terms:
+    # fl(a + b) in either order
+    r.sum_bound = np.maximum(r.counts.astype(np.float64) - 1, 0) * 2.0 ** -24 * r.sum_abs
+    few = r.counts <= 2
+    r.sum[few], r.sum_bound[few] = r.sum_float[few], 0.0
+    r.unclear = r.unclear.astype(bool)
+    r.branch = {name: int(v) for name, v in zip(FRONT_BRANCHES, branch)}
+    r.shape = (H, W)
+    return r
+
+
+def plain_winners(res):
+    """The plain rule's supporting surfel per pixel: the least (secondary bit, slot) of the pixel's supporters."""
+    best = np.full(res.first.size, INVALID, np.uint32)
+    np.minimum.at(best, res.sup_pixel, res.sup_key)
+    return np.where(best == INVALID, best, best & np.uint32(~SECONDARY_BIT & 0xFFFFFFFF))
+
+
+def supporter_pairs(res):
+    return np.unique(res.sup_pixel.astype(np.uint64) << np.uint64(32) | (res.sup_key & np.uint32(0x7FFFFFFF)))
+
+
+def _member(sorted_pairs, pixels, values):
+    keys = pixels.astype(np.uint64) << np.uint64(32) | np.asarray(values, np.uint64)
+    at = np.minimum(np.searchsorted(sorted_pairs, keys), max(sorted_pairs.size - 1, 0))
+    return (sorted_pairs.size > 0) & (sorted_pairs[at] == keys) if sorted_pairs.size else np.zeros(keys.shape, bool)
+
+
+def hold_association(res, rasters, winner="member", label=""):
+    """Holds association rasters (download_rasters, or the recorded reference) to the walk `res` on its clear pixels:
+    min depth bit for bit, counts, conflicting surfel a legal one (INVALID where there is none), depth sums within the
+    order bound. winner: "plain" (the plain rule, bit for bit), "member" (one of the pixel's supporters), or None.
+    Returns a dict of counts; raises AssertionError with the first differing pixels."""
+    P = res.first.size
+    get = lambda k, dt: np.asarray(rasters[k]).reshape(-1).astype(dt, copy=False)
+    first, counts = get("first_surfel_depth", np.float32), get("supporting_surfel_counts", np.uint32)
+    conflicting, sums = get("conflicting_surfels", np.uint32), get("supporting_surfel_depth_sums", np.float32)
+    clear = ~res.unclear
+    pixels = np.arange(P, dtype=np.uint32)
+    bad = {}
+
+    def check(name, wrong):
+        wrong = wrong & clear
+        if wrong.any():
+            bad[name] = np.flatnonzero(wrong)[:8].tolist()
+
+    check("min depth", first.view(np.uint32) != res.first.view(np.uint32))
+    check("count", counts != res.counts)
+    ok_conflict = np.where(res.conflict_any & (conflicting != INVALID),
+                           _member(res.conflict_legal, pixels, conflicting), ~res.conflict_any & (conflicting == INVALID))
+    check("conflicting surfel", ~ok_conflict)
+    with np.errstate(invalid="ignore"):
+        check("depth sum", ~(np.abs(sums.astype(np.float64) - res.sum) <= res.sum_bound))
+    if winner is not None:
+        supporting = get("supporting_surfels", np.uint32)
+        if winner == "plain":
+            check("supporting surfel (plain rule)", supporting != plain_winners(res))
+        else:
+            supported = res.counts > 0
+            member = _member(supporter_pairs(res), pixels, np.where(supporting == INVALID, 0, supporting))
+            check("supporting surfel", ~np.where(supported, (supporting != INVALID) & member, supporting == INVALID))
+    stats = dict(pixels=P, unclear=int(res.unclear.sum()), supported=int((res.counts > 0).sum()),
+                 contested=int((res.counts > 1).sum()), conflicts=int(res.conflict_any.sum()),
+                 merge_stage_conflicts=int(res.merge_writes.sum()))
+    if bad:
+        W = res.shape[1]
+        detail = []
+        for name, pix in bad.items():
+            i = pix[0]
+            detail.append(f"{name}: pixels {pix}; pixel {i} (x {i % W}, y {i // W}): walk first {res.first[i]} count "
+                          f"{res.counts[i]} sum {res.sum[i]} +- {res.sum_bound[i]}; run first {first[i]} count {counts[i]} "
+                          f"sum {sums[i]} conflicting {conflicting[i]}")
+        raise AssertionError(f"{label}: association differs from the walk ({stats})\n" + "\n".join(detail))
+    return stats
+
+
+def blend(depth_pre, counts, sums, radius, depth_scaling, mutations=()):
+    """The blended depth of BlendMeasurementsCUDA from the pre-blend depth [H, W] and the association's counts and
+    depth sums as handed in. Returns depth, lo, hi ([H, W] u16: the depths the reciprocal bounds allow; lo == hi:
+    exact), level_counts [2, radius + 1] (pixels per ring and level) and the branch counters."""
+    depth_pre = np.ascontiguousarray(depth_pre, np.uint16)
+    H, W = depth_pre.shape
+    P = W * H
+    counts = np.ascontiguousarray(np.asarray(counts).reshape(-1), np.uint32)
+    sums = np.ascontiguousarray(np.asarray(sums).reshape(-1), np.float32)
+    assert counts.size == P and sums.size == P and radius >= 1
+    ip = SimpleNamespace(depth_scaling=depth_scaling, sensor_noise_factor=0.0, normal_compatibility_threshold_deg=0.0,
+                         surfel_integration_active_window_size=0)
+    p = _front_params((W, H, 1.0, 1.0, 0.0, 0.0), ip, 0, np.zeros(12), mutations)
+    out, lo, hi = (np.empty(P, np.uint16) for _ in range(3))
+    dist = [np.empty(P, np.uint8) for _ in range(2)]
+    delta = [np.empty(P, np.float32) for _ in range(2)]
+    bound = [np.empty(P, np.float64) for _ in range(2)]
+    level_counts = np.zeros((2, radius + 1), np.uint64)
+    branch = np.zeros(len(FRONT_BRANCHES) + 1, np.uint64)
+    load().iw_blend(C.byref(p), int(radius), _p(depth_pre), _p(counts), _p(sums), _p(out), _p(lo), _p(hi), _p(dist[0]),
+                    _p(dist[1]), _p(delta[0]), _p(delta[1]), _p(bound[0]), _p(bound[1]), _p(level_counts), _p(branch))
+    return SimpleNamespace(depth=out.reshape(H, W), lo=lo.reshape(H, W), hi=hi.reshape(H, W),
+                           level_counts=level_counts.astype(np.int64),
+                           branch={name: int(v) for name, v in zip(FRONT_BRANCHES, branch)})
+
+
+def hold_blend(res, depth, label=""):
+    """Holds a blended depth [H, W] to the walk `res`: bit for bit where lo == hi, inside [lo, hi] elsewhere. Returns a
+    dict of counts; raises AssertionError with the first differing pixels."""
+    depth = np.asarray(depth).reshape(res.depth.shape).astype(np.int64)
+    exact = res.lo == res.hi
+    wrong = np.where(exact, depth != res.depth, (depth < res.lo) | (depth > res.hi))
+    stats = dict(pixels=int(depth.size), blended=int((res.depth != 0).sum()), ranged=int((~exact).sum()),
+                 levels=[int((row > 0).sum()) for row in res.level_counts])
+    if wrong.any():
+        ys, xs = np.nonzero(wrong)
+        detail = [f"(x {x}, y {y}): run {depth[y, x]}, walk {res.depth[y, x]} [{res.lo[y, x]}, {res.hi[y, x]}]"
+                  for y, x in list(zip(ys, xs))[:8]]
+        raise AssertionError(f"{label}: blended depth differs from the walk at {int(wrong.sum())} pixels ({stats})\n"
+                             + "\n".join(detail))
     return stats
