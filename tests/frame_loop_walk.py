@@ -34,6 +34,15 @@ whatever value in [lo, hi] the run read, its flags are those of the walk fed wit
 those two give different flags, the run's creation scan could differ from the walk's at one pixel and with it the
 index of every later new surfel: the frame is excused as a whole and not compared. An excused frame does not break a
 chain, which continues from the run's own state.
+
+Chains
+------
+`Chain` holds frame after frame of one handle, each from the state the previous hold (or a call between pushes) left.
+Its `Inputs` pre-process each pushed frame on a second handle, after a `stage` hook that restates on the CPU what the
+frame loop's ring does to a raw frame before the pre-processing reads it: nothing (`stage_identity`), the input
+pyramid of --pyramid_level (`stage_pyramid`) or the MedianFilterAndDensifyDepthMap passes (`stage_median`). The hook
+is applied to the frame and to each of its outlier-filter neighbours. Frames and poses are indexed by push: a
+pose-free session that leaves lost frames out pushes source frames `pushed_sources(states)`.
 """
 from __future__ import annotations
 
@@ -43,6 +52,7 @@ import numpy as np
 
 from tests import integrate_walk as IW
 from tests.test_regularize_float64_gpu import check as check_sweeps, expected_integrate
+from tests.util import other_frames
 
 INVALID = IW.INVALID
 
@@ -194,8 +204,141 @@ class Totals:
         assert self.excused <= 0.005 * self.slots, self.report()
         assert self.excused_frames * 10 <= max(self.frames, 10), self.report()
 
-    def assert_floors(self, min_frames):
+    def assert_floors(self, min_frames, waive=()):
+        """waive: floors (FLOOR_BRANCHES names) a chain cannot reach at its size; the caller says why."""
         floors = self.floors()
         assert self.frames >= min_frames, f"{self.label}: {self.frames} frames held"
-        assert all(v > 0 for v in floors.values()) and self.new > 0, f"{self.label}: branches not reached {floors}"
+        assert all(v > 0 for k, v in floors.items() if k not in waive) and self.new > 0, \
+            f"{self.label}: branches not reached {floors}"
         self.assert_fractions()
+
+
+# ---------------------------------------------------------------------------------------------
+# chains: the inputs of each pushed frame, and frame after frame of one handle
+# ---------------------------------------------------------------------------------------------
+
+def camera_tuple(cam):
+    return cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy
+
+
+def stage_identity(depth, color):
+    """Frames read at the handle's size, as pushed."""
+    return depth, color
+
+
+def stage_pyramid(level, width, height):
+    """--pyramid_level L (APP/main.cc:951-952, 973-981): the depth map downscaled by the median of each block without
+    zeros straight to the handle's width x height, the colour image by L rounds of halving."""
+    from tests import pyramid_walk as PW
+
+    def stage(depth, color):
+        return PW.downscale_median_excluding(depth, width, height), PW.color_image_pyramid(color, level)
+    return stage
+
+
+def stage_median(passes):
+    """--median_filter_and_densify_iterations n (APP/main.cc:927-939): n passes over the depth map; colour as is."""
+    from oracle import cpu_walk
+
+    def stage(depth, color):
+        for _ in range(passes):
+            depth = cpu_walk.median_filter_and_densify(depth)
+        return depth, color
+    return stage
+
+
+def pushed_sources(states, held_out=True):
+    """The source frame of each push of a pose-free session from its per-frame states (TrackedSession.states): with
+    relocalisation on (held_out), a frame left "lost" is not pushed, so push index and source frame diverge."""
+    return [f for f, s in enumerate(states) if not (held_out and s == "lost")]
+
+
+class Inputs:
+    """The pre-processed inputs of the frames pushed into a handle, from a handle of their own (created on first use).
+
+    depth / color: raw frames by source index (tensors or arrays, any device); sources: the source frame of each push
+    (a list the caller may extend while the session runs; None: push p is source frame p); stage(raw_depth, raw_color)
+    -> (depth, color) at `cam`, the handle's camera."""
+
+    def __init__(self, cam, depth, color, pp, stage=stage_identity, sources=None):
+        self.cam, self.depth, self.color, self.pp, self.stage = cam, depth, color, pp, stage
+        self.sources = sources
+        self.rec = None
+        self.staged = {}
+
+    def source(self, push):
+        return push if self.sources is None else self.sources[push]
+
+    def others(self, push):
+        """The source frames of push `push`'s outlier-filter neighbours: the K/2 pushes before it and after it."""
+        return [self.source(p) for p in other_frames(push, self.pp.outlier_filtering_frame_count)]
+
+    def staged_frame(self, source):
+        """Source frame `source` after the stage hook: (depth [H, W] uint16, colour [H, W, 3] uint8) numpy arrays."""
+        if source not in self.staged:
+            host = lambda a: a.cpu().numpy() if hasattr(a, "cpu") else np.asarray(a)
+            self.staged[source] = self.stage(host(self.depth[source]), host(self.color[source]))
+        return self.staged[source]
+
+    def frame(self, push, global_T_frame, frame_T_global):
+        """hold_frame's `frame` for push `push`; global_T_frame / frame_T_global: the poses pushed, by push index."""
+        import torch
+        from surfelmeshing_b200 import reconstruction as R
+        cam, pp = self.cam, self.pp
+        if self.rec is None:
+            self.rec = R.CUDASurfelReconstruction(1024, *camera_tuple(cam))
+        K = pp.outlier_filtering_frame_count
+        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
+        raw_depth, color = self.staged_frame(self.source(push))
+        others = [dev(self.staged_frame(s)[0]) for s in self.others(push)]
+        g = np.asarray(global_T_frame[:push + K // 2 + 1], np.float32)
+        l = np.asarray(frame_T_global[:push + K // 2 + 1], np.float32)
+        transforms = R.outlier_filter_transforms(g, l, push, K, pp.depth_scaling)
+        H, W = cam.height, cam.width
+        assert raw_depth.shape == (H, W) and color.shape == (H, W, 3), (raw_depth.shape, color.shape)
+        d = torch.zeros((H, W), dtype=torch.uint16, device="cuda")
+        n = torch.zeros((H, W, 2), dtype=torch.float32, device="cuda")
+        r = torch.zeros((H, W), dtype=torch.float32, device="cuda")
+        self.rec.preprocess(None, pp, dev(raw_depth), others, transforms, d, n, r)
+        torch.cuda.synchronize()
+        return dict(depth_pre=d.cpu().numpy(), normals=n.cpu().numpy(), radius=r.cpu().numpy(), color=color)
+
+    def close(self):
+        if self.rec is not None:
+            self.rec.close()
+
+
+class Chain:
+    """Holds frame after frame of one handle, each from the state the previous hold (or a call between) left.
+    poses: (global_T_frame, frame_T_global), the poses pushed, by push index (lists the caller may extend)."""
+
+    def __init__(self, label, rec, inputs, ip, poses, first_frame_index=0, plain=False):
+        self.label, self.rec, self.inputs, self.ip, self.poses = label, rec, inputs, ip, poses
+        self.first = first_frame_index
+        self.winner = "plain" if plain else "member"
+        self.rows, self.merges = np.zeros((25, 0), np.float32), 0
+        self.totals = Totals(label)
+
+    def restart(self):
+        """The state after a call between pushes, or after a frame not held: the next frame starts from it."""
+        rows, _, merges = self.rec.dump_state()
+        self.rows, self.merges = rows.copy(), merges
+
+    def hold(self, frame_index):
+        rec = self.rec
+        push = frame_index - self.first
+        rows, n, merges = rec.dump_state()
+        rows = rows.copy()
+        rasters = rec.download_rasters()
+        counters = frame_counters(rec)
+        g, l = self.poses
+        stats = hold_frame(self.rows, rows, merges, rasters, self.inputs.frame(push, g, l), frame_index, g[push], l[push],
+                           camera_tuple(self.inputs.cam), self.ip, merges_before=self.merges, counters=counters,
+                           winner=self.winner, label=f"{self.label} frame {frame_index}")
+        self.totals.add(stats)
+        self.rows, self.merges = rows, merges
+
+    def finish(self, min_frames, waive=()):
+        self.inputs.close()
+        print(self.totals.report())
+        self.totals.assert_floors(min_frames, waive)

@@ -13,7 +13,9 @@ whole stream would only drift.
 
 Each frame's inputs come from a second handle outside the session: `preprocess` of the raw frame with the
 outlier-filter transforms of the pushed poses. The first-frame parity tests hold the frame loop's fused
-pre-processing to that call, so a difference here is a finding about the pre slot of the graph.
+pre-processing to that call, so a difference here is a finding about the pre slot of the graph. The chains here push
+raw frames at the handle's size with the stream's poses; tests/test_frame_loop_inputs_gpu.py holds the pyramid,
+median-densify and pose-free paths with the same Chain.
 
 Not held: the frames sm_session_end integrates in the frame-graph mode. It runs its last two steps without returning
 to the caller, so they cannot be dumped one by one.
@@ -29,7 +31,6 @@ from surfelmeshing_b200 import synthetic as S
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams
 from tests import frame_loop_walk as FW
 from tests.test_reloc_gpu import odd_camera
-from tests.util import other_frames
 
 pytestmark = pytest.mark.gpu
 
@@ -54,69 +55,7 @@ def make_stream(cam, frames, K=8):
     return st
 
 
-def camera_tuple(cam):
-    return cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy
-
-
-class Inputs:
-    """The pre-processed inputs of a stream's frames, from a handle of their own."""
-
-    def __init__(self, cam, st, pp):
-        self.cam, self.st, self.pp = cam, st, pp
-        self.rec = R.CUDASurfelReconstruction(1024, *camera_tuple(cam))
-
-    def frame(self, local):
-        cam, st, pp = self.cam, self.st, self.pp
-        K = pp.outlier_filtering_frame_count
-        others = [st.depth[f] for f in other_frames(local, K)]
-        transforms = R.outlier_filter_transforms(st.global_T_frame, st.frame_T_global, local, K, pp.depth_scaling)
-        H, W = cam.height, cam.width
-        d = torch.zeros((H, W), dtype=torch.uint16, device="cuda")
-        n = torch.zeros((H, W, 2), dtype=torch.float32, device="cuda")
-        r = torch.zeros((H, W), dtype=torch.float32, device="cuda")
-        self.rec.preprocess(None, pp, st.depth[local], others, transforms, d, n, r)
-        torch.cuda.synchronize()
-        return dict(depth_pre=d.cpu().numpy(), normals=n.cpu().numpy(), radius=r.cpu().numpy(),
-                    color=st.color[local].cpu().numpy())
-
-    def close(self):
-        self.rec.close()
-
-
-class Chain:
-    """Holds frame after frame of one handle, each from the state the previous hold (or a call between) left."""
-
-    def __init__(self, label, rec, cam, st, pp, ip, first_frame_index=0, plain=False):
-        self.label, self.rec, self.cam, self.st, self.ip = label, rec, cam, st, ip
-        self.first = first_frame_index
-        self.winner = "plain" if plain else "member"
-        self.inputs = Inputs(cam, st, pp)
-        self.rows, self.merges = np.zeros((25, 0), np.float32), 0
-        self.totals = FW.Totals(label)
-
-    def restart(self):
-        """The state after a call between pushes: the next frame starts from it."""
-        rows, _, merges = self.rec.dump_state()
-        self.rows, self.merges = rows.copy(), merges
-
-    def hold(self, frame_index):
-        rec, st = self.rec, self.st
-        local = frame_index - self.first
-        rows, n, merges = rec.dump_state()
-        rows = rows.copy()
-        rasters = rec.download_rasters()
-        counters = FW.frame_counters(rec)
-        stats = FW.hold_frame(self.rows, rows, merges, rasters, self.inputs.frame(local), frame_index,
-                              st.global_T_frame[local], st.frame_T_global[local], camera_tuple(self.cam), self.ip,
-                              merges_before=self.merges, counters=counters, winner=self.winner,
-                              label=f"{self.label} frame {frame_index}")
-        self.totals.add(stats)
-        self.rows, self.merges = rows, merges
-
-    def finish(self, min_frames):
-        self.inputs.close()
-        print(self.totals.report())
-        self.totals.assert_floors(min_frames)
+camera_tuple = FW.camera_tuple
 
 
 def params(cam, K=8):
@@ -126,28 +65,39 @@ def params(cam, K=8):
     return pp, IntegrateParams.defaults()
 
 
+def host_frame(a, kind):
+    """A frame tensor as pushed: "device" (CUDA, read in place), "pageable" or "pinned" host memory."""
+    return a if kind == "device" else (a.cpu().pin_memory() if kind == "pinned" else a.cpu())
+
+
 def session_chain(label, cam=QVGA, frames=FRAMES, K=8, pp_set=None, ip_set=None, plain=False, serial=False,
-                  first_frame_index=0, pinned=False, between=None, min_frames=15):
+                  first_frame_index=0, kinds=("device",), between=None, min_frames=15, st=None,
+                  stage=FW.stage_identity, configure=(), waive=()):
+    """A session on a handle at `cam` holding every frame it integrates. st: the stream (default: make_stream at cam),
+    its frames pushed as they are (at 2^L x cam with configure pyramid_level L) and held after `stage`; push i gives
+    kinds[i % len(kinds)] frames; configure: sm_configure (key, value) pairs."""
     pp, ip = params(cam, K)
     for k, v in (pp_set or {}).items():
         setattr(pp, k, v)
     for k, v in (ip_set or {}).items():
         setattr(ip, k, v)
-    st = make_stream(cam, frames, K)
+    st = st or make_stream(cam, frames, K)
     rec = R.CUDASurfelReconstruction(CAP, *camera_tuple(cam))
     if plain:
         rec.configure("tiebreak_wave", 0)
     if serial:
         rec.enable_timings(True)
-    chain = Chain(label, rec, cam, st, pp, ip, first_frame_index, plain)
+    for key, value in configure:
+        rec.configure(key, value)
+    chain = FW.Chain(label, rec, FW.Inputs(cam, st.depth, st.color, pp, stage), ip,
+                     (st.global_T_frame, st.frame_T_global), first_frame_index, plain)
     t0 = time.perf_counter()
     last = -1
     try:
-        with rec.session(pp, ip, (cam.width, cam.height), first_frame_index) as s:
+        with rec.session(pp, ip, (st.depth.shape[2], st.depth.shape[1]), first_frame_index) as s:
             for i in range(frames):
-                d, c = st.depth[i], st.color[i]
-                if pinned:
-                    d, c = d.cpu().pin_memory(), c.cpu().pin_memory()
+                kind = kinds[i % len(kinds)]
+                d, c = host_frame(st.depth[i], kind), host_frame(st.color[i], kind)
                 status = s.push(d, c, st.global_T_frame[i], st.frame_T_global[i])
                 f = status.last_integrated_frame
                 if f != last:
@@ -156,7 +106,7 @@ def session_chain(label, cam=QVGA, frames=FRAMES, K=8, pp_set=None, ip_set=None,
                     last = f
                     if between is not None and between(s, rec, f, ip):
                         chain.restart()
-        chain.finish(min_frames)
+        chain.finish(min_frames, waive)
     finally:
         rec.close()
     print(f"{label}: {time.perf_counter() - t0:.1f} s")
@@ -172,7 +122,7 @@ CASES = {
     "odd-camera-K4": dict(cam=odd_camera(), K=4),
     "bilateral-radius-4": dict(pp_set=dict(bilateral_filter_sigma_xy=2.0)),
     "first-frame-2^30-64": dict(first_frame_index=2**30 - 64),
-    "pinned-host-frames": dict(pinned=True),
+    "pinned-host-frames": dict(kinds=("pinned",)),
     "serial": dict(serial=True),
 }
 
@@ -210,20 +160,31 @@ def test_session_chain_vga(product):
     session_chain("640x480", cam=VGA, frames=24, min_frames=12)
 
 
-def test_stream_run_one_frame_per_call(product):
-    """sm_stream_run over [f, f + 1), sixteen times on one handle: every call runs the graph's placeholder steps around
-    its one frame, and continues from the state the previous call left."""
-    cam = QVGA
+def stream_run_chain(label, cam=QVGA, st=None, frames_on=lambda a: a, stage=FW.stage_identity, configure=()):
+    """sm_stream_run over [f, f + 1), sixteen times on one handle, holding each frame. st: the stream (default:
+    make_stream at cam), passed through frames_on (e.g. into pinned memory) and held after `stage`."""
     pp, ip = params(cam)
-    st = make_stream(cam, 24)
+    st = st or make_stream(cam, 24)
     others = R.stream_outlier_filter_transforms(st.global_T_frame, st.frame_T_global, 8, st.depth_scaling)
     rec = R.CUDASurfelReconstruction(CAP, *camera_tuple(cam))
-    chain = Chain("stream_run [f, f + 1)", rec, cam, st, pp, ip)
+    for key, value in configure:
+        rec.configure(key, value)
+    chain = FW.Chain(label, rec, FW.Inputs(cam, st.depth, st.color, pp, stage), ip,
+                     (st.global_T_frame, st.frame_T_global))
+    depth, color = frames_on(st.depth), frames_on(st.color)
+    t0 = time.perf_counter()
     try:
         for f in range(4, 20):
-            stats = rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, others, pp, ip, f, f + 1)
+            stats = rec.stream_run(None, depth, color, st.global_T_frame, st.frame_T_global, others, pp, ip, f, f + 1)
             assert stats.frames_integrated == 1
             chain.hold(f)
         chain.finish(min_frames=16)
     finally:
         rec.close()
+    print(f"{label}: {time.perf_counter() - t0:.1f} s")
+
+
+def test_stream_run_one_frame_per_call(product):
+    """sm_stream_run over [f, f + 1), sixteen times on one handle: every call runs the graph's placeholder steps around
+    its one frame, and continues from the state the previous call left."""
+    stream_run_chain("stream_run [f, f + 1)")

@@ -107,3 +107,56 @@ def test_a_ranged_pixel_that_flips_a_creation_excuses_the_frame(monkeypatch):
         if not flips:
             assert res.new_flag[U] == 1
             assert stats["excused"] >= 1 and stats["ranged"] >= 1
+
+
+# ---------------------------------------------------------------------------------------------
+# the inputs of a chain: stage hooks and the push -> source frame map
+# ---------------------------------------------------------------------------------------------
+
+def test_stage_hooks_on_recorded_frames(golden):
+    """Inputs' staged frames are the pyramid / median restatements of each recorded frame alone, whatever order the
+    frames are staged in and however often each is read (a frame is read as its neighbours' outlier frame too)."""
+    from oracle import cpu_walk
+    from tests import pyramid_walk as PW
+    depth, color = golden["depth"], golden["color"]
+    H, W = depth.shape[1:]
+    frames = (7, 2, 7, 5)
+    for level in (1, 2, 3):
+        w, h = W >> level, H >> level
+        inputs = FW.Inputs(None, depth, color, None, FW.stage_pyramid(level, w, h))
+        for f in frames:
+            d, c = inputs.staged_frame(f)
+            assert d.shape == (h, w) and c.shape == (h, w, 3)
+            assert np.array_equal(d, PW.downscale_median_excluding(depth[f], w, h))
+            assert np.array_equal(c, PW.color_image_pyramid(color[f], level))
+    for passes in (1, 2, 3):
+        inputs = FW.Inputs(None, depth, color, None, FW.stage_median(passes))
+        for f in frames:
+            d, c = inputs.staged_frame(f)
+            expect = depth[f]
+            for _ in range(passes):
+                expect = cpu_walk.median_filter_and_densify(expect)
+            assert np.array_equal(d, expect) and np.array_equal(c, color[f])
+            assert (d != 0).sum() > (depth[f] != 0).sum(), "the passes densify"
+    inputs = FW.Inputs(None, depth, color, None)
+    assert all(np.array_equal(inputs.staged_frame(f)[0], depth[f]) for f in frames)
+
+
+def test_push_to_source_map_with_frames_left_out():
+    """A relocalising session leaves its lost frames out: push p reads source frame sources[p], and its outlier
+    neighbours are the K/2 pushes on either side, which skip the frames left out. Without relocalisation every frame is
+    pushed, lost or not."""
+    states = ["tracked"] * 6 + ["lost", "lost", "relocalised"] + ["tracked"] * 7
+    sources = FW.pushed_sources(states)
+    assert sources == [0, 1, 2, 3, 4, 5, 8, 9, 10, 11, 12, 13, 14, 15]
+    assert FW.pushed_sources(states, held_out=False) == list(range(len(states)))
+    pp = golden_params(load_golden())[0]
+    assert pp.outlier_filtering_frame_count == 8
+    inputs = FW.Inputs(None, None, None, pp, sources=sources)
+    assert inputs.source(6) == 8
+    assert inputs.others(4) == [3, 2, 1, 0, 5, 8, 9, 10]
+    assert inputs.others(7) == [8, 5, 4, 3, 10, 11, 12, 13]
+    # the caller extends the map while the session runs
+    sources.append(16)
+    assert inputs.source(10) == 12 and inputs.others(10) == [11, 10, 9, 8, 13, 14, 15, 16]
+    assert FW.Inputs(None, None, None, pp).others(6) == [5, 4, 3, 2, 7, 8, 9, 10]
