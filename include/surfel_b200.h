@@ -418,6 +418,41 @@ int sm_render_mesh(sm_reconstruction* r, void* stream, const sm_render_params* p
                    float* normal, size_t normal_pitch,
                    uint32_t* index, size_t index_pitch);
 
+/* ---- rendering the textured triangle mesh (DESIGN.md section 5.17) ---------------------------------------------
+ * sm_render_mesh with the colour of its triangles read from a texture atlas, such as the atlas and uv that
+ * sm_mesh_texture makes for the same list: to look at a textured mesh from new cameras, compare it with held-out
+ * frames or hand its images to something that consumes them. Same raster, rules T1-T7 and outputs; in the same
+ * arithmetic (fp32, denormals flushed to zero, no contraction, each operation rounded on its own):
+ *  T8. Textured colour, for a pixel whose winning key is a triangle t (every other output, and every disk or empty
+ *      pixel, is what sm_render_mesh gives for the same arguments). With s_0 < s_1 < s_2 t's corners sorted by slot
+ *      (T1), UV_k = (uv[6t + 2j], uv[6t + 2j + 1]) with j the list position of the corner whose slot is s_k, so
+ *      rotating or re-winding t together with its uv leaves the image unchanged. With q_k and z of T5 at the pixel,
+ *      U = ((q_0 * U_0 + q_1 * U_1) + q_2 * U_2) * z, and V alike. If U or V is not finite the pixel takes T7's
+ *      colour. Otherwise U and V are clamped to [0, 1], x = U * float(W) - 0.5, y = V * float(H) - 0.5, x0 = floor(x),
+ *      fx = x - x0, y0 = floor(y), fy = y - y0, and texel (i, j) is read with i clamped to [0, W - 1] and j to
+ *      [0, H - 1]. Per channel, with V_ab the texel (x0 + a, y0 + b) as a float, sample = top + fy * (bot - top),
+ *      top = V_00 + fx * (V_10 - V_00), bot = V_01 + fx * (V_11 - V_01) (X6's form), and the colour is the u8 of
+ *      sample + 0.5, truncated, 255 if that is >= 255. The lookup is done in software: the 8-bit weights of hardware
+ *      texture filtering cannot meet this rule.
+ * atlas is a DEVICE buffer of packed u8x3 texels (r, g, b), W = atlas_width by H = atlas_height, atlas_pitch bytes
+ * per row; uv (DEVICE, 6 x triangle_count floats) holds per triangle and per corner in list order the (u, v) of
+ * sm_mesh_texture's uv output, v = 0 at row 0. Asynchronous on `stream`, no host synchronisation; only reads the
+ * surfel state, the triangles, uv and the atlas; the same scratch and launches as sm_render_mesh.
+ * SM_ERR_INVALID_ARGUMENT, with no launch, for everything sm_render_mesh rejects, color NULL, uv or atlas NULL with
+ * triangle_count > 0, atlas_width or atlas_height outside [1, SM_TEXTURE_MAX_ATLAS_SIDE] with triangle_count > 0,
+ * atlas_pitch below 3 x atlas_width, and an output that overlaps the atlas or uv. An empty list with a 0 x 0 atlas
+ * is legal. */
+int sm_render_mesh_textured(sm_reconstruction* r, void* stream, const sm_render_params* p,
+                            const float view_T_global[12],      /* 3x4 row-major, global -> camera */
+                            const uint32_t* triangles /* device, 3 x triangle_count */, uint64_t triangle_count,
+                            int32_t flags,
+                            const float* uv,          /* device, 6 x triangle_count: sm_mesh_texture's uv output */
+                            const uint8_t* atlas, size_t atlas_pitch, int32_t atlas_width, int32_t atlas_height,
+                            float* depth, size_t depth_pitch,
+                            uint8_t* color, size_t color_pitch,
+                            float* normal, size_t normal_pitch,
+                            uint32_t* index, size_t index_pitch);
+
 /* ---- camera tracking against the cloud (DESIGN.md section 1 row f8, section 5.6) ----------------------------
  * The reference reads every camera pose from a trajectory file (APP/main.cc:601-625) and has no tracker.
  * sm_track_frame estimates the pose of a depth map by projective point-to-plane ICP against a model view,

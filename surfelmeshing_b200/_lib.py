@@ -404,6 +404,8 @@ _PRODUCT_ONLY = {
     "render_surfels": (C.c_int, [_P, _P, C.POINTER(RenderParams), _P, _P, _SZ, _P, _SZ, _P, _SZ, _P, _SZ]),
     "render_mesh": (C.c_int, [_P, _P, C.POINTER(RenderParams), _P, _P, C.c_uint64, _I, _P, _SZ, _P, _SZ, _P, _SZ, _P,
                               _SZ]),
+    "render_mesh_textured": (C.c_int, [_P, _P, C.POINTER(RenderParams), _P, _P, C.c_uint64, _I, _P, _P, _SZ, _I, _I,
+                                       _P, _SZ, _P, _SZ, _P, _SZ, _P, _SZ]),
     "default_track_params": (None, [C.POINTER(TrackParams)]),
     "track_frame": (C.c_int, [_P, _P, C.POINTER(TrackParams), C.POINTER(PreprocessParams), _P, _SZ, _P, _P,
                               C.POINTER(TrackResult)]),

@@ -212,7 +212,8 @@ __global__ void __launch_bounds__(kResolveBlock) k_render_resolve(DeviceState d,
   }
 }
 
-// ---- sm_render_mesh (DESIGN.md section 5.9): rules T1-T7 of include/surfel_b200.h ----
+// ---- sm_render_mesh (DESIGN.md section 5.9): rules T1-T7 of include/surfel_b200.h; sm_render_mesh_textured
+// (section 5.17) adds T8 to the resolve ----
 
 constexpr int kMarkBlock = 256;
 constexpr int kTriBlock = 256;
@@ -225,6 +226,11 @@ struct MeshArgs {
   u32* marks;             // one bit per slot: a corner of a T1-valid triangle (SM_RENDER_UNMESHED_SURFELS only)
   u32* large_list;        // triangles whose rectangle has more than kSmallTrianglePixels pixels
   u32* large_count;
+  // sm_render_mesh_textured (T8): per triangle the (u, v) of its corners in list order, and the packed u8x3 atlas;
+  // atlas NULL: the colour of T7. Last, so the other kernels' parameter offsets stay where they were.
+  const float* uv;        // [triangle_count][3][2]
+  const u8* atlas; size_t atlas_pitch;
+  int atlas_width, atlas_height;
 };
 
 // T1 for triangle t: its three slots (in list order) if all are < n and present.
@@ -426,6 +432,48 @@ __device__ __forceinline__ float3 triangle_normal(const Triangle& tr) {
   return make_float3(fmul(g.x, inv), fmul(g.y, inv), fmul(g.z, inv));
 }
 
+// T8 channel ch of the bilinear lookup between texels t00, t10 (one row) and t01, t11 (the next), rounded half up and
+// clamped to 255: X6's form.
+__device__ __forceinline__ u32 bilinear_channel(const u8* t00, const u8* t10, const u8* t01, const u8* t11, int ch,
+                                                float fx, float fy) {
+  const float v00 = u2f(t00[ch]), v10 = u2f(t10[ch]), v01 = u2f(t01[ch]), v11 = u2f(t11[ch]);
+  const float top = fadd(v00, fmul(fx, fsub(v10, v00)));
+  const float bot = fadd(v01, fmul(fx, fsub(v11, v01)));
+  const float value = fadd(fadd(top, fmul(fy, fsub(bot, top))), 0.5f);
+  return value >= 255.f ? 255u : static_cast<u32>(f2i_trunc(value));
+}
+
+// T8: the atlas colour of triangle t at the pixel of T5's q and z; false (T7's colour) if U or V is not finite. Each
+// sorted corner takes the uv of its list position, so the lookup does not depend on the winding or the rotation.
+__device__ __forceinline__ bool texture_rgb(const MeshArgs& m, u32 t, const Triangle& tr, const float q[3], float z,
+                                            u32* rgb) {
+  const u32* p = m.triangles + 3 * static_cast<size_t>(t);
+  const float* uv = m.uv + 6 * static_cast<size_t>(t);
+  float cu[3], cv[3];
+  for (int k = 0; k < 3; ++k) {
+    const int j = p[0] == tr.s[k] ? 0 : (p[1] == tr.s[k] ? 1 : 2);
+    cu[k] = uv[2 * j];
+    cv[k] = uv[2 * j + 1];
+  }
+  float u = fmul(fadd(fadd(fmul(q[0], cu[0]), fmul(q[1], cu[1])), fmul(q[2], cu[2])), z);
+  float v = fmul(fadd(fadd(fmul(q[0], cv[0]), fmul(q[1], cv[1])), fmul(q[2], cv[2])), z);
+  if (!isfinite(u) || !isfinite(v)) return false;
+  u = fminf(fmaxf(u, 0.f), 1.f);
+  v = fminf(fmaxf(v, 0.f), 1.f);
+  const float x = fsub(fmul(u, i2f(m.atlas_width)), 0.5f), y = fsub(fmul(v, i2f(m.atlas_height)), 0.5f);
+  const float xf = floorf(x), yf = floorf(y);
+  const float fx = fsub(x, xf), fy = fsub(y, yf);
+  const int x0 = static_cast<int>(xf), y0 = static_cast<int>(yf);   // in [-1, W - 1] and [-1, H - 1]
+  const int i0 = max(x0, 0), i1 = min(x0 + 1, m.atlas_width - 1);
+  const int j0 = max(y0, 0), j1 = min(y0 + 1, m.atlas_height - 1);
+  const u8* r0 = m.atlas + static_cast<size_t>(j0) * m.atlas_pitch;
+  const u8* r1 = m.atlas + static_cast<size_t>(j1) * m.atlas_pitch;
+  const u8 *t00 = r0 + 3 * i0, *t10 = r0 + 3 * i1, *t01 = r1 + 3 * i0, *t11 = r1 + 3 * i1;
+  *rgb = bilinear_channel(t00, t10, t01, t11, 0, fx, fy) | (bilinear_channel(t00, t10, t01, t11, 1, fx, fy) << 8) |
+         (bilinear_channel(t00, t10, t01, t11, 2, fx, fy) << 16);
+  return true;
+}
+
 __global__ void __launch_bounds__(kResolveBlock) k_mesh_render_resolve(DeviceState d, RenderArgs a, MeshArgs m) {
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {   // the raster passes have finished
     *a.large_count = 0;
@@ -456,10 +504,12 @@ __global__ void __launch_bounds__(kResolveBlock) k_mesh_render_resolve(DeviceSta
           float w[3], q[3];
           triangle_weights(tr, px, py, w);
           const float z = triangle_depth(tr, w, q);
-          const u32 corner_rgb[3] = {SM_SU(SM_ROW_COLOR, tr.s[0]), SM_SU(SM_ROW_COLOR, tr.s[1]),
-                                     SM_SU(SM_ROW_COLOR, tr.s[2])};
-          rgb = blend_channel(q, corner_rgb, 0, z) | (blend_channel(q, corner_rgb, 8, z) << 8) |
-                (blend_channel(q, corner_rgb, 16, z) << 16);
+          if (!m.atlas || !texture_rgb(m, index, tr, q, z, &rgb)) {
+            const u32 corner_rgb[3] = {SM_SU(SM_ROW_COLOR, tr.s[0]), SM_SU(SM_ROW_COLOR, tr.s[1]),
+                                       SM_SU(SM_ROW_COLOR, tr.s[2])};
+            rgb = blend_channel(q, corner_rgb, 0, z) | (blend_channel(q, corner_rgb, 8, z) << 8) |
+                  (blend_channel(q, corner_rgb, 16, z) << 16);
+          }
         }
         if (a.normal) nrm = triangle_normal(tr);
       }
@@ -565,6 +615,99 @@ int EnsureMeshRenderBuffers(sm_reconstruction* r, cudaStream_t stream, u32 trian
   return SM_OK;
 }
 
+// The texture of sm_render_mesh_textured (T8).
+struct MeshTexture {
+  const float* uv;
+  const uint8_t* atlas; size_t atlas_pitch;
+  int32_t atlas_width, atlas_height;
+};
+
+// Bytes from the start of a raster of `rows` rows to the end of its last row, saturated.
+u64 RasterBytes(size_t pitch, int rows, u64 row_bytes) {
+  const u64 head = Bytes(static_cast<u64>(rows - 1), pitch == 0 ? 1 : pitch);
+  return head > UINT64_MAX - row_bytes ? UINT64_MAX : head + row_bytes;
+}
+
+// The checks sm_render_mesh_textured adds to sm_render_mesh's: the reason the texture is refused, or nullptr.
+const char* MeshTextureError(const MeshTexture& x, u64 count, const RenderArgs& a) {
+  if (!a.color) return "color is NULL";
+  if (x.atlas_width > 0 && x.atlas_pitch < 3 * static_cast<size_t>(x.atlas_width)) return "atlas_pitch is below 3 x atlas_width";
+  if (count == 0) return nullptr;   // nothing is read
+  if (!x.uv || !x.atlas) return "uv or atlas is NULL with a count > 0";
+  if (x.atlas_width < 1 || x.atlas_width > SM_TEXTURE_MAX_ATLAS_SIDE || x.atlas_height < 1 ||
+      x.atlas_height > SM_TEXTURE_MAX_ATLAS_SIDE)
+    return "atlas_width and atlas_height must be in [1, SM_TEXTURE_MAX_ATLAS_SIDE]";
+  const u64 uv_bytes = 24 * count, atlas_bytes = RasterBytes(x.atlas_pitch, x.atlas_height, 3 * static_cast<u64>(x.atlas_width));
+  const u64 w = static_cast<u64>(a.width);
+  const struct { const void* p; size_t pitch; u64 row; } outputs[4] = {
+      {a.depth, a.depth_pitch, 4 * w}, {a.color, a.color_pitch, 3 * w}, {a.normal, a.normal_pitch, 12 * w},
+      {a.index, a.index_pitch, 4 * w}};
+  for (const auto& o : outputs) {
+    if (!o.p) continue;
+    const u64 bytes = RasterBytes(o.pitch, a.height, o.row);
+    if (Overlap(o.p, bytes, x.uv, uv_bytes) || Overlap(o.p, bytes, x.atlas, atlas_bytes))
+      return "an output overlaps the atlas or uv";
+  }
+  return nullptr;
+}
+
+// sm_render_mesh, and with `texture` sm_render_mesh_textured: the same checks (then the texture's), scratch and
+// launches; only the resolve reads the texture.
+int DrawMesh(sm_reconstruction* r, cudaStream_t stream, const char* name, const sm_render_params& p,
+             const float* view_T_global, const uint32_t* triangles, uint64_t triangle_count, int32_t flags,
+             const MeshTexture* texture, float* depth, size_t depth_pitch, uint8_t* color, size_t color_pitch,
+             float* normal, size_t normal_pitch, uint32_t* index, size_t index_pitch) {
+  auto bad = [name](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string(name) + ": " + why).c_str()); };
+  RenderArgs a;
+  int status = MakeRenderArgs(r, stream, name, p, view_T_global, depth, depth_pitch, color, color_pitch, normal,
+                              normal_pitch, index, index_pitch, &a);
+  if (status != SM_OK) return status;
+  if (!triangles && triangle_count > 0) return bad("triangles is NULL with a count > 0");
+  if (triangle_count >= (1ull << 31)) return bad("triangle_count must be < 2^31");
+  if (flags & ~SM_RENDER_UNMESHED_SURFELS) return bad("unknown flag bits");
+  if (texture)
+    if (const char* why = MeshTextureError(*texture, triangle_count, a)) return bad(why);
+  const bool disks = (flags & SM_RENDER_UNMESHED_SURFELS) != 0;
+  status = EnsureRenderBuffers(r, stream, static_cast<size_t>(p.width) * static_cast<size_t>(p.height));
+  if (status == SM_OK) status = EnsureMeshRenderBuffers(r, stream, static_cast<u32>(triangle_count));
+  if (status != SM_OK) return status;
+  const RenderScratch& s = *r->render;
+  a.keys = s.keys;
+  a.large_list = s.large_list;
+  a.large_count = s.large_count;
+  MeshArgs m;
+  m.triangles = triangles;
+  m.triangle_count = static_cast<u32>(triangle_count);
+  m.marks = s.mesh_marks;
+  m.large_list = s.mesh_large_list;
+  m.large_count = s.mesh_large_count;
+  m.uv = texture ? texture->uv : nullptr;
+  m.atlas = texture && triangle_count > 0 ? texture->atlas : nullptr;
+  m.atlas_pitch = texture ? texture->atlas_pitch : 0;
+  m.atlas_width = texture ? texture->atlas_width : 0;
+  m.atlas_height = texture ? texture->atlas_height : 0;
+  r->last_stream = stream;
+  auto grid = [](u32 items, int block, int resident) {
+    const u32 blocks = (items + block - 1) / block;
+    return dim3(blocks == 0 ? 1u : (blocks < static_cast<u32>(resident) ? blocks : static_cast<u32>(resident)));
+  };
+  if (disks) {
+    SM_CUDA(cudaMemsetAsync(s.mesh_marks, 0, sizeof(u32) * ((r->d.stride + 31) / 32), stream));
+    LaunchScope scope(stream, KID_MESH_RENDER_MARK);
+    LaunchKernel(k_mesh_render_mark, grid(m.triangle_count, kMarkBlock, s.mesh_mark_blocks), dim3(kMarkBlock), 0,
+                 stream, r->d, a, m);
+  }
+  { LaunchScope scope(stream, KID_MESH_RENDER_TRI); LaunchKernel(k_mesh_render_tri, grid(m.triangle_count, kTriBlock, s.mesh_tri_blocks), dim3(kTriBlock), 0, stream, r->d, a, m); }
+  { LaunchScope scope(stream, KID_MESH_RENDER_LARGE); LaunchKernel(k_mesh_render_large, dim3(s.mesh_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a, m); }
+  if (disks) {
+    { LaunchScope scope(stream, KID_MESH_RENDER_SPLAT); LaunchKernel(k_mesh_render_splat, dim3(s.mesh_splat_blocks), dim3(kSplatBlock), 0, stream, r->d, a, m); }
+    { LaunchScope scope(stream, KID_MESH_RENDER_SPLAT_LARGE); LaunchKernel(k_mesh_render_splat_large, dim3(s.mesh_splat_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a); }
+  }
+  const dim3 resolve_grid((p.width + kResolveBlock - 1) / kResolveBlock, p.height < 65535 ? p.height : 65535);
+  { LaunchScope scope(stream, KID_MESH_RENDER_RESOLVE); LaunchKernel(k_mesh_render_resolve, resolve_grid, dim3(kResolveBlock), 0, stream, r->d, a, m); }
+  return CheckLaunch("render mesh");
+}
+
 }  // namespace
 
 int RenderSurfels(sm_reconstruction* r, cudaStream_t stream, const sm_render_params& p, const float* view_T_global,
@@ -591,48 +734,8 @@ int RenderMesh(sm_reconstruction* r, cudaStream_t stream, const sm_render_params
                const uint32_t* triangles, uint64_t triangle_count, int32_t flags, float* depth, size_t depth_pitch,
                uint8_t* color, size_t color_pitch, float* normal, size_t normal_pitch, uint32_t* index,
                size_t index_pitch) {
-  RenderArgs a;
-  int status = MakeRenderArgs(r, stream, "sm_render_mesh", p, view_T_global, depth, depth_pitch, color, color_pitch,
-                              normal, normal_pitch, index, index_pitch, &a);
-  if (status != SM_OK) return status;
-  if (!triangles && triangle_count > 0)
-    return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_mesh: triangles is NULL with a count > 0");
-  if (triangle_count >= (1ull << 31)) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_mesh: triangle_count must be < 2^31");
-  if (flags & ~SM_RENDER_UNMESHED_SURFELS) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_mesh: unknown flag bits");
-  const bool disks = (flags & SM_RENDER_UNMESHED_SURFELS) != 0;
-  status = EnsureRenderBuffers(r, stream, static_cast<size_t>(p.width) * static_cast<size_t>(p.height));
-  if (status == SM_OK) status = EnsureMeshRenderBuffers(r, stream, static_cast<u32>(triangle_count));
-  if (status != SM_OK) return status;
-  const RenderScratch& s = *r->render;
-  a.keys = s.keys;
-  a.large_list = s.large_list;
-  a.large_count = s.large_count;
-  MeshArgs m;
-  m.triangles = triangles;
-  m.triangle_count = static_cast<u32>(triangle_count);
-  m.marks = s.mesh_marks;
-  m.large_list = s.mesh_large_list;
-  m.large_count = s.mesh_large_count;
-  r->last_stream = stream;
-  auto grid = [](u32 items, int block, int resident) {
-    const u32 blocks = (items + block - 1) / block;
-    return dim3(blocks == 0 ? 1u : (blocks < static_cast<u32>(resident) ? blocks : static_cast<u32>(resident)));
-  };
-  if (disks) {
-    SM_CUDA(cudaMemsetAsync(s.mesh_marks, 0, sizeof(u32) * ((r->d.stride + 31) / 32), stream));
-    LaunchScope scope(stream, KID_MESH_RENDER_MARK);
-    LaunchKernel(k_mesh_render_mark, grid(m.triangle_count, kMarkBlock, s.mesh_mark_blocks), dim3(kMarkBlock), 0,
-                 stream, r->d, a, m);
-  }
-  { LaunchScope scope(stream, KID_MESH_RENDER_TRI); LaunchKernel(k_mesh_render_tri, grid(m.triangle_count, kTriBlock, s.mesh_tri_blocks), dim3(kTriBlock), 0, stream, r->d, a, m); }
-  { LaunchScope scope(stream, KID_MESH_RENDER_LARGE); LaunchKernel(k_mesh_render_large, dim3(s.mesh_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a, m); }
-  if (disks) {
-    { LaunchScope scope(stream, KID_MESH_RENDER_SPLAT); LaunchKernel(k_mesh_render_splat, dim3(s.mesh_splat_blocks), dim3(kSplatBlock), 0, stream, r->d, a, m); }
-    { LaunchScope scope(stream, KID_MESH_RENDER_SPLAT_LARGE); LaunchKernel(k_mesh_render_splat_large, dim3(s.mesh_splat_large_blocks), dim3(kLargeBlock), 0, stream, r->d, a); }
-  }
-  const dim3 resolve_grid((p.width + kResolveBlock - 1) / kResolveBlock, p.height < 65535 ? p.height : 65535);
-  { LaunchScope scope(stream, KID_MESH_RENDER_RESOLVE); LaunchKernel(k_mesh_render_resolve, resolve_grid, dim3(kResolveBlock), 0, stream, r->d, a, m); }
-  return CheckLaunch("render mesh");
+  return DrawMesh(r, stream, "sm_render_mesh", p, view_T_global, triangles, triangle_count, flags, nullptr, depth,
+                  depth_pitch, color, color_pitch, normal, normal_pitch, index, index_pitch);
 }
 
 void FreeRenderBuffers(sm_reconstruction* r) {
@@ -665,6 +768,19 @@ int sm_render_mesh(sm_reconstruction* r, void* stream, const sm_render_params* p
   if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_mesh: null argument");
   return RenderMesh(r, static_cast<cudaStream_t>(stream), *p, view_T_global, triangles, triangle_count, flags, depth,
                     depth_pitch, color, color_pitch, normal, normal_pitch, index, index_pitch);
+}
+
+int sm_render_mesh_textured(sm_reconstruction* r, void* stream, const sm_render_params* p,
+                            const float view_T_global[12], const uint32_t* triangles, uint64_t triangle_count,
+                            int32_t flags, const float* uv, const uint8_t* atlas, size_t atlas_pitch,
+                            int32_t atlas_width, int32_t atlas_height, float* depth, size_t depth_pitch,
+                            uint8_t* color, size_t color_pitch, float* normal, size_t normal_pitch, uint32_t* index,
+                            size_t index_pitch) {
+  if (!r || !p || !view_T_global) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_render_mesh_textured: null argument");
+  const MeshTexture texture{uv, atlas, atlas_pitch, atlas_width, atlas_height};
+  return DrawMesh(r, static_cast<cudaStream_t>(stream), "sm_render_mesh_textured", *p, view_T_global, triangles,
+                  triangle_count, flags, &texture, depth, depth_pitch, color, color_pitch, normal, normal_pitch, index,
+                  index_pitch);
 }
 
 }  // extern "C"

@@ -136,6 +136,18 @@ struct sm_reconstruction {
 };
 
 namespace smb {
+// Whether the bytes [a, a + a_bytes) and [b, b + b_bytes) overlap. An end past the top of the address space is taken
+// as the top, so a range of any length from the caller compares correctly.
+inline bool Overlap(const void* a, u64 a_bytes, const void* b, u64 b_bytes) {
+  const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+  const uintptr_t a1 = a_bytes > UINTPTR_MAX - a0 ? UINTPTR_MAX : a0 + a_bytes;
+  const uintptr_t b1 = b_bytes > UINTPTR_MAX - b0 ? UINTPTR_MAX : b0 + b_bytes;
+  return a0 < b1 && b0 < a1;
+}
+
+// Bytes of `count` items of `size` bytes, saturated like the end of an address range.
+inline u64 Bytes(u64 count, u64 size) { return count > UINT64_MAX / size ? UINT64_MAX : count * size; }
+
 // api.cu
 // Calls that would change what an open session builds on (sm_session_begin, include/surfel_b200.h).
 int RejectInSession(const char* call);

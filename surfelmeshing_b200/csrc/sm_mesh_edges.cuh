@@ -146,18 +146,6 @@ inline const char* TriangleListError(const uint32_t* triangles, u64 count, const
   return nullptr;
 }
 
-// Whether the bytes [a, a + a_bytes) and [b, b + b_bytes) overlap. An end past the top of the address space is taken
-// as the top, so a range of any length from the caller compares correctly.
-inline bool Overlap(const void* a, u64 a_bytes, const void* b, u64 b_bytes) {
-  const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
-  const uintptr_t a1 = a_bytes > UINTPTR_MAX - a0 ? UINTPTR_MAX : a0 + a_bytes;
-  const uintptr_t b1 = b_bytes > UINTPTR_MAX - b0 ? UINTPTR_MAX : b0 + b_bytes;
-  return a0 < b1 && b0 < a1;
-}
-
-// Bytes of `count` items of `size` bytes, saturated like the end of an address range.
-inline u64 Bytes(u64 count, u64 size) { return count > UINT64_MAX / size ? UINT64_MAX : count * size; }
-
 // The SM_ERR_CAPACITY of `who` when an output list of `capacity` triangles cannot take `count`.
 inline int TriangleCapacityError(const char* who, u64 count, u64 capacity) {
   return SetError(SM_ERR_CAPACITY, (std::string(who) + ": " + std::to_string(count) +

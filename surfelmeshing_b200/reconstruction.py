@@ -83,6 +83,23 @@ def _check_triangles(triangles) -> None:
         raise ValueError("triangles must be an int32 CUDA tensor [T, 3]")
 
 
+def _check_texture(texture, count: int):
+    """The (atlas, uv) pair of a textured render_mesh(): atlas uint8 CUDA [H, W, 3] with packed rows, uv float32 CUDA
+    [T, 3, 2] for a list of `count` triangles. Returns (atlas, contiguous uv)."""
+    if not (isinstance(texture, (tuple, list)) and len(texture) == 2):
+        raise ValueError("texture must be the (atlas, uv) pair that texture_mesh() returns")
+    atlas, uv = texture
+    if not (isinstance(atlas, torch.Tensor) and atlas.is_cuda and atlas.dtype == torch.uint8 and atlas.dim() == 3
+            and atlas.shape[2] == 3 and atlas.stride(2) == 1 and atlas.stride(1) == 3):
+        raise ValueError("the atlas must be a uint8 CUDA tensor [H, W, 3] with packed rows")
+    if not (isinstance(uv, torch.Tensor) and uv.is_cuda and uv.dtype == torch.float32 and uv.dim() == 3
+            and tuple(uv.shape[1:]) == (3, 2)):
+        raise ValueError("uv must be a float32 CUDA tensor [T, 3, 2]")
+    if uv.shape[0] != count:
+        raise ValueError(f"uv has {uv.shape[0]} triangles, the list {count}")
+    return atlas, uv.contiguous()
+
+
 def _mat12(m) -> np.ndarray:
     a = np.ascontiguousarray(np.asarray(m, dtype=np.float32).reshape(-1)[:12])
     assert a.size == 12
@@ -408,11 +425,15 @@ class CUDASurfelReconstruction:
 
     def render_mesh(self, triangles, view_T_global, width: int, height: int, fx: float, fy: float, cx: float,
                     cy: float, near: float = 0.1, far: float = 100.0, unmeshed_surfels: bool = True, stream=None,
-                    outputs=RENDER_OUTPUTS) -> dict:
+                    outputs=RENDER_OUTPUTS, texture=None) -> dict:
         """sm_render_mesh: a triangle list over the current cloud (the int32 CUDA tensor [T, 3] of slot indices that
         triangulate() and mesh_triangles() return) drawn into a pinhole camera of any size, with perspective-correct
         depth and colour; unmeshed_surfels=True also draws the slots no triangle names as disks, as render() does.
         Triangles naming merged or out-of-range slots, or with a corner outside [near, far], are not drawn.
+
+        texture: the (atlas, uv) pair texture_mesh() returns for `triangles` (atlas uint8 CUDA [H, W, 3] with packed
+        rows, uv float32 CUDA [T, 3, 2]); the triangles are then coloured by bilinear lookups in the atlas at
+        perspective-correct texture coordinates (sm_render_mesh_textured), and "color" must be among the outputs.
 
         Returns the dict of render(): "depth", "color", "normal" (the unit triangle normal facing the camera) and
         "index" (the triangle's row in `triangles`; a disk's slot with bit 31 set, so negative in int32; -1 = empty),
@@ -423,12 +444,18 @@ class CUDASurfelReconstruction:
             raise ValueError(f"outputs must be a non-empty subset of {RENDER_OUTPUTS}, got {outputs}")
         _check_triangles(triangles)
         triangles = triangles.contiguous()
+        count = int(triangles.shape[0])
+        if texture is not None:
+            atlas, uv = _check_texture(texture, count)
+            if "color" not in outputs:
+                raise ValueError("a textured render needs 'color' among the outputs")
         H, W = int(height), int(width)
         shapes = {"depth": ((H, W), torch.float32), "color": ((H, W, 3), torch.uint8),
                   "normal": ((H, W, 3), torch.float32), "index": ((H, W), torch.int32)}
         out = {k: torch.empty(shapes[k][0], dtype=shapes[k][1], device="cuda") for k in outputs}
         if isinstance(stream, torch.cuda.Stream):
-            for t in (*out.values(), triangles):
+            used = (*out.values(), triangles) if texture is None else (*out.values(), triangles, atlas, uv)
+            for t in used:
                 t.record_stream(stream)   # allocated on the current stream, used on `stream`
         args = []
         for k in RENDER_OUTPUTS:
@@ -436,10 +463,15 @@ class CUDASurfelReconstruction:
             args += [C.c_void_p(t.data_ptr()), t.stride(0) * t.element_size()] if t is not None else [None, 0]
         p = RenderParams(W, H, float(fx), float(fy), float(cx), float(cy), float(near), float(far))
         T = _mat12(view_T_global)
-        count = int(triangles.shape[0])
-        self.lib.call("render_mesh", self._h, _stream_handle(stream), C.byref(p), T.ctypes.data_as(C.c_void_p),
-                      C.c_void_p(triangles.data_ptr()) if count else None, count,
-                      _lib.RENDER_UNMESHED_SURFELS if unmeshed_surfels else 0, *args)
+        head = (self._h, _stream_handle(stream), C.byref(p), T.ctypes.data_as(C.c_void_p),
+                C.c_void_p(triangles.data_ptr()) if count else None, count,
+                _lib.RENDER_UNMESHED_SURFELS if unmeshed_surfels else 0)
+        if texture is None:
+            self.lib.call("render_mesh", *head, *args)
+        else:
+            self.lib.call("render_mesh_textured", *head, C.c_void_p(uv.data_ptr()) if count else None,
+                          C.c_void_p(atlas.data_ptr()) if atlas.numel() else None, atlas.stride(0),
+                          int(atlas.shape[1]), int(atlas.shape[0]), *args)
         return out
 
     def track(self, depth, guess, params: Optional[TrackParams] = None, pp: Optional[PreprocessParams] = None,

@@ -4,6 +4,7 @@ product first and last and every --lib name=path build in between (a variant is 
 `python -m surfelmeshing_b200.build --out variants/lib_<name>.so -- <nvcc flags>`). Prints frames/s (best and
 median of --reps passes, CUDA events) and the surfel counts; writes probe_out/ab_probe.json."""
 import argparse
+import ctypes as C
 import json
 import sys
 from pathlib import Path
@@ -15,6 +16,19 @@ sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 from surfelmeshing_b200 import _lib, synthetic as S  # noqa: E402
 from surfelmeshing_b200 import reconstruction as R  # noqa: E402
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams  # noqa: E402
+
+
+def load_build(path):
+    """Another build of the product library, bound to the entry points it exports: an older build (the parent
+    commit's) may lack ones added since, and the A/B only calls the ones both have."""
+    lib = _lib.Library.__new__(_lib.Library)
+    lib.path, lib.prefix, lib.cdll, lib.fn = Path(path).resolve(), "sm_", C.CDLL(str(Path(path).resolve()), mode=C.RTLD_LOCAL), {}
+    for name, (restype, argtypes) in {**_lib._SIGNATURES, **_lib._PRODUCT_ONLY}.items():
+        f = getattr(lib.cdll, "sm_" + name, None)
+        if f is not None:
+            f.restype, f.argtypes = restype, argtypes
+            lib.fn[name] = f
+    return lib
 
 
 def main():
@@ -36,7 +50,7 @@ def main():
     arms = [("default", product)]
     for item in args.lib:
         name, path = item.split("=", 1)
-        arms.append((name, _lib.Library(Path(path).resolve(), "sm_", product=True)))
+        arms.append((name, load_build(path)))
     arms.append(("default_again", product))
 
     cam = S.Camera.tum(args.width, args.height)
