@@ -1171,6 +1171,78 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream, const sm_texture_params*
                     float* uv /* device, 6 x count: (u, v) per corner in the listed order, in [0, 1]; may be NULL */,
                     sm_texture_stats* stats);
 
+/* ---- exposure compensation between the texture views (DESIGN.md section 1 row f20, section 5.18) ---------------
+ * Cameras with auto-exposure and auto white balance give the views of one surface different brightness, and X6's
+ * mean then shows patches whose edges follow the set of views. sm_mesh_texture_compensated fits one gain per view
+ * and channel jointly over surface points the views share (Brown & Lowe 2007, gain compensation) and textures with
+ * each view's samples scaled by its gains. Everything of sm_mesh_texture holds (arguments, checks, layout,
+ * capacity protocol, X1-X8, the stats, read-only on the surfel state), with these rules added:
+ *  G1. Sample points. P = min(count, floor(max_samples / view_count)), 0 without views. Point p in [0, P) lies on
+ *      triangle t_p = floor(p * count / P) (u64): its corners in LIST order as (a, b, c) and alpha = beta =
+ *      float(1/3) in X5's form give its position X and normal n (no X2 rotation, no clamp).
+ *  G2. Samples. s_pv (3 channels) is X6's bilinear sample of view v at point p: the same depth raster, visibility,
+ *      angle and footprint tests; the weight w is not used. The sample is absent if X6 rejects the view or any
+ *      channel lies outside [min_level, max_level]. k_p = the present samples of p; p takes part in the fit iff
+ *      k_p >= 2. n_v = the present samples of view v at such points; a view with n_v = 0 keeps gain 1.
+ *  G3. Objective, per channel: E(g) = sum_p sum_(v in p) (g_v s_pv - m_p)^2 / sigma_noise^2 + sum_v n_v (g_v -
+ *      1)^2 / sigma_gain^2, m_p = (1 / k_p) sum_(u in p) g_u s_pu. Its normal equations A g = b are, per view,
+ *      (A x)_v = y_v(x) * cN + (n_v * cG) * x_v and b_v = n_v * cG with cN = 1 / (sigma_noise * sigma_noise),
+ *      cG = 1 / (sigma_gain * sigma_gain) and y_v(x) = sum_p s_pv * (s_pv * x_v - m_p(x)).
+ *  G4. Solve. fp64 from here on (samples and sigmas promoted; each product, sum, quotient and square root rounded
+ *      alone), the three channels independently. m_p(x) = (sum over views in order of s_pv * x_v, from 0) / k_p.
+ *      A column sum over points (y_v, and the data terms of G6) is a 32-ary tree: TREE(t_0 .. t_31) = t_0 after
+ *      t_i = t_i + t_(i + off) for i < off, off = 16, 8, 4, 2, 1; level 1 is TREE of each 32 consecutive points
+ *      (term 0 for a point past P, not in the fit or without a sample of v), level 2 the TREE of each 32
+ *      consecutive level-1 sums (a block of 1024 points, 0 past the last); then, while more than one value is
+ *      left, the TREE of each 32 consecutive values (0 past the last) replaces them. A sum over views (dot
+ *      products) is TREE of the 32 TREEs of views 32w .. 32w + 31 (0 past view_count). Conjugate gradients from
+ *      x = 1: r = b - A x, d = r, rr = r . r; each of `iterations` steps of a channel whose rr != 0: pAp = d . A d;
+ *      if !(pAp > 0) the channel stops; else alpha = rr / pAp, x = x + alpha * d, r = r - alpha * (A d), rr' =
+ *      r . r, beta = rr' / rr, d = r + beta * d, rr = rr'. The prior alone fixes the common scale only loosely
+ *      (views that disagree for other reasons than exposure pull every gain down), so a view with n_v > 0 gets
+ *      g = float(x / xbar) (every other view 1), xbar = (sum over views of n_v * x_v) / (sum over views of n_v) (two sums over views; xbar
+ *      = 1 when the second is 0 or the quotient is not > 0): their n_v-weighted mean is 1 per channel.
+ *  G5. Application. X6 with each channel's sample replaced by float(g_v,ch * sample_ch) before the product with w;
+ *      X7 unchanged (the corner blend is not compensated). With iterations = 0 every gain is 1 and the atlas equals
+ *      sm_mesh_texture's.
+ *  G6. Stats: points = P, samples = sum of n_v, views_fitted = the views with n_v > 0; rms_before and rms_after =
+ *      sqrt(D / (3 samples)) (0 without samples) at x = 1 and at x = the float gains, where D = (D_r + D_g) + D_b
+ *      and D_ch = the sum over views of the G4 column sums of (s_pv * x_v - m_p(x))^2.
+ * gains (HOST, 3 x view_count floats: r, g, b per view; may be NULL) and gain_stats are written only by a call that
+ * fills the atlas (with count 0: every gain 1 and gain_stats zero); every other return leaves gains untouched and
+ * gain_stats zero, and a layout query or SM_ERR_CAPACITY sets stats as sm_mesh_texture does. SM_ERR_INVALID_ARGUMENT
+ * also for gp or gain_stats NULL, max_samples or iterations negative, sigma_noise or sigma_gain not finite and > 0,
+ * min_level or max_level not finite, or min_level > max_level. The call renders every view twice (once to sample,
+ * once to accumulate), adds one synchronisation (the gain read-back) and launches a number of kernels that depends
+ * only on view_count, iterations and whether P > 0. Memory, on top of sm_mesh_texture's: 12 bytes per sample
+ * (P x view_count, the sample matrix), 28 bytes per point (k_p and m_p), 24 bytes per view per 1024 points (the
+ * level-2 column sums) and a fixed 88 KB of solver state. */
+typedef struct sm_texture_gain_params {
+  int32_t max_samples;     /* P x view_count entries of the sample matrix; 1 << 23 (96 MB at 12 bytes) */
+  int32_t iterations;      /* conjugate-gradient steps; 0 = every gain 1; 32 */
+  float sigma_noise;       /* grey levels; 10 (Brown & Lowe) */
+  float sigma_gain;        /* the prior that fixes the common scale; 1 (Brown & Lowe's 0.1 undoes most of the
+                              correction along a chain of views, 3 lets noisy views shrink the common scale:
+                              DESIGN.md section 5.18) */
+  float min_level, max_level;   /* 5, 250: a sample with any channel outside takes no part in the fit */
+} sm_texture_gain_params;
+typedef struct sm_texture_gain_stats {
+  uint64_t points;         /* sample points P */
+  uint64_t samples;        /* (point, view) samples in the fit */
+  uint64_t views_fitted;   /* views with at least one such sample; every other view keeps gain 1 */
+  double rms_before, rms_after;   /* grey levels, at gain 1 and at the fitted gains */
+} sm_texture_gain_stats;
+/* Host only, no device needed. */
+void sm_default_texture_gain_params(sm_texture_gain_params* p);
+int sm_mesh_texture_compensated(sm_reconstruction* r, void* stream, const sm_texture_params* p,
+                                const sm_texture_gain_params* gp,
+                                const uint32_t* triangles /* device, 3 x count */, uint64_t count,
+                                const sm_texture_view* views /* host array */, int32_t view_count,
+                                uint8_t* atlas, size_t atlas_pitch, int32_t atlas_capacity_width,
+                                int32_t atlas_capacity_height, float* uv,
+                                float* gains /* HOST, 3 x view_count; may be NULL */,
+                                sm_texture_stats* stats, sm_texture_gain_stats* gain_stats);
+
 /* ---- connected pieces of a triangle mesh (DESIGN.md section 1 row f18, section 5.16) ----------------------------
  * The surfel mesher leaves small floating pieces behind: a pair of surfels at a depth edge, or a few surfels the
  * normal gate cut off from their neighbours. sm_mesh_components splits a caller's triangle list into its connected

@@ -217,6 +217,30 @@ class CUDASurfelReconstruction {
     return stats;
   }
 
+  // Extension: TextureMesh with one gain per view and channel fitted over the surface the views share, so that
+  // views of different exposure and white balance give one even atlas (sm_mesh_texture_compensated). `gains` (host,
+  // 3 x view_count, may be null) receives the fitted gains and `gain_stats` (may be null) the fit's statistics.
+  sm_texture_stats TextureMeshCompensated(cudaStream_t stream, const u32* triangles, uint64_t count,
+                                          const sm_texture_view* views, int view_count, u8* atlas, size_t atlas_pitch,
+                                          int capacity_width, int capacity_height, float* uv, float* gains = nullptr,
+                                          sm_texture_gain_stats* gain_stats = nullptr,
+                                          const sm_texture_params* params = nullptr,
+                                          const sm_texture_gain_params* gain_params = nullptr) {
+    sm_texture_params defaults;
+    sm_default_texture_params(&defaults);
+    sm_texture_gain_params gain_defaults;
+    sm_default_texture_gain_params(&gain_defaults);
+    sm_texture_stats stats;
+    sm_texture_gain_stats fit;
+    const int status = sm_mesh_texture_compensated(handle_, stream, params ? params : &defaults,
+                                                   gain_params ? gain_params : &gain_defaults, triangles, count, views,
+                                                   view_count, atlas, atlas_pitch, capacity_width, capacity_height, uv,
+                                                   gains, &stats, &fit);
+    if (!(status == SM_ERR_CAPACITY && atlas == nullptr)) Check(status);
+    if (gain_stats) *gain_stats = fit;
+    return stats;
+  }
+
  private:
   static void ToRowMajor(const SE3f& t, float* out) {
     const auto m = t.matrix3x4();

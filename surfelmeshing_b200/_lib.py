@@ -301,6 +301,28 @@ class TextureViewDesc(C.Structure):
                 ("color_pitch", C.c_size_t)]
 
 
+class TextureGainParams(C.Structure):
+    """sm_texture_gain_params: the most samples (points x views) of the gain fit, the conjugate-gradient steps
+    (0: every gain 1), the noise and gain sigmas of the objective, and the levels outside which a sample takes no
+    part in the fit."""
+    _fields_ = [("max_samples", C.c_int32), ("iterations", C.c_int32), ("sigma_noise", C.c_float),
+                ("sigma_gain", C.c_float), ("min_level", C.c_float), ("max_level", C.c_float)]
+
+    @classmethod
+    def defaults(cls, **overrides) -> "TextureGainParams":
+        p = cls(1 << 23, 32, 10.0, 1.0, 5.0, 250.0)
+        for k, v in overrides.items():
+            setattr(p, k, v)
+        return p
+
+
+class TextureGainStats(C.Structure):
+    """sm_texture_gain_stats: the sample points, the (point, view) samples in the fit, the views fitted, and the rms
+    residual in grey levels at gain 1 and at the fitted gains."""
+    _fields_ = [("points", C.c_uint64), ("samples", C.c_uint64), ("views_fitted", C.c_uint64),
+                ("rms_before", C.c_double), ("rms_after", C.c_double)]
+
+
 class ComponentParams(C.Structure):
     """sm_component_params: the fewest triangles and the least area (m^2) of a kept piece, and how many of the
     largest pieces may be kept (0: no limit)."""
@@ -441,6 +463,10 @@ _PRODUCT_ONLY = {
     "default_texture_params": (None, [C.POINTER(TextureParams)]),
     "mesh_texture": (C.c_int, [_P, _P, C.POINTER(TextureParams), _P, C.c_uint64, C.POINTER(TextureViewDesc), _I, _P,
                                _SZ, _I, _I, _P, C.POINTER(TextureStats)]),
+    "default_texture_gain_params": (None, [C.POINTER(TextureGainParams)]),
+    "mesh_texture_compensated": (C.c_int, [_P, _P, C.POINTER(TextureParams), C.POINTER(TextureGainParams), _P,
+                                           C.c_uint64, C.POINTER(TextureViewDesc), _I, _P, _SZ, _I, _I, _P, _P,
+                                           C.POINTER(TextureStats), C.POINTER(TextureGainStats)]),
     "default_component_params": (None, [C.POINTER(ComponentParams)]),
     "mesh_components": (C.c_int, [_P, _P, C.POINTER(ComponentParams), _P, C.c_uint64, _P, C.c_uint64, _P, _P,
                                   C.c_uint64, C.POINTER(ComponentStats)]),

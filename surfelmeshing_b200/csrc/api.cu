@@ -138,6 +138,7 @@ const char* KernelName(int id) {
       "k_compact_store", "k_compact_mesh", "k_simplify_edges", "k_simplify_fans", "k_simplify_sort",
       "k_simplify_quadrics", "k_simplify_candidates", "k_simplify_select", "k_simplify_apply", "k_simplify_scan",
       "k_simplify_write", "k_tex_classes", "k_tex_sort", "k_tex_place", "k_tex_uv", "k_tex_accumulate", "k_tex_resolve",
+      "k_tex_gain_sample", "k_tex_gain_count", "k_tex_gain_points", "k_tex_gain_views", "k_tex_gain_step",
       "k_cc_edges", "k_cc_hook", "k_cc_number", "k_cc_scan", "k_cc_sums", "k_cc_rank", "k_cc_write"};
   return (id >= 0 && id < KID_COUNT) ? names[id] : "?";
 }

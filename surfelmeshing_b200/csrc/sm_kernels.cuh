@@ -51,6 +51,7 @@ enum KernelId {
   KID_SIMPLIFY_EDGES, KID_SIMPLIFY_FANS, KID_SIMPLIFY_SORT, KID_SIMPLIFY_QUADRICS, KID_SIMPLIFY_CANDIDATES,
   KID_SIMPLIFY_SELECT, KID_SIMPLIFY_APPLY, KID_SIMPLIFY_SCAN, KID_SIMPLIFY_WRITE,
   KID_TEXTURE_CLASSES, KID_TEXTURE_SORT, KID_TEXTURE_PLACE, KID_TEXTURE_UV, KID_TEXTURE_ACCUMULATE, KID_TEXTURE_RESOLVE,
+  KID_TEXTURE_GAIN_SAMPLE, KID_TEXTURE_GAIN_COUNT, KID_TEXTURE_GAIN_POINTS, KID_TEXTURE_GAIN_VIEWS, KID_TEXTURE_GAIN_STEP,
   KID_COMPONENTS_EDGES, KID_COMPONENTS_HOOK, KID_COMPONENTS_NUMBER, KID_COMPONENTS_SCAN, KID_COMPONENTS_SUMS,
   KID_COMPONENTS_RANK, KID_COMPONENTS_WRITE,
   KID_COUNT

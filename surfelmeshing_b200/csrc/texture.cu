@@ -17,6 +17,19 @@
 //   (synchronisation: the end).
 // A texel code m is the Morton code of an atlas texel below the total area: the squares are aligned blocks of codes,
 // so m names its class, its square and its texel (i, j) in it without a search, and the accumulators are indexed by m.
+//
+// sm_mesh_texture_compensated (DESIGN.md section 5.18, rules G1-G6) adds, after k_tex_uv and before the views'
+// accumulation (whose k_tex_accumulate<true> scales each sample by the view's gains):
+//   per view: sm_render_mesh's depth pass, then k_tex_gain_sample (one thread per sample point: G1-G2 into the
+//     view's column of the [V][P] sample matrix);
+//   k_tex_gain_count     one thread per point: k_p, n_v (warp-aggregated), and the solver state set to x = d = 1;
+//   the data term at x = 1 and r = b - A 1, then per conjugate-gradient step three launches:
+//     k_tex_gain_points  one thread per point: m_p of the step's vector;
+//     k_tex_gain_views   one 1024-thread block per (1024 points, view): levels 1-2 of G4's column sums;
+//     k_tex_gain_step    one 1024-thread block, a thread per view: the rest of the column sums, then the step;
+//   then the float gains and the data term at them;
+//   (synchronisation: the gain read-back after the end's).
+// The launch count depends on view_count and iterations only; the gains never leave the device until the end.
 
 #include <cub/device/device_radix_sort.cuh>
 
@@ -60,6 +73,17 @@ struct TextureCounters {
   u32 view_used[SM_TEXTURE_MAX_VIEWS];
 };
 
+// The gain fit of sm_mesh_texture_compensated: what the host reads back first, then the solver's device state.
+struct GainState {
+  float gains[SM_TEXTURE_MAX_VIEWS][3];
+  u32 view_samples[SM_TEXTURE_MAX_VIEWS];   // n_v
+  double data[2];                           // D at x = 1 and at the float gains
+  // (device only from here)
+  double x[SM_TEXTURE_MAX_VIEWS][3], r[SM_TEXTURE_MAX_VIEWS][3], d[SM_TEXTURE_MAX_VIEWS][3];
+  double rr[3];
+  u32 done[3];
+};
+
 // The scratch of sm_mesh_texture: per triangle, per texel code and per pixel of the largest view.
 struct TextureScratch {
   CounterMirror<TextureCounters> counters;
@@ -72,6 +96,15 @@ struct TextureScratch {
   float4* accum = nullptr;        // by texel code: sum of w * (r, g, b), sum of w
   size_t pixel_capacity = 0;
   float* depth = nullptr;         // one view's sm_render_mesh depth
+  // sm_mesh_texture_compensated only (G1-G6)
+  CounterMirror<GainState> gain;
+  u64 sample_capacity = 0;
+  float* samples = nullptr;       // [V][P] x (r, g, b), NaN when absent
+  u64 point_capacity = 0;
+  u32* fit_count = nullptr;       // per point: k_p, 0 when not in the fit
+  double* mean = nullptr;         // per point: m_p per channel
+  u64 block_capacity = 0;
+  double* block_sums = nullptr;   // [V][ceil(P / 1024)] x 3: the level-2 column sums
 };
 
 namespace {
@@ -248,6 +281,23 @@ struct TexelPoint {
   bool has_normal;
 };
 
+// X5's position and normal at (alpha, beta) of the triangle p->corner (a, b, c).
+__device__ __forceinline__ void point_on(const TextureArgs& a, float alpha, float beta, TexelPoint* p) {
+  p->alpha = alpha;
+  p->beta = beta;
+  const float3 pa = position(a, p->corner[0]), pb = position(a, p->corner[1]), pc = position(a, p->corner[2]);
+  const float3 e1 = sub3(pb, pa), e2 = sub3(pc, pa);
+  p->X = make_float3(fadd(fadd(pa.x, fmul(alpha, e1.x)), fmul(beta, e2.x)),
+                     fadd(fadd(pa.y, fmul(alpha, e1.y)), fmul(beta, e2.y)),
+                     fadd(fadd(pa.z, fmul(alpha, e1.z)), fmul(beta, e2.z)));
+  const float3 g = make_float3(fsub(fmul(e1.y, e2.z), fmul(e1.z, e2.y)), fsub(fmul(e1.z, e2.x), fmul(e1.x, e2.z)),
+                               fsub(fmul(e1.x, e2.y), fmul(e1.y, e2.x)));
+  const float gg = dot3p(g, g);
+  p->has_normal = gg > 0.f && isfinite(gg);
+  const float inv = p->has_normal ? __fdiv_rn(1.f, __fsqrt_rn(gg)) : 0.f;
+  p->n = make_float3(fmul(g.x, inv), fmul(g.y, inv), fmul(g.z, inv));
+}
+
 // X5 for texel (i, j) of the tile `rec`.
 __device__ __forceinline__ void texel_point(const TextureArgs& a, uint4 rec, u32 i, u32 j, TexelPoint* p) {
   const u32 s = rec.w & 0xFFFFu, half = (rec.w >> 16) & 1u;
@@ -270,19 +320,7 @@ __device__ __forceinline__ void texel_point(const TextureArgs& a, uint4 rec, u32
     alpha = __fdiv_rn(alpha, sum);
     beta = fsub(1.f, alpha);
   }
-  p->alpha = alpha;
-  p->beta = beta;
-  const float3 pa = position(a, p->corner[0]), pb = position(a, p->corner[1]), pc = position(a, p->corner[2]);
-  const float3 e1 = sub3(pb, pa), e2 = sub3(pc, pa);
-  p->X = make_float3(fadd(fadd(pa.x, fmul(alpha, e1.x)), fmul(beta, e2.x)),
-                     fadd(fadd(pa.y, fmul(alpha, e1.y)), fmul(beta, e2.y)),
-                     fadd(fadd(pa.z, fmul(alpha, e1.z)), fmul(beta, e2.z)));
-  const float3 g = make_float3(fsub(fmul(e1.y, e2.z), fmul(e1.z, e2.y)), fsub(fmul(e1.z, e2.x), fmul(e1.x, e2.z)),
-                               fsub(fmul(e1.x, e2.y), fmul(e1.y, e2.x)));
-  const float gg = dot3p(g, g);
-  p->has_normal = gg > 0.f && isfinite(gg);
-  const float inv = p->has_normal ? __fdiv_rn(1.f, __fsqrt_rn(gg)) : 0.f;
-  p->n = make_float3(fmul(g.x, inv), fmul(g.y, inv), fmul(g.z, inv));
+  point_on(a, alpha, beta, p);
 }
 
 // X6: one view's weight and colour sample at the texel point; false if the view does not contribute.
@@ -313,7 +351,9 @@ __device__ __forceinline__ bool view_sample(const TextureView& v, const TexelPoi
   return true;
 }
 
-__global__ void __launch_bounds__(kBlock) k_tex_accumulate(TextureArgs a, TextureView v) {
+// X6 into the accumulators; with kGain each sample channel is first scaled by the view's gain (G5).
+template <bool kGain>
+__global__ void __launch_bounds__(kBlock) k_tex_accumulate(TextureArgs a, TextureView v, const float* gain) {
   const TextureLayout& l = a.counters->layout;
   bool any = false;
   for (u32 m = blockIdx.x * blockDim.x + threadIdx.x; m < a.area; m += gridDim.x * blockDim.x) {
@@ -324,6 +364,9 @@ __global__ void __launch_bounds__(kBlock) k_tex_accumulate(TextureArgs a, Textur
     texel_point(a, rec, i, j, &p);
     float w, rgb[3];
     if (!view_sample(v, p, &w, rgb)) continue;
+    if constexpr (kGain) {
+      for (int ch = 0; ch < 3; ++ch) rgb[ch] = fmul(gain[ch], rgb[ch]);
+    }
     float4 s = a.accum[m];
     s.x = fadd(s.x, fmul(w, rgb[0]));
     s.y = fadd(s.y, fmul(w, rgb[1]));
@@ -378,6 +421,246 @@ __global__ void __launch_bounds__(kBlock) k_tex_resolve(TextureArgs a) {
   }
 }
 
+// ---- the gain fit of sm_mesh_texture_compensated (G1-G6) ----------------------------------------------------------
+
+constexpr int kGainBlock = 1024;   // points per level-2 column sum; also the views of one k_tex_gain_step block
+static_assert(SM_TEXTURE_MAX_VIEWS <= kGainBlock, "k_tex_gain_step holds one view per thread");
+
+struct GainArgs {
+  float* samples;          // [V][P] x 3
+  u32* fit_count;          // [P]
+  double* mean;            // [P] x 3
+  double* block_sums;      // [V][blocks] x 3
+  GainState* state;
+  u32 points, views, blocks;
+  float min_level, max_level;
+  double cN, cG;           // 1 / sigma_noise^2, 1 / sigma_gain^2
+};
+
+__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double dsub(double a, double b) { return __dadd_rn(a, -b); }
+
+// TREE of G4 over the 32 lanes: the result in lane 0.
+__device__ __forceinline__ double warp_tree(double t) {
+  for (int off = 16; off > 0; off >>= 1) t = dadd(t, __shfl_down_sync(0xffffffffu, t, off));
+  return t;
+}
+
+// G1 and G2: one thread per point writes view `view`'s column of the sample matrix.
+__global__ void __launch_bounds__(kBlock) k_tex_gain_sample(TextureArgs a, TextureView v, GainArgs g, u32 view) {
+  const float third = 1.f / 3.f;
+  for (u32 p = blockIdx.x * blockDim.x + threadIdx.x; p < g.points; p += gridDim.x * blockDim.x) {
+    const u64 t = static_cast<u64>(p) * a.count / g.points;
+    TexelPoint pt;
+    for (int k = 0; k < 3; ++k) pt.corner[k] = a.tri[3 * t + k];
+    point_on(a, third, third, &pt);
+    float w, rgb[3];
+    bool present = view_sample(v, pt, &w, rgb);
+    for (int ch = 0; ch < 3; ++ch) present = present && rgb[ch] >= g.min_level && rgb[ch] <= g.max_level;
+    float* out = g.samples + 3 * (static_cast<size_t>(view) * g.points + p);
+    for (int ch = 0; ch < 3; ++ch) out[ch] = present ? rgb[ch] : __int_as_float(0x7fc00000);
+  }
+}
+
+// k_p per point (0 below two samples) and n_v per view; block 0 also sets x = d = 1 and clears the solver state.
+__global__ void __launch_bounds__(kBlock) k_tex_gain_count(GainArgs g) {
+  GainState* s = g.state;
+  if (blockIdx.x == 0) {
+    for (u32 i = threadIdx.x; i < 3 * SM_TEXTURE_MAX_VIEWS; i += blockDim.x) {
+      (&s->x[0][0])[i] = 1.0;
+      (&s->d[0][0])[i] = 1.0;
+      (&s->r[0][0])[i] = 0.0;
+    }
+    if (threadIdx.x < 3) { s->rr[threadIdx.x] = 0.0; s->done[threadIdx.x] = 0; }
+  }
+  const u32 lane = threadIdx.x & 31;
+  for (u32 base = blockIdx.x * blockDim.x; base < g.points; base += gridDim.x * blockDim.x) {
+    const u32 p = base + threadIdx.x;
+    const bool in = p < g.points;
+    u32 k = 0;
+    for (u32 v = 0; in && v < g.views; ++v) k += isnan(g.samples[3 * (static_cast<size_t>(v) * g.points + p)]) ? 0 : 1;
+    const bool fit = k >= 2;
+    if (in) g.fit_count[p] = fit ? k : 0;
+    if (!__any_sync(0xffffffffu, fit)) continue;
+    for (u32 v = 0; v < g.views; ++v) {
+      const bool here = fit && !isnan(g.samples[3 * (static_cast<size_t>(v) * g.points + p)]);
+      const u32 n = __popc(__ballot_sync(0xffffffffu, here));
+      if (lane == 0 && n) atomicAdd(&s->view_samples[v], n);
+    }
+  }
+}
+
+// G4's point sweep: m_p of the vector `x` (x or d of the state) for every point in the fit.
+__global__ void __launch_bounds__(kBlock) k_tex_gain_points(GainArgs g, const double* x) {
+  for (u32 p = blockIdx.x * blockDim.x + threadIdx.x; p < g.points; p += gridDim.x * blockDim.x) {
+    const u32 k = g.fit_count[p];
+    if (k == 0) continue;
+    double sum[3] = {0.0, 0.0, 0.0};
+    for (u32 v = 0; v < g.views; ++v) {
+      const float* sp = g.samples + 3 * (static_cast<size_t>(v) * g.points + p);
+      const float s0 = sp[0];
+      if (isnan(s0)) continue;
+      const float sv[3] = {s0, sp[1], sp[2]};
+      for (int ch = 0; ch < 3; ++ch) sum[ch] = dadd(sum[ch], dmul(static_cast<double>(sv[ch]), x[3 * v + ch]));
+    }
+    for (int ch = 0; ch < 3; ++ch) g.mean[3 * static_cast<size_t>(p) + ch] = __ddiv_rn(sum[ch], static_cast<double>(k));
+  }
+}
+
+// G4's view sweep, levels 1 and 2: block (b, v) sums points [1024 b, 1024 b + 1024) of view v's column, of
+// s (s x_v - m_p) (the product A x) or, with kSquares, of (s x_v - m_p)^2 (the data term of G6).
+template <bool kSquares>
+__global__ void __launch_bounds__(kGainBlock) k_tex_gain_views(GainArgs g, const double* x) {
+  __shared__ double warp_sums[32][3];
+  const u32 v = blockIdx.y, p = blockIdx.x * kGainBlock + threadIdx.x;
+  double t[3] = {0.0, 0.0, 0.0};
+  if (p < g.points && g.fit_count[p] != 0) {
+    const float* sp = g.samples + 3 * (static_cast<size_t>(v) * g.points + p);
+    const float s0 = sp[0];
+    if (!isnan(s0)) {
+      const float sv[3] = {s0, sp[1], sp[2]};
+      for (int ch = 0; ch < 3; ++ch) {
+        const double s = sv[ch];
+        const double e = dsub(dmul(s, x[3 * v + ch]), g.mean[3 * static_cast<size_t>(p) + ch]);
+        t[ch] = kSquares ? dmul(e, e) : dmul(s, e);
+      }
+    }
+  }
+  const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int ch = 0; ch < 3; ++ch) t[ch] = warp_tree(t[ch]);
+  if (lane == 0) for (int ch = 0; ch < 3; ++ch) warp_sums[warp][ch] = t[ch];
+  __syncthreads();
+  if (warp == 0) {
+    for (int ch = 0; ch < 3; ++ch) {
+      const double b = warp_tree(warp_sums[lane][ch]);
+      if (lane == 0) g.block_sums[3 * (static_cast<size_t>(v) * g.blocks + blockIdx.x) + ch] = b;
+    }
+  }
+}
+
+// The sum over views of G4 (0 past view_count) for the three channels, in every thread of the block.
+__device__ __forceinline__ void views_tree(double t[3], double (*warp_sums)[3], double out[3]) {
+  const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int ch = 0; ch < 3; ++ch) t[ch] = warp_tree(t[ch]);
+  __syncthreads();   // (warp_sums may still be read from the previous call)
+  if (lane == 0) for (int ch = 0; ch < 3; ++ch) warp_sums[warp][ch] = t[ch];
+  __syncthreads();
+  if (warp == 0)
+    for (int ch = 0; ch < 3; ++ch) {
+      const double s = warp_tree(warp_sums[lane][ch]);
+      if (lane == 0) warp_sums[32][ch] = s;
+    }
+  __syncthreads();
+  for (int ch = 0; ch < 3; ++ch) out[ch] = warp_sums[32][ch];
+}
+
+enum GainStep : int { kStepData0 = 0, kStepData1 = 1, kStepInit, kStepIterate, kStepFinish };
+
+// One block of kGainBlock threads, thread v = view v: the rest of the column sums (levels 3 and up, one warp per
+// view), then by `mode`: the data term D (into data[mode]), r = b - A x with d = r, one CG step, or the float gains
+// with d = the gains (for the data term at the fitted gains).
+__global__ void __launch_bounds__(kGainBlock) k_tex_gain_step(GainArgs g, int mode) {
+  __shared__ double column[SM_TEXTURE_MAX_VIEWS][3];
+  __shared__ double warp_sums[33][3];
+  GainState* s = g.state;
+  const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5, v = threadIdx.x;
+  if (mode != kStepFinish) {
+    for (u32 view = warp; view < g.views; view += kGainBlock / 32) {
+      double* b = g.block_sums + 3 * static_cast<size_t>(view) * g.blocks;
+      for (u32 n = g.blocks; n > 1; n = (n + 31) / 32) {
+        for (u32 group = 0; 32 * group < n; ++group) {
+          const u32 i = 32 * group + lane;
+          for (int ch = 0; ch < 3; ++ch) {
+            const double t = warp_tree(i < n ? b[3 * i + ch] : 0.0);
+            __syncwarp();
+            if (lane == 0) b[3 * group + ch] = t;
+            __syncwarp();
+          }
+        }
+      }
+      if (lane == 0) for (int ch = 0; ch < 3; ++ch) column[view][ch] = b[ch];
+    }
+    __syncthreads();
+  }
+  const bool is_view = v < g.views;
+  if (mode == kStepData0 || mode == kStepData1) {
+    double t[3], D[3];
+    for (int ch = 0; ch < 3; ++ch) t[ch] = is_view ? column[v][ch] : 0.0;
+    views_tree(t, warp_sums, D);
+    if (threadIdx.x == 0) s->data[mode] = dadd(dadd(D[0], D[1]), D[2]);
+    return;
+  }
+  if (mode == kStepFinish) {   // the common scale: x over its n_v-weighted mean
+    const double n = is_view ? static_cast<double>(s->view_samples[v]) : 0.0;
+    double t[3], weighted[3], total[3];
+    for (int ch = 0; ch < 3; ++ch) t[ch] = is_view ? dmul(n, s->x[v][ch]) : 0.0;
+    views_tree(t, warp_sums, weighted);
+    for (int ch = 0; ch < 3; ++ch) t[ch] = n;
+    views_tree(t, warp_sums, total);
+    if (is_view)
+      for (int ch = 0; ch < 3; ++ch) {
+        double mean = total[ch] > 0.0 ? __ddiv_rn(weighted[ch], total[ch]) : 1.0;
+        if (!(mean > 0.0)) mean = 1.0;
+        const float gain = n > 0.0 ? __double2float_rn(__ddiv_rn(s->x[v][ch], mean)) : 1.f;
+        s->gains[v][ch] = gain;
+        s->d[v][ch] = gain;
+      }
+    return;
+  }
+  const double nG = is_view ? dmul(static_cast<double>(s->view_samples[v]), g.cG) : 0.0;
+  double Ad[3];
+  for (int ch = 0; ch < 3; ++ch) Ad[ch] = is_view ? dadd(dmul(column[v][ch], g.cN), dmul(nG, s->d[v][ch])) : 0.0;
+  if (mode == kStepInit) {
+    double t[3], rr[3];
+    for (int ch = 0; ch < 3; ++ch) {
+      const double r = is_view ? dsub(nG, Ad[ch]) : 0.0;
+      if (is_view) { s->r[v][ch] = r; s->d[v][ch] = r; }
+      t[ch] = dmul(r, r);
+    }
+    views_tree(t, warp_sums, rr);
+    if (threadIdx.x == 0)
+      for (int ch = 0; ch < 3; ++ch) { s->rr[ch] = rr[ch]; s->done[ch] = !(rr[ch] != 0.0); }
+    return;
+  }
+  // kStepIterate
+  bool active[3];
+  double rr[3], t[3], pAp[3], alpha[3];
+  for (int ch = 0; ch < 3; ++ch) {
+    rr[ch] = s->rr[ch];
+    active[ch] = s->done[ch] == 0;
+    t[ch] = is_view ? dmul(s->d[v][ch], Ad[ch]) : 0.0;
+  }
+  views_tree(t, warp_sums, pAp);
+  for (int ch = 0; ch < 3; ++ch) {
+    active[ch] = active[ch] && pAp[ch] > 0.0;
+    alpha[ch] = active[ch] ? __ddiv_rn(rr[ch], pAp[ch]) : 0.0;
+    double r = 0.0;
+    if (is_view) {
+      r = s->r[v][ch];
+      if (active[ch]) {
+        s->x[v][ch] = dadd(s->x[v][ch], dmul(alpha[ch], s->d[v][ch]));
+        r = dsub(r, dmul(alpha[ch], Ad[ch]));
+        s->r[v][ch] = r;
+      }
+    }
+    t[ch] = dmul(r, r);
+  }
+  double rr_new[3];
+  views_tree(t, warp_sums, rr_new);
+  for (int ch = 0; ch < 3; ++ch) {
+    if (!active[ch]) continue;
+    const double beta = __ddiv_rn(rr_new[ch], rr[ch]);
+    if (is_view) s->d[v][ch] = dadd(s->r[v][ch], dmul(beta, s->d[v][ch]));
+  }
+  __syncthreads();   // every thread has read rr and done
+  if (threadIdx.x == 0)
+    for (int ch = 0; ch < 3; ++ch) {
+      if (active[ch]) s->rr[ch] = rr_new[ch];
+      s->done[ch] = !active[ch] || !(rr_new[ch] != 0.0);
+    }
+}
+
 void FreeTriangleScratch(TextureScratch& s) {
   FreeAndClear(s.keys, s.sorted, s.records, s.sort_temp);
   s.sort_temp_bytes = 0;
@@ -428,6 +711,43 @@ int EnsurePixelScratch(TextureScratch& s, size_t pixels) {
   return SM_OK;
 }
 
+void FreeGainScratch(TextureScratch& s) {
+  FreeAndClear(s.samples, s.fit_count, s.mean, s.block_sums);
+  s.sample_capacity = s.point_capacity = s.block_capacity = 0;
+}
+
+// The sample matrix (P x V entries), the per-point vectors (P) and the level-2 column sums (V x blocks), each group
+// grown by x 1.5 when it does not fit; the solver state once.
+int EnsureGainScratch(TextureScratch& s, u64 entries, u64 points, u64 block_sums) {
+  if (!s.gain.device) {
+    const int status = CreateCounters(s.gain);
+    if (status != SM_OK) return status;
+  }
+  if (entries > s.sample_capacity) {
+    const u64 cap = GrownCapacity(entries, 1 << 16);
+    FreeAndClear(s.samples);
+    s.sample_capacity = 0;
+    SM_CUDA(cudaMalloc(&s.samples, 3 * sizeof(float) * cap));
+    s.sample_capacity = cap;
+  }
+  if (points > s.point_capacity) {
+    const u64 cap = GrownCapacity(points);
+    FreeAndClear(s.fit_count, s.mean);
+    s.point_capacity = 0;
+    SM_CUDA(cudaMalloc(&s.fit_count, sizeof(u32) * cap));
+    SM_CUDA(cudaMalloc(&s.mean, 3 * sizeof(double) * cap));
+    s.point_capacity = cap;
+  }
+  if (block_sums > s.block_capacity) {
+    const u64 cap = GrownCapacity(block_sums);
+    FreeAndClear(s.block_sums);
+    s.block_capacity = 0;
+    SM_CUDA(cudaMalloc(&s.block_sums, 3 * sizeof(double) * cap));
+    s.block_capacity = cap;
+  }
+  return SM_OK;
+}
+
 }  // namespace
 
 void FreeTextureBuffers(sm_reconstruction* r) {
@@ -436,33 +756,37 @@ void FreeTextureBuffers(sm_reconstruction* r) {
   FreeTriangleScratch(*s);
   FreeTexelScratch(*s);
   FreePixelScratch(*s);
+  FreeGainScratch(*s);
   FreeCounters(s->counters);
+  FreeCounters(s->gain);
   delete s;
   r->texture = nullptr;
 }
 
-}  // namespace smb
+namespace {
 
-using namespace smb;
-
-extern "C" {
-
-void sm_default_texture_params(sm_texture_params* p) {
-  p->texel_size = 0.004f;
-  p->max_atlas_side = 16384;
-  p->max_view_angle_deg = 75.0f;
-  p->depth_tolerance = 0.01f;
-}
-
-int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_params* params, const uint32_t* triangles,
-                    uint64_t count, const sm_texture_view* views, int32_t view_count, uint8_t* atlas,
-                    size_t atlas_pitch, int32_t atlas_capacity_width, int32_t atlas_capacity_height, float* uv,
-                    sm_texture_stats* stats) {
-  if (!r || !params || !stats) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_texture: null argument");
-  auto bad = [](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (std::string("sm_mesh_texture: ") + why).c_str()); };
+// sm_mesh_texture, and with `gp` set sm_mesh_texture_compensated; `who` names the call in its messages.
+int Texture(const char* who, sm_reconstruction* r, void* stream_v, const sm_texture_params* params,
+            const sm_texture_gain_params* gp, const uint32_t* triangles, uint64_t count, const sm_texture_view* views,
+            int32_t view_count, uint8_t* atlas, size_t atlas_pitch, int32_t atlas_capacity_width,
+            int32_t atlas_capacity_height, float* uv, float* gains, sm_texture_stats* stats,
+            sm_texture_gain_stats* gain_stats) {
+  const std::string prefix = std::string(who) + ": ";
+  auto bad = [&prefix](const char* why) { return SetError(SM_ERR_INVALID_ARGUMENT, (prefix + why).c_str()); };
+  if (!r || !params || !stats) return bad("null argument");
   const cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   const sm_texture_params& p = *params;
   *stats = sm_texture_stats{};
+  if (gp) {
+    if (!gain_stats) return bad("null argument");
+    *gain_stats = sm_texture_gain_stats{};
+    if (gp->max_samples < 0) return bad("max_samples must be >= 0");
+    if (gp->iterations < 0) return bad("iterations must be >= 0");
+    if (!std::isfinite(gp->sigma_noise) || !(gp->sigma_noise > 0.f)) return bad("sigma_noise must be finite and > 0");
+    if (!std::isfinite(gp->sigma_gain) || !(gp->sigma_gain > 0.f)) return bad("sigma_gain must be finite and > 0");
+    if (!std::isfinite(gp->min_level) || !std::isfinite(gp->max_level) || gp->min_level > gp->max_level)
+      return bad("min_level and max_level must be finite with min_level <= max_level");
+  }
   if (!std::isfinite(p.texel_size) || !(p.texel_size > 0.f)) return bad("texel_size must be finite and > 0");
   if (p.max_atlas_side < 8 || p.max_atlas_side > SM_TEXTURE_MAX_ATLAS_SIDE)
     return bad("max_atlas_side must be in [8, SM_TEXTURE_MAX_ATLAS_SIDE]");
@@ -494,7 +818,10 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_param
   r->last_stream = stream;
   int status = FetchCounters(r, stream);
   if (status == SM_ERR_CUDA) return status;   // (a surfel-cap overflow of an earlier frame does not matter here)
-  if (count == 0) return SM_OK;               // a 0 x 0 atlas: nothing to write
+  if (count == 0) {                           // a 0 x 0 atlas: nothing to write
+    if (gains) std::fill(gains, gains + 3 * static_cast<size_t>(view_count), 1.f);
+    return SM_OK;
+  }
   const u32 n = r->host_counters->surfel_count[r->count_slot];
 
   if (!r->texture) {   // published only with its counters, so a failed first call is retried whole
@@ -549,11 +876,11 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_param
   stats->tiles_clamped = h.clamped;
   const u64 height = h.height;
   if (width > static_cast<u64>(p.max_atlas_side))
-    return SetError(SM_ERR_CAPACITY, ("sm_mesh_texture: the atlas needs a side of " + std::to_string(width) +
+    return SetError(SM_ERR_CAPACITY, (prefix + "the atlas needs a side of " + std::to_string(width) +
                                       " texels, above max_atlas_side " + std::to_string(p.max_atlas_side) +
                                       "; raise texel_size").c_str());
   if (width > static_cast<u64>(atlas_capacity_width) || height > static_cast<u64>(atlas_capacity_height))
-    return SetError(SM_ERR_CAPACITY, ("sm_mesh_texture: a " + std::to_string(width) + " x " + std::to_string(height) +
+    return SetError(SM_ERR_CAPACITY, (prefix + "a " + std::to_string(width) + " x " + std::to_string(height) +
                                       " atlas does not fit the capacity of " + std::to_string(atlas_capacity_width) +
                                       " x " + std::to_string(atlas_capacity_height)).c_str());
   // From here on a failure leaves the stats zero.
@@ -562,6 +889,13 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_param
   status = EnsureTexelScratch(s, area);
   if (status == SM_OK) status = EnsurePixelScratch(s, max_pixels);
   if (status != SM_OK) return status;
+  // G1: the sample points
+  const u64 points = gp && view_count > 0 ? std::min<u64>(count, static_cast<u64>(gp->max_samples) / view_count) : 0;
+  const u64 blocks = (points + kGainBlock - 1) / kGainBlock;
+  if (points > 0) {
+    status = EnsureGainScratch(s, points * view_count, points, blocks * view_count);
+    if (status != SM_OK) return status;
+  }
 
   a.accum = s.accum;
   a.area = static_cast<u32>(area);   // width <= SM_TEXTURE_MAX_ATLAS_SIDE: area <= 2^30
@@ -575,34 +909,140 @@ int sm_mesh_texture(sm_reconstruction* r, void* stream_v, const sm_texture_param
   if (uv) { LaunchScope scope(stream, KID_TEXTURE_UV); LaunchKernel(k_tex_uv, dim3(grid), dim3(kBlock), 0, stream, a); }
   const int texel_grid = Grid(area, r->sm_count);
   const float cos_max = CosDegrees(p.max_view_angle_deg);
-  for (int32_t k = 0; k < view_count; ++k) {
+  // View k's depth into the scratch raster, and its description for the kernels.
+  auto render_view = [&](int32_t k, TextureView* v) {
     const sm_texture_view& view = views[k];
     const sm_render_params& cam = view.camera;
     const size_t depth_pitch = sizeof(float) * static_cast<size_t>(cam.width);
-    status = RenderMesh(r, stream, cam, view.view_T_global, triangles, count, 0, s.depth, depth_pitch, nullptr, 0,
-                        nullptr, 0, nullptr, 0);
-    if (status != SM_OK) return status;
+    v->T = MakeMat3x4(view.view_T_global);
+    v->fx = cam.fx; v->fy = cam.fy; v->cx = cam.cx; v->cy = cam.cy;
+    v->near_depth = cam.near_depth; v->far_depth = cam.far_depth;
+    v->width = cam.width; v->height = cam.height;
+    v->color = view.color; v->color_pitch = view.color_pitch;
+    v->depth = s.depth; v->depth_pitch = depth_pitch;
+    v->cos_max = cos_max;
+    v->tolerance = p.depth_tolerance;
+    v->used = c->view_used + k;
+    return RenderMesh(r, stream, cam, view.view_T_global, triangles, count, 0, s.depth, depth_pitch, nullptr, 0,
+                      nullptr, 0, nullptr, 0);
+  };
+  GainState* gs = s.gain.device;
+  if (points > 0) {   // G2-G4 and the data terms of G6, all on `stream`
+    GainArgs g{};
+    g.samples = s.samples; g.fit_count = s.fit_count; g.mean = s.mean; g.block_sums = s.block_sums;
+    g.state = gs;
+    g.points = static_cast<u32>(points);   // points * view_count <= INT32_MAX
+    g.views = static_cast<u32>(view_count);
+    g.blocks = static_cast<u32>(blocks);
+    g.min_level = gp->min_level; g.max_level = gp->max_level;
+    const double sn = gp->sigma_noise, sg = gp->sigma_gain;
+    g.cN = 1.0 / (sn * sn);
+    g.cG = 1.0 / (sg * sg);
+    const int point_grid = Grid(points, r->sm_count);
+    const dim3 view_grid(static_cast<u32>(blocks), static_cast<u32>(view_count));
+    SM_CUDA(cudaMemsetAsync(gs, 0, offsetof(GainState, x), stream));
+    for (int32_t k = 0; k < view_count; ++k) {
+      TextureView v;
+      status = render_view(k, &v);
+      if (status != SM_OK) return status;
+      LaunchScope scope(stream, KID_TEXTURE_GAIN_SAMPLE);
+      LaunchKernel(k_tex_gain_sample, dim3(point_grid), dim3(kBlock), 0, stream, a, v, g, static_cast<u32>(k));
+    }
+    { LaunchScope scope(stream, KID_TEXTURE_GAIN_COUNT); LaunchKernel(k_tex_gain_count, dim3(point_grid), dim3(kBlock), 0, stream, g); }
+    auto sweep = [&](const double* x, bool squares, int mode) {
+      if (x) { LaunchScope scope(stream, KID_TEXTURE_GAIN_POINTS); LaunchKernel(k_tex_gain_points, dim3(point_grid), dim3(kBlock), 0, stream, g, x); }
+      {
+        LaunchScope scope(stream, KID_TEXTURE_GAIN_VIEWS);
+        const double* xv = x ? x : &gs->x[0][0];
+        if (squares) LaunchKernel(k_tex_gain_views<true>, view_grid, dim3(kGainBlock), 0, stream, g, xv);
+        else LaunchKernel(k_tex_gain_views<false>, view_grid, dim3(kGainBlock), 0, stream, g, xv);
+      }
+      LaunchScope scope(stream, KID_TEXTURE_GAIN_STEP);
+      LaunchKernel(k_tex_gain_step, dim3(1), dim3(kGainBlock), 0, stream, g, mode);
+    };
+    sweep(&gs->x[0][0], true, kStepData0);   // D at x = 1
+    sweep(nullptr, false, kStepInit);       // r = b - A 1 (the same m_p)
+    for (int32_t it = 0; it < gp->iterations; ++it) sweep(&gs->d[0][0], false, kStepIterate);
+    { LaunchScope scope(stream, KID_TEXTURE_GAIN_STEP); LaunchKernel(k_tex_gain_step, dim3(1), dim3(kGainBlock), 0, stream, g, static_cast<int>(kStepFinish)); }
+    sweep(&gs->d[0][0], true, kStepData1);   // D at the float gains
+  }
+  for (int32_t k = 0; k < view_count; ++k) {
     TextureView v;
-    v.T = MakeMat3x4(view.view_T_global);
-    v.fx = cam.fx; v.fy = cam.fy; v.cx = cam.cx; v.cy = cam.cy;
-    v.near_depth = cam.near_depth; v.far_depth = cam.far_depth;
-    v.width = cam.width; v.height = cam.height;
-    v.color = view.color; v.color_pitch = view.color_pitch;
-    v.depth = s.depth; v.depth_pitch = depth_pitch;
-    v.cos_max = cos_max;
-    v.tolerance = p.depth_tolerance;
-    v.used = c->view_used + k;
+    status = render_view(k, &v);
+    if (status != SM_OK) return status;
     LaunchScope scope(stream, KID_TEXTURE_ACCUMULATE);
-    LaunchKernel(k_tex_accumulate, dim3(texel_grid), dim3(kBlock), 0, stream, a, v);
+    if (points > 0) LaunchKernel(k_tex_accumulate<true>, dim3(texel_grid), dim3(kBlock), 0, stream, a, v, &gs->gains[k][0]);
+    else LaunchKernel(k_tex_accumulate<false>, dim3(texel_grid), dim3(kBlock), 0, stream, a, v, static_cast<const float*>(nullptr));
   }
   { LaunchScope scope(stream, KID_TEXTURE_RESOLVE); LaunchKernel(k_tex_resolve, dim3(texel_grid), dim3(kBlock), 0, stream, a); }
   status = ReadCounters(s.counters, stream);
+  if (status == SM_OK && points > 0) status = ReadCounters(s.gain, stream, offsetof(GainState, x));
   if (status != SM_OK) return status;
   *stats = layout;
   stats->texels_seen = h.seen;
   stats->texels_fallback = h.fallback;
   for (int32_t k = 0; k < view_count; ++k) stats->views_used += h.view_used[k] ? 1 : 0;
+  if (gp) {
+    const GainState& hg = *s.gain.host;
+    sm_texture_gain_stats out{};
+    out.points = points;
+    for (int32_t k = 0; points > 0 && k < view_count; ++k) {
+      out.samples += hg.view_samples[k];
+      out.views_fitted += hg.view_samples[k] ? 1 : 0;
+    }
+    if (out.samples > 0) {
+      const double scale = 3.0 * static_cast<double>(out.samples);
+      out.rms_before = std::sqrt(hg.data[0] / scale);
+      out.rms_after = std::sqrt(hg.data[1] / scale);
+    }
+    *gain_stats = out;
+    if (gains)
+      for (int32_t k = 0; k < view_count; ++k)
+        for (int ch = 0; ch < 3; ++ch) gains[3 * k + ch] = points > 0 ? hg.gains[k][ch] : 1.f;
+  }
   return CheckLaunch("texture");
+}
+
+}  // namespace
+
+}  // namespace smb
+
+using namespace smb;
+
+extern "C" {
+
+void sm_default_texture_params(sm_texture_params* p) {
+  p->texel_size = 0.004f;
+  p->max_atlas_side = 16384;
+  p->max_view_angle_deg = 75.0f;
+  p->depth_tolerance = 0.01f;
+}
+
+void sm_default_texture_gain_params(sm_texture_gain_params* p) {
+  p->max_samples = 1 << 23;
+  p->iterations = 32;
+  p->sigma_noise = 10.0f;
+  p->sigma_gain = 1.0f;
+  p->min_level = 5.0f;
+  p->max_level = 250.0f;
+}
+
+int sm_mesh_texture(sm_reconstruction* r, void* stream, const sm_texture_params* params, const uint32_t* triangles,
+                    uint64_t count, const sm_texture_view* views, int32_t view_count, uint8_t* atlas,
+                    size_t atlas_pitch, int32_t atlas_capacity_width, int32_t atlas_capacity_height, float* uv,
+                    sm_texture_stats* stats) {
+  return Texture("sm_mesh_texture", r, stream, params, nullptr, triangles, count, views, view_count, atlas,
+                 atlas_pitch, atlas_capacity_width, atlas_capacity_height, uv, nullptr, stats, nullptr);
+}
+
+int sm_mesh_texture_compensated(sm_reconstruction* r, void* stream, const sm_texture_params* params,
+                                const sm_texture_gain_params* gp, const uint32_t* triangles, uint64_t count,
+                                const sm_texture_view* views, int32_t view_count, uint8_t* atlas, size_t atlas_pitch,
+                                int32_t atlas_capacity_width, int32_t atlas_capacity_height, float* uv, float* gains,
+                                sm_texture_stats* stats, sm_texture_gain_stats* gain_stats) {
+  if (!gp) return SetError(SM_ERR_INVALID_ARGUMENT, "sm_mesh_texture_compensated: null argument");
+  return Texture("sm_mesh_texture_compensated", r, stream, params, gp, triangles, count, views, view_count, atlas,
+                 atlas_pitch, atlas_capacity_width, atlas_capacity_height, uv, gains, stats, gain_stats);
 }
 
 }  // extern "C"

@@ -22,7 +22,7 @@ from . import _lib
 from . import mesh_io
 from ._lib import (CompactStats, ComponentParams, ComponentStats, HoleParams, HoleStats, IntegrateParams, SimplifyParams, SimplifyStats, Library, MeshComponent, MeshParams, MeshStats, MeshUpdateStats,
                    PreprocessParams, RelocParams, RelocResult, RenderParams, SessionStatus, StreamDesc, StreamStats,
-                   TextureParams, TextureStats, TextureViewDesc, TrackParams, TrackResult,
+                   TextureGainParams, TextureGainStats, TextureParams, TextureStats, TextureViewDesc, TrackParams, TrackResult,
                    TrackRGBDParams, TrackRGBDResult,
                    TransferStats, TransferToken, VisualizationParams)
 
@@ -746,14 +746,19 @@ class CUDASurfelReconstruction:
         return out[:int(stats.triangles_out)], labels[:T], table, stats
 
     def texture_mesh(self, triangles, views: Sequence[TextureView], params: Optional[TextureParams] = None,
-                     stream=None):
+                     stream=None, gains: Optional[TextureGainParams] = None):
         """sm_mesh_texture: a texture atlas for `triangles` (an int32 CUDA tensor [T, 3] of present slots, any list
         without repeated corners) from the colour images of `views` (TextureView, in the order their samples are
         summed; include/surfel_b200.h gives the rules). Synchronous. Lays the atlas out first (a query that writes
         nothing), then fills it. Returns (atlas uint8 CUDA tensor [H, W, 3], row 0 first; uv float32 CUDA tensor
         [T, 3, 2], (u, v) in [0, 1] per corner of each triangle in its listed order, v = 0 at row 0; TextureStats).
         Raises SurfelError (SM_ERR_CAPACITY) when the atlas would be wider than params.max_atlas_side: raise
-        params.texel_size then."""
+        params.texel_size then.
+
+        With `gains` (TextureGainParams), sm_mesh_texture_compensated: one gain per view and channel is fitted over
+        surface points the views share, evening out their exposure and white balance, and each view's samples are
+        scaled by its gains. Returns (atlas, uv, stats, gains float32 CPU tensor [V, 3] (r, g, b per view),
+        TextureGainStats)."""
         p = TextureParams.defaults() if params is None else params
         _check_triangles(triangles)
         tri = triangles.contiguous()
@@ -761,13 +766,27 @@ class CUDASurfelReconstruction:
         descs = (TextureViewDesc * max(len(views), 1))(*[v.desc() for v in views])
         handle = _stream_handle(stream)
         stats = TextureStats()
-        fn = self.lib.fn["mesh_texture"]
         tri_ptr = C.c_void_p(tri.data_ptr()) if len(tri) else None
-        status = fn(self._h, handle, C.byref(p), tri_ptr, len(tri), descs, len(views), None, 0, 0, 0, None,
-                    C.byref(stats))
+        if gains is not None:
+            gain_out = torch.ones((len(views), 3), dtype=torch.float32)
+            gain_stats = TextureGainStats()
+
+        def call(atlas_ptr, pitch, W, H, uv_ptr):
+            if gains is None:
+                return self.lib.fn["mesh_texture"](self._h, handle, C.byref(p), tri_ptr, len(tri), descs, len(views),
+                                                   atlas_ptr, pitch, W, H, uv_ptr, C.byref(stats))
+            return self.lib.fn["mesh_texture_compensated"](
+                self._h, handle, C.byref(p), C.byref(gains), tri_ptr, len(tri), descs, len(views), atlas_ptr, pitch,
+                W, H, uv_ptr, C.c_void_p(gain_out.data_ptr()) if len(views) else None, C.byref(stats),
+                C.byref(gain_stats))
+
+        def finish(atlas, uv):
+            return (atlas, uv, stats) if gains is None else (atlas, uv, stats, gain_out, gain_stats)
+
+        status = call(None, 0, 0, 0, None)
         if status == _lib.SM_OK:   # an empty list: an empty atlas
-            return (torch.zeros((0, 0, 3), dtype=torch.uint8, device="cuda"),
-                    torch.zeros((0, 3, 2), dtype=torch.float32, device="cuda"), stats)
+            return finish(torch.zeros((0, 0, 3), dtype=torch.uint8, device="cuda"),
+                          torch.zeros((0, 3, 2), dtype=torch.float32, device="cuda"))
         if status != _lib.SM_ERR_CAPACITY or stats.atlas_width > p.max_atlas_side:
             raise self.lib.error(status)
         W, H = int(stats.atlas_width), int(stats.atlas_height)
@@ -776,9 +795,10 @@ class CUDASurfelReconstruction:
         if isinstance(stream, torch.cuda.Stream):
             atlas.record_stream(stream)
             uv.record_stream(stream)
-        self.lib.call("mesh_texture", self._h, handle, C.byref(p), tri_ptr, len(tri), descs, len(views),
-                      C.c_void_p(atlas.data_ptr()), 3 * W, W, H, C.c_void_p(uv.data_ptr()), C.byref(stats))
-        return atlas, uv, stats
+        status = call(C.c_void_p(atlas.data_ptr()), 3 * W, W, H, C.c_void_p(uv.data_ptr()))
+        if status != _lib.SM_OK:
+            raise self.lib.error(status)
+        return finish(atlas, uv)
 
     def export_vertices_host(self, stream=None):
         """sm_export_vertices into host arrays: positions [n, 3] float32 (NaN rows for merged slots), colours
@@ -795,7 +815,8 @@ class CUDASurfelReconstruction:
                       holes: Optional[HoleParams] = None, simplify: Optional[SimplifyParams] = None,
                       texture: Optional[TextureParams] = None,
                       views: Optional[Sequence[TextureView]] = None,
-                      components: Optional[ComponentParams] = None) -> MeshStats:
+                      components: Optional[ComponentParams] = None,
+                      gains: Optional[TextureGainParams] = None) -> MeshStats:
         """The reference's SaveMeshAsOBJ (main.cc:128-175): the non-merged slots in slot order with their colour,
         and the triangles of triangulate() over them (1-based, remapped to that order). With `holes`, the
         triangles of fill_holes(holes) follow the mesh's. With `components`, only the triangles of the pieces that
@@ -804,7 +825,8 @@ class CUDASurfelReconstruction:
         `simplify`, only the slots that are corners of the final triangles are written, in slot order.
         With `texture`, the final triangles are textured from `views` by texture_mesh(texture): the OBJ gets one
         texture coordinate per triangle corner and names the material of `path` with the suffix .mtl, whose
-        diffuse map is the atlas written to `path` with the suffix .png."""
+        diffuse map is the atlas written to `path` with the suffix .png. With `gains` as well, the atlas is
+        texture_mesh(texture, gains=gains)'s: the views' exposure evened out."""
         tri, stats = self.triangulate(params, stream)
         if holes is not None:
             fill, _ = self.fill_holes(tri, holes, stream)
@@ -816,7 +838,7 @@ class CUDASurfelReconstruction:
         uvs, material = None, None
         if texture is not None:
             from pathlib import Path
-            atlas, uv, _ = self.texture_mesh(tri, views or [], texture, stream)
+            atlas, uv = self.texture_mesh(tri, views or [], texture, stream, gains=gains)[:2]
             png, mtl = Path(path).with_suffix(".png"), Path(path).with_suffix(".mtl")
             image = atlas.cpu().numpy() if atlas.numel() else np.zeros((1, 1, 3), np.uint8)
             mesh_io.write_png(png, image)
