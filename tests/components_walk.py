@@ -1,21 +1,17 @@
 """ctypes loader for tests/components_walk.c (TEST INFRASTRUCTURE): the plain-C restatement of sm_mesh_components,
-and the hand-built meshes the host and GPU tests share. The library is compiled on first use into a temporary
-directory (keyed by the source's digest), so the repository tree stays untouched."""
+and the hand-built meshes the host and GPU tests share."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
 from surfelmeshing_b200 import _lib as L
+from tests import cbuild
 from tests import mesh_walk as M
 from tests import simplify_walk as SW
+from tests.cbuild import ptr
 
 SOURCE = Path(__file__).resolve().parent / "components_walk.c"
 STATS = [f for f, _ in L.ComponentStats._fields_]
@@ -26,34 +22,12 @@ TABLE_DTYPE = np.dtype({"names": ["triangles", "area", "lo", "hi", "first_triang
                         "offsets": [getattr(L.MeshComponent, f).offset for f, _ in L.MeshComponent._fields_],
                         "itemsize": C.sizeof(L.MeshComponent)})
 
-_lib = None
-
 
 def load():
-    global _lib
-    if _lib is None:
-        tag = hashlib.sha256(SOURCE.read_bytes()).hexdigest()[:16]
-        out_dir = Path(tempfile.gettempdir()) / f"components_walk_{os.getuid()}"
-        out_dir.mkdir(parents=True, exist_ok=True)
-        path = out_dir / f"libcomponents_walk_{tag}.so"
-        if not path.exists():
-            cc = shutil.which("gcc") or shutil.which("cc")
-            if cc is None:
-                raise RuntimeError("a C compiler is needed to build the components checker")
-            tmp = out_dir / f"{path.name}.{os.getpid()}.tmp"
-            subprocess.run([cc, "-O2", "-fPIC", "-shared", "-std=gnu11", "-ffp-contract=off", "-o", str(tmp),
-                            str(SOURCE), "-lm"], check=True, capture_output=True)
-            os.replace(tmp, path)
-        _lib = C.CDLL(str(path))
-        _lib.cw_components.restype = C.c_int64
-        _lib.cw_components.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64,
-                                       C.POINTER(L.ComponentParams), C.c_void_p, C.c_void_p, C.c_void_p,
-                                       C.POINTER(L.ComponentStats)]
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return cbuild.library(SOURCE, cbuild.WALK_FLAGS, {
+        "cw_components": (C.c_int64, [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64,
+                                      C.POINTER(L.ComponentParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.POINTER(L.ComponentStats)])})
 
 
 class InvalidMesh(ValueError):
@@ -79,8 +53,8 @@ def components(rows, tri, params=None):
     labels = np.zeros(max(count, 1), np.int32)
     table = np.zeros(max(count, 1), TABLE_DTYPE)
     stats = L.ComponentStats()
-    total = load().cw_components(_p(rows), rows.shape[1], n, _p(tri) if count else None, count, C.byref(p), _p(out),
-                                 _p(labels), _p(table), C.byref(stats))
+    total = load().cw_components(ptr(rows), rows.shape[1], n, ptr(tri) if count else None, count, C.byref(p), ptr(out),
+                                 ptr(labels), ptr(table), C.byref(stats))
     if total < 0:
         raise InvalidMesh(ERRORS[total])
     return out[:total], labels[:count], table[:stats.components].copy(), stats_dict(stats)

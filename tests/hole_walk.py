@@ -1,52 +1,26 @@
 """ctypes loader for tests/hole_walk.c (TEST INFRASTRUCTURE): the plain-C restatement of sm_mesh_fill_holes, and
-the hand-built meshes the host and GPU tests share. The library is compiled on first use into a temporary
-directory (keyed by the source's digest), so the repository tree stays untouched."""
+the hand-built meshes the host and GPU tests share."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
 from surfelmeshing_b200 import _lib as L
+from tests import cbuild
 from tests import mesh_walk as M
+from tests.cbuild import ptr
 
 SOURCE = Path(__file__).resolve().parent / "hole_walk.c"
 STAT_NAMES = [f for f, _ in L.HoleStats._fields_]
 ERRORS = {-1: "bad corner", -2: "repeated corner", -3: "duplicate edge"}
 
-_lib = None
-
 
 def load():
-    global _lib
-    if _lib is None:
-        tag = hashlib.sha256(SOURCE.read_bytes()).hexdigest()[:16]
-        out_dir = Path(tempfile.gettempdir()) / f"hole_walk_{os.getuid()}"
-        out_dir.mkdir(parents=True, exist_ok=True)
-        path = out_dir / f"libhole_walk_{tag}.so"
-        if not path.exists():
-            cc = shutil.which("gcc") or shutil.which("cc")
-            if cc is None:
-                raise RuntimeError("a C compiler is needed to build the hole-filling checker")
-            tmp = out_dir / f"{path.name}.{os.getpid()}.tmp"
-            subprocess.run([cc, "-O2", "-fPIC", "-shared", "-std=gnu11", "-ffp-contract=off", "-o", str(tmp),
-                            str(SOURCE), "-lm"], check=True, capture_output=True)
-            os.replace(tmp, path)
-        _lib = C.CDLL(str(path))
-        _lib.hw_fill_holes.restype = C.c_int64
-        _lib.hw_fill_holes.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.c_int, C.c_float,
-                                       C.c_float, C.c_void_p, C.c_uint64, C.c_void_p]
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return cbuild.library(SOURCE, cbuild.WALK_FLAGS, {
+        "hw_fill_holes": (C.c_int64, [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.c_int, C.c_float,
+                                      C.c_float, C.c_void_p, C.c_uint64, C.c_void_p])})
 
 
 class InvalidMesh(ValueError):
@@ -64,13 +38,13 @@ def fill_holes(rows, tri, params=None):
     tri = np.ascontiguousarray(np.asarray(tri, np.uint32).reshape(-1, 3))
     stats = np.zeros(7, np.uint64)
     lib = load()
-    args = (_p(rows), rows.shape[1], n, _p(tri) if len(tri) else None, len(tri), p.max_hole_edges,
+    args = (ptr(rows), rows.shape[1], n, ptr(tri) if len(tri) else None, len(tri), p.max_hole_edges,
             p.max_angle_between_normals_deg, p.max_triangle_angle_deg)
-    total = lib.hw_fill_holes(*args, None, 0, _p(stats))
+    total = lib.hw_fill_holes(*args, None, 0, ptr(stats))
     if total < 0:
         raise InvalidMesh(ERRORS[total])
     fill = np.zeros((max(total, 1), 3), np.uint32)
-    lib.hw_fill_holes(*args, _p(fill), total, _p(stats))
+    lib.hw_fill_holes(*args, ptr(fill), total, ptr(stats))
     return fill[:total], {k: int(v) for k, v in zip(STAT_NAMES, stats)}
 
 

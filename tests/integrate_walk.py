@@ -46,16 +46,14 @@ merges in the same frame: the only ones where the reference may differ (it then 
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
 import re
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 from types import SimpleNamespace
 
 import numpy as np
+
+from tests import cbuild
+from tests.cbuild import ptr
 
 SOURCE = Path(__file__).resolve().parent / "integrate_walk.c"
 ROW_COUNT = 25
@@ -90,36 +88,11 @@ class Params(C.Structure):
                 ("local_T_global", C.c_float * 12), ("mutations", C.c_uint32)]
 
 
-_lib = None
-
-
 def load():
-    global _lib
-    if _lib is None:
-        tag = hashlib.sha256(SOURCE.read_bytes()).hexdigest()[:16]
-        out_dir = Path(tempfile.gettempdir()) / f"integrate_walk_{os.getuid()}"
-        out_dir.mkdir(parents=True, exist_ok=True)
-        path = out_dir / f"libintegrate_walk_{tag}.so"
-        if not path.exists():
-            cc = shutil.which("gcc") or shutil.which("cc")
-            if cc is None:
-                raise RuntimeError("a C compiler is needed to build the integration walk")
-            tmp = out_dir / f"{path.name}.{os.getpid()}.tmp"
-            subprocess.run([cc, "-O2", "-fPIC", "-shared", "-std=gnu11", "-ffp-contract=off", "-o", str(tmp), str(SOURCE),
-                            "-lm"], check=True, capture_output=True)
-            os.replace(tmp, path)
-        _lib = C.CDLL(str(path))
-        _lib.iw_integrate.restype = C.c_uint64
-        _lib.iw_integrate.argtypes = [C.POINTER(Params), C.c_uint64, C.c_uint64] + [C.c_void_p] * 22
-        _lib.iw_associate.restype = None
-        _lib.iw_associate.argtypes = [C.POINTER(Params), C.c_uint64] + [C.c_void_p] * 17
-        _lib.iw_blend.restype = None
-        _lib.iw_blend.argtypes = [C.POINTER(Params), C.c_int] + [C.c_void_p] * 14
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return cbuild.library(SOURCE, cbuild.WALK_FLAGS, {
+        "iw_integrate": (C.c_uint64, [C.POINTER(Params), C.c_uint64, C.c_uint64] + [C.c_void_p] * 22),
+        "iw_associate": (None, [C.POINTER(Params), C.c_uint64] + [C.c_void_p] * 17),
+        "iw_blend": (None, [C.POINTER(Params), C.c_int] + [C.c_void_p] * 14)})
 
 
 def invert_rigid(m):
@@ -160,9 +133,10 @@ def walk(rows_before, frame, rasters, camera, ip, frame_index, global_T_local, l
     branch = np.zeros(len(BRANCHES) + 1, np.uint64)
     counts = np.zeros(3, np.uint64)
     scratch = np.zeros((ROW_COUNT, max(n, 1)), np.float32)
-    n_after = load().iw_integrate(C.byref(p), n, stride, _p(rows), *[_p(a) for a in inputs], _p(out.merge_flag),
-                                  _p(out.new_flag), _p(out.new_index), _p(out.status), _p(out.pbound), _p(out.nbound),
-                                  _p(out.cbound), _p(out.color_lo), _p(out.color_hi), _p(branch), _p(counts), _p(scratch))
+    n_after = load().iw_integrate(C.byref(p), n, stride, ptr(rows), *[ptr(a) for a in inputs], ptr(out.merge_flag),
+                                  ptr(out.new_flag), ptr(out.new_index), ptr(out.status), ptr(out.pbound),
+                                  ptr(out.nbound), ptr(out.cbound), ptr(out.color_lo), ptr(out.color_hi), ptr(branch),
+                                  ptr(counts), ptr(scratch))
     assert n_after <= stride
     for k in ("status", "pbound", "nbound", "cbound", "color_lo", "color_hi"):
         setattr(out, k, getattr(out, k)[:n_after])
@@ -292,9 +266,9 @@ def associate(rows, depth_pre, normals, camera, ip, frame_index, local_T_global,
     conf_pixel, conf_surfel, conf_stage = np.empty(3 * n + 1, np.uint32), np.empty(3 * n + 1, np.uint32), np.empty(3 * n + 1, np.uint8)
     counts = np.zeros(2, np.uint64)
     branch = np.zeros(len(FRONT_BRANCHES) + 1, np.uint64)
-    load().iw_associate(C.byref(p), n, _p(rows), _p(depth_pre), _p(normals), _p(r.first), _p(r.counts), _p(r.sum_float),
-                        _p(r.sum), _p(r.sum_abs), _p(r.unclear), _p(ties), _p(sup_pixel), _p(sup_key), _p(conf_pixel),
-                        _p(conf_surfel), _p(conf_stage), _p(counts), _p(branch))
+    load().iw_associate(C.byref(p), n, ptr(rows), ptr(depth_pre), ptr(normals), ptr(r.first), ptr(r.counts),
+                        ptr(r.sum_float), ptr(r.sum), ptr(r.sum_abs), ptr(r.unclear), ptr(ties), ptr(sup_pixel),
+                        ptr(sup_key), ptr(conf_pixel), ptr(conf_surfel), ptr(conf_stage), ptr(counts), ptr(branch))
     ns, nc = int(counts[0]), int(counts[1])
     r.sup_pixel, r.sup_key = sup_pixel[:ns], sup_key[:ns]
     conf_pixel, conf_surfel, conf_stage = conf_pixel[:nc], conf_surfel[:nc], conf_stage[:nc]
@@ -401,8 +375,9 @@ def blend(depth_pre, counts, sums, radius, depth_scaling, mutations=()):
     bound = [np.empty(P, np.float64) for _ in range(2)]
     level_counts = np.zeros((2, radius + 1), np.uint64)
     branch = np.zeros(len(FRONT_BRANCHES) + 1, np.uint64)
-    load().iw_blend(C.byref(p), int(radius), _p(depth_pre), _p(counts), _p(sums), _p(out), _p(lo), _p(hi), _p(dist[0]),
-                    _p(dist[1]), _p(delta[0]), _p(delta[1]), _p(bound[0]), _p(bound[1]), _p(level_counts), _p(branch))
+    load().iw_blend(C.byref(p), int(radius), ptr(depth_pre), ptr(counts), ptr(sums), ptr(out), ptr(lo), ptr(hi),
+                    ptr(dist[0]), ptr(dist[1]), ptr(delta[0]), ptr(delta[1]), ptr(bound[0]), ptr(bound[1]),
+                    ptr(level_counts), ptr(branch))
     return SimpleNamespace(depth=out.reshape(H, W), lo=lo.reshape(H, W), hi=hi.reshape(H, W),
                            level_counts=level_counts.astype(np.int64),
                            branch={name: int(v) for name, v in zip(FRONT_BRANCHES, branch)})

@@ -4,20 +4,15 @@ umbrella and per-owner share of every slot in each state, and the mesh an update
 previous owners' triangles outside R, the new ones inside R."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 from scipy.spatial import cKDTree
 
 from surfelmeshing_b200 import _lib as L
 from tests import mesh_walk as M
+from tests.cbuild import ptr
 
 SNAPSHOT_ROWS = (3, 4, 5, 7, 8, 9, 10)   # smooth x y z, radius^2, normal x y z
 WIDE = 64                                # an umbrella cap no slot reaches: the exact umbrella, overflow or not
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def walk(rows, params=None, cap=M.U):
@@ -30,11 +25,11 @@ def walk(rows, params=None, cap=M.U):
     counts = np.zeros(max(n, 1), np.uint32)
     stats = np.zeros(4, np.uint64)
     lib = M.load()
-    args = (_p(store), store.shape[1], n, p.neighbor_radius_factor, p.max_angle_between_normals_deg,
-            p.max_triangle_angle_deg, cap, _p(umbrella), _p(counts))
-    total = lib.mw_triangulate(*args, None, 0, _p(stats))
+    args = (ptr(store), store.shape[1], n, p.neighbor_radius_factor, p.max_angle_between_normals_deg,
+            p.max_triangle_angle_deg, cap, ptr(umbrella), ptr(counts))
+    total = lib.mw_triangulate(*args, None, 0, ptr(stats))
     tri = np.zeros((max(total, 1), 3), np.uint32)
-    lib.mw_triangulate(*args, _p(tri), total, _p(stats))
+    lib.mw_triangulate(*args, ptr(tri), total, ptr(stats))
     names = ("triangle_count", "vertices_meshed", "boundary_edges", "umbrella_overflows")
     return tri[:total], {k: int(v) for k, v in zip(names, stats)}, umbrella[:n], counts[:n]
 

@@ -1,51 +1,25 @@
 """ctypes loader for tests/mesh_walk.c (TEST INFRASTRUCTURE): the plain-C restatement of sm_triangulate, plus the
-hand-built clouds and the mesh invariants the host and GPU tests share. The library is compiled on first use into
-a temporary directory (keyed by the source's digest), so the repository tree stays untouched."""
+hand-built clouds and the mesh invariants the host and GPU tests share."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
 from surfelmeshing_b200 import _lib as L
+from tests import cbuild
 from tests import knn_cases
+from tests.cbuild import ptr
 
 SOURCE = Path(__file__).resolve().parent / "mesh_walk.c"
 U = L.MESH_MAX_UMBRELLA
 
-_lib = None
-
 
 def load():
-    global _lib
-    if _lib is None:
-        tag = hashlib.sha256(SOURCE.read_bytes()).hexdigest()[:16]
-        out_dir = Path(tempfile.gettempdir()) / f"mesh_walk_{os.getuid()}"
-        out_dir.mkdir(parents=True, exist_ok=True)
-        path = out_dir / f"libmesh_walk_{tag}.so"
-        if not path.exists():
-            cc = shutil.which("gcc") or shutil.which("cc")
-            if cc is None:
-                raise RuntimeError("a C compiler is needed to build the meshing checker")
-            tmp = out_dir / f"{path.name}.{os.getpid()}.tmp"
-            subprocess.run([cc, "-O2", "-fPIC", "-shared", "-std=gnu11", "-ffp-contract=off", "-o", str(tmp),
-                            str(SOURCE), "-lm"], check=True, capture_output=True)
-            os.replace(tmp, path)
-        _lib = C.CDLL(str(path))
-        _lib.mw_triangulate.restype = C.c_uint64
-        _lib.mw_triangulate.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_int,
-                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return cbuild.library(SOURCE, cbuild.WALK_FLAGS, {
+        "mw_triangulate": (C.c_uint64, [C.c_void_p, C.c_uint64, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_int,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p])})
 
 
 def triangulate(rows, params=None):
@@ -60,11 +34,11 @@ def triangulate(rows, params=None):
     counts = np.zeros(max(n, 1), np.uint32)
     stats = np.zeros(4, np.uint64)
     lib = load()
-    args = (_p(rows), rows.shape[1], n, p.neighbor_radius_factor, p.max_angle_between_normals_deg,
-            p.max_triangle_angle_deg, U, _p(umbrella), _p(counts))
-    total = lib.mw_triangulate(*args, None, 0, _p(stats))
+    args = (ptr(rows), rows.shape[1], n, p.neighbor_radius_factor, p.max_angle_between_normals_deg,
+            p.max_triangle_angle_deg, U, ptr(umbrella), ptr(counts))
+    total = lib.mw_triangulate(*args, None, 0, ptr(stats))
     tri = np.zeros((max(total, 1), 3), np.uint32)
-    lib.mw_triangulate(*args, _p(tri), total, _p(stats))
+    lib.mw_triangulate(*args, ptr(tri), total, ptr(stats))
     names = ("triangle_count", "vertices_meshed", "boundary_edges", "umbrella_overflows")
     return tri[:total], {k: int(v) for k, v in zip(names, stats)}, counts[:n]
 

@@ -8,10 +8,10 @@ from __future__ import annotations
 
 import numpy as np
 import torch
-from scipy.spatial.transform import Rotation
 
 from surfelmeshing_b200 import synthetic as S
 from tests import pyramid_walk as PW
+from tests.util import offset
 
 MASK64 = (1 << 64) - 1
 MAX_CANDIDATES = 8
@@ -151,11 +151,6 @@ class Database:
 
 
 # ---- kidnapped-camera frames ----------------------------------------------------------------------------------------
-
-def offset(rotvec_deg, translation) -> np.ndarray:
-    Rm = Rotation.from_rotvec(np.radians(rotvec_deg)).as_matrix()
-    return np.concatenate([Rm, np.asarray(translation, float)[:, None]], axis=1)
-
 
 def compose(a, b) -> np.ndarray:
     a, b = np.asarray(a, np.float64).reshape(3, 4), np.asarray(b, np.float64).reshape(3, 4)

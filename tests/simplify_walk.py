@@ -1,54 +1,28 @@
 """ctypes loader for tests/simplify_walk.c (TEST INFRASTRUCTURE): the plain-C restatement of sm_mesh_simplify, and
-the hand-built meshes the host and GPU tests share. The library is compiled on first use into a temporary directory
-(keyed by the source's digest), so the repository tree stays untouched."""
+the hand-built meshes the host and GPU tests share."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
 from surfelmeshing_b200 import _lib as L
+from tests import cbuild
 from tests import hole_walk as HW
 from tests import mesh_walk as M
+from tests.cbuild import ptr
 
 SOURCE = Path(__file__).resolve().parent / "simplify_walk.c"
 STAT_NAMES = [f for f, _ in L.SimplifyStats._fields_]
 ERRORS = {-1: "bad corner", -2: "repeated corner", -3: "duplicate edge"}
 
-_lib = None
-
 
 def load():
-    global _lib
-    if _lib is None:
-        tag = hashlib.sha256(SOURCE.read_bytes()).hexdigest()[:16]
-        out_dir = Path(tempfile.gettempdir()) / f"simplify_walk_{os.getuid()}"
-        out_dir.mkdir(parents=True, exist_ok=True)
-        path = out_dir / f"libsimplify_walk_{tag}.so"
-        if not path.exists():
-            cc = shutil.which("gcc") or shutil.which("cc")
-            if cc is None:
-                raise RuntimeError("a C compiler is needed to build the simplification checker")
-            tmp = out_dir / f"{path.name}.{os.getpid()}.tmp"
-            subprocess.run([cc, "-O2", "-fPIC", "-shared", "-std=gnu11", "-ffp-contract=off", "-o", str(tmp),
-                            str(SOURCE), "-lm"], check=True, capture_output=True)
-            os.replace(tmp, path)
-        _lib = C.CDLL(str(path))
-        _lib.sw_simplify.restype = C.c_int64
-        _lib.sw_simplify.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64,
-                                     C.POINTER(L.SimplifyParams), C.c_void_p, C.c_uint64, C.POINTER(L.SimplifyStats),
-                                     C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return cbuild.library(SOURCE, cbuild.WALK_FLAGS, {
+        "sw_simplify": (C.c_int64, [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64,
+                                    C.POINTER(L.SimplifyParams), C.c_void_p, C.c_uint64, C.POINTER(L.SimplifyStats),
+                                    C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)])})
 
 
 class InvalidMesh(ValueError):
@@ -80,8 +54,8 @@ def simplify(rows, tri, params=None, log=False):
     round_log = np.zeros((max(p.max_rounds, 1), 2), np.uint64)
     last = np.zeros(max(count, 1), np.uint64)
     last_count = C.c_uint64()
-    total = load().sw_simplify(_p(rows), rows.shape[1], n, _p(tri) if count else None, count, C.byref(p), _p(out),
-                               count, C.byref(stats), _p(round_log), _p(last), C.byref(last_count))
+    total = load().sw_simplify(ptr(rows), rows.shape[1], n, ptr(tri) if count else None, count, C.byref(p), ptr(out),
+                               count, C.byref(stats), ptr(round_log), ptr(last), C.byref(last_count))
     if total == -4:
         raise OrderDependent("a round's collapses depend on their order")
     if total < 0:

@@ -16,14 +16,11 @@ from surfelmeshing_b200 import reconstruction as R
 from surfelmeshing_b200._lib import SM_ERR_INVALID_ARGUMENT, SurfelError
 from tests import integrate_walk as IW
 from tests.test_association_walk_host import CASES, TILE, front_case, front_params
+from tests.util import dev
 
 pytestmark = pytest.mark.gpu
 
 PITCHED = {"tile-past-r18", "odd-r33", "flipped-r34"}   # the depth view starts 2 bytes into a wider row
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def depth_buffer(depth, pitched):

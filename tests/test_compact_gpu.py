@@ -9,10 +9,10 @@ import torch
 
 from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
-from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, TransferToken
+from surfelmeshing_b200._lib import TransferToken
 from tests import compact_walk as W
 from tests.test_compact_host import state as hand_state
-from tests.util import load_golden
+from tests.util import load_golden, params
 
 pytestmark = pytest.mark.gpu
 
@@ -24,12 +24,6 @@ SMOOTH_TOLERANCE = 1e-4   # metres
 CAP = 400_000
 K = 8
 INV = W.INVALID
-
-
-def params(cam=CAM):
-    pp = PreprocessParams.defaults()
-    pp.depth_valid_region_radius = cam.valid_region_radius()
-    return pp, IntegrateParams.defaults()
 
 
 def make(cap=CAP, cam=CAM):
@@ -44,7 +38,7 @@ def stream48():
 
 
 def run(rec, st, first, last):
-    pp, ip = params()
+    pp, ip = params(CAM)
     return rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp,
                           ip, first, last)
 
@@ -214,7 +208,7 @@ def near(a, b):
 
 @pytest.mark.parametrize("serial", [False, True], ids=["frame_graph", "serial"])
 def test_session_compacts_between_pushes(stream48, serial):
-    pp, ip = params()
+    pp, ip = params(CAM)
     st = stream48
     p = 30
     a = make()
@@ -287,7 +281,7 @@ def test_hand_off_after_compaction(stream48):
 # is 25 % + 0.1 mm. The cap is set from the plain run, so the test holds for any stream.
 def test_compacting_session_stays_under_the_cap():
     st = S.make_stream(CAM, 96, device="cuda")
-    pp, ip = params()
+    pp, ip = params(CAM)
     plain = make(cap=CAP)
     with plain.session(pp, ip, (CAM.width, CAM.height)) as s:
         for f in range(st.frame_count):
@@ -329,7 +323,7 @@ def test_compacting_session_stays_under_the_cap():
 
 
 def test_session_policy_compacts_when_headroom_runs_low(stream48):
-    pp, ip = params()
+    pp, ip = params(CAM)
     probe = make()
     run(probe, stream48, *stream48.integrated_range())
     cap = probe.surfels_size() + 2000

@@ -10,15 +10,11 @@ import torch
 from surfelmeshing_b200 import reconstruction as R
 from tests import integrate_walk as IW
 from tests.test_integrate_walk_host import CASES, build_case, integrate_params
-from tests.util import check_state_invariants
+from tests.util import check_state_invariants, dev
 
 pytestmark = pytest.mark.gpu
 
 META_DETACH = 0x80000000
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 @pytest.mark.parametrize("plain_tiebreak", [False, True], ids=["wave", "plain"])

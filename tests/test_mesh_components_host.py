@@ -2,12 +2,11 @@
 flood fill) checked against independent numpy / scipy code (scipy.sparse.csgraph.connected_components over the
 shared-edge graph, numpy sums) on the hand-built meshes, every mesh_walk case and golden f7; pieces that touch at a
 slot, a non-manifold edge, isolated triangles, ties in area, every threshold on both sides of its boundary, and the
-ABI. The GPU is held to the restatement bit for bit in tests/test_mesh_components_gpu.py.
+header's rules. The GPU is held to the restatement bit for bit in tests/test_mesh_components_gpu.py.
 
 Golden f7, meshed by the restated sm_triangulate: 21 217 triangles in 34 pieces; 11 pieces of fewer than 10
 triangles (42 triangles), 19 of fewer than 50 (219 triangles); 0.942 m^2 in all.
 """
-import ctypes as C
 from pathlib import Path
 
 import numpy as np
@@ -15,7 +14,6 @@ import pytest
 from scipy.sparse import coo_matrix
 from scipy.sparse.csgraph import connected_components
 
-from surfelmeshing_b200 import _lib
 from surfelmeshing_b200._lib import ComponentParams
 from tests import components_walk as CW
 from tests import mesh_walk as M
@@ -204,22 +202,8 @@ def test_invalid_inputs_are_refused():
     assert len(out) == len(labels) == len(table) == 0 and stats == dict.fromkeys(CW.STATS, 0)
 
 
-def test_struct_layouts_and_defaults():
-    assert C.sizeof(_lib.ComponentParams) == 24 and C.sizeof(_lib.ComponentStats) == 48
-    assert C.sizeof(_lib.MeshComponent) == 48 and CW.TABLE_DTYPE.itemsize == 48
-    assert [f for f, _ in _lib.ComponentParams._fields_] == ["min_triangles", "min_area", "keep_largest"]
-    p = ComponentParams.defaults()
-    assert (p.min_triangles, p.min_area, p.keep_largest) == (10, 0.0, 0)
-    assert "sm_mesh_components" in _lib.EXPORTED_SYMBOLS and "sm_default_component_params" in _lib.EXPORTED_SYMBOLS
+def test_header_declares_the_call():
     h = (Path(__file__).resolve().parents[1] / "include" / "surfel_b200.h").read_text()
     assert "int sm_mesh_components(" in h and "} sm_mesh_component;" in h
     for rule in ("C1. Input.", "C2. Adjacency.", "C3. Numbering.", "C4. Area.", "C5. Bounds.", "C6. Keep.", "C7. Output."):
         assert rule in h
-
-
-def test_default_params_match_the_library(product):
-    p = ComponentParams()
-    product.fn["default_component_params"](C.byref(p))
-    d = ComponentParams.defaults()
-    for name, _ in p._fields_:
-        assert getattr(p, name) == getattr(d, name), name

@@ -15,7 +15,8 @@ from tests import mesh_render_walk as MRW
 from tests import mesh_walk as M
 from tests.test_mesh_render_host import CAM as GRID_CAM, fan, grid_mesh, vertex_rows
 from tests.test_render_gpu import (BEHIND, CAM, FAR, IDENTITY, NEAR, OUTPUT_CAMERAS, VGA, ODD, assert_bit_equal, make,
-                                   orbit_pose, params)
+                                   orbit_pose)
+from tests.util import params
 
 pytestmark = pytest.mark.gpu
 
@@ -125,7 +126,7 @@ def test_golden_state_with_its_mesh():
 def integrated():
     """The cloud after 40 integrated frames of the VGA synthetic stream and its sm_triangulate mesh."""
     st = S.make_stream(CAM, 48, device="cuda")
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     first, last = st.integrated_range()
     rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
@@ -222,7 +223,7 @@ def test_pitched_outputs_and_subsets(integrated):
 
 def test_render_mesh_only_reads_the_state_and_repeats():
     st = S.make_stream(CAM, 24, device="cuda")
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     first, last = st.integrated_range()
     rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
@@ -244,7 +245,7 @@ def test_render_mesh_only_reads_the_state_and_repeats():
 
 def test_render_mesh_between_session_pushes():
     st = S.make_stream(CAM, 40, device="cuda")
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     seen = []
     with rec.session(pp, ip, (CAM.width, CAM.height)) as s:
@@ -321,7 +322,7 @@ SCENE_LIMITS = {
 @pytest.mark.parametrize("sigma", [None, 0.0], ids=["nominal_noise", "noise_free"])
 def test_rendered_mesh_depth_matches_the_scene(sigma):
     st = S.make_stream(CAM, 48, sigma_depth=sigma, device="cuda")
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     first, last = st.integrated_range()
     rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,

@@ -17,14 +17,10 @@ from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, SurfelError
 from tests.util import (GOLDEN_DIR, INTEGRATE_ROWS, INVALID, NEIGHBOR_ROWS, SMOOTH_ROWS, check_state_invariants,
-                        count_mismatch, digest, golden_camera, golden_params, link_stable_slots, load_npz_xz,
+                        count_mismatch, dev, digest, golden_camera, golden_params, link_stable_slots, load_npz_xz,
                         oracle_answers, other_frames, regularization_threshold, smooth_violations)
 
 pytestmark = pytest.mark.gpu
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def u16(h, w):

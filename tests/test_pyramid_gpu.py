@@ -11,17 +11,13 @@ from surfelmeshing_b200 import reconstruction as R
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, SurfelError
 from tests import pyramid_walk
 from tests.test_pyramid_host import depth_case
-from tests.util import count_mismatch
+from tests.util import count_mismatch, dev
 
 pytestmark = pytest.mark.gpu
 
 # SoA rows compared exactly after one frame: positions, confidence, radius, normals, stamps (the smooth rows
 # are left out: the regularisation sums with float atomics)
 EXACT_ROWS = (0, 1, 2, 6, 7, 8, 9, 10, 17, 18)
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def make(cam, cap=400_000, lib=None):

@@ -10,9 +10,10 @@ import torch
 
 from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
-from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, RelocParams, RelocResult, TrackRGBDParams
+from surfelmeshing_b200._lib import PreprocessParams, RelocParams, RelocResult, TrackRGBDParams
 from tests import reloc_walk as W
 from tests import track_walk as TW
+from tests.util import offset, params
 
 pytestmark = pytest.mark.gpu
 
@@ -24,12 +25,6 @@ MAX_T, MAX_R = 0.01, 0.5   # test_track_gpu.py::test_pose_free_stream at nominal
 
 def make(cam=VGA):
     return R.CUDASurfelReconstruction(CAP, cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy)
-
-
-def params(cam=VGA):
-    pp = PreprocessParams.defaults()
-    pp.depth_valid_region_radius = cam.valid_region_radius()
-    return pp, IntegrateParams.defaults()
 
 
 def with_(base=None, **kw):
@@ -154,7 +149,7 @@ def mapped():
     """The cloud of the first 150 frames of the VGA desk stream integrated with their true poses, and a database of
     those frames offered at their true poses with the default params."""
     st = S.make_stream(VGA, MAPPED, device="cuda")
-    pp, ip = params()
+    pp, ip = params(VGA)
     rec = make()
     first, last = st.integrated_range()
     rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
@@ -183,7 +178,7 @@ def cloud_params():
 @pytest.mark.parametrize("rgbd", [False, True], ids=["depth", "rgbd"])
 def test_accepted_pose_is_the_tracking_call_from_that_keyframe(mapped, revisits, rgbd):
     st, rec, db = mapped
-    pp, _ = params()
+    pp, _ = params(VGA)
     rp = TrackRGBDParams.defaults() if rgbd else None
     depth, color, truth = revisits[1]
     pose, res = rec.relocalise(db, depth, color, rgbd=rp, pp=pp)
@@ -200,7 +195,7 @@ def test_accepted_pose_is_the_tracking_call_from_that_keyframe(mapped, revisits,
     # the handle's previous frame is the accepted call's: a previous-frame track after sm_relocalise equals one after
     # that same tracking call
     nxt_depth, nxt_color, nxt_truth = revisits[1][0], revisits[1][1], truth
-    guess = TW.compose(nxt_truth, W.offset((0.3, 0, 0), (0.004, 0, 0))).astype(np.float32)
+    guess = TW.compose(nxt_truth, offset((0.3, 0, 0), (0.004, 0, 0))).astype(np.float32)
     rec.relocalise(db, depth, color, rgbd=rp, pp=pp)
     if rgbd:
         a, ra = rec.track_rgbd(nxt_depth, nxt_color, guess, rgbd=rp, pp=pp, source="previous")
@@ -215,7 +210,7 @@ def test_accepted_pose_is_the_tracking_call_from_that_keyframe(mapped, revisits,
 
 def test_relocalisation_only_reads_the_state(mapped, revisits):
     st, rec, db = mapped
-    pp, _ = params()
+    pp, _ = params(VGA)
     before, n0, m0 = rec.dump_state()
     before = before.copy()
     count = len(db)
@@ -229,7 +224,7 @@ def test_relocalisation_only_reads_the_state(mapped, revisits):
 
 def test_launch_counts(product, mapped, revisits):
     st, rec, db = mapped
-    pp, _ = params()
+    pp, _ = params(VGA)
     launches = product.fn["kernel_launch_count"]
     depth, color, truth = revisits[2]
     empty = R.KeyframeDatabase(rec)
@@ -261,7 +256,7 @@ def test_launch_counts(product, mapped, revisits):
 
 def test_invalid_arguments_are_rejected_without_a_launch(product, mapped):
     st, rec, db = mapped
-    pp, _ = params()
+    pp, _ = params(VGA)
     launches = product.fn["kernel_launch_count"]
     fn = rec.lib.fn
     bad = _lib.SM_ERR_INVALID_ARGUMENT
@@ -331,7 +326,7 @@ def test_invalid_arguments_are_rejected_without_a_launch(product, mapped):
 def test_relocalisation_during_a_session(mapped, revisits):
     """Relocalisation is allowed while a stream session is open, like tracking."""
     st, rec0, db0 = mapped
-    pp, ip = params()
+    pp, ip = params(VGA)
     rec = make()
     db = R.KeyframeDatabase(rec)
     with rec.session(pp, ip, (VGA.width, VGA.height)) as s:
@@ -353,7 +348,7 @@ def test_kidnapped_camera(mapped, revisits):
     the tracker from the pose before the jump reports them lost, sm_relocalise recovers them within the pose-free
     bounds, and frames of the never-mapped far side of the orbit are not accepted at a wrong pose."""
     st, rec, db = mapped
-    pp, _ = params()
+    pp, _ = params(VGA)
     pre_jump = st.global_T_frame[MAPPED - 1]
     report = []
     for (depth, color, truth), f in zip(revisits, REVISITS):
@@ -383,7 +378,7 @@ def jump_session(reloc):
     noise), through a TrackedSession."""
     st = S.make_stream(VGA, MAPPED, device="cuda")
     tail = W.jump_frames(VGA, 60, 20)
-    pp, ip = params()
+    pp, ip = params(VGA)
     rec = make()
     truth = list(st.global_T_frame) + [p for _, _, p in tail]
     with R.TrackedSession(rec, pp, ip, st.global_T_frame[0], reloc=reloc) as s:
@@ -423,7 +418,7 @@ def test_pose_free_session_without_relocalisation_pushes_wrong_poses():
 
 def test_pose_free_stream_without_loss_never_relocalises():
     st = S.make_stream(VGA, 120, device="cuda")
-    pp, ip = params()
+    pp, ip = params(VGA)
     rec = make()
     with R.TrackedSession(rec, pp, ip, st.global_T_frame[0], reloc=RelocParams.defaults()) as s:
         for f in range(st.frame_count):

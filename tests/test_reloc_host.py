@@ -1,18 +1,9 @@
 """The keyframe database's rules without a GPU: the numpy restatement (tests/reloc_walk.py) of the splitmix64 fern
-tables, the colour block means, nibble packing and distances, the query order and the add rule, and the ctypes
-layout and defaults of sm_reloc_*."""
-import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
-
+tables, the colour block means, nibble packing and distances, the query order and the add rule."""
 import numpy as np
 import pytest
 
-from surfelmeshing_b200 import _lib
 from tests import reloc_walk as W
-
-ROOT = Path(__file__).resolve().parents[1]
 
 
 def test_splitmix64_matches_the_published_sequence():
@@ -118,50 +109,3 @@ def test_encode_restatement_on_a_hand_built_frame():
     assert ((nib >> 1 & 1) == (t["g"] == 0)).all() and ((nib >> 2 & 1) == (t["b"] == 0)).all()
     assert ((nib >> 3 & 1) == (5000.0 >= t["depth"] * 5000.0)).all()
     assert ((enc.nibbles(np.zeros_like(depth), color) >> 3) == 0).all()   # D = 0 never sets bit 3
-
-
-def test_defaults_and_struct_layouts_match_the_header(product):
-    p = _lib.RelocParams()
-    product.fn["default_reloc_params"](C.byref(p))
-    d = _lib.RelocParams.defaults()
-    for name, _ in p._fields_:
-        if name != "track":
-            assert getattr(p, name) == getattr(d, name), name
-    assert bytes(p.track) == bytes(d.track)
-    track = _lib.TrackParams.defaults()
-    track.max_point_distance = 0.1
-    assert bytes(p.track) == bytes(track)
-    assert p.ferns % 8 == 0 and 1 <= p.level <= 4 and 1 <= p.candidates <= _lib.RELOC_MAX_CANDIDATES
-    cc = shutil.which("gcc") or shutil.which("cc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    src = r"""
-#include <stddef.h>
-#include <stdio.h>
-#include "surfel_b200.h"
-#define F(T, m) printf(#T "." #m " %zu\n", offsetof(T, m));
-int main(void) {
-  printf("sizeof.params %zu\nsizeof.result %zu\n", sizeof(sm_reloc_params), sizeof(sm_reloc_result));
-  F(sm_reloc_params, level) F(sm_reloc_params, ferns) F(sm_reloc_params, seed) F(sm_reloc_params, min_depth)
-  F(sm_reloc_params, max_depth) F(sm_reloc_params, capacity) F(sm_reloc_params, add_fraction)
-  F(sm_reloc_params, candidates) F(sm_reloc_params, max_query_fraction) F(sm_reloc_params, track)
-  F(sm_reloc_params, accept_inlier_fraction) F(sm_reloc_params, accept_rms)
-  F(sm_reloc_result, relocalised) F(sm_reloc_result, attempts) F(sm_reloc_result, keyframe)
-  F(sm_reloc_result, rank) F(sm_reloc_result, distance) F(sm_reloc_result, track)
-  printf("max %d\n", SM_RELOC_MAX_CANDIDATES);
-  return 0;
-}
-"""
-    import tempfile
-    with tempfile.TemporaryDirectory() as tmp:
-        c_file, exe = Path(tmp) / "layout.c", Path(tmp) / "layout"
-        c_file.write_text(src)
-        subprocess.run([cc, "-I", str(ROOT / "include"), "-o", str(exe), str(c_file)], check=True, capture_output=True)
-        out = dict(line.rsplit(" ", 1) for line in subprocess.run([str(exe)], capture_output=True, text=True,
-                                                                   check=True).stdout.splitlines())
-    assert int(out["sizeof.params"]) == C.sizeof(_lib.RelocParams)
-    assert int(out["sizeof.result"]) == C.sizeof(_lib.RelocResult)
-    assert int(out["max"]) == _lib.RELOC_MAX_CANDIDATES
-    for T, S in (("sm_reloc_params", _lib.RelocParams), ("sm_reloc_result", _lib.RelocResult)):
-        for name, _ in S._fields_:
-            assert int(out[f"{T}.{name}"]) == getattr(S, name).offset, (T, name)

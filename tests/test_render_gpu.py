@@ -9,9 +9,10 @@ import torch
 
 from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
-from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, RenderParams
+from surfelmeshing_b200._lib import RenderParams
 from tests import render_walk
 from tests.test_render_host import make_rows
+from tests.util import params
 
 pytestmark = pytest.mark.gpu
 
@@ -29,12 +30,6 @@ OUTPUT_CAMERAS = {"vga": VGA, "odd": ODD, "negative_fy": FLIPPED}
 
 def make(lib=None):
     return R.CUDASurfelReconstruction(CAP, CAM.width, CAM.height, CAM.fx, CAM.fy, CAM.cx, CAM.cy, lib=lib)
-
-
-def params(cam=CAM):
-    pp = PreprocessParams.defaults()
-    pp.depth_valid_region_radius = cam.valid_region_radius()
-    return pp, IntegrateParams.defaults()
 
 
 def walk(rows, T, near=NEAR, far=FAR, **cam):
@@ -108,7 +103,7 @@ def test_hand_built_clouds_bit_exact(case, cam):
 def integrated():
     """The cloud after 40 integrated frames of the VGA synthetic stream."""
     st = S.make_stream(CAM, 48, device="cuda")
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     first, last = st.integrated_range()
     rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
@@ -224,7 +219,7 @@ def test_invalid_arguments_are_rejected_without_a_launch(integrated, product):
 
 def test_render_between_session_pushes():
     st = S.make_stream(CAM, 40, device="cuda")
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     seen = []
 
@@ -269,7 +264,7 @@ SCENE_LIMITS = {
 @pytest.mark.parametrize("sigma", [None, 0.0], ids=["nominal_noise", "noise_free"])
 def test_rendered_depth_matches_the_scene(sigma):
     st = S.make_stream(CAM, 48, sigma_depth=sigma, device="cuda")
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     first, last = st.integrated_range()
     rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,

@@ -1,8 +1,5 @@
 """sm_render_surfels on the CPU: the plain-C restatement (tests/render_walk.c) against float64 geometry, its tie and
-merge rules, and the layout of sm_render_params. The GPU kernels are compared with the restatement bit for bit in
-tests/test_render_gpu.py."""
-import ctypes as C
-
+merge rules. The GPU kernels are compared with the restatement bit for bit in tests/test_render_gpu.py."""
 import numpy as np
 
 from surfelmeshing_b200 import _lib
@@ -113,11 +110,3 @@ def test_disk_around_the_camera_plane_is_clipped_by_the_ray_test():
     out = walk(make_rows([((0.0, 0.0, 0.2), (0, 0.3, -1), 1.0, (7, 7, 7))]))
     cover, _ = analytic_cover((0.0, 0.0, 0.2), (0, 0.3, -1), 1.0)
     assert cover.all() and np.all(out["index"] == 0)
-
-
-def test_render_params_layout():
-    p = _lib.RenderParams
-    assert C.sizeof(p) == 32
-    assert [(name, getattr(p, name).offset) for name, _ in p._fields_] == [
-        ("width", 0), ("height", 4), ("fx", 8), ("fy", 12), ("cx", 16), ("cy", 20), ("near_depth", 24),
-        ("far_depth", 28)]

@@ -15,14 +15,10 @@ from surfelmeshing_b200 import reconstruction as R
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams
 from tests.test_parity_gpu import (ENVELOPE_FACTOR, envelope_floors, envelope_limit, golden_final_state,
                                    golden_reconstruction)
-from tests.util import (INTEGRATE_ROWS, INVALID, NEIGHBOR_ROWS, check_state_invariants, count_mismatch, digest,
+from tests.util import (INTEGRATE_ROWS, INVALID, NEIGHBOR_ROWS, check_state_invariants, count_mismatch, dev, digest,
                         golden_camera, golden_params, oracle_answers, other_frames)
 
 pytestmark = pytest.mark.gpu
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def u16(h, w):

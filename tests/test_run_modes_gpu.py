@@ -4,14 +4,15 @@ import pytest
 
 from surfelmeshing_b200 import _lib
 from surfelmeshing_b200._lib import SurfelError
-from tests.test_session_gpu import assert_one_frame_equal, make, near, params, run_session, run_stream, vga  # noqa: F401
+from tests.test_session_gpu import CAM, assert_one_frame_equal, make, near, run_session, run_stream, vga  # noqa: F401
+from tests.util import params
 
 pytestmark = pytest.mark.gpu
 
 
 def radius4():
     """bilateral_filter_sigma_xy = 2 with the default radius factor 2: radius 4."""
-    pp, ip = params()
+    pp, ip = params(CAM)
     pp.bilateral_filter_sigma_xy = 2.0
     assert int(pp.bilateral_filter_radius_factor * pp.bilateral_filter_sigma_xy + 0.5) == 4
     return pp, ip
@@ -45,11 +46,11 @@ def test_session_against_stream(product, vga):
 
 def test_negative_radius_is_rejected(product, vga):
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     pp.bilateral_filter_sigma_xy = -3.0
     with pytest.raises(SurfelError) as err:
         run_stream(rec, st, others, 9, pp, ip)
     assert err.value.code == _lib.SM_ERR_INVALID_ARGUMENT
-    pp, ip = params()
+    pp, ip = params(CAM)
     assert run_stream(rec, st, others, 9, pp, ip).frames_integrated == 1

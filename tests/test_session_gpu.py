@@ -10,8 +10,8 @@ import torch
 
 from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
-from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, TransferToken
-from tests.util import check_state_invariants, count_mismatch
+from surfelmeshing_b200._lib import TransferToken
+from tests.util import check_state_invariants, count_mismatch, params
 
 pytestmark = pytest.mark.gpu
 
@@ -28,12 +28,6 @@ def vga():
     others = R.stream_outlier_filter_transforms(st.global_T_frame, st.frame_T_global, K, st.depth_scaling)
     torch.cuda.synchronize()
     return st, others
-
-
-def params(cam=CAM):
-    pp = PreprocessParams.defaults()
-    pp.depth_valid_region_radius = cam.valid_region_radius()
-    return pp, IntegrateParams.defaults()
 
 
 def make(cam=CAM, lib=None):
@@ -82,7 +76,7 @@ def near(a, b):
 @pytest.mark.parametrize("mode", ["device", "pageable", "pinned"])
 def test_one_integrated_frame(product, vga, mode):
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     ref = make()
     run_stream(ref, st, others, 9, pp, ip)
     rec = make()
@@ -94,7 +88,7 @@ def test_one_integrated_frame(product, vga, mode):
 
 def test_serial_mode_with_timings(product, vga):
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     ref = make()
     ref.enable_timings(True)
     run_stream(ref, st, others, 9, pp, ip)
@@ -110,7 +104,7 @@ def test_serial_mode_with_timings(product, vga):
 
 def test_whole_stream(product, vga):
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     ref = make()
     want = run_stream(ref, st, others, 60, pp, ip)
     rec = make()
@@ -178,7 +172,7 @@ def test_every_feature_allocates_and_frees_its_scratch(product, vga):
 
 def test_hand_off_between_pushes(product, vga):
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     persistent = R.make_cpu_buffers(CAP)
     token = TransferToken()
@@ -222,7 +216,7 @@ def test_hand_off_between_pushes(product, vga):
 
 def test_ordering_of_calls_on_the_stream(product, vga):
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     rec = make()
     with rec.session(pp, ip, (640, 480)) as s:
         for f in range(20):
@@ -252,7 +246,7 @@ def test_regularize_between_pushes(product, vga):
     integrated per push, nothing of the next frame in flight) given the same Regularize() calls at the same newest
     integrated frames; a serial session without them is the control that shows what the calls change."""
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     regularize_at = (12, 15)
 
     def run(serial, regularize):
@@ -290,7 +284,7 @@ def test_regularize_between_pushes(product, vga):
 
 def test_rejected_calls(product, vga):
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     ref = make()
     run_stream(ref, st, others, 9, pp, ip)
     rec = make()
@@ -339,7 +333,7 @@ def test_rejected_calls(product, vga):
 
 def test_against_reference(product, reference, vga):
     st, others = vga
-    pp, ip = params()
+    pp, ip = params(CAM)
     oracle = make(lib=reference)
     want = run_stream(oracle, st, others, 20, pp, ip)
     got = run_session(make(), st, 20, pp, ip)

@@ -1,4 +1,4 @@
-"""sm_outlier_filter_transforms (host only, APP/main.cc:1039-1058) and the layout of sm_session_status."""
+"""sm_outlier_filter_transforms (host only, APP/main.cc:1039-1058)."""
 import ctypes as C
 
 import numpy as np
@@ -90,11 +90,6 @@ def test_rejections(product, poses):
     assert product.fn["outlier_filter_transforms"](8, DEPTH_SCALING, FRAMES, None, None, 100,
                                                    out.ctypes.data_as(C.c_void_p)) == _lib.SM_ERR_INVALID_ARGUMENT
     assert b"other_count" in product.fn["last_error"]() or b"null" in product.fn["last_error"]()
-
-
-def test_session_status_layout():
-    assert C.sizeof(_lib.SessionStatus) == 16
-    assert _lib.SessionStatus.last_integrated_frame.offset == 8
 
 
 def test_stream_transforms_match_per_frame_call(product, poses):

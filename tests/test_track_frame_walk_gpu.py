@@ -17,6 +17,7 @@ from surfelmeshing_b200 import reconstruction as R
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, TrackParams, TrackRGBDParams
 from tests import track_rgbd_walk as RW
 from tests import track_walk as TW
+from tests.util import offset
 
 pytestmark = pytest.mark.gpu
 
@@ -37,11 +38,6 @@ def pre(cam):
     pp = PreprocessParams.defaults()
     pp.depth_valid_region_radius = cam.valid_region_radius()
     return pp
-
-
-def offset(rotvec_deg, translation):
-    Rm = Rotation.from_rotvec(np.radians(rotvec_deg)).as_matrix()
-    return np.concatenate([Rm, np.asarray(translation, float)[:, None]], axis=1)
 
 
 def schedule(levels=3, iterations=(4, 5, 10, 0), **fields):

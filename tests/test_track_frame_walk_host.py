@@ -10,6 +10,7 @@ from scipy.spatial.transform import Rotation
 
 from surfelmeshing_b200._lib import TrackParams
 from tests import track_walk as TW
+from tests.util import offset
 
 CAM = (160, 120, 131.25, 131.25, 80.0, 60.0)   # TUM fr1 intrinsics at 160 x 120, pixel-corner convention
 EPS = np.finfo(np.float64).eps
@@ -18,11 +19,6 @@ EPS = np.finfo(np.float64).eps
 def pack(A, g):
     """The 27 sums of a system J^T J = A, J^T r = g."""
     return np.array([A[i, j] for i in range(6) for j in range(i, 6)] + list(g), np.float64)
-
-
-def offset(rotvec_deg, translation):
-    R = Rotation.from_rotvec(np.radians(rotvec_deg)).as_matrix()
-    return np.concatenate([R, np.asarray(translation, float)[:, None]], axis=1)
 
 
 # ---- the solve -------------------------------------------------------------------------------------------------------

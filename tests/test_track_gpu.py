@@ -6,12 +6,12 @@ import ctypes as C
 import numpy as np
 import pytest
 import torch
-from scipy.spatial.transform import Rotation
 
 from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
-from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams, TrackParams, TrackResult
+from surfelmeshing_b200._lib import PreprocessParams, TrackParams, TrackResult
 from tests import track_walk as TW
+from tests.util import offset, params
 
 pytestmark = pytest.mark.gpu
 
@@ -27,17 +27,6 @@ def cam_tuple(cam):
 
 def make(cam=VGA):
     return R.CUDASurfelReconstruction(CAP, cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy)
-
-
-def params(cam=VGA):
-    pp = PreprocessParams.defaults()
-    pp.depth_valid_region_radius = cam.valid_region_radius()
-    return pp, IntegrateParams.defaults()
-
-
-def offset(rotvec_deg, translation):
-    Rm = Rotation.from_rotvec(np.radians(rotvec_deg)).as_matrix()
-    return np.concatenate([Rm, np.asarray(translation, float)[:, None]], axis=1)
 
 
 pose_error = TW.pose_error
@@ -83,7 +72,7 @@ def test_linearize_matches_restatement_on_planes(scene, level, off):
 def integrated():
     """The cloud after 40 integrated frames of the VGA synthetic stream."""
     st = S.make_stream(VGA, 48, device="cuda")
-    pp, ip = params()
+    pp, ip = params(VGA)
     rec = make()
     first, last = st.integrated_range()
     rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
@@ -130,7 +119,7 @@ def test_recovers_the_pose_of_exact_data(integrated, perturbation):
     guess = TW.compose(pose, offset(*perturbation)).astype(np.float32)
     t0, r0 = pose_error(guess, pose)
     assert t0 > 0.01 or r0 > 1.5
-    pp, _ = params()
+    pp, _ = params(VGA)
     out, res = rec.track(live, guess, pp=pp)
     dt, dr = pose_error(out, pose)
     print(f"exact data, start {t0 * 1000:.1f} mm / {r0:.2f} deg: {dt * 1000:.3f} mm, {dr:.4f} deg, "
@@ -147,7 +136,7 @@ def test_a_five_degree_tilt_is_reported_lost(integrated):
     pose = st.global_T_frame[30]
     guess = TW.compose(pose, offset(TILT_5, (0, 0, 0))).astype(np.float32)
     assert abs(pose_error(guess, pose)[1] - 5.0) < 1e-3
-    pp, _ = params()
+    pp, _ = params(VGA)
     out, res = rec.track(quantized_render(rec, pose), guess, pp=pp)
     assert res.tracked == 0 and np.array_equal(out, guess)
 
@@ -160,7 +149,7 @@ def test_a_guess_off_so3_is_projected(integrated):
     guess = TW.compose(pose, offset((0.5, 0, 0), (0.005, 0, 0))).astype(np.float32)
     guess[:, :3] *= np.float32(1.002)
     guess[0, 1] += np.float32(0.001)
-    pp, _ = params()
+    pp, _ = params(VGA)
     out, res = rec.track(quantized_render(rec, pose), guess, pp=pp)
     rot = out[:, :3].astype(np.float64)
     assert res.tracked == 1
@@ -171,7 +160,7 @@ def test_a_guess_off_so3_is_projected(integrated):
 
 def test_two_calls_are_bit_identical(integrated):
     st, rec = integrated
-    pp, _ = params()
+    pp, _ = params(VGA)
     live = st.depth[32].cuda()
     guess = TW.compose(st.global_T_frame[32], offset((0.5, 0.5, 0), (0.01, 0, 0))).astype(np.float32)
     a, ra = rec.track(live, guess, pp=pp)
@@ -183,7 +172,7 @@ def test_two_calls_are_bit_identical(integrated):
 
 def test_tracking_only_reads_the_state(integrated):
     st, rec = integrated
-    pp, _ = params()
+    pp, _ = params(VGA)
     before, n0, m0 = rec.dump_state()
     before = before.copy()
     rec.track(st.depth[33].cuda(), st.global_T_frame[33], pp=pp)
@@ -195,7 +184,7 @@ def test_tracking_only_reads_the_state(integrated):
 
 def test_lost_frames_return_the_guess(integrated):
     st, rec = integrated
-    pp, _ = params()
+    pp, _ = params(VGA)
     empty = make()
     guess = st.global_T_frame[20]
     out, res = empty.track(st.depth[20].cuda(), guess, pp=pp)
@@ -290,7 +279,7 @@ def test_invalid_arguments_are_rejected_without_a_launch(product):
 
 def test_tracking_between_session_pushes():
     st = S.make_stream(VGA, 30, device="cuda")
-    pp, ip = params()
+    pp, ip = params(VGA)
     rec = make()
     tracked = []
     with rec.session(pp, ip, (VGA.width, VGA.height)) as s:
@@ -322,7 +311,7 @@ def median_scene_error(rec, st, f):
 @pytest.mark.parametrize("sigma,max_t,max_r", [(None, 0.01, 0.5), (0.0, 0.002, 0.1)], ids=["nominal_noise", "noise_free"])
 def test_pose_free_stream(sigma, max_t, max_r):
     st = S.make_stream(VGA, 120, sigma_depth=sigma, device="cuda")
-    pp, ip = params()
+    pp, ip = params(VGA)
     rec = make()
     with R.TrackedSession(rec, pp, ip, st.global_T_frame[0]) as s:
         for f in range(st.frame_count):

@@ -1,21 +1,15 @@
 """The tracking rules without a GPU: the numpy restatement (tests/track_walk.py) against finite differences, scipy's
-rotation vector and a Gauss-Newton loop on analytic plane scenes; the ctypes layout and defaults of sm_track_*."""
-import ctypes as C
+rotation vector and a Gauss-Newton loop on analytic plane scenes."""
 import math
 
 import numpy as np
 import pytest
 from scipy.spatial.transform import Rotation
 
-from surfelmeshing_b200 import _lib
 from tests import track_walk as TW
+from tests.util import offset
 
 CAM = (160, 120, 131.25, 131.25, 80.0, 60.0)   # TUM fr1 intrinsics at 160 x 120, pixel-corner convention
-
-
-def offset(rotvec_deg, translation):
-    R = Rotation.from_rotvec(np.radians(rotvec_deg)).as_matrix()
-    return np.concatenate([R, np.asarray(translation, float)[:, None]], axis=1)
 
 
 def scene_images(name, model_T_live, level=0, holes=False):
@@ -85,26 +79,6 @@ def test_restatement_rules_on_holes_and_gates():
     assert lin["valid"] < interior and lin["inliers"] < lin["valid"]
     far = offset((0, 0, 0), (0, 0, 1.0)).astype(np.float32)
     assert TW.linearize(live, 5000.0, lc[2:], md, mn, CAM[2:], far)["inliers"] == 0
-
-
-def test_track_struct_layouts():
-    assert C.sizeof(_lib.TrackParams) == 44
-    assert C.sizeof(_lib.TrackResult) == 20
-    assert [f for f, _ in _lib.TrackParams._fields_] == [
-        "levels", "iterations", "max_point_distance", "max_normal_angle_deg", "min_inlier_fraction",
-        "convergence_rotation", "convergence_translation", "model_source"]
-
-
-def test_default_track_params_match(product):
-    tp = _lib.TrackParams()
-    product.fn["default_track_params"](C.byref(tp))
-    d = _lib.TrackParams.defaults()
-    for name, _ in tp._fields_:
-        a, b = getattr(tp, name), getattr(d, name)
-        if name == "iterations":
-            a, b = list(a), list(b)
-        assert a == b, name
-    assert list(tp.iterations) == [4, 5, 10, 0] and tp.levels == 3 and tp.model_source == _lib.TRACK_CLOUD
 
 
 def test_pose_chain_stays_rigid():

@@ -11,9 +11,10 @@ from scipy.spatial.transform import Rotation
 
 from surfelmeshing_b200 import _lib, synthetic as S
 from surfelmeshing_b200 import reconstruction as R
-from surfelmeshing_b200._lib import (IntegrateParams, PreprocessParams, TrackParams, TrackRGBDParams, TrackRGBDResult)
+from surfelmeshing_b200._lib import TrackParams, TrackRGBDParams, TrackRGBDResult
 from tests import track_rgbd_walk as RW
 from tests import track_walk as TW
+from tests.util import offset, params
 
 pytestmark = pytest.mark.gpu
 
@@ -31,17 +32,6 @@ def cam_tuple(cam):
 
 def make(cam=VGA):
     return R.CUDASurfelReconstruction(CAP, cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy)
-
-
-def params(cam=VGA):
-    pp = PreprocessParams.defaults()
-    pp.depth_valid_region_radius = cam.valid_region_radius()
-    return pp, IntegrateParams.defaults()
-
-
-def offset(rotvec_deg, translation):
-    Rm = Rotation.from_rotvec(np.radians(rotvec_deg)).as_matrix()
-    return np.concatenate([Rm, np.asarray(translation, float)[:, None]], axis=1)
 
 
 def cuda(a, dtype=None):
@@ -100,7 +90,7 @@ def test_linearize_rgbd_matches_restatement_on_textured_planes(scene, level, off
 def integrated():
     """The cloud after 40 integrated frames of the VGA synthetic stream."""
     st = S.make_stream(VGA, 48, device="cuda")
-    pp, ip = params()
+    pp, ip = params(VGA)
     rec = make()
     first, last = st.integrated_range()
     rec.stream_run(None, st.depth, st.color, st.global_T_frame, st.frame_T_global, st.others_TR_reference, pp, ip,
@@ -131,7 +121,7 @@ def test_linearize_rgbd_matches_restatement_on_a_rendered_cloud(integrated, leve
 
 def test_weight_zero_is_sm_track_frame(integrated):
     st, rec = integrated
-    pp, _ = params()
+    pp, _ = params(VGA)
     rp = TrackRGBDParams.defaults()
     rp.photometric_weight = 0.0
     depth, color = st.depth[32].cuda(), st.color[32].cuda()
@@ -161,7 +151,7 @@ def test_recovers_the_pose_of_exact_data(integrated, perturbation):
     pose = st.global_T_frame[30]
     live, color = quantized_render(rec, pose)
     guess = TW.compose(pose, offset(*perturbation)).astype(np.float32)
-    pp, _ = params()
+    pp, _ = params(VGA)
     out, res = rec.track_rgbd(live, color, guess, pp=pp)
     dt, dr = pose_error(out, pose)
     print(f"exact data rgbd: {dt * 1000:.3f} mm, {dr:.4f} deg, {res.depth.iterations} steps, photometric inliers "
@@ -241,7 +231,7 @@ def test_pose_free_desk_stream(sigma, max_t, max_r):
 
 def test_two_calls_are_bit_identical_and_read_only(integrated):
     st, rec = integrated
-    pp, _ = params()
+    pp, _ = params(VGA)
     before, n0, m0 = rec.dump_state()
     before = before.copy()
     guess = TW.compose(st.global_T_frame[32], offset((0.5, 0.5, 0), (0.01, 0, 0))).astype(np.float32)
@@ -257,7 +247,7 @@ def test_two_calls_are_bit_identical_and_read_only(integrated):
 
 def test_lost_frames_return_the_guess(integrated):
     st, rec = integrated
-    pp, _ = params()
+    pp, _ = params(VGA)
     guess = st.global_T_frame[20]
     out, res = make().track_rgbd(st.depth[20].cuda(), st.color[20].cuda(), guess, pp=pp)
     assert res.depth.tracked == 0 and np.array_equal(out, np.asarray(guess, np.float32))
@@ -339,7 +329,7 @@ def test_invalid_arguments_are_rejected_without_a_launch(product):
 
 def test_launch_count_does_not_depend_on_the_data(integrated, product):
     st, rec = integrated
-    pp, _ = params()
+    pp, _ = params(VGA)
     counts = []
     for guess in (st.global_T_frame[32], TW.compose(st.global_T_frame[32], offset((0, 0, 0), (0, 0, 1.0)))):
         torch.cuda.synchronize()

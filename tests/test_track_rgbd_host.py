@@ -1,23 +1,16 @@
 """The RGB-D tracking rules without a GPU: the numpy restatement (tests/track_rgbd_walk.py) against finite differences,
 the pyramid's edge rule, the rank of the depth-only and the joint systems on a single textured plane, Gauss-Newton on
-the restatement, weight 0, and the ctypes layout and defaults of sm_track_rgbd_*."""
-import ctypes as C
-
+the restatement and weight 0."""
 import numpy as np
 import pytest
 from scipy.spatial.transform import Rotation
 
-from surfelmeshing_b200 import _lib
 from tests import track_rgbd_walk as RW
 from tests import track_walk as TW
+from tests.util import offset
 
 CAM = (160, 120, 131.25, 131.25, 80.0, 60.0)   # TUM fr1 intrinsics at 160 x 120, pixel-corner convention
 WEIGHTS = dict(photometric_weight=2e-4, max_intensity_residual=40.0, min_gradient=2.0)
-
-
-def offset(rotvec_deg, translation):
-    R = Rotation.from_rotvec(np.radians(rotvec_deg)).as_matrix()
-    return np.concatenate([R, np.asarray(translation, float)[:, None]], axis=1)
 
 
 def textured_images(name, model_T_live, level=0):
@@ -134,20 +127,3 @@ def test_weight_zero_is_the_depth_system(level):
     ref = TW.linearize(live, 5000.0, lc[2:], md, mn, CAM[2:], T)
     assert np.array_equal(lin["system"], ref["system"])
     assert lin["inliers"] == ref["inliers"] and lin["photometric_inliers"] > 0
-
-
-def test_track_rgbd_struct_layouts():
-    assert C.sizeof(_lib.TrackRGBDParams) == 12
-    assert C.sizeof(_lib.TrackRGBDResult) == 28
-    assert [f for f, _ in _lib.TrackRGBDParams._fields_] == ["photometric_weight", "max_intensity_residual",
-                                                             "min_gradient"]
-    assert [f for f, _ in _lib.TrackRGBDResult._fields_] == ["depth", "photometric_inliers", "rms_intensity"]
-    assert _lib.TrackRGBDResult.photometric_inliers.offset == 20
-
-
-def test_default_track_rgbd_params_match(product):
-    rp = _lib.TrackRGBDParams()
-    product.fn["default_track_rgbd_params"](C.byref(rp))
-    d = _lib.TrackRGBDParams.defaults()
-    for name, _ in rp._fields_:
-        assert getattr(rp, name) == getattr(d, name), name

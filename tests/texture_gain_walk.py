@@ -1,55 +1,27 @@
 """ctypes loader for tests/texture_gain_walk.c (TEST INFRASTRUCTURE): the plain-C restatement of
-sm_mesh_texture_compensated. The library is compiled on first use into a temporary directory (keyed by the digest
-of its sources), so the repository tree stays untouched."""
+sm_mesh_texture_compensated."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
 from surfelmeshing_b200._lib import TextureGainParams, TextureParams
+from tests import cbuild
 from tests import texture_walk as TW
+from tests.cbuild import ptr
 
-HERE = Path(__file__).resolve().parent
-SOURCE = HERE / "texture_gain_walk.c"
-SOURCES = (SOURCE, *TW.SOURCES)   # each includes the next
+SOURCE = Path(__file__).resolve().parent / "texture_gain_walk.c"
 
 GAIN_STATS = ("points", "samples", "views_fitted", "rms_before", "rms_after")
 
-_lib = None
-
 
 def load():
-    global _lib
-    if _lib is None:
-        tag = hashlib.sha256(b"".join(p.read_bytes() for p in SOURCES)).hexdigest()[:16]
-        out_dir = Path(tempfile.gettempdir()) / f"texture_gain_walk_{os.getuid()}"
-        out_dir.mkdir(parents=True, exist_ok=True)
-        path = out_dir / f"libtexture_gain_walk_{tag}.so"
-        if not path.exists():
-            cc = shutil.which("gcc") or shutil.which("cc")
-            if cc is None:
-                raise RuntimeError("a C compiler is needed to build the texture gain checker")
-            tmp = out_dir / f"{path.name}.{os.getpid()}.tmp"
-            subprocess.run([cc, "-O2", "-fPIC", "-shared", "-std=gnu11", "-ffp-contract=off", "-o", str(tmp),
-                            str(SOURCE), "-lm"], check=True, capture_output=True)
-            os.replace(tmp, path)
-        _lib = C.CDLL(str(path))
-        _lib.txg_texture.restype = C.c_uint32
-        _lib.txg_texture.argtypes = ([C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.c_float, C.c_float,
-                                      C.c_float, C.c_int] + [C.c_void_p] * 4 +
-                                     [C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float] + [C.c_void_p] * 6)
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return cbuild.library(SOURCE, cbuild.WALK_FLAGS, {
+        "txg_texture": (C.c_uint32, [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.c_float, C.c_float,
+                                     C.c_float, C.c_int] + [C.c_void_p] * 4 +
+                        [C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float] + [C.c_void_p] * 6)})
 
 
 def points(count: int, view_count: int, max_samples: int) -> int:
@@ -92,11 +64,11 @@ def texture(rows, triangles, views, params=None, gains=None, with_samples=False)
     P = points(count, V, gp.max_samples)
     samples = np.zeros((max(V, 1), max(P, 1), 3), np.float32)
     lib = load()
-    errors = lib.txg_texture(_p(rows), rows.shape[1], rows.shape[1], _p(tris), count, float(p.texel_size),
-                             TW.cos_max(p), float(p.depth_tolerance), V, _p(size), _p(cam), _p(T),
+    errors = lib.txg_texture(ptr(rows), rows.shape[1], rows.shape[1], ptr(tris), count, float(p.texel_size),
+                             TW.cos_max(p), float(p.depth_tolerance), V, ptr(size), ptr(cam), ptr(T),
                              C.cast(colors, C.c_void_p), int(gp.max_samples), int(gp.iterations),
                              float(gp.sigma_noise), float(gp.sigma_gain), float(gp.min_level), float(gp.max_level),
-                             _p(atlas), _p(uv), _p(st), _p(g), _p(gs), _p(samples))
+                             ptr(atlas), ptr(uv), ptr(st), ptr(g), ptr(gs), ptr(samples))
     if errors:
         raise ValueError(f"input error bits {errors}")
     stats = dict(zip(TW.STATS, (int(x) for x in st)))

@@ -1,53 +1,25 @@
 """ctypes loader for tests/texture_walk.c (TEST INFRASTRUCTURE): the plain-C restatement of sm_mesh_texture, and the
-hand-built scenes of the texture tests. The library is compiled on first use into a temporary directory (keyed by the
-digest of its sources), so the repository tree stays untouched."""
+hand-built scenes of the texture tests."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
 import math
-import os
-import shutil
-import subprocess
-import tempfile
 from pathlib import Path
 
 import numpy as np
 
 from surfelmeshing_b200._lib import TextureParams
+from tests import cbuild
 from tests import mesh_walk as M
+from tests.cbuild import ptr
 
-HERE = Path(__file__).resolve().parent
-SOURCE = HERE / "texture_walk.c"
-SOURCES = (SOURCE, HERE / "mesh_render_walk.c", HERE / "render_walk.c")   # each includes the next
-
-_lib = None
+SOURCE = Path(__file__).resolve().parent / "texture_walk.c"
 
 
 def load():
-    global _lib
-    if _lib is None:
-        tag = hashlib.sha256(b"".join(p.read_bytes() for p in SOURCES)).hexdigest()[:16]
-        out_dir = Path(tempfile.gettempdir()) / f"texture_walk_{os.getuid()}"
-        out_dir.mkdir(parents=True, exist_ok=True)
-        path = out_dir / f"libtexture_walk_{tag}.so"
-        if not path.exists():
-            cc = shutil.which("gcc") or shutil.which("cc")
-            if cc is None:
-                raise RuntimeError("a C compiler is needed to build the texture checker")
-            tmp = out_dir / f"{path.name}.{os.getpid()}.tmp"
-            subprocess.run([cc, "-O2", "-fPIC", "-shared", "-std=gnu11", "-ffp-contract=off", "-o", str(tmp),
-                            str(SOURCE), "-lm"], check=True, capture_output=True)
-            os.replace(tmp, path)
-        _lib = C.CDLL(str(path))
-        _lib.txw_texture.restype = C.c_uint32
-        _lib.txw_texture.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.c_float, C.c_float,
-                                     C.c_float, C.c_int] + [C.c_void_p] * 7
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return cbuild.library(SOURCE, cbuild.WALK_FLAGS, {
+        "txw_texture": (C.c_uint32, [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.c_float, C.c_float,
+                                     C.c_float, C.c_int] + [C.c_void_p] * 7)})
 
 
 STATS = ("triangles", "atlas_width", "atlas_height", "texels", "texels_seen", "texels_fallback", "tiles_clamped",
@@ -91,9 +63,9 @@ def texture(rows, triangles, views, params=None, layout_only=False):
     colors = (C.c_void_p * max(V, 1))(*[v.color.ctypes.data for v in views])
     st = np.zeros(8, np.uint64)
     lib = load()
-    args = (_p(rows), rows.shape[1], n, _p(tris), count, float(p.texel_size), cos_max(p), float(p.depth_tolerance),
-            V, _p(size), _p(cam), _p(T), C.cast(colors, C.c_void_p))
-    errors = lib.txw_texture(*args, None, None, _p(st))
+    args = (ptr(rows), rows.shape[1], n, ptr(tris), count, float(p.texel_size), cos_max(p), float(p.depth_tolerance),
+            V, ptr(size), ptr(cam), ptr(T), C.cast(colors, C.c_void_p))
+    errors = lib.txw_texture(*args, None, None, ptr(st))
     if errors:
         raise ValueError(f"input error bits {errors}")
     stats = dict(zip(STATS, (int(x) for x in st)))
@@ -102,7 +74,7 @@ def texture(rows, triangles, views, params=None, layout_only=False):
     W, H = stats["atlas_width"], stats["atlas_height"]
     atlas = np.zeros((max(H, 1), max(W, 1), 3), np.uint8)
     uv = np.zeros((max(count, 1), 3, 2), np.float32)
-    lib.txw_texture(*args, _p(atlas), _p(uv), _p(st))
+    lib.txw_texture(*args, ptr(atlas), ptr(uv), ptr(st))
     return atlas[:H, :W], uv[:count], dict(zip(STATS, (int(x) for x in st)))
 
 

@@ -6,6 +6,8 @@ import lzma
 from pathlib import Path
 
 import numpy as np
+import torch
+from scipy.spatial.transform import Rotation
 
 from surfelmeshing_b200._lib import IntegrateParams, PreprocessParams
 
@@ -71,6 +73,23 @@ def oracle_answers():
     if _ORACLE_ANSWERS is None:
         _ORACLE_ANSWERS = json.loads((GOLDEN_DIR / "oracle_answers.json").read_text())
     return _ORACLE_ANSWERS
+
+
+def dev(a):
+    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+
+def offset(rotvec_deg, translation):
+    """The 3x4 rigid transform that turns by a rotation vector given in degrees, then moves by `translation`."""
+    R = Rotation.from_rotvec(np.radians(rotvec_deg)).as_matrix()
+    return np.concatenate([R, np.asarray(translation, float)[:, None]], axis=1)
+
+
+def params(cam):
+    """The default pre-processing and integration parameters, with the valid-region radius of camera `cam`."""
+    pp = PreprocessParams.defaults()
+    pp.depth_valid_region_radius = cam.valid_region_radius()
+    return pp, IntegrateParams.defaults()
 
 
 def golden_params(golden):
